@@ -59,6 +59,9 @@ def parse():
     ap.add_argument("--cpu-sample-steps", type=int, default=60)
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--force-shard", action="store_true", help="shard the elimination tree even below SHARD_MIN_FLOPS")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (device-resident run, rank 0) as DIR/<name>.npy: the step "
+                         "direction d (float64) and the inertia (pos, zero, neg) of its last factorisation")
     return ap.parse_args()
 
 
@@ -96,7 +99,7 @@ def config_of(args, st, world):
 
 # ----------------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """samples nvidia-smi SM clocks / throttle reasons while the timed region runs (B200_PROFILING.md recipe)"""
+    """samples nvidia-smi SM clocks / throttle reasons while the timed region runs"""
 
     def __init__(self, index=0):
         self.index = index
@@ -241,7 +244,7 @@ def cpu_baseline_sample(args, st, its):
     return out
 
 
-# ----------------------------------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------------------------------- GPU arm
 def run_b200(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -387,6 +390,10 @@ def run_b200(args, rank, world, local_rank):
         sampler.start()
     dev_ms, dev_wall = timed_run(False)
     cnt_dev = dict(la.cnt)
+    outputs = None
+    if args.dump_outputs and rank == 0:
+        outputs = {"direction": la.d.values.detach().cpu().numpy().astype(np.float64),
+                   "inertia": np.asarray(la.last_inertia, dtype=np.float64)}
     ser_ms, ser_wall = timed_run(True)
     e2e_ms, e2e_wall = timed_pipelined()
     assert pipe.h2d_bytes == h2d_bytes and pipe.d2h_bytes == d2h_bytes
@@ -412,8 +419,8 @@ def run_b200(args, rank, world, local_rank):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         # algorithmic bytes (SURVEY.md 8d): numeric factorisation 8*(nnz K + nnz L); one solve 2 sweeps x (8+4) B x nnz L
         alg_bytes = 8.0 * (stats["nnz_a"] + stats["nnz_l"])
         achieved = alg_bytes / (fac_ms * 1e-3) / 1e9 if fac_ms else None
@@ -425,11 +432,6 @@ def run_b200(args, rank, world, local_rank):
         e2e_val = units / (e2e_ms * 1e-3)
         nfac = max(1, cnt_dev["factorizations"])
         solves = cnt_dev["backsolves"] / nfac
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(args.workload if world == 1 else "", None)
-        except Exception:
-            pass
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": dev_ms / args.steps, "higher_is_better": True, "scaling": "strong" if sharded else "weak",
@@ -453,7 +455,6 @@ def run_b200(args, rank, world, local_rank):
                                  + solves * (stats["n_solve_launches"] + 6)) * args.steps),
             "roofline": {"kernel": "numeric multifrontal LDL^T of the whole elimination tree (k_factor_dep, one launch)", "bound": "hbm",
                          "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": (achieved / hbm_peak) if achieved else None,
-                         "traffic": traffic, "traffic_source": "profiles/traffic.json (ncu --set full dram read+write per launch)",
                          "algorithmic_bytes": alg_bytes, "peak_source": peak_src,
                          "note": "latency-bound: %d fronts of order <= %d in %d levels, %.3g Mflop" % (
                              stats["n_supernodes"], stats["max_front"], stats["n_levels"], stats["flops"] / 1e6)},
@@ -468,6 +469,10 @@ def run_b200(args, rank, world, local_rank):
             line["secondary"] = secondary
         if world == 1 and args.cpu_sample_steps > 0:
             line["cpu_baseline"] = cpu_baseline_sample(args, st, its)
+        if outputs is not None:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, arr in outputs.items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.barrier()
@@ -482,8 +487,8 @@ def run_secondary(args, rank, world, dev):
     try:
         import bench_configs as BC
         if world == 1:
-            out["fp64_peak_tflops"] = {"cublas_dgemm_8192": BC.dgemm_peak(), "dmma_issue_peak": 37.0,
-                                       "note": "fp64 roofline denominators (MEASURED_PEAKS.json has none)"}
+            out["fp64_peak_tflops"] = {"cublas_dgemm_8192": BC.dgemm_peak(), "fp64_tensor_datasheet": BC.DMMA_PEAK,
+                                       "note": "fp64 roofline denominators: measured cuBLAS DGEMM, H100 SXM data sheet"}
             out["c2_dense_n4096_m2048"] = BC.config2(cpu=True)
             out["c2_dense_n4096_m2048_neq256"] = BC.config2(n_eq=256, cpu=False, lib=False)
             out["c3_case1354_pegase"] = BC.config_sparse_opf("case1354_pegase")

@@ -1,5 +1,5 @@
 /*
- * b200kkt.h -- C ABI of the B200-native KKT hot path (assembly -> LDL^T + inertia -> solve).
+ * b200kkt.h -- C ABI of the H100-native KKT hot path (assembly -> LDL^T + inertia -> solve).
  *
  * This is the drop-in boundary a MadNLP.jl maintainer binds with `ccall` (see INTEGRATION.md
  * and madnlp.jl_b200/julia/B200KKT.jl).  Plain pointers and sizes only; no exceptions cross
@@ -73,7 +73,7 @@ typedef struct b2_options {
                                 them runs in one flag-driven launch (instead of one launch per level)          */
     int32_t chain_merge_f;   /* > 0: a supernode with exactly ONE child absorbs it whatever the explicit zeros cost, as long as the
                                 merged front stays team-class (order <= min(chain_merge_f, 64)): on latency-bound trees every
-                                level of the critical path costs ~5 us of hand-off besides its pivots, the zeros nothing.
+                                level of the critical path costs microseconds of hand-off besides its pivots, the zeros nothing.
                                 Default 0 = off (measured slower on the OPF trees: the single-child chains sit at the bottom, where the
                                 tree is throughput-bound and bigger leaves hurt); kept as an option for trees with long chains on top */
     int32_t reserved[4];
@@ -238,8 +238,8 @@ int b2d_condensed_assemble(int32_t n, int32_t m, int32_t ns, int32_t n_eq,
                            const double* pr_diag_d, const double* du_diag_d,
                            double* diag_buffer_d, double* aug_d, void* stream);
 
-/* The same assembly with the J' D J contraction on the 5th-generation tensor cores: fp64 is cut into 8 signed 7-bit digits per entry
- * (Ozaki scheme) and the 36 digit-pair products run as exact int8 GEMMs on tcgen05.mma.kind::i8 with TMA-staged operands
+/* The same assembly with the J' D J contraction on the Hopper tensor cores: fp64 is cut into 8 signed 7-bit digits per entry
+ * (Ozaki scheme) and the 36 digit-pair products run as exact int8 GEMMs on wgmma.mma_async (s8) with TMA-staged operands
  * (csrc/ozaki_kernels.cuh); the result agrees with the fp64 contraction to ~1e-14 of max|W| (parity bar 1e-13,
  * tests/test_gpu_parity_large.py).  The plan owns the digit planes (8 * n_pad * ns_pad bytes), exponents, tile list and tensor maps.
  * ns <= 16384.  b2d_ozaki_plan_status reports whether a (bounded) pipeline wait ever timed out. */

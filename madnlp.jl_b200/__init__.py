@@ -1,7 +1,7 @@
-"""madnlp.jl_b200 -- B200-native KKT hot path for MadNLP-style interior-point solvers.
+"""madnlp.jl_b200 -- H100-native KKT hot path for MadNLP-style interior-point solvers.
 
 Only what the hot path needs lives here (SURVEY.md section 8):
-  csrc/           hand-written sm_100a CUDA kernels + the C ABI (include/b200kkt.h) -> libb200kkt.so
+  csrc/           hand-written sm_90a CUDA kernels + the C ABI (include/b200kkt.h) -> libb200kkt.so
   capi.py         ctypes binding of that ABI (the same boundary Julia would `ccall`)
   linear_solvers  mirror of MadNLP's AbstractLinearSolver surface (B200SparseSolver, B200DenseSolver)
   kkt             mirror of the AbstractKKTSystem surface (SparseKKTSystem, SparseCondensedKKTSystem,

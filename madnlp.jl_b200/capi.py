@@ -66,7 +66,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            f"(or `make -C madnlp.jl_b200/csrc`). The B200 KKT path has no CPU fallback.")
+            f"(or `make -C madnlp.jl_b200/csrc`). The GPU KKT path has no CPU fallback.")
     return C.CDLL(LIB_PATH)
 
 
@@ -205,7 +205,7 @@ def device_count() -> int:
 
 def require_device():
     if device_count() == 0:
-        raise B2Error(B2_ERR_NO_DEVICE, "no CUDA device visible; the B200 KKT path has no CPU fallback")
+        raise B2Error(B2_ERR_NO_DEVICE, "no CUDA device visible; the GPU KKT path has no CPU fallback")
 
 
 def default_options(**kw) -> Options:

@@ -361,7 +361,7 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
                 double z = (double)z2 / (double)nnz2;
                 bool ok = (w2 <= 4) || (w2 <= nemin && z < 0.8) || (w2 <= 3 * nemin && z < zr) || (z < 0.25 * zr);
                 // latency rule: an only child is absorbed while the merged front stays team-class -- one level less on the tree's
-                // critical path (hand-off + staging ~5 us per level on the device) for a few explicit zeros in a front of order <= 64
+                // critical path (hand-off + staging per level on the device) for a few explicit zeros in a front of order <= 64
                 if (!ok && opt.chain_merge_f > 0 && nd[p].kids.size() == 1 && f2 <= std::min(opt.chain_merge_f, 64)) ok = true;
                 if (!ok) continue;
                 // merge c into p

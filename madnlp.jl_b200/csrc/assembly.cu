@@ -236,7 +236,8 @@ extern "C" int b2_condensed_assemble(b2_condensed_plan* p, double* aug_nz_d, con
 
 // ---------------------------------------------------------------------------------------------------------
 // dense condensed KKT (lower triangle):  aug[0:n,0:n] = J_I' D J_I + H + diag(pr[0:n]);  equality rows/diag below.
-// The SYRK runs on the fp64 tensor pipe (mma.sync m8n8k4 -> DMMA): 128x64 tile per 256-thread CTA, k-chunks of 16
+// The SYRK runs on the fp64 tensor pipe (mma.sync m16n8k4 -> DMMA; on H100 twice the issue rate of m8n8k4, measured with
+// tools/microbench/dmma_shapes.cu): 128x64 tile per 256-thread CTA, k-chunks of 16
 // double-buffered in shared memory; the sqrt(D) scaling of the reference's `jac_ineq` prologue kernel is folded into
 // the B operand (D, not sqrt(D): one operand is scaled once), the +H +diag epilogue kernel into the store.
 // ---------------------------------------------------------------------------------------------------------
@@ -307,12 +308,12 @@ __global__ void __launch_bounds__(256) k_dense_syrk(int n, int m, int ns, int N,
 #pragma unroll
             for (int y = 0; y < 4; ++y) bf[y] = Bs[buf][k0 + q][wj + 8 * y + g];
 #pragma unroll
-            for (int x = 0; x < 4; ++x)
+            for (int x = 0; x < 4; x += 2)                            // m16n8k4 = two m8n8k4 row blocks 8 apart sharing B
 #pragma unroll
                 for (int y = 0; y < 4; ++y)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1])
-                                 : "d"(af[x]), "d"(bf[y]));
+                    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1]), "+d"(c[x + 1][y][0]), "+d"(c[x + 1][y][1])
+                                 : "d"(af[x]), "d"(af[x + 1]), "d"(bf[y]));
         }
         if (ch + 1 < nchunk) sstore(buf ^ 1);
         __syncthreads();

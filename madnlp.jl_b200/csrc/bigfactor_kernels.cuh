@@ -18,8 +18,8 @@ namespace b2 {
 
 constexpr int DB = 128;                   // outer block (== BS of the solve kernels)
 
-// Shared-memory / warp-shuffle issue is the scarce resource of a single SM here (measured on B200,
-// tools/microbench/fp64_pipes.cu: one LDS.64 or SHFL.64 per ~4.6-9 clk per scheduler vs one DFMA per ~2 clk), so the
+// Shared-memory / warp-shuffle issue is the scarce resource of a single SM here (measured on H100,
+// tools/microbench/fp64_pipes.cu: one LDS.64 or SHFL.64 per ~4.5-8 clk per scheduler vs one DFMA per ~2 clk), so the
 // block lives in REGISTERS: 256 threads as a 16 x 16 grid, thread (ty, tx) owns the 8 x 8 entries (ty + 16a, tx + 16b)
 // -- cyclic, so the shrinking trailing matrix stays balanced.  The matrix is kept fully symmetric, which makes the pivot
 // column also the pivot row: per pivot the 16 owner threads publish it (one barrier), and every thread then needs just
@@ -65,8 +65,8 @@ __device__ __forceinline__ void diag128_invert_store(Diag128Smem& sm, const int 
     //          in registers, every l(i,k) is a shared-memory broadcast;
     //      (2) X_ij = -X_ii * (sum_{k=j}^{i-1} L_ik X_kj) for i > j, block row by block row and j ascending (so that L_ij may be
     //          overwritten by X_ij), each 32^3 product on the fp64 tensor pipe (8 warps x 2 tiles of m8n8k4 DMMA).
-    //      The round-1 version applied the 127 elementary row operations one by one (one mbarrier hand-off each, ~340 clk per step,
-    //      22 us of the 60 us this kernel sits on the factorisation's critical path); this is ~16 dependent steps.
+    //      Applying the 127 elementary row operations one by one would cost one mbarrier hand-off each on the factorisation's
+    //      critical path; this is ~16 dependent steps.
     __syncthreads();                                               // (the caller's reads of sm.Lc -- write-back of L11 -- are complete)
     {
         const int warp = tid >> 5, lane = tid & 31;
@@ -339,12 +339,12 @@ __global__ void __launch_bounds__(256, 2) k_big_trsm(FactorArgs a, const int32_t
 #pragma unroll
             for (int y = 0; y < 4; ++y) bf[y] = Bb[(k0 + q) * GU_LDB + wj + 8 * y + g];
 #pragma unroll
-            for (int x = 0; x < 4; ++x)
+            for (int x = 0; x < 4; x += 2)                            // m16n8k4 = two m8n8k4 row blocks 8 apart sharing B
 #pragma unroll
                 for (int y = 0; y < 4; ++y)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1])
-                                 : "d"(af[x]), "d"(bf[y]));
+                    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1]), "+d"(c[x + 1][y][0]), "+d"(c[x + 1][y][1])
+                                 : "d"(af[x]), "d"(af[x + 1]), "d"(bf[y]));
         }
     }
     // epilogue: Ut -> shared memory as Cs[i][c], then coalesced stores of L21(i, c) = Ut(c, i) / d_c  (i fastest)
@@ -369,8 +369,8 @@ __global__ void __launch_bounds__(256, 2) k_big_trsm(FactorArgs a, const int32_t
 // Near-diagonal step of the dense look-ahead schedule (sparse_ldl.cu: enqueue_dense_factor_lookahead).  Between two diagonal-block
 // kernels the critical path only needs (1) the 128 x 128 block of L right below the diagonal block and (2) the update of the NEXT
 // diagonal block with it.  The general kernels above do these as parts of whole-panel launches whose latency is one 128 x 64 x 128
-// tile on one SM (12 + 8 us); here the same 2 x 2.1 Mflop are cut into pieces small enough that latency, not per-SM tensor rate,
-// is what remains (~2 x 3 us), and the rest of the panel moves to a side branch that runs beside the next diagonal block.
+// tile on one SM; here the same 2 x 2.1 Mflop are cut into pieces small enough that latency, not per-SM tensor rate,
+// is what remains, and the rest of the panel moves to a side branch that runs beside the next diagonal block.
 //
 //   k_near_trsm  16 CTAs x 8 rows:  L(i, c) = (sum_{k <= c} A(i, k) Linv(c, k)) / d_c   for the rows i of block k+1, in place.
 //                Whole operands land in shared memory in one cp.async round trip (8 x 128 of A, the lower part of Linv); warp w owns
@@ -488,12 +488,9 @@ __global__ void __launch_bounds__(256, 2) k_near_syrk(FactorArgs a, const int32_
     for (int k0 = 0; k0 < DB; k0 += 4) {
         const double sc = dneg[k0 + q];
         const double bf = Bs[(k0 + q) * NS_LD + nb + g];
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-            const double af = As[(k0 + q) * NS_LD + mb + 8 * x + g] * sc;
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                         : "+d"(c[x][0]), "+d"(c[x][1]) : "d"(af), "d"(bf));
-        }
+        const double af0 = As[(k0 + q) * NS_LD + mb + g] * sc, af1 = As[(k0 + q) * NS_LD + mb + 8 + g] * sc;
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0][0]), "+d"(c[0][1]), "+d"(c[1][0]), "+d"(c[1][1]) : "d"(af0), "d"(af1), "d"(bf));
     }
 #pragma unroll
     for (int x = 0; x < 2; ++x)

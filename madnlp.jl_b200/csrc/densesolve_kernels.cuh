@@ -1,7 +1,7 @@
 // Dense triangular solves  x <- (L D L')^{-1} x  in ONE launch: a dataflow over the 128-wide block rows of the factor.
 //
-// The launch-per-block sweeps (bigsolve_kernels.cuh) cost 2 * N/128 dependent launches (64 at N = 4096: 0.59 ms for a job whose
-// HBM time is 20 us).  Here CTA k OWNS block row k of the forward sweep and block column k of the backward sweep:
+// The launch-per-block sweeps (bigsolve_kernels.cuh) cost 2 * N/128 dependent launches (64 at N = 4096, for a job whose
+// HBM time is tens of microseconds).  Here CTA k OWNS block row k of the forward sweep and block column k of the backward sweep:
 //
 //   forward :  t_k = b_k - sum_{c<k} L(k,c) y_c   accumulated as the y_c become available,  y_k = Linv_k t_k
 //   diagonal:  z_k = y_k ./ d_k

@@ -248,7 +248,7 @@ __device__ __forceinline__ double fast_rcp_d(double x) {
 // Trailing update of the blocked factorisation (> 95 % of the flops of a big front; see bigfactor_kernels.cuh):
 //   C(i,j) -= sum_{k in [kb0, kb0+kcount)} L(i,k) d_k L(j,k),  i >= j, jlo <= j < jhi
 // (jlo = kb0 + min(jlo_rel, kcount) when clip_jlo, else kb0 + jlo_rel; jhi = min(f, kb0 + jhi_rel))
-// 128 x 64 tiles, 8 warps as 4 x 2 (32 x 32 per warp = 4 x 4 m8n8k4 DMMA fragments).  Both operands are raw panel
+// 128 x 64 tiles, 8 warps as 4 x 2 (32 x 32 per warp = 2 x 4 m16n8k4 DMMA fragments: on H100 twice the m8n8k4 issue rate).  Both operands are raw panel
 // columns of L streamed by cp.async through a GU_STAGES-deep ring of K = 16 slices (no register staging, loads stay in
 // flight under the tensor pipe); the -d_k scaling is applied to the A fragments in registers (4 DMUL per 16 DMMA), and
 // the epilogue adds the (negative) accumulators to C.
@@ -340,12 +340,12 @@ __device__ __forceinline__ void big_update_tile(const FactorArgs& a, const Front
 #pragma unroll
             for (int y = 0; y < 4; ++y) bf[y] = Bb[(k0 + q) * GU_LDB + wj + 8 * y + g];
 #pragma unroll
-            for (int x = 0; x < 4; ++x)
+            for (int x = 0; x < 4; x += 2)                            // m16n8k4 = two m8n8k4 row blocks 8 apart sharing B
 #pragma unroll
                 for (int y = 0; y < 4; ++y)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1])
-                                 : "d"(af[x]), "d"(bf[y]));
+                    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1]), "+d"(c[x + 1][y][0]), "+d"(c[x + 1][y][1])
+                                 : "d"(af[x]), "d"(af[x + 1]), "d"(bf[y]));
         }
     }
     // epilogue: accumulators -> shared memory (column-major tile), then a coalesced read-modify-write of C with all of
@@ -541,12 +541,12 @@ __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const 
 #pragma unroll
             for (int y = 0; y < 4; ++y) bf[y] = Bb[(k0 + q) * GU_LDB + wj + 8 * y + g];
 #pragma unroll
-            for (int x = 0; x < 4; ++x)
+            for (int x = 0; x < 4; x += 2)                            // m16n8k4 = two m8n8k4 row blocks 8 apart sharing B
 #pragma unroll
                 for (int y = 0; y < 4; ++y)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1])
-                                 : "d"(af[x]), "d"(bf[y]));
+                    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                                 : "+d"(c[x][y][0]), "+d"(c[x][y][1]), "+d"(c[x + 1][y][0]), "+d"(c[x + 1][y][1])
+                                 : "d"(af[x]), "d"(af[x + 1]), "d"(bf[y]));
         }
         __syncwarp();
         if (lane == 0) gu_mbar_arrive(&empty[st]);

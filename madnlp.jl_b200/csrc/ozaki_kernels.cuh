@@ -1,19 +1,21 @@
-// Ozaki-scheme fp64 SYRK on the 5th-generation tensor cores: W = A' A with A (K x n) cut into S = 8 signed 7-bit digits per
-// entry, the 36 digit-pair products run as EXACT int8 GEMMs on tcgen05.mma.kind::i8 (accumulators in TMEM), operands staged by
-// TMA (cp.async.bulk.tensor, 64-byte swizzle), fp64 reconstruction in the epilogue.  See tools/microbench/ozaki_syrk_tcgen05.cu
+// Ozaki-scheme fp64 SYRK on the Hopper tensor cores: W = A' A with A (K x n) cut into S = 8 signed 7-bit digits per entry, the
+// 36 digit-pair products run as EXACT int8 GEMMs on wgmma.mma_async (s8 x s8 -> s32, accumulators in registers), operands staged
+// by TMA (cp.async.bulk.tensor, 64-byte swizzle), fp64 reconstruction in the epilogue.  See tools/microbench/ozaki_syrk_wgmma.cu
 // for the stand-alone measurement and DESIGN.md section 3 for the error analysis; used by b2d_condensed_assemble_ozaki
 // (build_kkt!(::DenseCondensedKKTSystem), src/KKT/Dense/condensed.jl:157-186, in place of cuBLAS mul!(W, J', J)).
 //
 //   1. per column m:  e_m = exponent of max_i |a_im|;  x = a_im * 2^-e_m in (-1, 1) is cut into S = 8 signed 7-bit digits
 //      x = sum_s q_s 2^(-7(s+1))   (q_s int8, exact: 56 bits cover the fp64 mantissa of the column's largest entries)
 //   2. G_d = sum_{s+t=d} Q_s' Q_t  for d = 0..S-1 : 36 exact int8 x int8 -> int32 GEMMs (|G_d| <= 8 * K * 127^2 < 2^31 for
-//      K <= 16384), the d-sums accumulate inside the tensor-core accumulators (8 accumulators of 64 columns = the SM's whole TMEM)
+//      K <= 16384), the d-sums accumulate inside the wgmma accumulators
 //   3. W(m,n) = 2^(e_m + e_n - 14) * sum_d 2^(-7d) G_d(m,n)   evaluated in fp64 (Horner) by the epilogue
 //
-// Kernel (one 128 x 64 output tile per CTA, 192 threads):
-//   warp 4 lane 0 : TMA producer  -- the 8 A-digit tiles and 8 B-digit tiles of a 64-deep K block into a 2-stage ring
-//   warp 5 lane 0 : MMA issuer    -- 72 tcgen05.mma.cta_group::1.kind::i8 (M128 N64 K32) per K block, tcgen05.commit frees the stage
-//   warps 0..3    : epilogue      -- tcgen05.ld of the 8 accumulators, Horner in fp64, scaling, coalesced stores
+// Kernel (one 64 x 64 output tile per CTA, 288 threads):
+//   warp 8 lane 0 : TMA producer  -- the 8 A-digit tiles and 8 B-digit tiles of a 64-deep K block into a 3-stage ring
+//   warps 0..7    : two consumer warpgroups; each owns 4 of the 8 accumulators G_d (4 x m64n64 s32 = 128 registers a thread:
+//                   all 8 would not fit the register file), split so that both issue 18 digit pairs = 36 wgmma m64n64k32 per
+//                   K block.  Epilogue: both park their accumulators in shared memory, then all 256 threads run the Horner
+//                   sum over d, the scaling and coalesced column-major stores.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -23,13 +25,15 @@ namespace ozk {
 
 constexpr int S = 8;             // digits
 constexpr int WB = 7;            // bits per digit
-constexpr int BM = 128, BN = 64; // output tile
+constexpr int BM = 64, BN = 64;  // output tile
 constexpr int BKB = 64;          // K bytes (= int8 elements) per pipeline stage: one 64-byte swizzle row
-constexpr int STAGES = 2;
+constexpr int STAGES = 3;
 constexpr int A_TILE = BM * BKB, B_TILE = BN * BKB;                 // bytes of one digit tile
-constexpr int STAGE_BYTES = S * (A_TILE + B_TILE);                  // 96 KiB
+constexpr int STAGE_BYTES = S * (A_TILE + B_TILE);                  // 64 KiB
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;             // + alignment slack
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 288;
+constexpr int GLD = BM + 4;                                         // int32 row stride of the parked accumulators (no bank conflicts)
+static_assert(S * BN * GLD * 4 <= STAGES * STAGE_BYTES, "the parked accumulators reuse the operand ring");
 constexpr uint32_t SPIN_MAX = 1u << 22;
 
 // ------------------------------------------------------------------------------------------------ digit split
@@ -74,6 +78,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* err) {     // bounded: never hang the device
     uint32_t done = 0;
     for (uint32_t it = 0; it < SPIN_MAX; ++it) {
@@ -92,161 +99,150 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// K-major operand tile, 64-byte swizzle: rows of 64 bytes, 8-row groups 512 bytes apart (SBO), version 1 (Blackwell)
-__device__ __forceinline__ uint64_t umma_desc_k_sw64(uint32_t saddr) {
+// wgmma shared-memory descriptor of a K-major operand tile with 64-byte swizzle: rows of 64 bytes, 8-row groups 512 bytes
+// apart (stride byte offset), leading byte offset unused (1), layout type 2 = SWIZZLE_64B
+__device__ __forceinline__ uint64_t gmma_desc_k_sw64(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major): 1
-    d |= (uint64_t)(512 >> 4) << 32;                // stride byte offset between 8-row groups
-    d |= (uint64_t)1 << 46;                         // descriptor version
-    d |= (uint64_t)4 << 61;                         // SWIZZLE_64B
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;
     return d;
 }
-// instruction descriptor, kind::i8: D = S32, A = B = signed int8, both K-major, M = 128, N = 64
-constexpr uint32_t IDESC = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// D(64 x 64, s32) += A(64 x 32, s8, K-major) * B(32 x 64, s8, K-major), both operands from shared memory
+__device__ __forceinline__ void wgmma_s8(int (&d)[32], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "{\n.reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate) : "memory");
+        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),
+          "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),
+          "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]),
+          "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(adesc), "l"(bdesc));
 }
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}\n" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-          "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-          "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // warps 0..7 only
 
 // 2^e for |e| <= 1022 (exponent field only)
 __device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(min(max(e, -1022), 1023) + 1023) << 52); }
 
+// accumulators of consumer warpgroup G: {0, 1, 6, 7} and {2, 3, 4, 5} -- d has d + 1 digit pairs, 18 pairs each
+__host__ __device__ constexpr int acc_digit(int G, int j) { return G == 0 ? (j < 2 ? j : j + 4) : j + 2; }
+
+// one K block of warpgroup G: every digit pair (s, t = d - s) of its accumulators, two k32 steps each
+template <int G>
+__device__ __forceinline__ void mma_kblock(int (&acc)[4][32], uint64_t ad0, uint64_t bd0) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int d = acc_digit(G, j);
+#pragma unroll
+        for (int s = 0; s <= d; ++s)
+#pragma unroll
+            for (int k2 = 0; k2 < BKB / 32; ++k2)
+                wgmma_s8(acc[j], ad0 + (uint64_t)((s * A_TILE + k2 * 32) >> 4), bd0 + (uint64_t)(((d - s) * B_TILE + k2 * 32) >> 4));
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ the GEMM
-// tile list: tiles[t] = (bm, bn) with bn*BN < (bm+1)*BM  (touches the lower triangle)
+// tile list: tiles[t] = (bm, bn) with bn <= bm (touches the lower triangle); A and B tiles are both boxes of the digit planes
 // epilogue: C(m, n) = W(m, n) [+ hess(m, n)] [+ pr(m) on the diagonal] for m, n < nvalid (and m >= n when lower_only); ld = ldc / ldh
-__global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                                                            int K, int nvalid, const int2* __restrict__ tiles, const int* __restrict__ expo,
+__global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constant__ CUtensorMap mapQ, int K, int nvalid,
+                                                            const int2* __restrict__ tiles, const int* __restrict__ expo,
                                                             double* __restrict__ C, int64_t ldc, const double* __restrict__ hess, int64_t ldh,
                                                             const double* __restrict__ pr, int lower_only, int* err) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], accum_bar;
-    __shared__ uint32_t tmem_base_sm;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
+    // warp index through a shuffle: the compiler then knows it is warp-uniform and does not serialise the wgmma sequence
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int bm = tiles[blockIdx.x].x, bn = tiles[blockIdx.x].y;
     const int nkb = K / BKB;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&accum_bar, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {                                   // the whole tensor memory of the SM: 8 accumulators x 64 columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_sm)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_sm;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == 8) {
         // ---------------- TMA producer
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int st = kb % STAGES;
-            if (kb >= STAGES && !mbar_wait(&empty_bar[st], ((kb / STAGES) - 1) & 1, err)) break;
-            uint8_t* sa = smem + (size_t)st * STAGE_BYTES;
-            uint8_t* sb = sa + S * A_TILE;
-            mbar_expect_tx(&full_bar[st], STAGE_BYTES);
-            tma_load_3d(sa, &mapA, &full_bar[st], kb * BKB, bm * BM, 0);      // box (64 B of K, 128 rows, 8 digits)
-            tma_load_3d(sb, &mapB, &full_bar[st], kb * BKB, bn * BN, 0);      // box (64 B of K,  64 rows, 8 digits)
-        }
-    } else if (warp == 5) {
-        // ---------------- MMA issuer: the WHOLE warp runs the (warp-uniform) loop so that descriptors and predicates live in uniform
-        // registers; one elected lane issues.  The 72 MMAs of a K block are straight-line code: their operand descriptors differ from
-        // the stage's base descriptors by compile-time constants (digit tile offset + 32-byte K step), the accumulator by d * 64
-        // columns -- a single thread cannot afford ~100 cycles of address arithmetic per 32-cycle MMA (measured: v1 of this kernel).
-        const bool leader = elect_one();
-        bool ok = true;
-        for (int kb = 0; kb < nkb && ok; ++kb) {
-            const int st = kb % STAGES;
-            ok = mbar_wait(&full_bar[st], (kb / STAGES) & 1, err);
-            if (!ok) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (leader) {
-                const uint32_t sa = smem_u32(smem + (size_t)st * STAGE_BYTES);
-                const uint64_t ad0 = umma_desc_k_sw64(sa), bd0 = umma_desc_k_sw64(sa + S * A_TILE);
-                const uint32_t acc_any = kb > 0 ? 1u : 0u;
-#pragma unroll
-                for (int t = 0; t < S; ++t) {
-#pragma unroll
-                    for (int s = 0; s < S - t; ++s) {
-#pragma unroll
-                        for (int k2 = 0; k2 < BKB / 32; ++k2) {
-                            // first write of accumulator d = s + t: K block 0, t == 0, k2 == 0 (t is the outer loop, so every d is first met at t = 0)
-                            const uint32_t acc = (t > 0 || k2 > 0) ? 1u : acc_any;
-                            umma_i8(tmem_base + (uint32_t)((s + t) * BN), ad0 + (uint64_t)((s * A_TILE + k2 * 32) >> 4),
-                                    bd0 + (uint64_t)((t * B_TILE + k2 * 32) >> 4), acc);
-                        }
-                    }
-                }
-                umma_commit(&empty_bar[st]);            // the stage may be refilled once these MMAs have read it
+        if (lane == 0) {
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int st = kb % STAGES;
+                if (kb >= STAGES && !mbar_wait(&empty_bar[st], ((kb / STAGES) - 1) & 1, err)) break;
+                uint8_t* sa = smem + (size_t)st * STAGE_BYTES;
+                uint8_t* sb = sa + S * A_TILE;
+                mbar_expect_tx(&full_bar[st], STAGE_BYTES);
+                tma_load_3d(sa, &mapQ, &full_bar[st], kb * BKB, bm * BM, 0);      // box (64 B of K, 64 rows, 8 digits)
+                tma_load_3d(sb, &mapQ, &full_bar[st], kb * BKB, bn * BN, 0);
             }
-            __syncwarp();
         }
-        if (leader) umma_commit(&accum_bar);             // all accumulators final
-        __syncwarp();
-    } else if (warp < 4) {
-        // ---------------- epilogue: warp w owns TMEM lanes 32w .. 32w+31 = tile rows
-        if (mbar_wait(&accum_bar, 0, err)) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int m = bm * BM + warp * 32 + lane;
-            const int em = expo[m];
-            const double pm = pow2i(em - 2 * WB);                 // 2^(e_m - 14): exact scaling factors, applied as two
-                                                                       // multiplications (cheaper than one ldexp per entry)
-            const uint32_t lane_base = tmem_base + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
-            for (int half = 0; half < 2; ++half) {      // 32 columns at a time (register budget)
-                double h[32];
+        return;
+    }
+
+    // ---------------- consumers: warpgroup g = warp / 4
+    const int g = warp >> 2;
+    int acc[4][32];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) h[j] = 0.0;
-#pragma unroll 1
-                for (int d = S - 1; d >= 0; --d) {
-                    uint32_t r[32];
-                    tmem_ld32(lane_base + d * BN + half * 32, r);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    for (int j = 0; j < 4; ++j)
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) h[j] = fma(h[j], 1.0 / (1 << WB), (double)(int)r[j]);
-                }
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0;
+    bool ok = true;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int st = kb % STAGES;
+        ok = __all_sync(0xffffffffu, mbar_wait(&full_bar[st], (kb / STAGES) & 1, err));
+        if (!ok) break;
+        const uint32_t sa = smem_u32(smem + (size_t)st * STAGE_BYTES);
+        const uint64_t ad0 = gmma_desc_k_sw64(sa), bd0 = gmma_desc_k_sw64(sa + S * A_TILE);
+        wgmma_fence();
+        if (g == 0) mma_kblock<0>(acc, ad0, bd0);
+        else mma_kblock<1>(acc, ad0, bd0);
+        wgmma_commit();
+        wgmma_wait_all();
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[st]);    // this warpgroup has read the stage
+    }
+    wgmma_wait_all();
+
+    // ---------------- epilogue: park G_d(m, n) at Gs[d][n][m] (over the operand ring, which every wgmma has finished reading)
+    consumers_sync();
+    int32_t* Gs = reinterpret_cast<int32_t*>(smem);
+    {
+        const int w = warp & 3;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = bn * BN + half * 32 + j;
-                    if (n < nvalid && m < nvalid && (!lower_only || m >= n)) {
-                        double v = (h[j] * pm) * pow2i(expo[n]);
-                        if (hess) v += hess[(size_t)n * ldh + m];
-                        if (pr && m == n) v += pr[m];
-                        C[(size_t)n * ldc + m] = v;
-                    }
-                }
+        for (int j = 0; j < 4; ++j) {
+            int32_t* Gd = Gs + (size_t)acc_digit(g, j) * BN * GLD;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const int r = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);     // wgmma accumulator fragment: row, column
+                const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+                Gd[c * GLD + r] = acc[j][i];
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    consumers_sync();
+    if (!ok) return;
+    const int ml = threadIdx.x & (BM - 1);
+    const int m = bm * BM + ml;
+    const int em = expo[m];
+    const double pm = pow2i(em - 2 * WB);                 // 2^(e_m - 14): exact scaling factors, applied as two
+                                                          // multiplications (cheaper than one ldexp per entry)
+#pragma unroll 4
+    for (int nl = threadIdx.x >> 6; nl < BN; nl += 256 / BM) {
+        const int n = bn * BN + nl;
+        double h = 0.0;
+#pragma unroll
+        for (int d = S - 1; d >= 0; --d) h = fma(h, 1.0 / (1 << WB), (double)Gs[((size_t)d * BN + nl) * GLD + ml]);
+        if (n < nvalid && m < nvalid && (!lower_only || m >= n)) {
+            double v = (h * pm) * pow2i(expo[n]);
+            if (hess) v += hess[(size_t)n * ldh + m];
+            if (pr && m == n) v += pr[m];
+            C[(size_t)n * ldc + m] = v;
+        }
+    }
 }
 
 

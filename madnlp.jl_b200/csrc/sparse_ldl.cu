@@ -141,7 +141,7 @@ void launch_big_step(const FactorArgs& a, const int32_t* lb, int nfronts, int ob
 //   bulk  S2:  R(k) update of the columns >= k+2 incl. the front's update block (persistent, dynamic tiles, leaves the reserved SMs
 //              to the chain)
 // N1(k+1) waits for C(k), N2(k) and C(k) wait for R(k-1).  While the trailing update is long (first panels) the chain waits for it;
-// once it is short the period is D + N1 + N2 instead of D + whole-panel trsm + whole-column update (42 + 12 + 8 us).
+// once it is short the period is D + N1 + N2 instead of D + whole-panel trsm + whole-column update.
 // Block columns whose successor is not a full pivot block (tail of the pivots, w not a multiple of 128) take the general path:
 // whole-panel trsm and whole-column update on the chain.  B2_DENSE_NEAR=0 forces it everywhere (the two-branch schedule).
 // ----------------------------------------------------------------------------------------------------------
@@ -540,8 +540,8 @@ int capture(b2_solver* s, cudaGraphExec_t* out, Fn fn) {
 
 void build_schedule(b2_solver* s) {
     // fronts with at least this many pivot columns get the look-ahead schedule (B2_LOOKAHEAD_MIN_W; 0 = off, the default: on the 64^3
-    // augmented grid one front at a time with look-ahead measured 52.6 ms against 51.2 ms for the level-batched launches, whose
-    // diagonal-block kernels already run side by side across the fronts of a level -- profiles/r02_c5_lookahead.txt)
+    // augmented grid one front at a time with look-ahead measured slower than the level-batched launches, whose diagonal-block
+    // kernels already run side by side across the fronts of a level)
     int la_min_w = 0, la_tiles = 0;
     if (const char* e = getenv("B2_LOOKAHEAD_MIN_W")) la_min_w = atoi(e);
     const Symbolic& S = s->S;
@@ -1004,11 +1004,11 @@ int b2_options_default(b2_options* opt) {
     opt->pivot_eps = 1e-13;
     opt->use_cuda_graph = 1;
     opt->small_front_max = 160;
-    opt->fuse_max_fronts = 8;      // measured optimum on OPF-10k (profiles/r02_sweep.txt)
+    opt->fuse_max_fronts = 8;      // measured optimum on OPF-10k (tools/sweep_headline.sh)
     opt->dep_schedule = 1;
     if (const char* e = getenv("B2_DEP_SCHEDULE")) opt->dep_schedule = atoi(e);
-    opt->chain_merge_f = 0;      // measured on the OPF-10k tree: 16 -> 11 levels but the merged (two-warp, 14 us) leaves make the
-                                 // throughput-bound bottom of the tree 30 us longer: factorize 0.145 -> 0.172 ms (profiles/r02_chain_merge.txt)
+    opt->chain_merge_f = 0;      // measured on the OPF-10k tree: 16 -> 11 levels but the merged (two-warp) leaves make the
+                                 // throughput-bound bottom of the tree longer, and the factorisation slower
     if (const char* e = getenv("B2_CHAIN_MERGE_F")) opt->chain_merge_f = atoi(e);
     opt->n_parts = 1;
     opt->part_rank = 0;

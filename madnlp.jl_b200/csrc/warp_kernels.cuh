@@ -119,7 +119,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // as one branch-free block.  The publish is a predicated st.shared + bar.arrive in ONE asm without a memory clobber, so that most
 // of the pending update (which reads the OTHER column buffers) follows the arrive and overlaps the partner warp's barrier latency.
 // The empty volatile asm statements (B2_TIE) keep NVVM from sinking the whole chain below the update; ptxas then issues the six tied
-// FMA pairs under the latency of the d_k load and runs the chain contiguously.  (Measured, profiles/r02_pivot_loop.txt: forcing a
+// FMA pairs under the latency of the d_k load and runs the chain contiguously.  (Measured: forcing a
 // finer interleave with real data dependencies -- one LOP3 per link -- costs more issue slots than the latency it hides.)
 struct PivotCtx { const double* cb; const double* pb; double* nb; double* Fk; double eps; int tid, k, f, team; };
 #define B2_TIE(c, x, y) asm volatile("" : "+d"(c), "+d"(x), "+d"(y))
@@ -607,9 +607,9 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
     if (DEP && tid == 0) flag_set(done + s);
 }
 
-// NTEAM teams per CTA.  Measured on OPF-10k (profiles/r02_sweep.txt): sweeping the fused bottom subtrees with 8 one-warp teams per
-// CTA instead of 4 is SLOWER (0.139 -> 0.164 ms per solve: fewer resident CTAs, wider barriers), while smaller subtrees
-// (fuse_max_fronts 16 -> 8) are faster (0.150 -> 0.139 ms) -- so the fused launches keep TeamsPerCta teams.
+// NTEAM teams per CTA.  Measured on OPF-10k (tools/sweep_headline.sh): sweeping the fused bottom subtrees with 8 one-warp teams per
+// CTA instead of 4 is SLOWER (fewer resident CTAs, wider barriers), while smaller subtrees (fuse_max_fronts 16 -> 8) are
+// faster -- so the fused launches keep TeamsPerCta teams.
 constexpr int SOLVE_FUSED_TEAMS = 4;
 template <int NW, int NTEAM = TeamsPerCta<NW>::value>
 __global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2(SolveArgs a, const ChildRec* childrec, WarpSched ws) {

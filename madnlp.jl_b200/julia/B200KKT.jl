@@ -100,7 +100,7 @@ function improve!(M::B200Solver)
     return ch[] != 0
 end
 
-introduce(::B200Solver) = "b200kkt (sm_100a multifrontal LDL')"
+introduce(::B200Solver) = "b200kkt (sm_90a multifrontal LDL')"
 input_type(::Type{<:B200Solver}) = :csc
 default_options(::Type{<:B200Solver}) = B200Options()
 is_supported(::Type{<:B200Solver}, ::Type{Float64}) = true

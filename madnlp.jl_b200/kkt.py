@@ -444,7 +444,7 @@ class DenseCondensedKKTSystem(_KKTBase):
         ii = np.ascontiguousarray(ind_ineq, dtype=np.int64)
         check(lib.b2d_kkt_create(n, m, ns, ii.ctypes.data if ns else None, C.byref(h)))
         self._dk = _Plan(h, lib.b2d_kkt_destroy)
-        # J' D J on the 5th-generation tensor cores (tcgen05 int8 digits + TMA, csrc/ozaki_kernels.cuh) when the contraction is big
+        # J' D J on the Hopper tensor cores (wgmma int8 digits + TMA, csrc/ozaki_kernels.cuh) when the contraction is big
         # enough to pay for the digit split; B2_OZAKI=0/1 forces the DMMA kernel / the tensor-core kernel
         import os
         want = os.environ.get("B2_OZAKI")
@@ -483,7 +483,7 @@ class DenseCondensedKKTSystem(_KKTBase):
 
     def build_kkt(self):
         """Dense/condensed.jl:157-186 as diag-buffer + ONE contraction kernel with fused scaling/epilogue + equality rows; the
-        contraction runs on tcgen05 (int8 Ozaki digits, TMA) when self._ozaki is set, else on the fp64 DMMA path."""
+        contraction runs on wgmma (int8 Ozaki digits, TMA) when self._ozaki is set, else on the fp64 DMMA path."""
         if self._ozaki is not None:
             check(lib.b2d_condensed_assemble_ozaki(self._ozaki.h, self.n, self.m, self.ns, self.n_eq, ptr(self._ind_ineq_d), ptr(self._ind_eq_d),
                                                    ptr(self.hess), ptr(self.jac), ptr(self.pr_diag), ptr(self.du_diag),
@@ -494,7 +494,7 @@ class DenseCondensedKKTSystem(_KKTBase):
                                          ptr(self.diag_buffer), ptr(self.aug_com), _sp(self.stream)))
 
     def tensor_core_status(self):
-        """True if the tcgen05 assembly is active and none of its (bounded) pipeline waits ever timed out"""
+        """True if the tensor-core (wgmma) assembly is active and none of its (bounded) pipeline waits ever timed out"""
         if self._ozaki is None:
             return None
         t = C.c_int32(0)

@@ -1,5 +1,5 @@
 """Host-side mirror of MadNLP's AbstractLinearSolver plugin surface
-(src/LinearSolvers/linearsolvers.jl:13-95) for the B200 back-ends.
+(src/LinearSolvers/linearsolvers.jl:13-95) for the H100 back-ends.
 
 Same method names and meaning as the reference (Python spelling: `factorize!` -> `factorize`):
     Solver(A; opt)            constructor, A kept BY REFERENCE, symbolic analysis happens here
@@ -8,7 +8,7 @@ Same method names and meaning as the reference (Python spelling: `factorize!` ->
     is_inertia() / inertia()  -> (num_pos, num_zero, num_neg)   (code order, src/IPM/solver.jl:626)
     improve()                 -> bool
     introduce(), input_type, default_options(), is_supported(T), is_async()
-Everything numeric is a call through the C ABI (capi.py) into hand-written sm_100a kernels.
+Everything numeric is a call through the C ABI (capi.py) into hand-written sm_90a kernels.
 """
 from __future__ import annotations
 
@@ -37,7 +37,7 @@ class DeviceCSC:
 
 
 class B200SparseSolver:
-    """Supernodal multifrontal LDL^T with static pivoting on one B200
+    """Supernodal multifrontal LDL^T with static pivoting on one H100
     (role of CUDSSSolver, lib/MadNLPGPU/ext/MadNLPGPUCUDAExt/cudss.jl:88-214)."""
     input_type = "csc"
 

@@ -172,7 +172,7 @@ def test_coo_to_csc_random(m, n, nnz, seed):
 
 def test_reference_arm_runs_without_the_product_library():
     """bench.py --impl reference: one JSON line with the contract's keys, the requested --steps/--warmup, the same `config` dict the
-    B200 arm prints, and NO import of the product package (whose __init__ loads libb200kkt.so) -- VERDICT r1 'fix the import so
+    GPU arm prints, and NO import of the product package (whose __init__ loads libb200kkt.so) -- VERDICT r1 'fix the import so
     the record is clean'."""
     import json, os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -585,8 +585,8 @@ def test_ipm_reductions_match_the_reference_formulas(n_tot, m, seed):
 
 @pytest.mark.parametrize("n,m,n_eq", [(640, 300, 0), (515, 333, 40), (1024, 512, 0)])
 def test_dense_assembly_on_tensor_cores_matches_oracle(n, m, n_eq, monkeypatch):
-    """A8 with the contraction on tcgen05.mma.kind::i8 (Ozaki digits, csrc/ozaki_kernels.cuh): ragged sizes (n, ns not multiples of the
-    128 / 64 tile and K-block sizes: zero padding), equality rows, D spanning 18 decades.  Bar: 1e-13 of max|K| against the oracle's
+    """A8 with the contraction on wgmma.mma_async s8 (Ozaki digits, csrc/ozaki_kernels.cuh): ragged sizes (n, ns not multiples of the
+    64 x 64 tile and K-block sizes: zero padding), equality rows, D spanning 18 decades.  Bar: 1e-13 of max|K| against the oracle's
     fp64 assembly (Dense/condensed.jl:157-186), and agreement with the DMMA kernel to the same bar."""
     _need_gpu()
     from madnlp_jl_b200 import kkt as K

@@ -93,7 +93,7 @@ def test_headline_first_factorisation_inertia_matches_ldl_oracle_when_indefinite
 
 @pytest.mark.parametrize("n_eq,ozaki", [(0, "1"), (256, "1"), (0, "0")])
 def test_dense_condensed_full_size(n_eq, ozaki, monkeypatch):
-    """configs[1] at n = 4096, m = 2048; `ozaki` = J' D J on tcgen05 (int8 digits + TMA) / on the fp64 DMMA path."""
+    """configs[1] at n = 4096, m = 2048; `ozaki` = J' D J on wgmma (int8 digits + TMA) / on the fp64 DMMA path."""
     _need_gpu()
     monkeypatch.setenv("B2_OZAKI", ozaki)
     from madnlp_jl_b200 import kkt as K

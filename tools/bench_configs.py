@@ -15,8 +15,8 @@ W = pkg.workloads
 dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
 flush = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device="cuda")
 PEAKS = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-HBM = float(PEAKS.get("hbm_gbs", 6650.0))
-DMMA_PEAK = 37.0      # TFLOP/s, register-resident mma.sync m8n8k4 f64 issue peak measured on the pool (tools/microbench/dmma_shapes.cu)
+HBM = float(PEAKS.get("hbm_gbs", 3350.0))      # GB/s, H100 SXM data sheet unless measured
+DMMA_PEAK = 67.0      # TFLOP/s, fp64 tensor-core peak of the H100 SXM data sheet (700 W); a power-limited card reaches less
 
 
 class _CB:

@@ -7,7 +7,7 @@ sys.path.insert(0, ROOT)
 import numpy as np, torch
 import madnlp_jl_b200 as pkg
 from madnlp_jl_b200.capi import lib, check
-PEAK = 6577.4
+PEAK = 3350.0          # GB/s, H100 SXM data sheet unless measured
 try:
     PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:

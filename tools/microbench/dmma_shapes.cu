@@ -1,6 +1,6 @@
-// Throughput + fragment-layout check of the fp64 tensor-core shapes on sm_100a:
+// Throughput + fragment-layout check of the fp64 tensor-core shapes on sm_90a:
 //   mma.sync.aligned.{m8n8k4, m16n8k4, m16n8k8, m16n8k16}.row.col.f64.f64.f64.f64
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dmma_shapes dmma_shapes.cu ; run: ./dmma_shapes
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dmma_shapes dmma_shapes.cu ; run: ./dmma_shapes
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

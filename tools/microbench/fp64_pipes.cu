@@ -1,6 +1,6 @@
-// Per-SM issue rates that bound the small-front kernels on sm_100a: vector DFMA, 64-bit warp shuffles, LDS.64 broadcast,
+// Per-SM issue rates that bound the small-front kernels on sm_90a: vector DFMA, 64-bit warp shuffles, LDS.64 broadcast,
 // rcp.approx.f64, and the dependent-chain latency of DFMA / SHFL.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_pipes fp64_pipes.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_pipes fp64_pipes.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
