@@ -66,11 +66,11 @@ typedef struct b2_options {
                                 primal neighbours, so that a zero (2,2) block never yields a structurally zero pivot */
     int32_t fuse_max_fronts; /* bottom elimination subtrees with at most this many (warp-class) fronts run inside ONE
                                 CTA of a single launch (0 = plain level-by-level schedule)                      */
-    int32_t dep_schedule;    /* bit 0 (factorisation), bit 1 (solves): when every front is team-class (order <= 64) run the sweep
-                                as ONE launch whose CTAs wait on their children's completion flags instead of on
-                                kernel boundaries.  Default 1: measured faster for the factorisation only.
-                                bit 2 (hybrid sweeps): the fused bottom subtrees keep their staged kernel, every front above
-                                them runs in one flag-driven launch (instead of one launch per level)          */
+    int32_t dep_schedule;    /* bit 0 (default 1): for a single-part solver whose fronts are all team-class (order <= 64),
+                                the factorisation and b2_solve each run as ONE launch whose CTAs wait on completion
+                                flags instead of on kernel boundaries (b2_solve: one launch per right-hand side, with
+                                the same arithmetic as the level-launch solve).  0: level-by-level launches.  Other
+                                bits are ignored (earlier flag-driven sweep variants)                            */
     int32_t chain_merge_f;   /* > 0: a supernode with exactly ONE child absorbs it whatever the explicit zeros cost, as long as the
                                 merged front stays team-class (order <= min(chain_merge_f, 64)): on latency-bound trees every
                                 level of the critical path costs microseconds of hand-off besides its pivots, the zeros nothing.

@@ -23,6 +23,10 @@ struct SolveArgs {
     const double* dvec;
     double* xp;
     double* cbv;
+    // single-launch solve (k_solve_dep): the caller's vector in original order, read as x[perm[j]] by the forward sweep and
+    // written there by the backward sweep, so that no permutation kernels run; null for the level-launch solve
+    const int32_t* perm = nullptr;
+    double* x = nullptr;
 };
 
 __global__ void k_perm_in(int n, const int32_t* __restrict__ perm, const double* __restrict__ x, double* __restrict__ xp) {

@@ -43,9 +43,8 @@ struct Phase {
     // single-launch dependency-driven schedule (used instead of fused + levels when every front is team-class)
     int offAllC = 0, nAllC = 0, maxwAllC = 0;       // every M/B front of the phase (diagonal-block inversion)
     int dep_ngroup = 0, dep_type_off = 0, dep_ptr_off = 0, dep_tasks_off = 0, dep_maxf1 = 0, dep_maxf2 = 0;
-    // hybrid sweeps (dep_schedule bit 2): the fused bottom subtrees by their staged kernel, every front above them as ONE flag-driven
-    // launch (groups in level order of the upper tree); flags of the fused fronts are preset from d_flags_tpl
-    int dep2_ngroup = 0, dep2_type_off = 0, dep2_ptr_off = 0, dep2_tasks_off = 0;
+    // single-launch solve (k_solve_dep: the same groups, condition and phase 0 only): persistent CTAs (0: the level-launch solve)
+    int sol_grid = 0;
     cudaGraphExec_t g_factor = nullptr, g_fwd = nullptr, g_bwd = nullptr;
     int64_t n_factor_launches = 0, n_solve_launches = 0;
     int64_t n_fused_fronts = 0;
@@ -72,8 +71,9 @@ struct b2_solver {
     DevBuf<int32_t> d_counters;
     DevBuf<double> d_Linv, d_side;
     DevBuf<int64_t> d_linv_off;
-    DevBuf<int32_t> d_flags, d_parent;   // dependency flags [3][nsuper], supernode parents
-    DevBuf<int32_t> d_flags_tpl;         // [nsuper] 1 for fronts of the fused bottom subtrees (hybrid sweeps), else 0
+    // dependency flags [3][nsuper] (factorisation, forward sweep, backward sweep), then the factorisation's group ticket and the
+    // single-launch solve's {ticket, epoch}; supernode parents
+    DevBuf<int32_t> d_flags, d_parent;
     int32_t* h_counters = nullptr;   // pinned
     std::vector<int64_t> cbv_off;
     int64_t exch_cbv = 0;
@@ -439,35 +439,6 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
         }
         ++nl;
     };
-    if (P.dep_ngroup && (s->opt.dep_schedule & 2)) {
-        DepSched ds;
-        ds.grp_type = sched + P.dep_type_off; ds.grp_ptr = sched + P.dep_ptr_off; ds.tasks = sched + P.dep_tasks_off; ds.ngroup = P.dep_ngroup;
-        int* flags = s->d_flags.p + (size_t)(forward ? 1 : 2) * s->S.nsuper;
-        int* ticket = s->d_flags.p + (size_t)3 * s->S.nsuper;
-        cudaMemsetAsync(flags, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
-        const size_t smd = sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1>::doubles, (size_t)SolveSmem<2>::doubles);
-        if (forward) k_fwd_dep<<<P.dep_ngroup, 128, smd, st>>>(a, s->d_childrec.p, ds, flags, s->d_counters.p + 4, ticket);
-        else k_bwd_dep<<<P.dep_ngroup, 128, smd, st>>>(a, ds, s->d_parent.p, flags, s->d_counters.p + 4, ticket);
-        return 2;
-    }
-    if (P.dep2_ngroup && (s->opt.dep_schedule & 4)) {
-        // hybrid: the bottom subtrees in their fused staged kernel, everything above them in one flag-driven launch
-        DepSched ds;
-        ds.grp_type = sched + P.dep2_type_off; ds.grp_ptr = sched + P.dep2_ptr_off; ds.tasks = sched + P.dep2_tasks_off; ds.ngroup = P.dep2_ngroup;
-        int* flags = s->d_flags.p + (size_t)(forward ? 1 : 2) * s->S.nsuper;
-        int* ticket = s->d_flags.p + (size_t)3 * s->S.nsuper;
-        const size_t smd = sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1>::doubles, (size_t)SolveSmem<2>::doubles);
-        if (forward) {
-            if (P.fused.n_cta) warp_launch(P.fused, true);
-            cudaMemcpyAsync(flags, s->d_flags_tpl.p, (size_t)s->S.nsuper * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);   // fused fronts: done
-            k_fwd_dep<<<P.dep2_ngroup, 128, smd, st>>>(a, s->d_childrec.p, ds, flags, s->d_counters.p + 4, ticket);
-        } else {
-            cudaMemsetAsync(flags, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
-            k_bwd_dep<<<P.dep2_ngroup, 128, smd, st>>>(a, ds, s->d_parent.p, flags, s->d_counters.p + 4, ticket);
-            if (P.fused.n_cta) warp_launch(P.fused, true);
-        }
-        return nl + 2;
-    }
     if (forward && P.fused.n_cta) warp_launch(P.fused, true);
     if (!forward && P.topfused.n_cta) warp_launch(P.topfused);
     const int nlev = (int)P.lev.size();
@@ -506,6 +477,22 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
     return nl;
 }
 
+constexpr size_t SOLVE_DEP_SMEM = sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1>::doubles, (size_t)SolveSmem<2>::doubles);
+
+// the whole solve of one right-hand side x (original order, in place) as ONE launch of k_solve_dep
+void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
+    const Phase& P = s->phase[0];
+    SolveArgs a = solve_args(s);
+    a.perm = s->d_perm.p;
+    a.x = x;
+    DepSched ds;
+    ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
+    ds.ngroup = P.dep_ngroup;
+    const size_t ns = (size_t)s->S.nsuper;
+    k_solve_dep<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_parent.p, s->d_flags.p + ns, s->d_flags.p + 2 * ns,
+                                                         s->d_counters.p + 4, s->d_flags.p + 3 * ns + 1, s->S.n);
+}
+
 int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_front_smem<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
@@ -517,8 +504,7 @@ int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute((k_bwd_warp2<1, SOLVE_FUSED_TEAMS>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_fwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_fwd_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_bwd_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_solve_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_big_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     return B2_OK;
 }
@@ -581,11 +567,11 @@ void build_schedule(b2_solver* s) {
     };
     for (int ph = 0; ph < 2; ++ph) {
         Phase& P = s->phase[ph];
-        P.lev.clear(); P.fused = WarpLaunch(); P.n_fused_fronts = 0; P.dep_ngroup = 0;
+        P.lev.clear(); P.fused = WarpLaunch(); P.n_fused_fronts = 0; P.dep_ngroup = 0; P.sol_grid = 0;
         std::vector<char> mine(ns, 0);
         for (int sn = 0; sn < ns; ++sn) mine[sn] = (ph == 0) ? (S.owner[sn] == rank) : (S.owner[sn] == -1);
         // ---- dependency-driven single launch: every front of the phase is team-class and the tree is not sharded
-        if (s->opt.dep_schedule && s->opt.n_parts <= 1 && wmax > 32) {
+        if ((s->opt.dep_schedule & 1) && s->opt.n_parts <= 1 && wmax > 32) {
             bool all_team = true;
             int cntm = 0;
             for (int sn = 0; sn < ns && all_team; ++sn) if (mine[sn]) { int w, f; fdim(sn, w, f); all_team = f <= wmax; ++cntm; }
@@ -686,40 +672,6 @@ void build_schedule(b2_solver* s) {
         P.maxwAllC = 0;
         std::vector<std::vector<int32_t>> by_level(nul);
         for (int sn = 0; sn < ns; ++sn) if (ulev[sn] >= 0) by_level[ulev[sn]].push_back(sn);
-        // ---- hybrid sweeps: one flag-driven launch for the whole upper tree (only when all of it is team-class and unsharded)
-        P.dep2_ngroup = 0;
-        if ((s->opt.dep_schedule & 4) && s->opt.n_parts <= 1 && wmax > 32 && ph == 0) {
-            bool all_team = nul > 0;
-            for (int l = 0; l < nul && all_team; ++l)
-                for (int sn : by_level[l]) { int w, f; fdim(sn, w, f); if (f > wmax) { all_team = false; break; } }
-            if (all_team) {
-                std::vector<int32_t> order;
-                for (int l = 0; l < nul; ++l) order.insert(order.end(), by_level[l].begin(), by_level[l].end());
-                std::vector<int32_t> gtype, gptr(1, 0), tasks;
-                size_t k = 0;
-                while (k < order.size()) {
-                    int w, f; fdim(order[k], w, f);
-                    if (f > 32) { gtype.push_back(2); tasks.push_back(order[k]); ++k; }
-                    else {
-                        gtype.push_back(1);
-                        int c = 0;
-                        while (k < order.size() && c < FW_WARPS) {
-                            int w2, f2; fdim(order[k], w2, f2);
-                            if (f2 > 32) break;
-                            tasks.push_back(order[k]); ++k; ++c;
-                        }
-                    }
-                    gptr.push_back((int32_t)tasks.size());
-                }
-                P.dep2_ngroup = (int)gtype.size();
-                P.dep2_type_off = (int)sched.size(); sched.insert(sched.end(), gtype.begin(), gtype.end());
-                P.dep2_ptr_off = (int)sched.size(); sched.insert(sched.end(), gptr.begin(), gptr.end());
-                P.dep2_tasks_off = (int)sched.size(); sched.insert(sched.end(), tasks.begin(), tasks.end());
-                std::vector<int32_t> tpl(ns, 0);
-                for (int sn = 0; sn < ns; ++sn) if (mine[sn] && root_of[sn] >= 0) tpl[sn] = 1;
-                B2_CUDA_THROW(s->d_flags_tpl.upload(tpl.data(), tpl.size()));
-            }
-        }
         // ---- the top of the tree: trailing levels that hold at most 4 team-class fronts each are chained inside ONE CTA
         //      (stage = level): a launch boundary per level would cost more than the fronts themselves.
         P.topfused = WarpLaunch();
@@ -930,7 +882,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(s->d_cbv.alloc((size_t)std::max<int64_t>(1, s->cbv_off[ns])));
         B2_CUDA_THROW(s->d_counters.alloc(8));
         B2_CUDA_THROW(cudaMemset(s->d_counters.p, 0, 8 * sizeof(int32_t)));
-        B2_CUDA_THROW(s->d_flags.alloc((size_t)3 * ns + 1));
+        B2_CUDA_THROW(s->d_flags.alloc((size_t)3 * ns + 3));
         B2_CUDA_THROW(cudaMemset(s->d_flags.p, 0, s->d_flags.bytes()));
         B2_CUDA_THROW(s->d_parent.upload(S.sn_parent.data(), S.sn_parent.size()));
         B2_CUDA_THROW(cudaMemset(s->d_ws.p, 0, s->d_ws.bytes()));
@@ -941,6 +893,14 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(cudaStreamCreateWithFlags(&s->la_side, cudaStreamNonBlocking));
         build_schedule(s);
         if (set_smem_attrs() != B2_OK) throw std::runtime_error("attr");
+        if (Phase& P = s->phase[0]; P.dep_ngroup) {
+            // persistent grid: as many CTAs as fit on the device at once (a size, not a correctness condition), at most one per task
+            int per_sm = 0;
+            B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_dep, 128, SOLVE_DEP_SMEM));
+            const int ntask = 2 * P.dep_ngroup;
+            P.sol_grid = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
+            P.n_solve_launches = 1;
+        }
     } catch (std::exception&) {
         delete s;
         return B2_ERR_CUDA;
@@ -1138,6 +1098,13 @@ int b2_solve_bwd_local(b2_solver* s, double* x_d, void* stream) {
 int b2_solve(b2_solver* s, double* x_d, int32_t nrhs, void* stream) {
     if (!s || s->symbolic_only || !x_d || nrhs < 1) { set_error("b2_solve: invalid argument"); return B2_ERR_INVALID; }
     if (s->opt.n_parts > 1) { set_error("b2_solve: multi-part solver needs the phased solve"); return B2_ERR_INVALID; }
+    if (s->phase[0].sol_grid) {          // every front team-class: one launch per right-hand side, in place on x
+        if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
+        for (int c = 0; c < nrhs; ++c) enqueue_solve_dep(s, x_d + (size_t)c * s->S.n, as_stream(stream));
+        s->phase[0].n_solve_launches = 1;
+        B2_CUDA(cudaGetLastError());
+        return B2_OK;
+    }
     for (int c = 0; c < nrhs; ++c) {
         double* x = x_d + (size_t)c * s->S.n;
         int rc = b2_solve_fwd_local(s, x, stream);

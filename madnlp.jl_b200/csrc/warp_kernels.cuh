@@ -98,19 +98,23 @@ __device__ __forceinline__ void cp_async16_cg(void* smem_dst, const void* gsrc) 
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
 }
-// dependency flags of the single-launch ("dependency-driven") schedule
-__device__ __forceinline__ void flag_wait(const int* flag, int* err) {
+// dependency flags of the single-launch ("dependency-driven") schedules.  A flag is ready when it holds `want`: the factorisation
+// zeroes its flags and sets them to 1; the solve never clears its flags and sets them to the launch's epoch instead.
+__device__ __forceinline__ void flag_wait(const int* flag, int* err, int want = 1) {
     int v = 0;
     unsigned it = 0;
     do {
         asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
-        if (v) break;
+        if (v == want) break;
         __nanosleep(32);
     } while (++it < (1u << 24));
-    if (!v) atomicExch(err, 1);          // bounded spin: never hang the device, report instead
+    if (v != want) {                     // bounded spin: never hang the device, report instead
+        atomicExch(err, 1);
+        __threadfence();                 // (visible before this CTA's next ticket claim: k_solve_dep checks it after the last claim)
+    }
 }
-__device__ __forceinline__ void flag_set(int* flag) {
-    asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(1) : "memory");
+__device__ __forceinline__ void flag_set(int* flag, int v = 1) {
+    asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(v) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
@@ -419,9 +423,12 @@ struct SolveSmem {
     static constexpr int doubles = FMAX + 16 + 4 * MAXC + FMAX * FMAX;
 };
 
+// DEP: the front runs inside a single-launch solve -- values other CTAs produced are read from L2, and when `done` is given the
+// front waits for its children's flags (== epoch) and sets its own.  With a.x set (single-launch solve) the forward sweep reads its
+// right-hand side straight from the caller's x[perm[j]] and the backward sweep writes its solution there too, beside xp.
 template <int NW, bool DEP = false>
 __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRec* childrec, int s, double* sm_team, int tid, int team,
-                                               int* done = nullptr, int* err = nullptr) {
+                                               int* done = nullptr, int* err = nullptr, int epoch = 1) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* ys = sm_team;                              // [FMAX] assembly of the front's rhs
     double* yb = ys + FMAX;                            // [2][8] broadcast slots
@@ -433,19 +440,21 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
         const double* Lp = a.L + d.lp_off;
         for (int e = tid; e < f * w; e += TEAM) cp_async8(P + e, Lp + e);
     }
+    const int pj = (a.x && tid < w) ? a.perm[d.col0 + tid] : 0;
     for (int c0 = 0; c0 < max(d.nchild, 1); c0 += MAXC) {
         const int nc = min(MAXC, d.nchild - c0);
-        if (tid < nc) {
-            recs[tid] = childrec[d.child_off + c0 + tid];
-            if (DEP) flag_wait(done + recs[tid].sn, err);
-        }
+        if (tid < nc) recs[tid] = childrec[d.child_off + c0 + tid];
         team_sync<NW>(team);
         int tg[MAXC]; double vv[MAXC];
 #pragma unroll
         for (int c = 0; c < MAXC; ++c) tg[c] = (c < nc && tid < recs[c].rc) ? a.rel[recs[c].rel_off + tid] : -1;
+        if (DEP && done) {                              // (the relative indices are in flight while the children finish)
+            if (tid < nc) flag_wait(done + recs[tid].sn, err, epoch);
+            team_sync<NW>(team);
+        }
         if (c0 == 0) {                                  // (constant data is in flight; now the values of the levels below)
             if (!DEP) pdl_wait();
-            ys[tid] = (tid < w) ? a.xp[d.col0 + tid] : 0.0;
+            ys[tid] = (tid < w) ? (a.x ? a.x[pj] : a.xp[d.col0 + tid]) : 0.0;
         }
 #pragma unroll
         for (int c = 0; c < MAXC; ++c)
@@ -515,12 +524,12 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
     // hand-off: the team barrier orders every thread's stores before thread 0's st.release.gpu (release is cumulative over the
     // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed
     team_sync<NW>(team);
-    if (DEP && tid == 0) flag_set(done + s);
+    if (DEP && done && tid == 0) flag_set(done + s, epoch);
 }
 
 template <int NW, bool DEP = false>
 __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double* sm_team, int tid, int team,
-                                               int* done = nullptr, int* err = nullptr, const int32_t* parent = nullptr) {
+                                               int* done = nullptr, int* err = nullptr, const int32_t* parent = nullptr, int epoch = 1) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* xs = sm_team;                              // [FMAX] gathered ancestor values
     double* xb = xs + FMAX;                            // [2][8]
@@ -533,13 +542,14 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
     }
     const int32_t* rows = a.rows + d.rows_off + w;
     const int myrow = (tid < r) ? rows[tid] : 0;
+    const int pj = (a.x && tid < w) ? a.perm[d.col0 + tid] : 0;
     const double dinv = (tid < w) ? fast_rcp(a.dvec[d.col0 + tid]) : 0.0;
     if (DEP) {      // all ancestors are final once the parent is
-        if (tid == 0) { const int p = parent[s]; if (p >= 0) flag_wait(done + p, err); }
+        if (tid == 0 && done) { const int p = parent[s]; if (p >= 0) flag_wait(done + p, err, epoch); }
         team_sync<NW>(team);
     } else pdl_wait();
     if (tid < r) xs[tid] = DEP ? __ldcg(a.xp + myrow) : a.xp[myrow];
-    double t = (tid < w) ? a.xp[d.col0 + tid] * dinv : 0.0;
+    double t = (tid < w) ? (DEP ? __ldcg(a.xp + d.col0 + tid) : a.xp[d.col0 + tid]) * dinv : 0.0;
     cp_async_wait_all();
     team_sync<NW>(team);
     {   // t_j -= sum_{i >= w} L(i,j) x_i : no recurrence
@@ -600,11 +610,14 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
             }
         }
     }
-    if (tid < w) a.xp[d.col0 + tid] = t;
+    if (tid < w) {
+        a.xp[d.col0 + tid] = t;
+        if (a.x) a.x[pj] = t;
+    }
     // hand-off: the team barrier orders every thread's stores before thread 0's st.release.gpu (release is cumulative over the
     // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed
     team_sync<NW>(team);
-    if (DEP && tid == 0) flag_set(done + s);
+    if (DEP && done && tid == 0) flag_set(done + s, epoch);
 }
 
 // NTEAM teams per CTA.  Measured on OPF-10k (tools/sweep_headline.sh): sweeping the fused bottom subtrees with 8 one-warp teams per
@@ -686,31 +699,72 @@ __global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec
     }
 }
 
-__global__ void __launch_bounds__(128) k_fwd_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, int* done, int* err, int* ticket) {
+// ------------------------------------------------------------------------------------------------ single-launch solve
+// Forward sweep, D^-1 and backward sweep of the whole (team-class, unsharded) tree in ONE launch.  The tasks are the groups of
+// k_factor_dep (DepSched: fronts in (level, id) order, four fronts of order <= 32 as one-warp teams or one front of order <= 64 as a
+// two-warp team per group), every front with its own flag:
+//   ticket [0, ngroup)          forward sweep of group t: a front waits on its children's forward flags
+//   ticket [ngroup, 2 ngroup)   backward sweep of the groups in reverse order: a front waits on its parent's backward flag (a root:
+//                               on its own forward flag)
+// A persistent grid claims the tickets through an atomic counter, one task at a time.  A front waits only on fronts of smaller
+// tickets or of its own group (another team: no CTA-wide barrier inside a task), and a CTA claims a ticket only while it runs, so
+// forward progress does not depend on how many CTAs are resident or in which order they are dispatched.
+// Fronts of order <= 32 run as one-warp teams here and as two-warp teams in the level-launch solve above the fused subtrees; for
+// w <= f <= 32 the two-warp code runs warp 0 alone through the same loops, so the result is bit-identical to the level solve.
+// Flags are spaced per front (measured: a flag per front beats running fused bottom subtrees stage by stage inside one CTA, whose
+// stages each cost a front's full latency and which need more than two waves of the resident CTAs on OPF-10k).
+// Re-arming without any other graph node: flags hold the epoch of the launch that set them; there are exactly ntask + gridDim
+// claims (each CTA ends with one failing claim), every CTA reads the epoch before its first claim, and the CTA that makes the last
+// claim resets the ticket and advances the epoch.  ctl = {ticket, epoch}.
+// (six CTAs per SM: what the 35 KB of shared memory allows; the bound also keeps ptxas from spilling)
+__global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, const int32_t* parent,
+                                                   int* fdone, int* bdone, int* err, int* ctl, int n) {
     extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
-    double (*sm)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
-    const int g = claim_group(ticket, ds.ngroup);
-    const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
-    if (type == 1) {
-        const int team = threadIdx.x >> 5, tid = threadIdx.x & 31;
-        if (team < n) front_fwd_team<1, true>(a, childrec, ds.tasks[t0 + team], sm[team], tid, team, done, err);
-    } else {
-        const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
-        if (team < n) front_fwd_team<2, true>(a, childrec, ds.tasks[t0 + team], smd, tid, team, done, err);
+    double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
+    __shared__ int tk_sh, ep_sh, nan_sh;
+    const int ntask = 2 * ds.ngroup;
+    if (threadIdx.x == 0) {
+        int e;
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(e) : "l"(ctl + 1) : "memory");
+        ep_sh = e + 1;
+        nan_sh = 0;
     }
-}
-
-__global__ void __launch_bounds__(128) k_bwd_dep(SolveArgs a, DepSched ds, const int32_t* parent, int* done, int* err, int* ticket) {
-    extern __shared__ __align__(16) double smd[];
-    double (*sm)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
-    const int g = ds.ngroup - 1 - claim_group(ticket, ds.ngroup);   // reverse topological order
-    const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
-    if (type == 1) {
-        const int team = threadIdx.x >> 5, tid = threadIdx.x & 31;
-        if (team < n) front_bwd_team<1, true>(a, ds.tasks[t0 + team], sm[team], tid, team, done, err, parent);
-    } else {
-        const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
-        if (team < n) front_bwd_team<2, true>(a, ds.tasks[t0 + team], smd, tid, team, done, err, parent);
+    for (;;) {
+        if (threadIdx.x == 0) {
+            const int t = atomicAdd(ctl, 1);
+            if (t == ntask + (int)gridDim.x - 1) {      // last claim: every other CTA is done and has read the epoch
+                atomicExch(ctl, 0);
+                atomicExch(ctl + 1, ep_sh);
+                __threadfence();
+                nan_sh = *(volatile int*)err;           // a timed-out wait anywhere (or in the factorisation): x := NaN
+            }
+            tk_sh = t;
+        }
+        __syncthreads();
+        const int t = tk_sh;
+        const int E = ep_sh;
+        if (t >= ntask) {
+            if (nan_sh)
+                for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double(0x7ff8000000000000ll);
+            return;
+        }
+        const bool fwd = t < ds.ngroup;
+        const int g = fwd ? t : ntask - 1 - t;
+        const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
+        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
+        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        if (team < cnt) {
+            const int s = ds.tasks[t0 + team];
+            if (fwd) {
+                if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, fdone, err, E);
+                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, fdone, err, E);
+            } else {
+                if (tid == 0 && parent[s] < 0) flag_wait(fdone + s, err, E);   // a root: its own forward sweep
+                if (type == 1) front_bwd_team<1, true>(a, s, sm1[team], tid, team, bdone, err, parent, E);
+                else front_bwd_team<2, true>(a, s, smd, tid, team, bdone, err, parent, E);
+            }
+        }
+        __syncthreads();                                // (tk_sh is rewritten by the next claim)
     }
 }
 
