@@ -175,7 +175,7 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
 int b2d_destroy(b2d_solver* s);
 /* Debug: device timeline of the dense look-ahead factorisation.  With B2_DENSE_TRACE=1 in the environment at b2d_create, every kernel
  * of b2d_factorize stamps %globaltimer (ns) at its first entry and last exit; slot = 8 * block column + kind (0 diagonal block, 1 near
- * trsm, 2 near syrk, 3 panel trsm, 4 block-column update, 5 trailing update, 6 inverse), two uint64 per slot.  *count = number of
+ * trsm, 2 near syrk, 3 panel trsm, 4 block-column update, 5 trailing update), two uint64 per slot.  *count = number of
  * uint64 values (0 when tracing is off); stamps are copied when capacity >= *count. */
 int b2d_debug_trace(b2d_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count);
 int b2d_factorize(b2d_solver* s, void* stream);

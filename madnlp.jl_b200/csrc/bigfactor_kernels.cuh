@@ -7,10 +7,11 @@
 //                   Linv buffer -- the same blocks the multi-CTA triangular solves use (bigsolve_kernels.cuh).
 //   k_big_trsm      rows below the block:  L21 = A21 * L11^{-T} * D^{-1}  as a DMMA GEMM against Linv (64 rows per CTA,
 //                   operands streamed by cp.async), in place.
-//   k_big_update_pipe (front_kernels.cuh)  trailing update with all 128 pivots at once.
+//   k_big_update_pipe_bulk (front_kernels.cuh)  trailing update with all 128 pivots at once.
 //
 // so a front of order N costs 3*N/128 dependent launches instead of 13*N/128, and the diagonal-block inversion is no
-// longer a separate pass.  Pivoting is static (front_kernels.cuh): |d| < eps is replaced by sign(d)*eps and counted.
+// longer a separate pass.  The dense solver's look-ahead schedule (sparse_ldl.cu) runs the same diagonal-block kernel and adds
+// the near-diagonal kernels below.  Pivoting is static (front_kernels.cuh): |d| < eps is replaced by sign(d)*eps and counted.
 #pragma once
 #include "front_kernels.cuh"
 
@@ -57,7 +58,7 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, int parity) {
         "}\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(parity) : "memory");
 }
 
-// Phase I of the diagonal-block kernel as a function (also the body of k_big_inv128): on entry sm.Lc[k*DB_LDS + i] = l(i,k) for i > k and
+// Phase I of the diagonal-block kernel: on entry sm.Lc[k*DB_LDS + i] = l(i,k) for i > k and
 // 0 for i <= k; on exit the unit-lower inverse is in sm.Lc and has been stored to `out` (column-major, ld DB, zero outside nb x nb).
 __device__ __forceinline__ void diag128_invert_store(Diag128Smem& sm, const int tid, const int nb, double* __restrict__ out) {
     // ---- phase I: X = L11^{-1}, BLOCKED (4 x 4 blocks of 32), in place in sm.Lc (L11 has been written back to global memory):
@@ -144,8 +145,7 @@ __device__ __forceinline__ void diag128_invert_store(Diag128Smem& sm, const int 
 }
 
 __global__ void __launch_bounds__(256, 1) k_big_diag128(FactorArgs a, const int32_t* __restrict__ list, int kb,
-                                                        double* __restrict__ Linv, const int64_t* __restrict__ linv_off, int with_inv) {
-    pdl_sync();                                                    // (no-op unless launched with the PDL attribute: dense chain)
+                                                        double* __restrict__ Linv, const int64_t* __restrict__ linv_off) {
     const int s = list[blockIdx.x];
     const FrontDesc d = a.desc[s];
     if (kb >= d.w) return;
@@ -257,7 +257,6 @@ __global__ void __launch_bounds__(256, 1) k_big_diag128(FactorArgs a, const int3
         a.dvec[d.col0 + kb + tid] = sm.dd[tid];
     }
     DPROF();
-    if (!with_inv) { trace_exit(a, 8 * (kb / DB) + TR_DIAG); return; }   // dense chain: the inverse is formed off the critical path (k_big_inv128)
     diag128_invert_store(sm, tid, nb, Linv + linv_off[s] + (size_t)(kb / DB) * DB * DB);
     trace_exit(a, 8 * (kb / DB) + TR_DIAG);
     DPROF();
@@ -388,7 +387,6 @@ __device__ __forceinline__ void cp_async16_l2(void* smem_dst, const void* gsrc) 
 }
 __global__ void __launch_bounds__(256, 1) k_near_trsm(FactorArgs a, const int32_t* __restrict__ list, int kb,
                                                       const double* __restrict__ Linv, const int64_t* __restrict__ linv_off) {
-    pdl_sync();
     const int s = list[0];
     const FrontDesc d = a.desc[s];
     const int f = d.f;
@@ -448,7 +446,6 @@ constexpr int NS_T = 32;                         // tile order of k_near_syrk
 constexpr int NS_LD = NS_T + 4;                  // 36 = 4 (mod 16)
 constexpr size_t NS_SMEM = (size_t)(2 * DB * NS_LD + DB) * sizeof(double);
 __global__ void __launch_bounds__(256, 2) k_near_syrk(FactorArgs a, const int32_t* __restrict__ list, int kb) {
-    pdl_sync();
     const int s = list[0];
     const FrontDesc d = a.desc[s];
     const int f = d.f;
@@ -500,76 +497,6 @@ __global__ void __launch_bounds__(256, 2) k_near_syrk(FactorArgs a, const int32_
             if (i >= j) Lp[(size_t)j * f + i] = cold[x][e] + c[x][e];
         }
     trace_exit(a, 8 * (kb / DB) + TR_NEAR2);
-}
-
-// The inverse of a finished diagonal block as its own kernel (one CTA): the dense chain leaves it to the side branch, where it runs
-// beside the next diagonal block instead of in front of the near-diagonal step (16k + 5k of the diagonal kernel's 81k cycles).
-__global__ void __launch_bounds__(256, 1) k_big_inv128(FactorArgs a, const int32_t* __restrict__ list, int kb,
-                                                       double* __restrict__ Linv, const int64_t* __restrict__ linv_off) {
-    const int s = list[blockIdx.x];
-    const FrontDesc d = a.desc[s];
-    if (kb >= d.w) return;
-    extern __shared__ __align__(16) unsigned char dsm_raw[];
-    Diag128Smem& sm = *reinterpret_cast<Diag128Smem*>(dsm_raw);
-    const int f = d.f, nb = min(DB, d.w - kb), tid = threadIdx.x;
-    const double* Lp = a.L + d.lp_off;
-    for (int e = tid; e < DB * DB; e += 256) {
-        const int i = e & (DB - 1), j = e >> 7;
-        const bool in = i < nb && j < nb && i > j;
-        cp_async8_zfill(sm.Lc + j * DB_LDS + i, Lp + (size_t)(kb + (in ? j : 0)) * f + kb + (in ? i : 0), in);
-    }
-    cp_async_commit_group();
-    cp_async_wait_group_n<0>();
-    __syncthreads();
-    trace_enter(a, 8 * (kb / DB) + TR_INV);
-    diag128_invert_store(sm, tid, nb, Linv + linv_off[s] + (size_t)(kb / DB) * DB * DB);
-    trace_exit(a, 8 * (kb / DB) + TR_INV);
-}
-
-// Near-diagonal trsm WITHOUT the inverse: the 128 rows right below a finished diagonal block by forward substitution against L11
-// itself, one warp per row (16 CTAs x 8 rows).  Lane l holds the row's entries c = l + 32 j (cyclic, so the shrinking active part
-// stays spread over the lanes); step k broadcasts x_k by shuffle and every lane applies it to its entries c > k with L11(c, k) read
-// from shared memory (consecutive lanes, consecutive addresses).  Dependent chain per step: SHFL + DFMA; 128 steps.
-constexpr size_t NV_SMEM = (size_t)DB * NT_LDB * sizeof(double);
-__global__ void __launch_bounds__(256, 1) k_near_trsv(FactorArgs a, const int32_t* __restrict__ list, int kb) {
-    pdl_sync();
-    const int s = list[0];
-    const FrontDesc d = a.desc[s];
-    const int f = d.f;
-    extern __shared__ __align__(16) double nv_sm[];
-    double* Ls = nv_sm;                            // Ls[k*NT_LDB + c] = L11(c, k), c > k
-    double* Lp = a.L + d.lp_off;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int row = kb + DB + blockIdx.x * NT_ROWS + warp;
-    trace_enter(a, 8 * (kb / DB) + TR_NEAR1);
-    for (int e = tid; e < DB * DB; e += 256) {
-        const int c = e & (DB - 1), k = e >> 7;
-        if (c > k) cp_async8_zfill(Ls + k * NT_LDB + c, Lp + (size_t)(kb + k) * f + kb + c, true);
-    }
-    cp_async_commit_group();
-    double x[4], dinv[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        x[j] = Lp[(size_t)(kb + lane + 32 * j) * f + row];
-        dinv[j] = 1.0 / a.dvec[d.col0 + kb + lane + 32 * j];
-    }
-    cp_async_wait_group_n<0>();
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-#pragma unroll 8
-        for (int o = 0; o < 32; ++o) {
-            const int k = 32 * j + o;
-            const double xk = __shfl_sync(0xffffffffu, x[j], o);
-            const double* lk = Ls + k * NT_LDB + lane;
-            if (lane > o) x[j] = fma(-xk, lk[32 * j], x[j]);
-#pragma unroll
-            for (int jj = j + 1; jj < 4; ++jj) x[jj] = fma(-xk, lk[32 * jj], x[jj]);
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) Lp[(size_t)(kb + lane + 32 * j) * f + row] = x[j] * dinv[j];
-    trace_exit(a, 8 * (kb / DB) + TR_NEAR1);
 }
 
 }  // namespace b2

@@ -1,7 +1,6 @@
 // Error plumbing and device queries shared by all translation units.
 #include "common.cuh"
 
-#include <cstdlib>
 #include <mutex>
 
 namespace b2 {
@@ -16,11 +15,6 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
     g_err = buf;
     cudaGetLastError();   // clear sticky-less errors
     return B2_ERR_CUDA;
-}
-
-bool pdl_enabled() {
-    static const bool on = [] { const char* e = getenv("B2_PDL"); return !(e && e[0] == '0'); }();
-    return on;
 }
 
 int sm_count() {

@@ -57,8 +57,7 @@ int sm_count();
 // ---- programmatic dependent launch (PDL).  A kernel launched through launch_pdl() may be scheduled while its predecessor
 // in the stream is still running; it must not touch anything the predecessor produces before pdl_wait() returns (and must
 // pass pdl_wait() before it exits, so that ITS completion implies the predecessor's).  Kernels with nothing to prefetch
-// simply start with pdl_sync(): what overlaps is the launch latency.  B2_PDL=0 turns the attribute off (plain stream order).
-bool pdl_enabled();
+// simply start with pdl_sync(): what overlaps is the launch latency.
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -70,7 +69,7 @@ inline cudaError_t launch_pdl(void (*kern)(P...), dim3 grid, dim3 block, size_t 
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.attrs = at; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
 }
 #endif

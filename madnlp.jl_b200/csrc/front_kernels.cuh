@@ -43,7 +43,7 @@ struct FactorArgs {
 };
 
 // Timeline stamps of the dense look-ahead schedule (b2d_debug_trace): slot = 8 * block column + kernel kind
-enum { TR_DIAG = 0, TR_NEAR1 = 1, TR_NEAR2 = 2, TR_TRSM = 3, TR_COL = 4, TR_BULK = 5, TR_INV = 6 };
+enum { TR_DIAG = 0, TR_NEAR1 = 1, TR_NEAR2 = 2, TR_TRSM = 3, TR_COL = 4, TR_BULK = 5 };
 __device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void trace_enter(const FactorArgs& a, int slot) {
     if (a.trace && threadIdx.x == 0) atomicMin(a.trace + 2 * slot, global_ns());
@@ -405,29 +405,6 @@ __global__ void __launch_bounds__(256, 2) k_big_update_rows(FactorArgs a, const 
     trace_exit(a, 8 * (kb0 / 128) + TR_COL);
 }
 
-// The same update as a PERSISTENT kernel with a dynamic tile queue, for the look-ahead schedule of the dense factorisation:
-// CTAs that land on the first `n_reserved` SMs exit at once, so those SMs stay free for the next panel's diagonal-block kernel
-// (one CTA that needs a whole SM) while this kernel works through the trailing update on all the others.  Tiles are handed out
-// by an atomic counter (`*tile_counter`, zeroed by the host before the launch), so it does not matter which CTAs left.
-__device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
-__global__ void __launch_bounds__(256, 2) k_big_update_dyn(FactorArgs a, const int32_t* __restrict__ list, int kb0, int kmax, int jlo_rel,
-                                                           int jhi_rel, int clip_jlo, int nbx, int nby, int* tile_counter, int n_reserved) {
-    extern __shared__ __align__(16) double gu_sm[];
-    __shared__ int t_sh;
-    if ((int)smid() < n_reserved) return;
-    const FrontDesc d = a.desc[list[0]];
-    const int ntile = nbx * nby;
-    trace_enter(a, 8 * (kb0 / 128) + TR_BULK);
-    for (;;) {
-        __syncthreads();                                 // (the previous tile's epilogue has finished with shared memory)
-        if (threadIdx.x == 0) t_sh = atomicAdd(tile_counter, 1);
-        __syncthreads();
-        const int t = t_sh;
-        if (t >= ntile) { trace_exit(a, 8 * (kb0 / 128) + TR_BULK); return; }
-        big_update_tile(a, d, kb0, kmax, jlo_rel, jhi_rel, clip_jlo, t % nbx, t / nbx, gu_sm);
-    }
-}
-
 // ----------------------------------------------------------------------------------------------------------
 // The same 128 x 64 tile with operands staged by the TMA unit: 1-D bulk copies (cp.async.bulk.shared::cluster.global, one per
 // K-row of each operand: 1 KB of A, 512 B of B) issued by a ninth, producer warp into the same 4-stage ring, completion counted in
@@ -599,7 +576,7 @@ __device__ __forceinline__ void gu_bulk_setup(double* gu_sm) {
     __syncthreads();
 }
 
-// k_big_update_pipe / k_big_update_dyn with bulk-copy operand staging (288 threads: 8 consumer warps + 1 producer warp)
+// k_big_update_pipe with bulk-copy operand staging (288 threads: 8 consumer warps + 1 producer warp)
 __global__ void __launch_bounds__(GU_NT_BULK, 2) k_big_update_pipe_bulk(FactorArgs a, const int32_t* __restrict__ list, int kb0, int kmax,
                                                                        int jlo_rel, int jhi_rel, int clip_jlo) {
     extern __shared__ __align__(16) double gu_sm[];
@@ -615,6 +592,12 @@ __global__ void __launch_bounds__(GU_NT_BULK, 2) k_big_update_pipe_bulk(FactorAr
     unsigned it = 0;
     big_update_tile_bulk(a, d, kb0, kmax, jlo_rel, jhi_rel, clip_jlo, blockIdx.x, blockIdx.y, gu_sm, it);
 }
+
+// The same update as a PERSISTENT kernel with a dynamic tile queue, for the look-ahead schedule of the dense factorisation:
+// CTAs that land on the first `n_reserved` SMs exit at once, so those SMs stay free for the next panel's diagonal-block kernel
+// (one CTA that needs a whole SM) while this kernel works through the trailing update on all the others.  Tiles are handed out
+// by an atomic counter (`*tile_counter`, zeroed by the host before the launch), so it does not matter which CTAs left.
+__device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
 __global__ void __launch_bounds__(GU_NT_BULK, 2) k_big_update_dyn_bulk(FactorArgs a, const int32_t* __restrict__ list, int kb0, int kmax,
                                                                       int jlo_rel, int jhi_rel, int clip_jlo, int nbx, int nby, int* tile_counter,
                                                                       int n_reserved) {

@@ -5,7 +5,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <stdexcept>
-#include <array>
 #include <vector>
 
 #include "analysis.hpp"
@@ -30,10 +29,6 @@ struct LevelSched {
     WarpLaunch W, W2;                               // fronts of order <= 32 / <= 64
     int offM = 0, nM = 0, maxfM = 0;                // shared-memory CTA class
     int offB = 0, nB = 0, maxfB = 0, maxwB = 0, maxchildB = 0, maxamapB = 0, maxrB = 0;   // HBM-resident class
-    // the first nLA fronts of the B list are factorised ONE AT A TIME with the three-branch look-ahead schedule (enqueue_front_lookahead);
-    // la[i] = {w, f, offset of its tile counters}; maxfBr / maxwBr: maxima over the remaining (batched) fronts
-    int nLA = 0, maxfBr = 0, maxwBr = 0;
-    std::vector<std::array<int, 3>> la;
     int offC = 0, nC = 0, maxfC = 0, maxwC = 0;     // M and B fronts together, for the multi-CTA solve kernels
 };
 struct Phase {
@@ -79,11 +74,7 @@ struct b2_solver {
     int64_t exch_cbv = 0;
     Phase phase[2];                  // 0 = local (owned subtrees), 1 = shared top tree
     cudaStream_t cap_stream = nullptr;
-    cudaStream_t la_bulk = nullptr, la_side = nullptr;   // side branches of the look-ahead schedule of the largest fronts
-    std::vector<cudaEvent_t> ev_pool;
-    size_t ev_next = 0;
     DevBuf<unsigned long long> d_ftrace;                 // B2_SPARSE_TRACE=1: per-front stamps of the team-class factor kernels (b2_debug_trace)
-    DevBuf<int32_t> d_tilecnt;                           // dynamic-tile counters, one per 128-column block of every look-ahead front
     bool factorized = false;
     int64_t last_perturbed = 0;
     std::vector<uint8_t> owned_mask;  // original numbering
@@ -95,9 +86,6 @@ struct b2_solver {
             if (p.g_bwd) cudaGraphExecDestroy(p.g_bwd);
         }
         if (cap_stream) cudaStreamDestroy(cap_stream);
-        if (la_bulk) cudaStreamDestroy(la_bulk);
-        if (la_side) cudaStreamDestroy(la_side);
-        for (auto e : ev_pool) cudaEventDestroy(e);
         if (h_counters) cudaFreeHost(h_counters);
     }
 };
@@ -105,198 +93,22 @@ struct b2_solver {
 namespace {
 
 // one outer step of every big front in `lb`: diagonal block (factor + inverse), rows below, trailing update
-inline bool lookahead_bulk() {
-    static const bool on = [] { const char* e = getenv("B2_UPDATE_BULK"); return !e || atoi(e) != 0; }();
-    return on;
-}
 void launch_big_step(const FactorArgs& a, const int32_t* lb, int nfronts, int ob, int maxf, double* Linv, const int64_t* linv_off,
                      cudaStream_t st, int64_t* nl) {
     static bool attr = false;
     if (!attr) {
         cudaFuncSetAttribute(k_big_diag128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Diag128Smem));
         cudaFuncSetAttribute(k_big_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
-        cudaFuncSetAttribute(k_big_update_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
+        cudaFuncSetAttribute(k_big_update_pipe_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK);
         attr = true;
     }
-    k_big_diag128<<<nfronts, 256, sizeof(Diag128Smem), st>>>(a, lb, ob, Linv, linv_off, 1);
+    k_big_diag128<<<nfronts, 256, sizeof(Diag128Smem), st>>>(a, lb, ob, Linv, linv_off);
     if (nl) ++*nl;
     const int rem = maxf - ob - 1;                  // rows below the first pivot of the block (upper bound over the fronts)
     if (rem <= 0) return;
     k_big_trsm<<<dim3((rem + TR_ROWS - 1) / TR_ROWS, nfronts), 256, GU_SMEM, st>>>(a, lb, ob, Linv, linv_off, 0);
-    if (lookahead_bulk()) {
-        static bool battr = false;
-        if (!battr) { cudaFuncSetAttribute(k_big_update_pipe_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK); battr = true; }
-        k_big_update_pipe_bulk<<<dim3((rem + GU_M - 1) / GU_M, (rem + GU_N - 1) / GU_N, nfronts), GU_NT_BULK, GU_SMEM_BULK, st>>>(a, lb, ob, DB, DB, 1 << 30, 1);
-    } else
-    k_big_update_pipe<<<dim3((rem + GU_M - 1) / GU_M, (rem + GU_N - 1) / GU_N, nfronts), 256, GU_SMEM, st>>>(a, lb, ob, DB, DB, 1 << 30, 1);
+    k_big_update_pipe_bulk<<<dim3((rem + GU_M - 1) / GU_M, (rem + GU_N - 1) / GU_N, nfronts), GU_NT_BULK, GU_SMEM_BULK, st>>>(a, lb, ob, DB, DB, 1 << 30, 1);
     if (nl) *nl += 2;
-}
-
-// ----------------------------------------------------------------------------------------------------------
-// Look-ahead schedule of ONE HBM-resident front (the dense solver's matrix: f = w = N; a big front of the multifrontal tree: f > w),
-// three stream branches joined back into S1 (captured into the caller's graph).  Per block column k of 128 pivots:
-//   chain S1:  D(k) diagonal block -> N1(k) the 128 x 128 block of L below it (k_near_trsm) -> N2(k) update of the NEXT diagonal block
-//              (k_near_syrk) -> D(k+1) ...                         -- the only kernels on the critical path, each a few SMs wide
-//   side  S3:  T(k) trsm of the rows from block k+2 on (after D(k)) -> C(k) rest of block column k+1 (after N1(k), R(k-1))
-//   bulk  S2:  R(k) update of the columns >= k+2 incl. the front's update block (persistent, dynamic tiles, leaves the reserved SMs
-//              to the chain)
-// N1(k+1) waits for C(k), N2(k) and C(k) wait for R(k-1).  While the trailing update is long (first panels) the chain waits for it;
-// once it is short the period is D + N1 + N2 instead of D + whole-panel trsm + whole-column update.
-// Block columns whose successor is not a full pivot block (tail of the pivots, w not a multiple of 128) take the general path:
-// whole-panel trsm and whole-column update on the chain.  B2_DENSE_NEAR=0 forces it everywhere (the two-branch schedule).
-// ----------------------------------------------------------------------------------------------------------
-__global__ void k_trace_reset(unsigned long long* t, int nslot) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < 2 * nslot) t[i] = (i & 1) ? 0ull : ~0ull;
-}
-
-struct LookaheadCtx {
-    cudaStream_t S2 = nullptr, S3 = nullptr;
-    std::vector<cudaEvent_t>* pool = nullptr;        // events, created on demand, handed out in order
-    size_t* next = nullptr;
-    int32_t* tilecnt = nullptr;                      // one dynamic-tile counter per block column (zeroed by the caller)
-    cudaEvent_t ev() {
-        if (*next == pool->size()) { cudaEvent_t e; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); pool->push_back(e); }
-        return (*pool)[(*next)++];
-    }
-};
-
-struct LookaheadKnobs { int n_reserved, inv_side, use_near, relax, early_reserved, chain_pdl, bulk, depth2; };
-const LookaheadKnobs& lookahead_knobs() {
-    static LookaheadKnobs K = [] {
-        LookaheadKnobs k;
-        auto geti = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
-        // B2_DENSE_INV_SIDE=1: the diagonal-block kernel stops after writing L11 / D back; the near-diagonal trsm substitutes against L11
-        // (k_near_trsv) and the inverse (needed by the whole-panel trsm and by the solves) is formed by k_big_inv128 on the side branch
-        k.inv_side = geti("B2_DENSE_INV_SIDE", 0) != 0;
-        k.n_reserved = std::max(1, geti("B2_DENSE_RESERVED_SMS", k.inv_side ? 2 : 1));   // SMs the trailing update leaves to the chain
-        k.use_near = geti("B2_DENSE_NEAR", 1) != 0;
-        // B2_DENSE_RELAX (default 1): R(k) waits for the panel's trsm only (not for the block-column update C(k), which it does not touch), and
-        // while the trailing update is long it leaves `early_reserved` SMs to the side branch so that T(k+1) / C(k+1) finish beside it
-        k.relax = geti("B2_DENSE_RELAX", 1) != 0;
-        k.early_reserved = std::max(1, geti("B2_DENSE_EARLY_RESERVED", 4));
-        // chain kernels launched programmatically dependent on their stream predecessor (each of them starts with pdl_sync())
-        k.chain_pdl = geti("B2_DENSE_PDL", 0) != 0;
-        // trailing updates with TMA bulk-copy operand staging + mbarrier ring + producer warp (front_kernels.cuh: big_update_tile_bulk)
-        k.bulk = geti("B2_UPDATE_BULK", 1) != 0;
-        // B2_DENSE_DEPTH2=1: the side branch updates TWO block columns (k+1, k+2) and the bulk update starts at k+3, so the next diagonal
-        // block only waits for the bulk update of two panels back: the chain of panel k+1 (and its panel trsm) runs a whole bulk period
-        // ahead and R(k+1) can follow R(k) without a gap while the trailing update is long
-        k.depth2 = geti("B2_DENSE_DEPTH2", 0) != 0;
-        return k;
-    }();
-    return K;
-}
-
-void lookahead_attrs() {
-    static bool attr = false;
-    if (attr) return;
-    cudaFuncSetAttribute(k_big_diag128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Diag128Smem));
-    cudaFuncSetAttribute(k_big_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
-    cudaFuncSetAttribute(k_big_update_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
-    cudaFuncSetAttribute(k_big_update_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
-    cudaFuncSetAttribute(k_big_update_dyn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
-    cudaFuncSetAttribute(k_big_update_dyn_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK);
-    cudaFuncSetAttribute(k_big_update_pipe_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK);
-    cudaFuncSetAttribute(k_near_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NT_SMEM);
-    cudaFuncSetAttribute(k_near_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NS_SMEM);
-    cudaFuncSetAttribute(k_near_trsv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NV_SMEM);
-    cudaFuncSetAttribute(k_big_inv128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Diag128Smem));
-    attr = true;
-}
-
-// `list1`: device pointer to the front's supernode id; f, w: its order and pivot count.  Returns the number of launches.
-int64_t enqueue_front_lookahead(const FactorArgs& a, const int32_t* list1, int f, int w, double* Linv, const int64_t* linv_off,
-                                LookaheadCtx& cx, cudaStream_t S1) {
-    const LookaheadKnobs& K = lookahead_knobs();
-    lookahead_attrs();
-    const int nb = (w + DB - 1) / DB, nsm = sm_count();
-    cudaStream_t S2 = cx.S2, S3 = cx.S3;
-    int64_t nl = 0;
-    auto launch_chain = [&](auto kern, dim3 grid, size_t smem, auto... args) {
-        if (K.chain_pdl) launch_pdl(kern, grid, dim3(256), smem, S1, args...);
-        else kern<<<grid, 256, smem, S1>>>(args...);
-        ++nl;
-    };
-    cudaEvent_t ev_bulk = nullptr, ev_side = nullptr;            // most recent R(.) / side-branch completion
-    cudaEvent_t ev_bulk_prev = nullptr;                          // R(.) before the most recent one (depth-2 look-ahead)
-    const int cw = K.depth2 ? 2 * DB : DB;                       // columns the side branch updates per panel
-    for (int k = 0; k < nb; ++k) {
-        const int ob = k * DB;
-        const int nbk = std::min(DB, w - ob);                    // pivots of this block column
-        const int j1 = ob + nbk;                                 // first trailing row / column
-        const int rem2 = f - (ob + 2 * DB);                      // rows / columns from the block after the next on
-        const bool near_step = K.use_near && ob + 2 * DB <= w;   // the next diagonal block is a full pivot block
-        const int with_inv = (near_step && K.inv_side) ? 0 : 1;  // inverse of this block formed on the side branch?
-        if (K.use_near && k > 0) launch_chain(k_big_diag128, dim3(1), sizeof(Diag128Smem), a, list1, ob, Linv, linv_off, with_inv);
-        else { k_big_diag128<<<1, 256, sizeof(Diag128Smem), S1>>>(a, list1, ob, Linv, linv_off, with_inv); ++nl; }
-        if (j1 >= f) continue;                                   // no rows below (last block of a dense matrix)
-        if (near_step) {
-            cudaEvent_t ev_diag = cx.ev(), ev_near = cx.ev();
-            cudaEventRecord(ev_diag, S1);
-            if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);                          // C(k-1) wrote the rows N1(k) reads
-            if (K.inv_side) launch_chain(k_near_trsv, dim3(DB / NT_ROWS), NV_SMEM, a, list1, ob);
-            else launch_chain(k_near_trsm, dim3(DB / NT_ROWS), NT_SMEM, a, list1, ob, (const double*)Linv, linv_off);
-            cudaEventRecord(ev_near, S1);
-            // R(k-1) also wrote the next diagonal block -- unless the side branch covers two block columns: then R(k-1) starts at
-            // block column k+2 and the last bulk writer of this tile is R(k-2)
-            if (K.depth2) { if (ev_bulk_prev) cudaStreamWaitEvent(S1, ev_bulk_prev, 0); }
-            else if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);
-            launch_chain(k_near_syrk, dim3(10), NS_SMEM, a, list1, ob);
-            if (K.inv_side) {
-                cudaStreamWaitEvent(S3, ev_diag, 0);
-                k_big_inv128<<<1, 256, sizeof(Diag128Smem), S3>>>(a, list1, ob, Linv, linv_off);
-                ++nl;
-                if (rem2 <= 0) { ev_side = cx.ev(); cudaEventRecord(ev_side, S3); }
-            }
-            if (rem2 > 0) {
-                if (!K.inv_side) cudaStreamWaitEvent(S3, ev_diag, 0);
-                k_big_trsm<<<dim3((rem2 + TR_ROWS - 1) / TR_ROWS, 1), 256, GU_SMEM, S3>>>(a, list1, ob, Linv, linv_off, DB / TR_ROWS);
-                cudaEvent_t ev_panel = nullptr;
-                if (K.relax) { ev_panel = cx.ev(); cudaEventRecord(ev_panel, S3); }    // "panel k's L is complete"
-                cudaStreamWaitEvent(S3, ev_near, 0);
-                if (ev_bulk) cudaStreamWaitEvent(S3, ev_bulk, 0);                      // R(k-1) also wrote these block columns
-                k_big_update_rows<<<dim3((rem2 + GU_M - 1) / GU_M, (cw + GU_N - 1) / GU_N, 1), 256, GU_SMEM, S3>>>(a, list1, ob, DB, DB, DB + cw, 1, 1);
-                ev_side = cx.ev();
-                cudaEventRecord(ev_side, S3);
-                nl += 2;
-                const int remb = f - (ob + DB + cw);                                   // columns left to the bulk branch
-                if (remb > 0) {
-                    cudaStreamWaitEvent(S2, K.relax ? ev_panel : ev_side, 0);
-                    const int nbx = (remb + GU_M - 1) / GU_M, nby = (remb + GU_N - 1) / GU_N;
-                    const int nres = (K.relax && remb >= 2048) ? std::max(K.n_reserved, K.early_reserved) : K.n_reserved;
-                    if (K.bulk) k_big_update_dyn_bulk<<<2 * nsm, GU_NT_BULK, GU_SMEM_BULK, S2>>>(a, list1, ob, DB, DB + cw, 1 << 30, 0, nbx, nby, cx.tilecnt + k, nres);
-                    else k_big_update_dyn<<<2 * nsm, 256, GU_SMEM, S2>>>(a, list1, ob, DB, DB + cw, 1 << 30, 0, nbx, nby, cx.tilecnt + k, nres);
-                    ev_bulk_prev = ev_bulk;
-                    ev_bulk = cx.ev();
-                    cudaEventRecord(ev_bulk, S2);
-                    ++nl;
-                }
-            }
-            continue;
-        }
-        // general path: whole-panel trsm and the update of the next 128 columns on the chain, the rest on the bulk branch
-        if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);
-        k_big_trsm<<<dim3((f - j1 + TR_ROWS - 1) / TR_ROWS, 1), 256, GU_SMEM, S1>>>(a, list1, ob, Linv, linv_off, 0);
-        if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);                              // R(k-1) also wrote block column k+1
-        const int jhi = std::min(f, ob + 2 * DB);
-        k_big_update_pipe<<<dim3((f - j1 + GU_M - 1) / GU_M, (jhi - j1 + GU_N - 1) / GU_N, 1), 256, GU_SMEM, S1>>>(a, list1, ob, DB, DB, 2 * DB, 1);
-        nl += 2;
-        if (rem2 > 0) {
-            cudaEvent_t ev_chain = cx.ev();
-            cudaEventRecord(ev_chain, S1);
-            cudaStreamWaitEvent(S2, ev_chain, 0);
-            const int nbx = (rem2 + GU_M - 1) / GU_M, nby = (rem2 + GU_N - 1) / GU_N;
-            if (K.bulk) k_big_update_dyn_bulk<<<2 * nsm, GU_NT_BULK, GU_SMEM_BULK, S2>>>(a, list1, ob, DB, 2 * DB, 1 << 30, 0, nbx, nby, cx.tilecnt + k, K.n_reserved);
-                else k_big_update_dyn<<<2 * nsm, 256, GU_SMEM, S2>>>(a, list1, ob, DB, 2 * DB, 1 << 30, 0, nbx, nby, cx.tilecnt + k, K.n_reserved);
-            ev_bulk = cx.ev();
-            cudaEventRecord(ev_bulk, S2);
-            ++nl;
-        }
-    }
-    if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);                                  // join
-    if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);
-    return nl;
 }
 
 FactorArgs factor_args(b2_solver* s) {
@@ -363,8 +175,6 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
         return 2;
     }
     if (P.fused.n_cta) warp_launch(P.fused);
-    s->ev_next = 0;
-    if (s->d_tilecnt.p) cudaMemsetAsync(s->d_tilecnt.p, 0, s->d_tilecnt.bytes(), st);
     for (const LevelSched& lv : P.lev) {
         if (lv.W.n_cta) warp_launch(lv.W);
         if (lv.W2.n_cta) warp_launch(lv.W2);
@@ -383,17 +193,9 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
                 k_big_extend_add<<<dim3(std::max(1, std::min(8 * nsm / lv.nB + 1, (lv.maxrB * 32 + 255) / 256)), lv.nB), 256, 0, st>>>(a, lb, c);
                 ++nl;
             }
-            // the largest fronts one at a time, each with the whole GPU: diagonal blocks / near-diagonal steps of panel k+1 run beside
-            // the trailing update of panel k (three stream branches, joined back into `st`)
-            for (int i = 0; i < lv.nLA; ++i) {
-                LookaheadCtx cx;
-                cx.S2 = s->la_bulk; cx.S3 = s->la_side; cx.pool = &s->ev_pool; cx.next = &s->ev_next; cx.tilecnt = s->d_tilecnt.p + lv.la[i][2];
-                nl += enqueue_front_lookahead(a, lb + i, lv.la[i][1], lv.la[i][0], s->d_Linv.p, s->d_linv_off.p, cx, st);
-            }
-            // the others batched level-wide, three launches per 128 pivot columns
-            if (lv.nB > lv.nLA)
-                for (int ob = 0; ob < lv.maxwBr; ob += DB)
-                    launch_big_step(a, lb + lv.nLA, lv.nB - lv.nLA, ob, lv.maxfBr, s->d_Linv.p, s->d_linv_off.p, st, &nl);
+            // batched level-wide, three launches per 128 pivot columns
+            for (int ob = 0; ob < lv.maxwB; ob += DB)
+                launch_big_step(a, lb, lv.nB, ob, lv.maxfB, s->d_Linv.p, s->d_linv_off.p, st, &nl);
         }
     }
     if (P.topfused.n_cta) warp_launch(P.topfused);
@@ -411,14 +213,13 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
     int64_t nl = 0;
     const Phase& P = s->phase[ph];
     // level kernels are launched programmatically dependent on their predecessor (see warp_kernels.cuh: pdl_wait)
-    const bool pdl = pdl_enabled();
     cudaLaunchAttribute pattr[1];
     pattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     pattr[0].val.programmaticStreamSerializationAllowed = 1;
     auto cfg_of = [&](int grid, int block, size_t sm) {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = sm; cfg.stream = st;
-        cfg.attrs = pattr; cfg.numAttrs = pdl ? 1 : 0;
+        cfg.attrs = pattr; cfg.numAttrs = 1;
         return cfg;
     };
     auto warp_launch = [&](const WarpLaunch& L, bool fused = false) {
@@ -525,11 +326,6 @@ int capture(b2_solver* s, cudaGraphExec_t* out, Fn fn) {
 }
 
 void build_schedule(b2_solver* s) {
-    // fronts with at least this many pivot columns get the look-ahead schedule (B2_LOOKAHEAD_MIN_W; 0 = off, the default: on the 64^3
-    // augmented grid one front at a time with look-ahead measured slower than the level-batched launches, whose diagonal-block
-    // kernels already run side by side across the fronts of a level)
-    int la_min_w = 0, la_tiles = 0;
-    if (const char* e = getenv("B2_LOOKAHEAD_MIN_W")) la_min_w = atoi(e);
     const Symbolic& S = s->S;
     const int ns = S.nsuper;
     const int rank = std::max(0, s->opt.part_rank);
@@ -727,22 +523,6 @@ void build_schedule(b2_solver* s) {
             if (!Wx.empty()) lv.W = level_launch(Wx, 1);
             if (!W2x.empty()) lv.W2 = level_launch(W2x, 2);
             lv.offM = (int)sched.size(); lv.nM = (int)Mx.size(); sched.insert(sched.end(), Mx.begin(), Mx.end());
-            {   // look-ahead fronts first (stable: ascending supernode id inside both groups)
-                std::vector<int32_t> la_sn, rest;
-                for (int sn : Bx) {
-                    int w, f; fdim(sn, w, f);
-                    if (la_min_w > 0 && w >= la_min_w && s->la_bulk && s->la_side) {
-                        la_sn.push_back(sn);
-                        lv.la.push_back({w, f, la_tiles});
-                        la_tiles += (w + DB - 1) / DB;
-                    } else {
-                        rest.push_back(sn);
-                        lv.maxfBr = std::max(lv.maxfBr, f); lv.maxwBr = std::max(lv.maxwBr, w);
-                    }
-                }
-                lv.nLA = (int)la_sn.size();
-                Bx = la_sn; Bx.insert(Bx.end(), rest.begin(), rest.end());
-            }
             lv.offB = (int)sched.size(); lv.nB = (int)Bx.size(); sched.insert(sched.end(), Bx.begin(), Bx.end());
             lv.offC = lv.offM; lv.nC = lv.nM + lv.nB;        // M and B lists are adjacent
             P.lev.push_back(lv);
@@ -751,7 +531,6 @@ void build_schedule(b2_solver* s) {
     }
     if (sched.empty()) sched.push_back(0);
     B2_CUDA_THROW(s->d_sched.upload(sched.data(), sched.size()));
-    if (la_tiles) B2_CUDA_THROW(s->d_tilecnt.alloc((size_t)la_tiles));
 }
 
 int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t* rowval_h, const double* nzval_d,
@@ -889,8 +668,6 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(cudaMemset(s->d_cbv.p, 0, s->d_cbv.bytes()));
         B2_CUDA_THROW(cudaMallocHost((void**)&s->h_counters, 8 * sizeof(int32_t)));
         B2_CUDA_THROW(cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
-        B2_CUDA_THROW(cudaStreamCreateWithFlags(&s->la_bulk, cudaStreamNonBlocking));
-        B2_CUDA_THROW(cudaStreamCreateWithFlags(&s->la_side, cudaStreamNonBlocking));
         build_schedule(s);
         if (set_smem_attrs() != B2_OK) throw std::runtime_error("attr");
         if (Phase& P = s->phase[0]; P.dep_ngroup) {
@@ -966,10 +743,8 @@ int b2_options_default(b2_options* opt) {
     opt->small_front_max = 160;
     opt->fuse_max_fronts = 8;      // measured optimum on OPF-10k (tools/sweep_headline.sh)
     opt->dep_schedule = 1;
-    if (const char* e = getenv("B2_DEP_SCHEDULE")) opt->dep_schedule = atoi(e);
     opt->chain_merge_f = 0;      // measured on the OPF-10k tree: 16 -> 11 levels but the merged (two-warp) leaves make the
                                  // throughput-bound bottom of the tree longer, and the factorisation slower
-    if (const char* e = getenv("B2_CHAIN_MERGE_F")) opt->chain_merge_f = atoi(e);
     opt->n_parts = 1;
     opt->part_rank = 0;
     return B2_OK;
@@ -1303,11 +1078,51 @@ __global__ void k_copy_lower(int N, int lda, const double* __restrict__ A, doubl
         F[(size_t)j * N + i] = A[(size_t)j * lda + i];
 }
 
+__global__ void k_trace_reset(unsigned long long* t, int nslot) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < 2 * nslot) t[i] = (i & 1) ? 0ull : ~0ull;
+}
+
+// SMs the persistent trailing update leaves free for the chain and the side branch: always, and while at least 2048 columns remain
+// (so that the side branch's T(k+1) / C(k+1) finish beside the long early updates)
+constexpr int LA_RESERVED_SMS = 1, LA_EARLY_RESERVED_SMS = 4;
+
+void lookahead_attrs() {
+    static bool attr = false;
+    if (attr) return;
+    cudaFuncSetAttribute(k_big_diag128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Diag128Smem));
+    cudaFuncSetAttribute(k_big_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
+    cudaFuncSetAttribute(k_big_update_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
+    cudaFuncSetAttribute(k_big_update_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
+    cudaFuncSetAttribute(k_big_update_dyn_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK);
+    cudaFuncSetAttribute(k_near_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NT_SMEM);
+    cudaFuncSetAttribute(k_near_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NS_SMEM);
+    attr = true;
+}
+
+// ----------------------------------------------------------------------------------------------------------
+// Look-ahead schedule of the dense factorisation (N > 4 * 128), three stream branches joined back into S1 (captured into the
+// caller's graph).  Per block column k of 128 pivots:
+//   chain S1:  D(k) diagonal block -> N1(k) the 128 x 128 block of L below it (k_near_trsm) -> N2(k) update of the NEXT diagonal block
+//              (k_near_syrk) -> D(k+1) ...                         -- the only kernels on the critical path, each a few SMs wide
+//   side  S3:  T(k) trsm of the rows from block k+2 on (after D(k)) -> C(k) rest of block column k+1 (after N1(k), R(k-1))
+//   bulk  S2:  R(k) update of the columns >= k+2 (persistent, dynamic tiles, leaves the reserved SMs to the other branches); it waits
+//              for T(k) only, not for C(k), whose columns it does not touch
+// N1(k+1) waits for C(k), N2(k) and C(k) wait for R(k-1).  While the trailing update is long (first panels) the chain waits for it;
+// once it is short the period is D + N1 + N2 instead of D + whole-panel trsm + whole-column update.
+// When N is not a multiple of 128, block column nb - 2 has no full pivot block after it and takes the general path: whole-panel
+// trsm and update of the remaining columns on the chain.
+// ----------------------------------------------------------------------------------------------------------
 void enqueue_dense_factor_lookahead(b2d_solver* s, cudaStream_t S1) {
+    lookahead_attrs();
     FactorArgs a;
     a.desc = s->desc.p; a.child_idx = nullptr; a.rel = nullptr; a.amap_src = nullptr; a.amap_dst = nullptr;
     a.A = nullptr; a.L = s->fact.p; a.ws = nullptr; a.dvec = s->dvec.p; a.counters = s->counters.p; a.eps = s->opt.pivot_eps;
-    const int N = s->N, nb = (N + DB - 1) / DB;
+    const int N = s->N, nb = (N + DB - 1) / DB, nsm = sm_count();
+    const int32_t* list1 = s->list.p;
+    double* Linv = s->linv.p;
+    const int64_t* linv_off = s->linv_off.p;
+    cudaStream_t S2 = s->aux_stream, S3 = s->side_stream;
     if (s->trace.p) {
         a.trace = s->trace.p;
         k_trace_reset<<<(16 * nb + 255) / 256, 256, 0, S1>>>(s->trace.p, 8 * nb);
@@ -1315,15 +1130,56 @@ void enqueue_dense_factor_lookahead(b2d_solver* s, cudaStream_t S1) {
     cudaMemsetAsync(s->counters.p, 0, 2 * sizeof(int32_t), S1);
     cudaMemsetAsync(s->tilecnt.p, 0, s->tilecnt.bytes(), S1);
     k_copy_lower<<<dim3(std::max(1, std::min(8, (N + 255) / 256)), N), 256, 0, S1>>>(N, s->lda, s->A_d, s->fact.p);
-    LookaheadCtx cx;
-    cx.S2 = s->aux_stream; cx.S3 = s->side_stream; cx.pool = &s->ev_pool; s->ev_next = 0; cx.next = &s->ev_next; cx.tilecnt = s->tilecnt.p;
-    enqueue_front_lookahead(a, s->list.p, N, N, s->linv.p, s->linv_off.p, cx, S1);
+    s->ev_next = 0;
+    auto ev = [s] {                                              // events, created on demand, handed out in order
+        if (s->ev_next == s->ev_pool.size()) { cudaEvent_t e; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); s->ev_pool.push_back(e); }
+        return s->ev_pool[s->ev_next++];
+    };
+    cudaEvent_t ev_bulk = nullptr, ev_side = nullptr;            // most recent R(.) / side-branch completion
+    for (int k = 0; k < nb; ++k) {
+        const int ob = k * DB;
+        const int j1 = std::min(N, ob + DB);                     // first trailing row / column
+        const int rem2 = N - (ob + 2 * DB);                      // rows / columns from the block after the next on
+        k_big_diag128<<<1, 256, sizeof(Diag128Smem), S1>>>(a, list1, ob, Linv, linv_off);
+        if (j1 >= N) continue;                                   // last block column
+        if (rem2 < 0) {
+            // general path (the next diagonal block is not a full pivot block)
+            if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);
+            k_big_trsm<<<dim3((N - j1 + TR_ROWS - 1) / TR_ROWS, 1), 256, GU_SMEM, S1>>>(a, list1, ob, Linv, linv_off, 0);
+            if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);                          // R(k-1) also wrote block column k+1
+            k_big_update_pipe<<<dim3((N - j1 + GU_M - 1) / GU_M, (N - j1 + GU_N - 1) / GU_N, 1), 256, GU_SMEM, S1>>>(a, list1, ob, DB, DB, 2 * DB, 1);
+            continue;
+        }
+        cudaEvent_t ev_diag = ev(), ev_near = ev();
+        cudaEventRecord(ev_diag, S1);
+        if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);                              // C(k-1) wrote the rows N1(k) reads
+        k_near_trsm<<<DB / NT_ROWS, 256, NT_SMEM, S1>>>(a, list1, ob, Linv, linv_off);
+        cudaEventRecord(ev_near, S1);
+        if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);                              // R(k-1) also wrote the next diagonal block
+        k_near_syrk<<<10, 256, NS_SMEM, S1>>>(a, list1, ob);
+        if (rem2 == 0) continue;
+        cudaStreamWaitEvent(S3, ev_diag, 0);
+        k_big_trsm<<<dim3((rem2 + TR_ROWS - 1) / TR_ROWS, 1), 256, GU_SMEM, S3>>>(a, list1, ob, Linv, linv_off, DB / TR_ROWS);
+        cudaEvent_t ev_panel = ev();
+        cudaEventRecord(ev_panel, S3);                                                 // "panel k's L is complete"
+        cudaStreamWaitEvent(S3, ev_near, 0);
+        if (ev_bulk) cudaStreamWaitEvent(S3, ev_bulk, 0);                              // R(k-1) also wrote these block columns
+        k_big_update_rows<<<dim3((rem2 + GU_M - 1) / GU_M, (DB + GU_N - 1) / GU_N, 1), 256, GU_SMEM, S3>>>(a, list1, ob, DB, DB, 2 * DB, 1, 1);
+        ev_side = ev();
+        cudaEventRecord(ev_side, S3);
+        cudaStreamWaitEvent(S2, ev_panel, 0);
+        const int nbx = (rem2 + GU_M - 1) / GU_M, nby = (rem2 + GU_N - 1) / GU_N;
+        const int nres = rem2 >= 2048 ? LA_EARLY_RESERVED_SMS : LA_RESERVED_SMS;
+        k_big_update_dyn_bulk<<<2 * nsm, GU_NT_BULK, GU_SMEM_BULK, S2>>>(a, list1, ob, DB, 2 * DB, 1 << 30, 0, nbx, nby, s->tilecnt.p + k, nres);
+        ev_bulk = ev();
+        cudaEventRecord(ev_bulk, S2);
+    }
+    if (ev_bulk) cudaStreamWaitEvent(S1, ev_bulk, 0);                                  // join
+    if (ev_side) cudaStreamWaitEvent(S1, ev_side, 0);
 }
 
 void enqueue_dense_factor(b2d_solver* s, cudaStream_t st) {
-    static int lookahead = -1;
-    if (lookahead < 0) { const char* e = getenv("B2_DENSE_LOOKAHEAD"); lookahead = e ? (atoi(e) != 0) : 1; }
-    if (lookahead && s->aux_stream && s->side_stream && s->N > 4 * DB) { enqueue_dense_factor_lookahead(s, st); return; }
+    if (s->N > 4 * DB) { enqueue_dense_factor_lookahead(s, st); return; }
     FactorArgs a;
     a.desc = s->desc.p; a.child_idx = nullptr; a.rel = nullptr; a.amap_src = nullptr; a.amap_dst = nullptr;
     a.A = nullptr; a.L = s->fact.p; a.ws = nullptr; a.dvec = s->dvec.p; a.counters = s->counters.p; a.eps = s->opt.pivot_eps;
@@ -1434,11 +1290,8 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream) {
     cudaStream_t st = as_stream(stream);
     const int N = s->N;
     const int nblk = (N + BS - 1) / BS;
-    static int flow_ok = -1;            // every CTA of the dataflow kernel must be resident: one per SM
-    if (flow_ok < 0) {
-        flow_ok = cudaFuncSetAttribute(k_dense_solve_flow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess ? 1 : 0;
-        if (const char* e = getenv("B2_DENSE_SOLVE_FLOW")) flow_ok = flow_ok && atoi(e) != 0;
-    }
+    static const bool flow_ok =         // every CTA of the dataflow kernel must be resident: one per SM
+        cudaFuncSetAttribute(k_dense_solve_flow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
     for (int c = 0; c < nrhs; ++c) {
         double* x = x_d + (size_t)c * N;
         if (flow_ok && nblk <= sm_count()) {

@@ -215,10 +215,9 @@ def test_condensed_opf_step_direction_and_inertia(case, seed):
         assert res < 1e-12
 
 
-@pytest.mark.parametrize("dep_schedule,chain_merge_f", [(3, 0), (5, 0), (1, 48), (0, 0)])
+@pytest.mark.parametrize("dep_schedule,chain_merge_f", [(1, 0), (1, 48), (0, 0)])
 def test_schedule_and_amalgamation_options_give_the_same_answers(dep_schedule, chain_merge_f):
-    """b2_options.dep_schedule (bit 0: single-launch factorisation, bit 1: single-launch flag-driven sweeps, bit 2: hybrid sweeps --
-    fused bottom subtrees + one flag-driven launch for the tree above them; 0: level launches) and
+    """b2_options.dep_schedule (bit 0: single-launch factorisation and solve; 0: level launches) and
     chain_merge_f (only children absorbed while the front stays team-class) change the schedule / the supernode partition, never the
     mathematics: same inertia as the oracle, refined direction within 1e-6, single-solve residual within fp64 backward stability."""
     _need_gpu()
@@ -311,13 +310,16 @@ def test_big_front_path_3d_grid():
             assert np.abs(x2 - x).max() / np.abs(x).max() < 1e-10
 
 
-@pytest.mark.parametrize("n_eq", [0, 24])
-def test_dense_condensed_qp(n_eq):
+@pytest.mark.parametrize("n,m,n_eq", [(320, 130, 0), (320, 130, 24), (900, 300, 0), (900, 300, 24)],
+                         ids=["0", "24", "n900-0", "n900-24"])
+def test_dense_condensed_qp(n, m, n_eq):
     """configs[1] structure at a size the oracle finishes in seconds: DenseCondensedKKTSystem assembly (A8),
-    dense LDL^T + inertia (neg == n_eq) and solve_kkt vs LAPACK dsytrf/dsytrs."""
+    dense LDL^T + inertia (neg == n_eq) and solve_kkt vs LAPACK dsytrf/dsytrs.  N = n + n_eq = 320 / 344 is factorised with
+    three launches per block column; N = 900 / 924 with the look-ahead schedule, and since N is not a multiple of 128 its
+    block column nb - 2 takes that schedule's general path."""
     _need_gpu()
     from madnlp_jl_b200 import kkt as K
-    qp = W.dense_qp(n=320, m=130, n_eq=n_eq, seed=3)
+    qp = W.dense_qp(n=n, m=m, n_eq=n_eq, seed=3)
     it = W.dense_qp_iterate(qp, mu=1e-3, seed=4)
     ns = qp.m - n_eq
     cb = o.Callback(qp.n, qp.m, [], [], [], [], qp.ind_ineq, qp.ind_lb, qp.ind_ub)

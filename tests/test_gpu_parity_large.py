@@ -152,10 +152,9 @@ def _product_perm(N, cp, rv, **opts):
     return perm
 
 
-@pytest.mark.parametrize("nx,la_min_w", [(32, None), (32, 512)])
-def test_augmented_grid_delta_1e8_against_the_ldl_oracle(nx, la_min_w, monkeypatch):
-    """(la_min_w = None: every big front through the level-batched launches, the default; 512: fronts with >= 512 pivot columns are
-    factorised one at a time with the three-branch look-ahead schedule the dense solver uses -- the 32^2 and 32 x 16 separators here.)
+@pytest.mark.parametrize("nx,la_min_w", [(32, None)])
+def test_augmented_grid_delta_1e8_against_the_ldl_oracle(nx, la_min_w):
+    """(la_min_w = None: every big front through the level-batched launches, the default.)
     SparseKKTSystem-style quasi-definite matrix with delta = 1e-8 (SURVEY 8d C5), big (HBM-resident) fronts: inertia
     identical to the LDL^T oracle (src/LinearSolvers/ldl.jl restated) and the solution after Richardson refinement on K x = b
     within 1e-6 of the oracle's refined solution.  The oracle is the scalar up-looking LDL^T (no supernodes, no amalgamation, a
@@ -165,8 +164,6 @@ def test_augmented_grid_delta_1e8_against_the_ldl_oracle(nx, la_min_w, monkeypat
     _need_gpu()
     from madnlp_jl_b200.linear_solvers import B200SparseSolver, DeviceCSC
     from madnlp_jl_b200 import kkt as K
-    if la_min_w is not None:
-        monkeypatch.setenv("B2_LOOKAHEAD_MIN_W", str(la_min_w))
     N, n_tot, m, I, J, V = W.augmented_grid_kkt(nx, nx, nx, delta=1e-8)
     cp, rv, mp = o.coo_to_csc(I, J, N, N)
     nz = np.zeros(len(rv)); o.transfer(nz, V, mp)
