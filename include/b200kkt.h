@@ -166,6 +166,12 @@ int b2_debug_profile_front(b2_solver* s, int32_t sn, int32_t reps, int64_t* stam
  * finished: stamps_h[3 * sn + {0,1,2}].  Also returns the supernode parents and (w, f) of every front.  *count = number of
  * supernodes; data is copied when capacity >= *count (stamps are zero when tracing is off). */
 int b2_debug_trace(b2_solver* s, uint64_t* stamps_h, int32_t* parent_h, int32_t* w_h, int32_t* f_h, int64_t capacity, int64_t* count);
+/* Debug: per-front device timeline of the single-launch solve, under the same B2_SPARSE_TRACE=1 switch.  Each front stamps
+ * %globaltimer (ns) for its forward and its backward task: when the task is claimed, when its inputs have arrived (children's
+ * contributions / ancestor values and own forward result) and when it has handed its outputs on: stamps_h[6 * sn + {0,1,2}]
+ * forward, {3,4,5} backward, as left by the last solve.  *count = number of uint64 values (0 when tracing is off); stamps are
+ * copied when capacity >= *count. */
+int b2_debug_trace_solve(b2_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count);
 
 /* ------------------------------------------------------------------ dense LDL^T */
 typedef struct b2d_solver b2d_solver;

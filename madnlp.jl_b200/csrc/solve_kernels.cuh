@@ -27,6 +27,14 @@ struct SolveArgs {
     // written there by the backward sweep, so that no permutation kernels run; null for the level-launch solve
     const int32_t* perm = nullptr;
     double* x = nullptr;
+    // hand-off slots of the single-launch solve (warp_kernels.cuh: slot_take): contribution vectors child -> parent (`up`) and
+    // ancestor values parent -> child (`down`), both at the cbv_off offsets, and each front's forward result for its own backward
+    // task (`ypiv`, permuted order)
+    double* up = nullptr;
+    double* down = nullptr;
+    double* ypiv = nullptr;
+    unsigned long long* strace = nullptr;  // debug (B2_SPARSE_TRACE): [supernode][6] = forward {claimed, inputs arrived, done},
+                                           // backward {claimed, inputs arrived, done} of k_solve_dep (b2_debug_trace_solve)
 };
 
 __global__ void k_perm_in(int n, const int32_t* __restrict__ perm, const double* __restrict__ x, double* __restrict__ xp) {

@@ -66,15 +66,17 @@ struct b2_solver {
     DevBuf<int32_t> d_counters;
     DevBuf<double> d_Linv, d_side;
     DevBuf<int64_t> d_linv_off;
-    // dependency flags [3][nsuper] (factorisation, forward sweep, backward sweep), then the factorisation's group ticket and the
-    // single-launch solve's {ticket, epoch}; supernode parents
-    DevBuf<int32_t> d_flags, d_parent;
+    // the factorisation's dependency flags [nsuper], then its group ticket and the single-launch solve's {ticket, CTAs out}
+    DevBuf<int32_t> d_flags;
+    // hand-off slots of the single-launch solve (k_solve_dep), SLOT_EMPTY between launches: up [sum r] | down [sum r] | ypiv [n]
+    DevBuf<double> d_slots;
     int32_t* h_counters = nullptr;   // pinned
     std::vector<int64_t> cbv_off;
     int64_t exch_cbv = 0;
     Phase phase[2];                  // 0 = local (owned subtrees), 1 = shared top tree
     cudaStream_t cap_stream = nullptr;
     DevBuf<unsigned long long> d_ftrace;                 // B2_SPARSE_TRACE=1: per-front stamps of the team-class factor kernels (b2_debug_trace)
+    DevBuf<unsigned long long> d_strace;                 // B2_SPARSE_TRACE=1: per-front stamps of k_solve_dep (b2_debug_trace_solve)
     bool factorized = false;
     int64_t last_perturbed = 0;
     std::vector<uint8_t> owned_mask;  // original numbering
@@ -167,11 +169,11 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
     if (P.dep_ngroup && (s->opt.dep_schedule & 1)) {
         DepSched ds;
         ds.grp_type = sched + P.dep_type_off; ds.grp_ptr = sched + P.dep_ptr_off; ds.tasks = sched + P.dep_tasks_off; ds.ngroup = P.dep_ngroup;
-        // (the group ticket in slot 3*nsuper re-arms itself: the CTA that takes the last group resets it)
+        // (the group ticket in slot nsuper re-arms itself: the CTA that takes the last group resets it)
         cudaMemsetAsync(s->d_flags.p, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
         const size_t sm = sizeof(double) * std::max<size_t>((size_t)FW_WARPS * TeamSmem<1>::doubles(P.dep_maxf1), (size_t)TeamSmem<2>::doubles(P.dep_maxf2));
         k_factor_dep<<<P.dep_ngroup, 128, sm, st>>>(a, s->d_childrec.p, ds, P.dep_maxf1, P.dep_maxf2, s->d_flags.p, s->d_counters.p + 4,
-                                                    s->d_flags.p + (size_t)3 * s->S.nsuper);
+                                                    s->d_flags.p + s->S.nsuper);
         return 2;
     }
     if (P.fused.n_cta) warp_launch(P.fused);
@@ -286,12 +288,16 @@ void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
     SolveArgs a = solve_args(s);
     a.perm = s->d_perm.p;
     a.x = x;
+    a.strace = s->d_strace.p;
+    const int64_t nr = s->cbv_off[s->S.nsuper];
+    a.up = s->d_slots.p;
+    a.down = s->d_slots.p + nr;
+    a.ypiv = s->d_slots.p + 2 * nr;
     DepSched ds;
     ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
     ds.ngroup = P.dep_ngroup;
-    const size_t ns = (size_t)s->S.nsuper;
-    k_solve_dep<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_parent.p, s->d_flags.p + ns, s->d_flags.p + 2 * ns,
-                                                         s->d_counters.p + 4, s->d_flags.p + 3 * ns + 1, s->S.n);
+    k_solve_dep<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1, s->S.n,
+                                                         s->d_slots.p, (int64_t)s->d_slots.n);
 }
 
 int set_smem_attrs() {
@@ -639,7 +645,11 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             }
             B2_CUDA_THROW(s->d_childrec.upload(cr.data(), cr.size()));
         }
-        if (const char* e = getenv("B2_SPARSE_TRACE")) if (atoi(e)) B2_CUDA_THROW(s->d_ftrace.alloc((size_t)3 * ns));
+        if (const char* e = getenv("B2_SPARSE_TRACE"); e && atoi(e)) {
+            B2_CUDA_THROW(s->d_ftrace.alloc((size_t)3 * ns));
+            B2_CUDA_THROW(s->d_strace.alloc((size_t)6 * ns));
+            B2_CUDA_THROW(cudaMemset(s->d_strace.p, 0, s->d_strace.bytes()));
+        }
         B2_CUDA_THROW(s->d_L.alloc((size_t)S.lp_off[ns] + 2));          // (+2: the bulk-copy staging may read one aligned pair past a panel)
         B2_CUDA_THROW(s->d_Lt.alloc((size_t)S.lp_off[ns]));
         {
@@ -661,9 +671,8 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(s->d_cbv.alloc((size_t)std::max<int64_t>(1, s->cbv_off[ns])));
         B2_CUDA_THROW(s->d_counters.alloc(8));
         B2_CUDA_THROW(cudaMemset(s->d_counters.p, 0, 8 * sizeof(int32_t)));
-        B2_CUDA_THROW(s->d_flags.alloc((size_t)3 * ns + 3));
+        B2_CUDA_THROW(s->d_flags.alloc((size_t)ns + 3));
         B2_CUDA_THROW(cudaMemset(s->d_flags.p, 0, s->d_flags.bytes()));
-        B2_CUDA_THROW(s->d_parent.upload(S.sn_parent.data(), S.sn_parent.size()));
         B2_CUDA_THROW(cudaMemset(s->d_ws.p, 0, s->d_ws.bytes()));
         B2_CUDA_THROW(cudaMemset(s->d_cbv.p, 0, s->d_cbv.bytes()));
         B2_CUDA_THROW(cudaMallocHost((void**)&s->h_counters, 8 * sizeof(int32_t)));
@@ -677,6 +686,8 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             const int ntask = 2 * P.dep_ngroup;
             P.sol_grid = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
             P.n_solve_launches = 1;
+            B2_CUDA_THROW(s->d_slots.alloc((size_t)(2 * s->cbv_off[ns] + n)));
+            B2_CUDA_THROW(cudaMemset(s->d_slots.p, 0xff, s->d_slots.bytes()));     // every slot SLOT_EMPTY
         }
     } catch (std::exception&) {
         delete s;
@@ -1010,6 +1021,16 @@ int b2_debug_trace(b2_solver* s, uint64_t* stamps_h, int32_t* parent_h, int32_t*
         B2_CUDA(cudaMemcpy(stamps_h, s->d_ftrace.p, s->d_ftrace.bytes(), cudaMemcpyDeviceToHost));
     } else if (stamps_h) {
         std::memset(stamps_h, 0, (size_t)3 * ns * sizeof(uint64_t));
+    }
+    return B2_OK;
+}
+
+int b2_debug_trace_solve(b2_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count) {
+    if (!s || !count) { set_error("b2_debug_trace_solve: invalid argument"); return B2_ERR_INVALID; }
+    *count = s->d_strace.p ? (int64_t)6 * s->S.nsuper : 0;
+    if (stamps_h && *count && capacity >= *count) {
+        B2_CUDA(cudaDeviceSynchronize());
+        B2_CUDA(cudaMemcpy(stamps_h, s->d_strace.p, s->d_strace.bytes(), cudaMemcpyDeviceToHost));
     }
     return B2_OK;
 }

@@ -98,8 +98,7 @@ __device__ __forceinline__ void cp_async16_cg(void* smem_dst, const void* gsrc) 
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
 }
-// dependency flags of the single-launch ("dependency-driven") schedules.  A flag is ready when it holds `want`: the factorisation
-// zeroes its flags and sets them to 1; the solve never clears its flags and sets them to the launch's epoch instead.
+// dependency flags of the single-launch factorisation (k_factor_dep): zeroed before the launch, a flag is ready when it holds `want`
 __device__ __forceinline__ void flag_wait(const int* flag, int* err, int want = 1) {
     int v = 0;
     unsigned it = 0;
@@ -110,13 +109,60 @@ __device__ __forceinline__ void flag_wait(const int* flag, int* err, int want = 
     } while (++it < (1u << 24));
     if (v != want) {                     // bounded spin: never hang the device, report instead
         atomicExch(err, 1);
-        __threadfence();                 // (visible before this CTA's next ticket claim: k_solve_dep checks it after the last claim)
+        __threadfence();
     }
 }
 __device__ __forceinline__ void flag_set(int* flag, int v = 1) {
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(v) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Hand-off slots of the single-launch solve: the value is its own flag.  A slot holds SLOT_EMPTY until its one producer stores the
+// value; its one consumer polls the value itself (no flag, no release fence, one L2 round trip per hand-off) and stores SLOT_EMPTY
+// back once it has it, which arms the slot for the next launch.  SLOT_EMPTY is all-ones -- a negative NaN with a full payload, which
+// a byte-wise cudaMemset(0xff) writes and fp64 arithmetic never produces; a producer stores a value with that bit pattern (a NaN
+// from the caller's right-hand side) as the canonical NaN instead.
+constexpr unsigned long long SLOT_EMPTY = ~0ull;
+constexpr unsigned long long CANON_NAN = 0x7ff8000000000000ull;
+__device__ __forceinline__ unsigned long long slot_ld(const double* p) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(v) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ void slot_st(double* p, unsigned long long v) {
+    asm volatile("st.relaxed.gpu.global.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ void slot_put(double* p, double v) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+    slot_st(p, b == SLOT_EMPTY ? CANON_NAN : b);
+}
+// take the slots p[c] with bit c of `need` set: poll them all at once until none is empty, then re-arm each.  Bounded like flag_wait:
+// a slot still empty at the time-out sets *err (the solve then writes NaN into x) and reads as NaN.
+template <int K>
+__device__ __forceinline__ void slot_take(double* const (&p)[K], unsigned need, double (&v)[K], int* err) {
+    unsigned long long b[K];
+#pragma unroll
+    for (int c = 0; c < K; ++c) b[c] = (need >> c & 1u) ? slot_ld(p[c]) : 0ull;
+    unsigned it = 0;
+    for (;;) {
+        unsigned pend = 0;
+#pragma unroll
+        for (int c = 0; c < K; ++c) pend |= ((need >> c & 1u) && b[c] == SLOT_EMPTY) ? 1u << c : 0u;
+        if (!pend) break;
+        if (++it >= (1u << 24)) {            // never hang the device, report instead
+            atomicExch(err, 1);
+            break;
+        }
+        __nanosleep(32);
+#pragma unroll
+        for (int c = 0; c < K; ++c) if (pend >> c & 1u) b[c] = slot_ld(p[c]);
+    }
+#pragma unroll
+    for (int c = 0; c < K; ++c) {
+        v[c] = __longlong_as_double((long long)b[c]);
+        if ((need >> c & 1u) && b[c] != SLOT_EMPTY) slot_st(p[c], SLOT_EMPTY);
+    }
+}
 
 // One pivot of front_factor_team's software-pipelined loop, for a window of NB live 8-column blocks: the latency chain of pivot k
 // (d_k -> reciprocal (approx + 2 Newton steps) -> l_k -> column k+1 -> publish -> arrive) and the pending row update of pivot k-1,
@@ -423,17 +469,20 @@ struct SolveSmem {
     static constexpr int doubles = FMAX + 16 + 4 * MAXC + FMAX * FMAX;
 };
 
-// DEP: the front runs inside a single-launch solve -- values other CTAs produced are read from L2, and when `done` is given the
-// front waits for its children's flags (== epoch) and sets its own.  With a.x set (single-launch solve) the forward sweep reads its
-// right-hand side straight from the caller's x[perm[j]] and the backward sweep writes its solution there too, beside xp.
+// DEP: the front runs inside the single-launch solve (k_solve_dep).  It reads its right-hand side straight from the caller's
+// x[perm[j]] and takes its children's contribution vectors from their `up` slots; it puts its own contribution vector into its `up`
+// slots and its forward result into its `ypiv` slots (for its own backward task).  The backward sweep takes the ancestor values
+// from its `down` slots and its forward result from `ypiv`, writes its solution into x[perm[j]] and puts each child's ancestor
+// values into that child's `down` slots.  Without DEP (level-launch solve) the values go through xp and cbv instead.
 template <int NW, bool DEP = false>
 __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRec* childrec, int s, double* sm_team, int tid, int team,
-                                               int* done = nullptr, int* err = nullptr, int epoch = 1) {
+                                               int* err = nullptr) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* ys = sm_team;                              // [FMAX] assembly of the front's rhs
     double* yb = ys + FMAX;                            // [2][8] broadcast slots
     ChildRec* recs = (ChildRec*)(yb + 16);             // [MAXC]
     double* P = (double*)(recs + MAXC);                // panel, column-major, ld f
+    if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s] = global_ns();
     const FrontDesc d = a.desc[s];
     const int f = d.f, w = d.w;
     {
@@ -441,6 +490,7 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
         for (int e = tid; e < f * w; e += TEAM) cp_async8(P + e, Lp + e);
     }
     const int pj = (a.x && tid < w) ? a.perm[d.col0 + tid] : 0;
+    const int64_t cvo = a.cbv_off[s];                  // (loaded early: the address of the hand-off at the end)
     for (int c0 = 0; c0 < max(d.nchild, 1); c0 += MAXC) {
         const int nc = min(MAXC, d.nchild - c0);
         if (tid < nc) recs[tid] = childrec[d.child_off + c0 + tid];
@@ -448,17 +498,23 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
         int tg[MAXC]; double vv[MAXC];
 #pragma unroll
         for (int c = 0; c < MAXC; ++c) tg[c] = (c < nc && tid < recs[c].rc) ? a.rel[recs[c].rel_off + tid] : -1;
-        if (DEP && done) {                              // (the relative indices are in flight while the children finish)
-            if (tid < nc) flag_wait(done + recs[tid].sn, err, epoch);
-            team_sync<NW>(team);
-        }
         if (c0 == 0) {                                  // (constant data is in flight; now the values of the levels below)
             if (!DEP) pdl_wait();
             ys[tid] = (tid < w) ? (a.x ? a.x[pj] : a.xp[d.col0 + tid]) : 0.0;
         }
+        if (DEP) {                                      // every child's slots at once: one L2 round trip once the last one lands
+            double* p[MAXC];
+            unsigned need = 0;
 #pragma unroll
-        for (int c = 0; c < MAXC; ++c)
-            vv[c] = (tg[c] >= 0) ? (DEP ? __ldcg(a.cbv + recs[c].cbv_off + tid) : a.cbv[recs[c].cbv_off + tid]) : 0.0;
+            for (int c = 0; c < MAXC; ++c) {
+                p[c] = a.up + (tg[c] >= 0 ? recs[c].cbv_off + tid : 0);
+                need |= (tg[c] >= 0) ? 1u << c : 0u;
+            }
+            slot_take(p, need, vv, err);
+        } else {
+#pragma unroll
+            for (int c = 0; c < MAXC; ++c) vv[c] = (tg[c] >= 0) ? a.cbv[recs[c].cbv_off + tid] : 0.0;
+        }
         if (c0 == 0) team_sync<NW>(team);
 #pragma unroll
         for (int c = 0; c < MAXC; ++c) {               // ascending child order: deterministic sums
@@ -468,6 +524,7 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
             }
         }
     }
+    if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s + 1] = global_ns();
     cp_async_wait_all();
     team_sync<NW>(team);
     double y = ys[tid];
@@ -520,43 +577,66 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
             }
         }
     }
-    if (tid < f) { if (tid < w) a.xp[d.col0 + tid] = y; else a.cbv[a.cbv_off[s] + tid - w] = y; }
-    // hand-off: the team barrier orders every thread's stores before thread 0's st.release.gpu (release is cumulative over the
-    // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed
-    team_sync<NW>(team);
-    if (DEP && done && tid == 0) flag_set(done + s, epoch);
+    if (DEP) {
+        if (tid < f) slot_put(tid < w ? a.ypiv + d.col0 + tid : a.up + cvo + tid - w, y);
+        if (a.strace) { team_sync<NW>(team); if (tid == 0) a.strace[6 * (size_t)s + 2] = global_ns(); }
+    } else {
+        if (tid < f) { if (tid < w) a.xp[d.col0 + tid] = y; else a.cbv[cvo + tid - w] = y; }
+        team_sync<NW>(team);
+    }
 }
 
 template <int NW, bool DEP = false>
 __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double* sm_team, int tid, int team,
-                                               int* done = nullptr, int* err = nullptr, const int32_t* parent = nullptr, int epoch = 1) {
+                                               const ChildRec* childrec = nullptr, int* err = nullptr) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
-    double* xs = sm_team;                              // [FMAX] gathered ancestor values
+    double* xs = sm_team;                              // [FMAX] gathered ancestor values at [xa, xa + r)
     double* xb = xs + FMAX;                            // [2][8]
+    ChildRec* recs = (ChildRec*)(xb + 16);             // [MAXC] (DEP: the children, whose `down` slots this front fills)
     double* P = xb + 16 + 4 * MAXC;                    // row-major f x w panel (same slice layout as the forward sweep)
+    if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s + 3] = global_ns();
     const FrontDesc d = a.desc[s];
     const int f = d.f, w = d.w, r = f - w;
+    // DEP: xs is the whole front vector -- own pivots' x at [0, w), the ancestors' at [w, f) -- from which the children's
+    // hand-offs are gathered
+    const int xa = DEP ? w : 0;
     {
         const double* Lt = a.Lt + d.lp_off;
         for (int e = tid; e < f * w; e += TEAM) cp_async8(P + e, Lt + e);
     }
     const int32_t* rows = a.rows + d.rows_off + w;
-    const int myrow = (tid < r) ? rows[tid] : 0;
+    const int myrow = (!DEP && tid < r) ? rows[tid] : 0;
     const int pj = (a.x && tid < w) ? a.perm[d.col0 + tid] : 0;
     const double dinv = (tid < w) ? fast_rcp(a.dvec[d.col0 + tid]) : 0.0;
-    if (DEP) {      // all ancestors are final once the parent is
-        if (tid == 0 && done) { const int p = parent[s]; if (p >= 0) flag_wait(done + p, err, epoch); }
+    const int nc0 = min(MAXC, d.nchild);
+    int tg[MAXC];                                      // DEP: row of the front that child c's slot `tid` takes
+    double t;
+    if (DEP) {
+        // the children's records and relative indices are constant: fetched before the wait, so that the hand-off to the
+        // children follows the back-substitution directly
+        if (tid < nc0) recs[tid] = childrec[d.child_off + tid];
         team_sync<NW>(team);
-    } else pdl_wait();
-    if (tid < r) xs[tid] = DEP ? __ldcg(a.xp + myrow) : a.xp[myrow];
-    double t = (tid < w) ? (DEP ? __ldcg(a.xp + d.col0 + tid) : a.xp[d.col0 + tid]) * dinv : 0.0;
+#pragma unroll
+        for (int c = 0; c < MAXC; ++c) tg[c] = (c < nc0 && tid < recs[c].rc) ? a.rel[recs[c].rel_off + tid] : -1;
+        // ancestor values (the parent's hand-off) and own forward result, at once
+        double* const p[2] = {a.down + a.cbv_off[s] + tid, a.ypiv + d.col0 + tid};
+        double v[2];
+        slot_take(p, (tid < r ? 1u : 0u) | (tid < w ? 2u : 0u), v, err);
+        if (tid < r) xs[xa + tid] = v[0];
+        t = (tid < w) ? v[1] * dinv : 0.0;
+    } else {
+        pdl_wait();
+        if (tid < r) xs[xa + tid] = a.xp[myrow];
+        t = (tid < w) ? a.xp[d.col0 + tid] * dinv : 0.0;
+    }
     cp_async_wait_all();
     team_sync<NW>(team);
+    if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s + 4] = global_ns();
     {   // t_j -= sum_{i >= w} L(i,j) x_i : no recurrence
         double acc = 0.0;
         if (tid < w) {
 #pragma unroll 8
-            for (int i = 0; i < r; ++i) acc = fma(P[(w + i) * w + tid], xs[i], acc);
+            for (int i = 0; i < r; ++i) acc = fma(P[(w + i) * w + tid], xs[xa + i], acc);
         }
         t -= acc;
     }
@@ -574,7 +654,8 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
         }
     } else {
         // blocked by warp (see the forward sweep): warp 1 finishes columns 32.. with shuffles and publishes them in
-        // xs[32..] (the gathered ancestors occupy xs[0 .. f-w) with f - w < 32 here); warp 0 applies them in one pass
+        // xs[32..w) (the gathered ancestors occupy xs[0 .. f-w) with f - w < 32 here, or xs[w .. f) with DEP); warp 0 applies
+        // them in one pass
         if (w > 32) {
             if (tid >= 32) {
                 for (int k0 = w - 1; k0 >= 33; k0 -= 8) {
@@ -610,14 +691,25 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
             }
         }
     }
-    if (tid < w) {
-        a.xp[d.col0 + tid] = t;
-        if (a.x) a.x[pj] = t;
+    if (DEP) {
+        if (tid < w) { xs[tid] = t; a.x[pj] = t; }
+        team_sync<NW>(team);
+        // hand-off to the children: slot i of child c takes the front's value at row rel_c[i]
+#pragma unroll
+        for (int c = 0; c < MAXC; ++c) if (tg[c] >= 0) slot_put(a.down + recs[c].cbv_off + tid, xs[tg[c]]);
+        for (int c0 = MAXC; c0 < d.nchild; c0 += MAXC) {          // (fronts with more than MAXC children)
+            const int nc = min(MAXC, d.nchild - c0);
+            team_sync<NW>(team);
+            if (tid < nc) recs[tid] = childrec[d.child_off + c0 + tid];
+            team_sync<NW>(team);
+            for (int c = 0; c < nc; ++c)
+                if (tid < recs[c].rc) slot_put(a.down + recs[c].cbv_off + tid, xs[a.rel[recs[c].rel_off + tid]]);
+        }
+        if (a.strace) { team_sync<NW>(team); if (tid == 0) a.strace[6 * (size_t)s + 5] = global_ns(); }
+    } else {
+        if (tid < w) a.xp[d.col0 + tid] = t;
+        team_sync<NW>(team);
     }
-    // hand-off: the team barrier orders every thread's stores before thread 0's st.release.gpu (release is cumulative over the
-    // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed
-    team_sync<NW>(team);
-    if (DEP && done && tid == 0) flag_set(done + s, epoch);
 }
 
 // NTEAM teams per CTA.  Measured on OPF-10k (tools/sweep_headline.sh): sweeping the fused bottom subtrees with 8 one-warp teams per
@@ -702,52 +794,44 @@ __global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec
 // ------------------------------------------------------------------------------------------------ single-launch solve
 // Forward sweep, D^-1 and backward sweep of the whole (team-class, unsharded) tree in ONE launch.  The tasks are the groups of
 // k_factor_dep (DepSched: fronts in (level, id) order, four fronts of order <= 32 as one-warp teams or one front of order <= 64 as a
-// two-warp team per group), every front with its own flag:
-//   ticket [0, ngroup)          forward sweep of group t: a front waits on its children's forward flags
-//   ticket [ngroup, 2 ngroup)   backward sweep of the groups in reverse order: a front waits on its parent's backward flag (a root:
-//                               on its own forward flag)
+// two-warp team per group):
+//   ticket [0, ngroup)          forward sweep of group t: a front takes its children's contribution vectors from their `up` slots
+//   ticket [ngroup, 2 ngroup)   backward sweep of the groups in reverse order: a front takes its ancestors' values from its `down`
+//                               slots (its parent's hand-off) and its own forward result from its `ypiv` slots
 // A persistent grid claims the tickets through an atomic counter, one task at a time.  A front waits only on fronts of smaller
 // tickets or of its own group (another team: no CTA-wide barrier inside a task), and a CTA claims a ticket only while it runs, so
 // forward progress does not depend on how many CTAs are resident or in which order they are dispatched.
 // Fronts of order <= 32 run as one-warp teams here and as two-warp teams in the level-launch solve above the fused subtrees; for
 // w <= f <= 32 the two-warp code runs warp 0 alone through the same loops, so the result is bit-identical to the level solve.
-// Flags are spaced per front (measured: a flag per front beats running fused bottom subtrees stage by stage inside one CTA, whose
-// stages each cost a front's full latency and which need more than two waves of the resident CTAs on OPF-10k).
-// Re-arming without any other graph node: flags hold the epoch of the launch that set them; there are exactly ntask + gridDim
-// claims (each CTA ends with one failing claim), every CTA reads the epoch before its first claim, and the CTA that makes the last
-// claim resets the ticket and advances the epoch.  ctl = {ticket, epoch}.
+// Hand-offs are per front (measured: that beats running fused bottom subtrees stage by stage inside one CTA, whose stages each
+// cost a front's full latency and which need more than two waves of the resident CTAs on OPF-10k).
+//
+// Every hand-off is a slot that holds the value itself (slot_take / slot_put): a consumer polls the data, so a tree hop costs one
+// L2 round trip and no release fence.  Why each value read across CTAs inside the launch is safe:
+//   * an `up`, `down` or `ypiv` slot has exactly one writer and one reader per launch, and 8-byte aligned accesses are
+//     single-copy atomic: a reader that sees anything but SLOT_EMPTY sees the whole value, and nothing else it reads depends on
+//     the writer's other stores (each value a front needs from another CTA travels in its own slot);
+//   * the reader re-arms the slot after it has the value, and the next launch is ordered behind that store by the kernel boundary;
+//   * everything else a task reads (descriptors, panels, D, indices, the right-hand side x) was written by earlier launches;
+//   * the caller's x[perm[j]] is read by front s's forward task and written by its backward task, which takes that forward
+//     task's result (ypiv) first: the write data-depends on the read having completed.
+// Re-arming needs no other graph node.  There are exactly ntask + gridDim claims (each CTA ends with one failing claim); a CTA
+// then fences its stores and counts itself out, and the last CTA out -- every task of the launch has finished -- resets both
+// counters (ctl = {ticket, CTAs out}).  If a wait timed out anywhere (or in the factorisation), that CTA writes NaN into x so
+// that Richardson refinement rejects the step, and fills every slot with SLOT_EMPTY again: a slot whose consumer gave up may
+// hold a value the next launch must not see.
 // (six CTAs per SM: what the 35 KB of shared memory allows; the bound also keeps ptxas from spilling)
-__global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, const int32_t* parent,
-                                                   int* fdone, int* bdone, int* err, int* ctl, int n) {
+__global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
+                                                   double* slots, int64_t nslot) {
     extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
     double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
-    __shared__ int tk_sh, ep_sh, nan_sh;
+    __shared__ int tk_sh, bad_sh;
     const int ntask = 2 * ds.ngroup;
-    if (threadIdx.x == 0) {
-        int e;
-        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(e) : "l"(ctl + 1) : "memory");
-        ep_sh = e + 1;
-        nan_sh = 0;
-    }
     for (;;) {
-        if (threadIdx.x == 0) {
-            const int t = atomicAdd(ctl, 1);
-            if (t == ntask + (int)gridDim.x - 1) {      // last claim: every other CTA is done and has read the epoch
-                atomicExch(ctl, 0);
-                atomicExch(ctl + 1, ep_sh);
-                __threadfence();
-                nan_sh = *(volatile int*)err;           // a timed-out wait anywhere (or in the factorisation): x := NaN
-            }
-            tk_sh = t;
-        }
+        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
         __syncthreads();
         const int t = tk_sh;
-        const int E = ep_sh;
-        if (t >= ntask) {
-            if (nan_sh)
-                for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double(0x7ff8000000000000ll);
-            return;
-        }
+        if (t >= ntask) break;
         const bool fwd = t < ds.ngroup;
         const int g = fwd ? t : ntask - 1 - t;
         const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
@@ -756,15 +840,29 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRe
         if (team < cnt) {
             const int s = ds.tasks[t0 + team];
             if (fwd) {
-                if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, fdone, err, E);
-                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, fdone, err, E);
+                if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, err);
+                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
             } else {
-                if (tid == 0 && parent[s] < 0) flag_wait(fdone + s, err, E);   // a root: its own forward sweep
-                if (type == 1) front_bwd_team<1, true>(a, s, sm1[team], tid, team, bdone, err, parent, E);
-                else front_bwd_team<2, true>(a, s, smd, tid, team, bdone, err, parent, E);
+                if (type == 1) front_bwd_team<1, true>(a, s, sm1[team], tid, team, childrec, err);
+                else front_bwd_team<2, true>(a, s, smd, tid, team, childrec, err);
             }
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)
+    }
+    if (threadIdx.x == 0) {
+        bad_sh = 0;
+        __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
+        if (atomicAdd(ctl + 1, 1) == (int)gridDim.x - 1) {
+            atomicExch(ctl, 0);
+            atomicExch(ctl + 1, 0);
+            __threadfence();
+            bad_sh = *(volatile int*)err;
+        }
+    }
+    __syncthreads();
+    if (bad_sh) {
+        for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
+        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) slot_st(slots + i, SLOT_EMPTY);
     }
 }
 
