@@ -21,6 +21,7 @@
  *                                          kernels_sparse.jl:161-167.
  *   b2_condensed_*                       : src/KKT/Sparse/condensed.jl:201-366, gpu_sparse.jl:308-340.
  *   b2d_condensed_assemble               : src/KKT/Dense/condensed.jl:120-186, kernels_dense.jl:81-119.
+ *   b2d_aug_assemble, b2d_copy_diag      : src/KKT/Dense/augmented.jl:116-161, kernels_dense.jl:39-75.
  *   b2_set_aug_diagonal .. b2_kkt_mul_*  : src/IPM/kernels.jl:4-27,161-204, src/IPM/factorization.jl:41-46,
  *                                          143-167,190-237,303-324, src/KKT/KKTsystem.jl:222-226.
  */
@@ -243,6 +244,16 @@ int b2d_condensed_assemble(int32_t n, int32_t m, int32_t ns, int32_t n_eq,
                            const double* hess_d, const double* jac_d,
                            const double* pr_diag_d, const double* du_diag_d,
                            double* diag_buffer_d, double* aug_d, void* stream);
+
+/* ------------------------------------------------------------------ assembly: dense augmented */
+/* src/KKT/Dense/augmented.jl:116-156.  hess n x n (ld n; strict lower triangle read), jac m x n (ld m),
+ * aug N x N (ld N), N = n + ns + m, ind_ineq 0-based (ns entries).  Writes EVERY element of the lower triangle of aug
+ * (structural zeros included) and nothing above the diagonal. */
+int b2d_aug_assemble(int32_t n, int32_t m, int32_t ns, const int64_t* ind_ineq_d,
+                     const double* hess_d, const double* jac_d, const double* pr_diag_d,
+                     const double* du_diag_d, const double* diag_hess_d, double* aug_d, void* stream);
+/* compress_hessian!(::DenseKKTSystem) = diag!(diag_hess, hess)  (augmented.jl:158-161): d[i] = A[i, i], i < n */
+int b2d_copy_diag(int32_t n, int32_t lda, const double* A_d, double* d_d, void* stream);
 
 /* The same assembly with the J' D J contraction on the Hopper tensor cores: fp64 is cut into 8 signed 7-bit digits per entry
  * (Ozaki scheme) and the 36 digit-pair products run as exact int8 GEMMs on wgmma.mma_async (s8) with TMA-staged operands

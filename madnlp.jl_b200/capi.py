@@ -143,6 +143,8 @@ PROTOTYPES = {
     "b2_condensed_plan_destroy": (C.c_int, [_p]),
     "b2_condensed_assemble": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
     "b2d_condensed_assemble": (C.c_int, [_i32, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b2d_aug_assemble": (C.c_int, [_i32, _i32, _i32] + [_p] * 8),
+    "b2d_copy_diag": (C.c_int, [_i32, _i32, _p, _p, _p]),
     "b2_bounds_create": (C.c_int, [_i64, _i64, _i64, _p, _p, _PP]),
     "b2_bounds_destroy": (C.c_int, [_p]),
     "b2_set_aug_diagonal": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),

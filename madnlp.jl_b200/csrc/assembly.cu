@@ -2,6 +2,7 @@
 //   b2_coo_to_csc / b2_transfer*    -- src/matrixtools.jl:55-95, kernels_sparse.jl:161-167 (rows A3/A4/A5 of SURVEY 8a)
 //   b2_condensed_*                  -- src/KKT/Sparse/condensed.jl:201-366, gpu_sparse.jl:308-340 (rows A6/A7)
 //   b2d_condensed_assemble          -- src/KKT/Dense/condensed.jl:120-186, kernels_dense.jl:81-119 (row A8)
+//   b2d_aug_assemble, b2d_copy_diag -- src/KKT/Dense/augmented.jl:116-161, kernels_dense.jl:39-75
 // All sparse kernels are "one thread per destination slot" gathers: race-free, no atomics, and the per-slot
 // summation order equals the reference's sequential CPU loops, so results are bit-identical to them
 // (adds and multiplies are issued with explicit rounding intrinsics so the compiler cannot contract them to FMA).
@@ -389,4 +390,66 @@ extern "C" int b2d_condensed_assemble(int32_t n, int32_t m, int32_t ns, int32_t 
     k_dense_syrk<<<grid, 256, syrk_smem, st>>>(n, m, ns, N, ind_ineq_d, hess_d, jac_d, pr_diag_d, diag_buffer_d, aug_d);
     B2_CUDA(cudaGetLastError());
     return b2d_assemble_parts(n, m, ns, n_eq, ind_ineq_d, ind_eq_d, jac_d, pr_diag_d, du_diag_d, diag_buffer_d, aug_d, false, st);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// dense augmented KKT (lower triangle), N = n + ns + m:
+//   [ H + diag(pr_diag[0:n]) (diagonal: pr_diag + diag_hess)                ]
+//   [ 0                        diag(pr_diag[n:n+ns])                        ]
+//   [ J                        -1 at (ind_ineq[k], k)        diag(du_diag)  ]
+// Column j of aug below the diagonal is one contiguous run, and so are the sources that fill it (column j of hess and of
+// jac), so one CTA sweeps one column: coalesced reads and writes, every lower element written once (zeros included),
+// nothing above the diagonal touched.  Pure copy: the only arithmetic is the diagonal's single add, in the reference's order.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_dense_aug(int n, int m, int ns, const int64_t* __restrict__ ind_ineq,
+                                                   const double* __restrict__ hess, const double* __restrict__ jac,
+                                                   const double* __restrict__ pr, const double* __restrict__ du,
+                                                   const double* __restrict__ dh, double* __restrict__ aug) {
+    const int64_t nns = (int64_t)n + ns, N = nns + m;
+    const int64_t j = blockIdx.x;
+    double* __restrict__ col = aug + j * N;
+    if (j < n) {
+        const double* __restrict__ hc = hess + j * n;
+        const double* __restrict__ jc = jac + j * m;
+#pragma unroll 4
+        for (int64_t i = j + threadIdx.x; i < N; i += blockDim.x)
+            col[i] = i < n ? (i == j ? __dadd_rn(pr[i], dh[i]) : hc[i]) : (i < nns ? 0.0 : jc[i - nns]);
+    } else if (j < nns) {
+        const int64_t r = nns + ind_ineq[j - n];             // row of the slack's -1
+#pragma unroll 4
+        for (int64_t i = j + threadIdx.x; i < N; i += blockDim.x)
+            col[i] = i == j ? pr[j] : (i == r ? -1.0 : 0.0);
+    } else {
+#pragma unroll 4
+        for (int64_t i = j + threadIdx.x; i < N; i += blockDim.x)
+            col[i] = i == j ? du[j - nns] : 0.0;
+    }
+}
+
+__global__ void k_copy_diag(int n, int lda, const double* __restrict__ A, double* __restrict__ d) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        d[i] = A[i * lda + i];
+}
+
+extern "C" int b2d_aug_assemble(int32_t n, int32_t m, int32_t ns, const int64_t* ind_ineq_d,
+                                const double* hess_d, const double* jac_d, const double* pr_diag_d,
+                                const double* du_diag_d, const double* diag_hess_d, double* aug_d, void* stream) {
+    const int64_t N = (int64_t)n + ns + m;
+    if (n <= 0 || m < 0 || ns < 0 || ns > m || N > INT32_MAX || !hess_d || !pr_diag_d || !diag_hess_d || !aug_d ||
+        (m && (!jac_d || !du_diag_d)) || (ns && !ind_ineq_d)) {
+        set_error("b2d_aug_assemble: invalid argument");
+        return B2_ERR_INVALID;
+    }
+    k_dense_aug<<<(unsigned)N, 256, 0, as_stream(stream)>>>(n, m, ns, ind_ineq_d, hess_d, jac_d, pr_diag_d, du_diag_d, diag_hess_d, aug_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2d_copy_diag(int32_t n, int32_t lda, const double* A_d, double* d_d, void* stream) {
+    if (n < 0 || lda < n || (n && (!A_d || !d_d))) { set_error("b2d_copy_diag: invalid argument"); return B2_ERR_INVALID; }
+    if (n == 0) return B2_OK;
+    const int g = std::min((n + 255) / 256, 8 * sm_count());
+    k_copy_diag<<<g, 256, 0, as_stream(stream)>>>(n, lda, A_d, d_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
 }

@@ -111,6 +111,7 @@ is_async(::B200Solver) = true
 # KKT-level overloads.  Dispatch is on OUR solver type in the `LS` parameter of the stock KKT structs
 #   SparseCondensedKKTSystem{T,VT,MT,QN,LS,...} (src/KKT/Sparse/condensed.jl:7)   with VT <: CuVector AND LS <: B200Solver
 #   DenseCondensedKKTSystem{T,VT,MT,QN,LS,VI}   (src/KKT/Dense/condensed.jl:10)   with VT <: CuVector AND LS <: B200DenseSolver
+#   DenseKKTSystem{T,VT,MT,QN,LS,VI}            (src/KKT/Dense/augmented.jl:10)   with VT <: CuVector AND LS <: B200DenseSolver
 # -- strictly more specific than MadNLPGPU's `VT <: AbstractGPUVector` methods (lib/MadNLPGPU/src/KKT/gpu_sparse.jl:308-382,
 # gpu_dense.jl:86-138), so loading both packages is neither ambiguous nor type piracy (a type this module owns is in every
 # signature).  The native plans live in the solver object (which this module owns), built lazily from the kkt's own maps at
@@ -239,8 +240,10 @@ is_supported(::Type{<:B200DenseSolver}, ::Type{Float64}) = true
 is_async(::B200DenseSolver) = true
 
 const B200DenseKKT{T} = MadNLP.DenseCondensedKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200DenseSolver}
+const B200DenseAugKKT{T} = MadNLP.DenseKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200DenseSolver}
+const B200AnyDenseKKT{T} = Union{B200DenseKKT{T},B200DenseAugKKT{T}}     # AbstractDenseKKTSystem with our solver
 
-function dense_plans(kkt::B200DenseKKT{T}) where T
+function dense_plans(kkt::B200AnyDenseKKT{T}) where T
     M = kkt.linear_solver
     if M.kkt_plan == C_NULL
         n = size(kkt.hess, 1); m = size(kkt.jac, 1); ii = Array(kkt.ind_ineq) .- 1; h = Ref{Ptr{Cvoid}}(C_NULL)
@@ -280,14 +283,56 @@ function MadNLP.solve_kkt!(kkt::B200DenseKKT{T}, w::MadNLP.AbstractKKTVector) wh
     return w
 end
 
-# mul!(w, ::AbstractDenseKKTSystem, x, alpha, beta) (src/IPM/factorization.jl:303-324)
-function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200DenseKKT{T}, x::MadNLP.AbstractKKTVector, alpha = one(T), beta = zero(T)) where T
+# mul!(w, ::AbstractDenseKKTSystem, x, alpha, beta) (src/IPM/factorization.jl:303-324): the same formula for both dense KKT types
+function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200AnyDenseKKT{T}, x::MadNLP.AbstractKKTVector, alpha = one(T), beta = zero(T)) where T
     kp, bp = dense_plans(kkt)
     check(ccall((:b2d_kkt_mul, libb200kkt), Cint,
         (Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
         kp, bp, pointer(kkt.hess), pointer(kkt.jac), pointer(kkt.reg), pointer(kkt.du_diag), pointer(kkt.l_lower), pointer(kkt.u_lower),
         pointer(kkt.l_diag), pointer(kkt.u_diag), alpha, beta, pointer(MadNLP.full(x)), pointer(MadNLP.full(w)), stream_ptr()), SolveException)
     return w
+end
+
+# ---------------------------------------------------------------------------------------------------------------------
+# DenseKKTSystem (src/KKT/Dense/augmented.jl): the augmented matrix of order n + ns + m, assembled by one kernel and factorised
+# whole by B200DenseSolver.  kkt.etc (augmented.jl:39) holds the 0-based device copy of ind_ineq, made on first use.
+# ---------------------------------------------------------------------------------------------------------------------
+ind_ineq0(kkt::B200DenseAugKKT) = get!(() -> CuVector{Int64}(Array(kkt.ind_ineq) .- 1), kkt.etc, :b200_ind_ineq0)
+
+# build_kkt! (augmented.jl:116-156): every element of the lower triangle written, so the one-time fill! is not relied on
+function MadNLP.build_kkt!(kkt::B200DenseAugKKT{T}) where T
+    n = size(kkt.hess, 1); m = size(kkt.jac, 1)
+    check(ccall((:b2d_aug_assemble, libb200kkt), Cint,
+        (Int32, Int32, Int32, CuPtr{Int64}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        n, m, length(kkt.ind_ineq), pointer(ind_ineq0(kkt)), pointer(kkt.hess), pointer(kkt.jac), pointer(kkt.pr_diag),
+        pointer(kkt.du_diag), pointer(kkt.diag_hess), pointer(kkt.aug_com), stream_ptr()), FactorizationException)
+end
+
+# compress_hessian! (augmented.jl:158-161) = diag!(diag_hess, hess)
+function MadNLP.compress_hessian!(kkt::B200DenseAugKKT{T}) where T
+    check(ccall((:b2d_copy_diag, libb200kkt), Cint, (Int32, Int32, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        size(kkt.hess, 1), stride(kkt.hess, 2), pointer(kkt.hess), pointer(kkt.diag_hess), stream_ptr()), FactorizationException)
+end
+
+# solve_kkt!(::AbstractReducedKKTSystem) (src/IPM/factorization.jl:41-46): reduce_rhs! -> solve on primal_dual(w) -> finish_aug_solve!;
+# primal_dual(w) is the leading n + ns + m entries of full(w)
+function MadNLP.solve_kkt!(kkt::B200DenseAugKKT{T}, w::MadNLP.AbstractKKTVector) where T
+    _, bp = dense_plans(kkt); wv = MadNLP.full(w); m = size(kkt.jac, 1)
+    check(ccall((:b2_reduce_rhs, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        bp, m, pointer(kkt.l_diag), pointer(kkt.u_diag), pointer(wv), stream_ptr()), SolveException)
+    check(ccall((:b2d_solve, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, Int32, Ptr{Cvoid}),
+        kkt.linear_solver.handle, pointer(wv), 1, stream_ptr()), SolveException)
+    check(ccall((:b2_finish_aug_solve, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        bp, m, pointer(kkt.l_lower), pointer(kkt.u_lower), pointer(kkt.l_diag), pointer(kkt.u_diag), pointer(wv), stream_ptr()), SolveException)
+    return w
+end
+
+# mul!(y, ::DenseKKTSystem, x) (augmented.jl:98-100) = _symv!('L', 1, aug_com, x, 0, y)
+function MadNLP.mul!(y::CuVector{T}, kkt::B200DenseAugKKT{T}, x::CuVector{T}) where T
+    N = size(kkt.aug_com, 1)
+    check(ccall((:b2d_symv_lower, libb200kkt), Cint, (Int32, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
+        N, stride(kkt.aug_com, 2), pointer(kkt.aug_com), pointer(x), pointer(y), one(T), zero(T), stream_ptr()), SolveException)
+    return y
 end
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -418,9 +418,48 @@ class SparseCondensedKKTSystem(_KKTBase):
 
 
 # ======================================================================================================
-class DenseCondensedKKTSystem(_KKTBase):
-    """src/KKT/Dense/condensed.jl.  Dense matrices are torch tensors whose MEMORY is the column-major matrix
-    (tensor[j, i] = M[i, j]), so pointers can be handed to the kernels exactly as Julia would hand them."""
+class _DenseKKTBase(_KKTBase):
+    """What both dense formulations share (AbstractDenseKKTSystem, src/KKT/Dense/utils.jl:3-29).  Dense matrices are
+    torch tensors whose MEMORY is the column-major matrix (tensor[j, i] = M[i, j]), so pointers can be handed to the kernels
+    exactly as Julia would hand them."""
+
+    def get_jacobian(self):
+        return self.jac
+
+    def get_hessian(self):
+        return self.hess
+
+    def set_dense(self, hess_np=None, jac_np=None):
+        """upload column-major host matrices (what hess_dense!/jac_dense! would have written)."""
+        if hess_np is not None:
+            self.hess.copy_(torch.from_numpy(np.ascontiguousarray(hess_np.T)))
+        if jac_np is not None:
+            self.jac.copy_(torch.from_numpy(np.ascontiguousarray(jac_np.T)))
+
+    def compress_jacobian(self):
+        pass
+
+    def _gemv(self, trans, x, y, alpha, beta):
+        """y = alpha*op(jac)*x + beta*y with jac the m x n column-major device matrix (own kernels, no cuBLAS)"""
+        fn = lib.b2d_gemv_t if trans else lib.b2d_gemv_n
+        check(fn(self.m, self.n, self.m, ptr(self.jac), ptr(x), ptr(y), float(alpha), float(beta), _sp(self.stream)))
+
+    def mul(self, w, x, alpha=1.0, beta=0.0):
+        """src/IPM/factorization.jl:303-324 (AbstractDenseKKTSystem): symv + 2 gemv + one fused tail kernel (b2d_kkt_mul)."""
+        check(lib.b2d_kkt_mul(self._dk.h, self._bounds.h, ptr(self.hess), ptr(self.jac), ptr(self.reg), ptr(self.du_diag),
+                              ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta),
+                              ptr(x.values), ptr(w.values), _sp(self.stream)))
+        return w
+
+    def jtprod(self, y, x):
+        """src/KKT/Dense/utils.jl:12-23: y[1:n] = jac' x ; y[n + k] = -x[ind_ineq[k]] (not on the per-iteration solve path)."""
+        self._gemv(True, x, y[: self.n], 1.0, 0.0)
+        y[self.n:] = -x[self._ind_ineq_d]
+
+
+# ======================================================================================================
+class DenseCondensedKKTSystem(_DenseKKTBase):
+    """src/KKT/Dense/condensed.jl."""
 
     def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None):
         n, m = cb.nvar, cb.ncon
@@ -462,22 +501,6 @@ class DenseCondensedKKTSystem(_KKTBase):
     def initialize(self):
         self._initialize_common()
 
-    def get_jacobian(self):
-        return self.jac
-
-    def get_hessian(self):
-        return self.hess
-
-    def set_dense(self, hess_np=None, jac_np=None):
-        """upload column-major host matrices (what hess_dense!/jac_dense! would have written)."""
-        if hess_np is not None:
-            self.hess.copy_(torch.from_numpy(np.ascontiguousarray(hess_np.T)))
-        if jac_np is not None:
-            self.jac.copy_(torch.from_numpy(np.ascontiguousarray(jac_np.T)))
-
-    def compress_jacobian(self):
-        pass
-
     def compress_hessian(self):
         pass
 
@@ -505,11 +528,6 @@ class DenseCondensedKKTSystem(_KKTBase):
         """Dense/condensed.jl:189-191."""
         return num_zero == 0 and num_neg == self.n_eq
 
-    def _gemv(self, trans, x, y, alpha, beta):
-        """y = alpha*op(jac)*x + beta*y with jac the m x n column-major device matrix (own kernels, no cuBLAS)"""
-        fn = lib.b2d_gemv_t if trans else lib.b2d_gemv_n
-        check(fn(self.m, self.n, self.m, ptr(self.jac), ptr(x), ptr(y), float(alpha), float(beta), _sp(self.stream)))
-
     def solve_kkt(self, w: UnreducedKKTVector):
         """src/IPM/factorization.jl:190-229: own kernels around the dense solve (b2d_kkt_solve_pre / _post)."""
         sp = _sp(self.stream)
@@ -521,21 +539,64 @@ class DenseCondensedKKTSystem(_KKTBase):
                                      ptr(self.pd_buffer), ptr(w.values), sp))
         return w
 
-    def mul(self, w, x, alpha=1.0, beta=0.0):
-        """src/IPM/factorization.jl:303-324 (AbstractDenseKKTSystem): symv + 2 gemv + one fused tail kernel (b2d_kkt_mul)."""
-        check(lib.b2d_kkt_mul(self._dk.h, self._bounds.h, ptr(self.hess), ptr(self.jac), ptr(self.reg), ptr(self.du_diag),
-                              ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta),
-                              ptr(x.values), ptr(w.values), _sp(self.stream)))
+
+
+# ======================================================================================================
+class DenseKKTSystem(_DenseKKTBase):
+    """src/KKT/Dense/augmented.jl: the augmented system of order N = n + ns + m as one dense column-major matrix,
+    factorised whole by the dense LDL^T (inertia (n + ns, 0, m) at a minimiser)."""
+
+    def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None):
+        n, m = cb.nvar, cb.ncon
+        ind_ineq = np.asarray(cb.ind_ineq, dtype=np.int64)
+        ns = len(ind_ineq)
+        self.n, self.m, self.ns = n, m, ns
+        N = n + ns + m
+        self.N = N
+        self.aug_com = torch.zeros((N, N), dtype=torch.float64, device=_DEV)
+        self.hess = torch.zeros((n, n), dtype=torch.float64, device=_DEV)      # memory: column-major n x n
+        self.jac = torch.zeros((n, m), dtype=torch.float64, device=_DEV)       # memory: column-major m x n
+        self.pr_diag = _dz(n + ns); self.du_diag = _dz(m); self.diag_hess = _dz(n)
+        self._init_common(cb, n + ns, m)
+        self.l_diag.fill_(1.0); self.u_diag.fill_(1.0)
+        self._ind_ineq_d = torch.from_numpy(ind_ineq).to(_DEV)
+        h = C.c_void_p()
+        check(lib.b2d_kkt_create(n, m, ns, ind_ineq.ctypes.data if ns else None, C.byref(h)))
+        self._dk = _Plan(h, lib.b2d_kkt_destroy)
+        self.linear_solver = linear_solver(self.aug_com, opt_linear_solver)
+
+    def num_variables(self):
+        """augmented.jl:96."""
+        return len(self.pr_diag)
+
+    def initialize(self):
+        """KKTsystem.jl:210-216."""
+        self._initialize_common()
+
+    def compress_hessian(self):
+        """augmented.jl:158-161: diag!(diag_hess, hess)."""
+        check(lib.b2d_copy_diag(self.n, self.n, ptr(self.hess), ptr(self.diag_hess), _sp(self.stream)))
+
+    def build_kkt(self):
+        """augmented.jl:116-156 as one kernel (k_dense_aug) that writes the whole lower triangle, zeros included."""
+        check(lib.b2d_aug_assemble(self.n, self.m, self.ns, ptr(self._ind_ineq_d), ptr(self.hess), ptr(self.jac),
+                                   ptr(self.pr_diag), ptr(self.du_diag), ptr(self.diag_hess), ptr(self.aug_com), _sp(self.stream)))
+
+    def solve_kkt(self, w: UnreducedKKTVector):
+        """src/IPM/factorization.jl:41-46 (AbstractReducedKKTSystem)."""
+        self.reduce_rhs(w)
+        self.linear_solver.solve_linear_system(w.primal_dual())
+        self.finish_aug_solve(w)
         return w
 
-    def jtprod(self, y, x):
-        """src/KKT/Dense/utils.jl:12-23: y[1:n] = jac' x ; y[n + k] = -x[ind_ineq[k]] (not on the per-iteration solve path)."""
-        self._gemv(True, x, y[: self.n], 1.0, 0.0)
-        y[self.n:] = -x[self._ind_ineq_d]
+    def mul_aug(self, y, x):
+        """augmented.jl:98-100: y = sym(aug_com) x from the lower triangle."""
+        check(lib.b2d_symv_lower(self.N, self.N, ptr(self.aug_com), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
+        return y
 
 
 def create_kkt_system(kkt_type, cb, linear_solver=None, opt_linear_solver=None):
     """src/IPM/IPM.jl:157-165 -> create_kkt_system(::Type{K}, cb, linear_solver; opt_linear_solver)."""
     if linear_solver is None:
-        linear_solver = B200DenseSolver if kkt_type is DenseCondensedKKTSystem else B200SparseSolver
+        linear_solver = B200DenseSolver if kkt_type in (DenseCondensedKKTSystem, DenseKKTSystem) else B200SparseSolver
     return kkt_type(cb, linear_solver, opt_linear_solver)
