@@ -22,6 +22,8 @@
  *   b2_condensed_*                       : src/KKT/Sparse/condensed.jl:201-366, gpu_sparse.jl:308-340.
  *   b2d_condensed_assemble               : src/KKT/Dense/condensed.jl:120-186, kernels_dense.jl:81-119.
  *   b2d_aug_assemble, b2d_copy_diag      : src/KKT/Dense/augmented.jl:116-161, kernels_dense.jl:39-75.
+ *   b2_set_aug_diagonal_unreduced,
+ *   b2_unreduced_solve_pre / _post       : src/IPM/kernels.jl:29-34, src/IPM/factorization.jl:29-39.
  *   b2_set_aug_diagonal .. b2_kkt_mul_*  : src/IPM/kernels.jl:4-27,161-204, src/IPM/factorization.jl:41-46,
  *                                          143-167,190-237,303-324, src/KKT/KKTsystem.jl:222-226.
  */
@@ -77,7 +79,12 @@ typedef struct b2_options {
                                 level of the critical path costs microseconds of hand-off besides its pivots, the zeros nothing.
                                 Default 0 = off (measured slower on the OPF trees: the single-child chains sit at the bottom, where the
                                 tree is throughput-bound and bigger leaves hurt); kept as an option for trees with long chains on top */
-    int32_t reserved[4];
+    int32_t kkt_n_dual;      /* with kkt_n_primal > 0: rows [kkt_n_primal, kkt_n_primal + kkt_n_dual) are constraint duals and every
+                                later row is a bound dual of the unreduced KKT system (src/KKT/Sparse/unreduced.jl): a row with exactly
+                                one off-diagonal entry, in a primal column.  The ordering places each bound row immediately before
+                                its primal neighbour, so that it is eliminated first and adds its barrier term to that variable's
+                                pivot.  0 (default): every non-primal row is a constraint dual.  Ignored with B2_ORDER_USER. */
+    int32_t reserved[3];
 } b2_options;
 
 int b2_options_default(b2_options* opt);
@@ -309,6 +316,19 @@ int b2_bounds_destroy(b2_bounds* b);
 /* pr_diag = reg; pr_diag[ind_lb] -= l_lower./l_diag; pr_diag[ind_ub] -= u_lower./u_diag  (IPM/kernels.jl:22-27) */
 int b2_set_aug_diagonal(b2_bounds* b, const double* reg_d, const double* l_lower_d, const double* l_diag_d,
                         const double* u_lower_d, const double* u_diag_d, double* pr_diag_d, void* stream);
+/* SparseUnreducedKKTSystem (src/KKT/Sparse/unreduced.jl).  _set_aug_diagonal!(::AbstractUnreducedKKTSystem) (IPM/kernels.jl:29-34)
+ * as one launch:  pr_diag = reg (n_tot);  l_lower_aug = sqrt(l_lower) (nlb);  u_lower_aug = sqrt(u_lower) (nub), correctly rounded */
+int b2_set_aug_diagonal_unreduced(int64_t n_tot, int64_t nlb, int64_t nub, const double* reg_d, const double* l_lower_d,
+                                  const double* u_lower_d, double* pr_diag_d, double* l_lower_aug_d, double* u_lower_aug_d,
+                                  void* stream);
+/* solve_kkt!(::SparseUnreducedKKTSystem) (IPM/factorization.jl:29-39) around b2_solve on the FULL vector
+ * w = [x (n_tot) | y (m) | zl (nlb) | zu (nub)]:
+ *   pre : wzl = iszero(l_lower_aug) ? wzl : wzl / l_lower_aug ; the same for wzu   (-0.0 counts as zero)
+ *   post: wzl = wzl * (-l_lower_aug) ; wzu = wzu * u_lower_aug */
+int b2_unreduced_solve_pre(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* l_lower_aug_d,
+                           const double* u_lower_aug_d, double* w_d, void* stream);
+int b2_unreduced_solve_post(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* l_lower_aug_d,
+                            const double* u_lower_aug_d, double* w_d, void* stream);
 /* reg += dw; pr_diag += dw; du_diag -= dc   (KKTsystem.jl:222-226) */
 int b2_regularize_diagonal(int64_t n_tot, int64_t m, double dw, double dc, double* reg_d, double* pr_diag_d,
                            double* du_diag_d, void* stream);

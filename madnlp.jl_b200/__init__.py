@@ -4,8 +4,8 @@ Only what the hot path needs lives here (SURVEY.md section 8):
   csrc/           hand-written sm_90a CUDA kernels + the C ABI (include/b200kkt.h) -> libb200kkt.so
   capi.py         ctypes binding of that ABI (the same boundary Julia would `ccall`)
   linear_solvers  mirror of MadNLP's AbstractLinearSolver surface (B200SparseSolver, B200DenseSolver)
-  kkt             mirror of the AbstractKKTSystem surface (SparseKKTSystem, SparseCondensedKKTSystem,
-                  DenseCondensedKKTSystem, DenseKKTSystem, UnreducedKKTVector)
+  kkt             mirror of the AbstractKKTSystem surface (SparseKKTSystem, SparseUnreducedKKTSystem,
+                  SparseCondensedKKTSystem, DenseCondensedKKTSystem, DenseKKTSystem, UnreducedKKTVector)
   richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric
   workloads       synthetic generators for the configurations named in BASELINE.json
   julia/          the Julia shim a MadNLP.jl maintainer would add (cannot be run in this image)

@@ -44,7 +44,7 @@ class Options(C.Structure):
     _fields_ = [
         ("ordering", C.c_int32), ("nemin", C.c_int32), ("relax_zeros", C.c_double), ("pivot_eps", C.c_double),
         ("use_cuda_graph", C.c_int32), ("small_front_max", C.c_int32), ("n_parts", C.c_int32), ("part_rank", C.c_int32),
-        ("kkt_n_primal", C.c_int32), ("fuse_max_fronts", C.c_int32), ("dep_schedule", C.c_int32), ("chain_merge_f", C.c_int32), ("reserved", C.c_int32 * 4),
+        ("kkt_n_primal", C.c_int32), ("fuse_max_fronts", C.c_int32), ("dep_schedule", C.c_int32), ("chain_merge_f", C.c_int32), ("kkt_n_dual", C.c_int32), ("reserved", C.c_int32 * 3),
     ]
 
 
@@ -148,6 +148,9 @@ PROTOTYPES = {
     "b2_bounds_create": (C.c_int, [_i64, _i64, _i64, _p, _p, _PP]),
     "b2_bounds_destroy": (C.c_int, [_p]),
     "b2_set_aug_diagonal": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
+    "b2_set_aug_diagonal_unreduced": (C.c_int, [_i64, _i64, _i64] + [_p] * 7),
+    "b2_unreduced_solve_pre": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p, _p]),
+    "b2_unreduced_solve_post": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p, _p]),
     "b2_regularize_diagonal": (C.c_int, [_i64, _i64, _f64, _f64, _p, _p, _p, _p]),
     "b2_reduce_rhs": (C.c_int, [_p, _i64, _p, _p, _p, _p]),
     "b2_finish_aug_solve": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p]),

@@ -200,6 +200,21 @@ void colcounts(int32_t n, const std::vector<int64_t>& rptr, const std::vector<in
 
 inline int64_t trap_nnz(int64_t w, int64_t f) { return w * f - w * (w - 1) / 2; }
 
+// off-diagonal neighbours of the rows [nc, n): cnt[b - nc] = how many (each stored entry counted once, upper or lower),
+// nb[b - nc] = the last one seen
+void bound_neighbours(int32_t n, const int32_t* colptr, const int32_t* rowval, int32_t nc, std::vector<int32_t>& nb,
+                      std::vector<int32_t>& cnt) {
+    nb.assign(n - nc, -1);
+    cnt.assign(n - nc, 0);
+    for (int32_t j = 0; j < n; ++j)
+        for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p) {
+            const int32_t i = rowval[p];
+            if (i == j) continue;
+            if (i >= nc) { nb[i - nc] = j; cnt[i - nc]++; }
+            if (j >= nc) { nb[j - nc] = i; cnt[j - nc]++; }
+        }
+}
+
 // B2_ANALYSIS_TIMING=1: print the wall time of each phase of analyse() to stderr
 struct PhaseTimer {
     bool on;
@@ -214,6 +229,26 @@ struct PhaseTimer {
 };
 }  // namespace
 
+std::string check_kkt_rows(int32_t n, const int32_t* colptr, const int32_t* rowval, int kkt_n_primal, int kkt_n_dual) {
+    if (kkt_n_dual == 0) return "";
+    if (kkt_n_dual < 0) return "kkt_n_dual < 0";
+    if ((int64_t)kkt_n_primal + kkt_n_dual > n) return "kkt_n_primal + kkt_n_dual > n";
+    if (kkt_n_primal <= 0) return "kkt_n_dual > 0 needs kkt_n_primal > 0";
+    const int32_t nc = kkt_n_primal + kkt_n_dual;
+    for (int32_t j = 0; j < n; ++j)
+        for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p)
+            if (rowval[p] < 0 || rowval[p] >= n) return "row index out of range";
+    std::vector<int32_t> nb, cnt;
+    bound_neighbours(n, colptr, rowval, nc, nb, cnt);
+    for (int32_t b = nc; b < n; ++b) {
+        if (cnt[b - nc] != 1)
+            return "bound row " + std::to_string(b) + " has " + std::to_string(cnt[b - nc]) + " off-diagonal entries (needs exactly 1)";
+        if (nb[b - nc] >= kkt_n_primal)
+            return "bound row " + std::to_string(b) + " is coupled to row " + std::to_string(nb[b - nc]) + ", which is not primal";
+    }
+    return "";
+}
+
 void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const AnalysisOptions& opt,
              const int32_t* user_perm, Symbolic& S) {
     if (n <= 0) throw std::runtime_error("n must be positive");
@@ -223,7 +258,11 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     const int64_t nnz = colptr[n];
     PhaseTimer timer;
 
-    // ---- 1. ordering
+    // ---- 1. ordering.  With bound-dual rows (kkt_n_dual > 0) the fill-reducing ordering runs on the leading nc rows only: the
+    //          bound rows are inserted at 1c as leaves, so the other rows get the order the reduced system's matrix would get.
+    const bool bound_rows = opt.kkt_n_dual > 0 && opt.ordering != 3;
+    const int32_t nc = bound_rows ? opt.kkt_n_primal + opt.kkt_n_dual : n;
+    if (bound_rows && (opt.kkt_n_primal <= 0 || nc > n)) throw std::runtime_error("invalid kkt_n_primal / kkt_n_dual");
     std::vector<int32_t> perm0;
     if (opt.ordering == 3) {
         if (!user_perm) throw std::runtime_error("user ordering requested but no permutation given");
@@ -233,17 +272,26 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
             if (perm0[i] < 0 || perm0[i] >= n || seen[perm0[i]]) throw std::runtime_error("user_perm is not a permutation");
             seen[perm0[i]] = 1;
         }
-    } else if (opt.ordering == 2 || n < 3) {
-        perm0.resize(n);
+    } else if (opt.ordering == 2 || nc < 3) {
+        perm0.resize(nc);
         std::iota(perm0.begin(), perm0.end(), 0);
     } else {
         std::vector<int64_t> xadj, adj;
-        build_adjacency(n, colptr, rowval, xadj, adj);
-        if (opt.ordering == 1 || adj.empty()) order_mindeg(n, xadj, adj, perm0);
-        else order_metis(n, xadj, adj, perm0);
+        if (nc == n) build_adjacency(n, colptr, rowval, xadj, adj);
+        else {
+            std::vector<int32_t> cp(nc + 1, 0), rv;
+            rv.reserve(colptr[nc]);
+            for (int32_t j = 0; j < nc; ++j) {
+                for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p) if (rowval[p] < nc) rv.push_back(rowval[p]);
+                cp[j + 1] = (int32_t)rv.size();
+            }
+            build_adjacency(nc, cp.data(), rv.data(), xadj, adj);
+        }
+        if (opt.ordering == 1 || adj.empty()) order_mindeg(nc, xadj, adj, perm0);
+        else order_metis(nc, xadj, adj, perm0);
     }
     std::vector<int32_t> iperm(n);
-    for (int32_t i = 0; i < n; ++i) iperm[perm0[i]] = i;
+    for (int32_t i = 0; i < nc; ++i) iperm[perm0[i]] = i;
 
     timer.lap("ordering");
     // ---- 1b. augmented-KKT constraint.  With static (1 x 1) pivoting a dual row of [[H, J'], [J, -D]] (D possibly zero) gets a
@@ -253,19 +301,21 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     //          over two consecutive 1 x 1 steps): duals are visited in elimination order; a dual keeps its place if an unused
     //          neighbour already precedes it, otherwise it is moved to just after its earliest unused neighbour (or, if every
     //          neighbour is taken, after its last neighbour).  Quasi-definite / condensed matrices do not need this (kkt_n_primal = 0).
-    if (opt.kkt_n_primal > 0 && opt.kkt_n_primal < n && opt.ordering != 3) {
+    //          Only the constraint duals [kkt_n_primal, nc) take part; bound rows are placed at 1c.
+    if (opt.kkt_n_primal > 0 && opt.kkt_n_primal < nc && opt.ordering != 3) {
         const int32_t np_ = opt.kkt_n_primal;
-        const int32_t nd_ = n - np_;
+        const int32_t nd_ = nc - np_;
         // primal neighbours of every dual (lower CSC: entry (i, j), i >= np_ > j, sits in column j)
         std::vector<int64_t> dptr(nd_ + 1, 0);
         for (int32_t j = 0; j < np_; ++j)
-            for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p) if (rowval[p] >= np_) dptr[rowval[p] - np_ + 1]++;
+            for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p) if (rowval[p] >= np_ && rowval[p] < nc) dptr[rowval[p] - np_ + 1]++;
         for (int32_t v = 0; v < nd_; ++v) dptr[v + 1] += dptr[v];
         std::vector<int32_t> dnb(dptr[nd_]);
         {
             std::vector<int64_t> fill(dptr.begin(), dptr.end() - 1);
             for (int32_t j = 0; j < np_; ++j)
-                for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p) if (rowval[p] >= np_) dnb[fill[rowval[p] - np_]++] = j;
+                for (int32_t p = colptr[j]; p < colptr[j + 1]; ++p)
+                    if (rowval[p] >= np_ && rowval[p] < nc) dnb[fill[rowval[p] - np_]++] = j;
         }
         for (int32_t v = 0; v < nd_; ++v)                     // neighbours in elimination order
             std::sort(dnb.begin() + dptr[v], dnb.begin() + dptr[v + 1], [&](int32_t a, int32_t b) { return iperm[a] < iperm[b]; });
@@ -273,8 +323,8 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
         std::iota(duals.begin(), duals.end(), np_);
         std::sort(duals.begin(), duals.end(), [&](int32_t a, int32_t b) { return iperm[a] < iperm[b]; });
         std::vector<char> used(np_, 0);
-        std::vector<std::pair<int64_t, int32_t>> key(n);
-        for (int32_t v = 0; v < n; ++v) key[v] = {2 * (int64_t)iperm[v], iperm[v]};
+        std::vector<std::pair<int64_t, int32_t>> key(nc);
+        for (int32_t v = 0; v < nc; ++v) key[v] = {2 * (int64_t)iperm[v], iperm[v]};
         for (int32_t v : duals) {
             const int64_t a = dptr[v - np_], b = dptr[v - np_ + 1];
             if (a == b) continue;                              // isolated dual row: nothing can help it
@@ -285,10 +335,38 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
             if (partner >= 0) { used[partner] = 1; key[v] = {2 * (int64_t)iperm[partner] + 1, iperm[v]}; }
             else key[v] = {2 * (int64_t)std::max(iperm[dnb[b - 1]], iperm[v]) + 1, iperm[v]};
         }
-        std::vector<int32_t> ord(n);
+        std::vector<int32_t> ord(nc);
         std::iota(ord.begin(), ord.end(), 0);
         std::sort(ord.begin(), ord.end(), [&](int32_t a, int32_t b) { return key[a] < key[b]; });
         perm0 = ord;
+        for (int32_t i = 0; i < nc; ++i) iperm[perm0[i]] = i;
+    }
+    // ---- 1c. bound-dual rows of the unreduced KKT system: row b = [l_diag, sqrt(z)] couples only to its variable u.  Eliminated
+    //          first, its pivot l_diag (< 0) adds -z / l_diag to u's pivot: the reduced system's barrier term.  Eliminated after u, it
+    //          would leave u the pivot H_uu + reg, which is 0 for an LP.  So each bound row goes immediately before u.
+    std::vector<int32_t> bnb;                                  // neighbour of bound row nc + k
+    if (nc < n) {
+        std::vector<int32_t> cnt;
+        bound_neighbours(n, colptr, rowval, nc, bnb, cnt);
+        const int32_t np_ = opt.kkt_n_primal;
+        std::vector<int32_t> bptr(np_ + 1, 0);
+        for (int32_t k = 0; k < n - nc; ++k) {
+            if (cnt[k] != 1 || bnb[k] < 0 || bnb[k] >= np_) throw std::runtime_error("bound row without exactly one primal neighbour");
+            bptr[bnb[k] + 1]++;
+        }
+        for (int32_t u = 0; u < np_; ++u) bptr[u + 1] += bptr[u];
+        std::vector<int32_t> brow(n - nc);
+        {
+            std::vector<int32_t> fill(bptr.begin(), bptr.end() - 1);
+            for (int32_t k = 0; k < n - nc; ++k) brow[fill[bnb[k]]++] = nc + k;
+        }
+        std::vector<int32_t> ord;
+        ord.reserve(n);
+        for (int32_t v : perm0) {
+            if (v < np_) ord.insert(ord.end(), brow.begin() + bptr[v], brow.begin() + bptr[v + 1]);
+            ord.push_back(v);
+        }
+        perm0.swap(ord);
         for (int32_t i = 0; i < n; ++i) iperm[perm0[i]] = i;
     }
 
@@ -307,6 +385,10 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     // ---- 3. structures under perm1
     permuted_lower_rows(n, colptr, rowval, iperm, rptr, rcol);
     etree(n, rptr, rcol, parent);
+    // a bound row is a leaf whose parent is its variable, so it still precedes the variable after the postorder, and amalgamation
+    // (children's columns before the parent's) and the final DFS keep that
+    for (size_t k = 0; k < bnb.size(); ++k)
+        if (parent[iperm[nc + k]] != iperm[bnb[k]]) throw std::runtime_error("internal: a bound row's etree parent is not its variable");
     std::vector<int64_t> cc;
     colcounts(n, rptr, rcol, parent, cc);
 

@@ -15,6 +15,7 @@ struct AnalysisOptions {
     double relax_zeros = 0.25;
     int n_parts = 1;           // multi-GPU partition count
     int kkt_n_primal = 0;      // augmented-KKT hint: dual rows are ordered after one primal neighbour
+    int kkt_n_dual = 0;        // > 0: rows from kkt_n_primal + kkt_n_dual on are bound duals, ordered just before their neighbour
     int chain_merge_f = 0;     // > 0: single-child chains are merged while the front order stays <= this (latency, not flops)
 };
 
@@ -51,6 +52,11 @@ struct Symbolic {
     int64_t top_rows = 0;             // sum of w over the shared top tree
     int64_t exch_cb = 0;              // doubles at the start of the update-block workspace that cross rank->top
 };
+
+// Checks the row classes of an unreduced KKT pattern: kkt_n_dual >= 0, kkt_n_primal + kkt_n_dual <= n, kkt_n_primal > 0 when
+// kkt_n_dual > 0, and every bound row (index >= kkt_n_primal + kkt_n_dual) has exactly one off-diagonal entry, in a primal column.
+// Returns "" when the options are valid, else what is wrong.
+std::string check_kkt_rows(int32_t n, const int32_t* colptr, const int32_t* rowval, int kkt_n_primal, int kkt_n_dual);
 
 // colptr/rowval: lower-triangular CSC (0-based).  Throws std::runtime_error on failure.
 void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const AnalysisOptions& opt,

@@ -68,6 +68,67 @@ extern "C" int b2_set_aug_diagonal(b2_bounds* b, const double* reg_d, const doub
     return B2_OK;
 }
 
+// _set_aug_diagonal!(::AbstractUnreducedKKTSystem) (IPM/kernels.jl:29-34): thread t < n_tot copies reg, the next nlb take
+// sqrt(zl), the last nub sqrt(zu).  __dsqrt_rn is correctly rounded, as Julia's and numpy's sqrt.
+__global__ void k_set_aug_diagonal_unreduced(int64_t n_tot, int64_t nlb, int64_t nub, const double* __restrict__ reg,
+                                             const double* __restrict__ ll, const double* __restrict__ ul, double* __restrict__ pr,
+                                             double* __restrict__ lla, double* __restrict__ ula) {
+    GRID_STRIDE(t, n_tot + nlb + nub) {
+        if (t < n_tot) pr[t] = reg[t];
+        else if (t < n_tot + nlb) lla[t - n_tot] = __dsqrt_rn(ll[t - n_tot]);
+        else ula[t - n_tot - nlb] = __dsqrt_rn(ul[t - n_tot - nlb]);
+    }
+}
+extern "C" int b2_set_aug_diagonal_unreduced(int64_t n_tot, int64_t nlb, int64_t nub, const double* reg_d, const double* l_lower_d,
+                                             const double* u_lower_d, double* pr_diag_d, double* l_lower_aug_d, double* u_lower_aug_d,
+                                             void* stream) {
+    if (n_tot < 0 || nlb < 0 || nub < 0 || (n_tot && (!reg_d || !pr_diag_d)) || (nlb && (!l_lower_d || !l_lower_aug_d)) ||
+        (nub && (!u_lower_d || !u_lower_aug_d))) {
+        set_error("b2_set_aug_diagonal_unreduced: invalid argument");
+        return B2_ERR_INVALID;
+    }
+    const int64_t tot = n_tot + nlb + nub;
+    if (tot == 0) return B2_OK;
+    k_set_aug_diagonal_unreduced<<<grid_for(tot), 256, 0, as_stream(stream)>>>(n_tot, nlb, nub, reg_d, l_lower_d, u_lower_d, pr_diag_d,
+                                                                               l_lower_aug_d, u_lower_aug_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+// solve_kkt!(::SparseUnreducedKKTSystem) (IPM/factorization.jl:29-39), the scalings of the bound-dual blocks of w around b2_solve.
+// pre:  w = iszero(s) ? w : w / s   (-0.0 == 0.0 in C as in Julia's iszero);   post: wzl = wzl * (-sl), wzu = wzu * su
+template <bool POST>
+__global__ void k_unreduced_scale(int64_t nlb, int64_t nub, const double* __restrict__ sl, const double* __restrict__ su,
+                                  double* __restrict__ wz) {
+    GRID_STRIDE(t, nlb + nub) {
+        const bool lower = t < nlb;
+        const double s = lower ? sl[t] : su[t - nlb];
+        const double v = wz[t];
+        if (POST) wz[t] = __dmul_rn(v, lower ? -s : s);
+        else if (s != 0.0) wz[t] = __ddiv_rn(v, s);
+    }
+}
+template <bool POST>
+static int unreduced_scale(const char* name, int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* sl, const double* su,
+                           double* w, void* stream) {
+    if (n_tot < 0 || m < 0 || nlb < 0 || nub < 0 || !w || (nlb && !sl) || (nub && !su)) {
+        set_error(std::string(name) + ": invalid argument");
+        return B2_ERR_INVALID;
+    }
+    if (nlb + nub == 0) return B2_OK;
+    k_unreduced_scale<POST><<<grid_for(nlb + nub), 256, 0, as_stream(stream)>>>(nlb, nub, sl, su, w + n_tot + m);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+extern "C" int b2_unreduced_solve_pre(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* l_lower_aug_d,
+                                      const double* u_lower_aug_d, double* w_d, void* stream) {
+    return unreduced_scale<false>("b2_unreduced_solve_pre", n_tot, m, nlb, nub, l_lower_aug_d, u_lower_aug_d, w_d, stream);
+}
+extern "C" int b2_unreduced_solve_post(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* l_lower_aug_d,
+                                       const double* u_lower_aug_d, double* w_d, void* stream) {
+    return unreduced_scale<true>("b2_unreduced_solve_post", n_tot, m, nlb, nub, l_lower_aug_d, u_lower_aug_d, w_d, stream);
+}
+
 __global__ void k_regularize(int64_t n_tot, int64_t m, double dw, double dc, double* __restrict__ reg, double* __restrict__ pr,
                              double* __restrict__ du) {
     GRID_STRIDE(i, n_tot + m) {

@@ -543,6 +543,10 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
                   const b2_options* opt, const int32_t* user_perm_h, bool symbolic_only, b2_solver** out) {
     if (!out || !colptr_h || !rowval_h || n <= 0) { set_error("b2_create: invalid argument"); return B2_ERR_INVALID; }
     if (colptr_h[n] != nnz) { set_error("b2_create: colptr[n] != nnz"); return B2_ERR_INVALID; }
+    if (opt && opt->kkt_n_dual != 0) {
+        const std::string bad = check_kkt_rows(n, colptr_h, rowval_h, opt->kkt_n_primal, opt->kkt_n_dual);
+        if (!bad.empty()) { set_error("b2_create: " + bad); return B2_ERR_INVALID; }
+    }
     b2_solver* s = new b2_solver();
     if (opt) s->opt = *opt; else b2_options_default(&s->opt);
     s->symbolic_only = symbolic_only;
@@ -555,6 +559,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         ao.chain_merge_f = s->opt.chain_merge_f;
         ao.n_parts = std::max(1, s->opt.n_parts);
         ao.kkt_n_primal = s->opt.kkt_n_primal;
+        ao.kkt_n_dual = s->opt.kkt_n_dual;
         analyse(n, colptr_h, rowval_h, ao, user_perm_h, s->S);
     } catch (std::exception& e) {
         set_error(std::string("b2_create: analysis failed: ") + e.what());

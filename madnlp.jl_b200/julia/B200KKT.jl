@@ -33,15 +33,17 @@ Base.@kwdef mutable struct B200Options <: AbstractOptions
     b200_fuse_max_fronts::Int32 = 8
     b200_dep_schedule::Int32 = 1
     b200_chain_merge_f::Int32 = 0
+    b200_kkt_n_dual::Int32 = 0          # set by create_kkt_system(SparseUnreducedKKTSystem, ...) below
 end
 
 struct CB2Options
     ordering::Int32; nemin::Int32; relax_zeros::Float64; pivot_eps::Float64
     use_cuda_graph::Int32; small_front_max::Int32; n_parts::Int32; part_rank::Int32
-    kkt_n_primal::Int32; fuse_max_fronts::Int32; dep_schedule::Int32; chain_merge_f::Int32; reserved::NTuple{4,Int32}
+    kkt_n_primal::Int32; fuse_max_fronts::Int32; dep_schedule::Int32; chain_merge_f::Int32; kkt_n_dual::Int32; reserved::NTuple{3,Int32}
 end
 CB2Options(o::B200Options) = CB2Options(o.b200_ordering, o.b200_nemin, o.b200_relax_zeros, o.b200_pivot_eps,
-    o.b200_use_cuda_graph, o.b200_small_front_max, 1, 0, o.b200_kkt_n_primal, o.b200_fuse_max_fronts, o.b200_dep_schedule, o.b200_chain_merge_f, ntuple(_ -> Int32(0), 4))
+    o.b200_use_cuda_graph, o.b200_small_front_max, 1, 0, o.b200_kkt_n_primal, o.b200_fuse_max_fronts, o.b200_dep_schedule, o.b200_chain_merge_f,
+    o.b200_kkt_n_dual, ntuple(_ -> Int32(0), 3))
 
 last_error() = unsafe_string(ccall((:b2_last_error, libb200kkt), Cstring, ()))
 function check(rc::Cint, exc)
@@ -112,6 +114,7 @@ is_async(::B200Solver) = true
 #   SparseCondensedKKTSystem{T,VT,MT,QN,LS,...} (src/KKT/Sparse/condensed.jl:7)   with VT <: CuVector AND LS <: B200Solver
 #   DenseCondensedKKTSystem{T,VT,MT,QN,LS,VI}   (src/KKT/Dense/condensed.jl:10)   with VT <: CuVector AND LS <: B200DenseSolver
 #   DenseKKTSystem{T,VT,MT,QN,LS,VI}            (src/KKT/Dense/augmented.jl:10)   with VT <: CuVector AND LS <: B200DenseSolver
+#   SparseUnreducedKKTSystem{T,VT,MT,QN,LS,...} (src/KKT/Sparse/unreduced.jl:8)   with VT <: CuVector AND LS <: B200Solver
 # -- strictly more specific than MadNLPGPU's `VT <: AbstractGPUVector` methods (lib/MadNLPGPU/src/KKT/gpu_sparse.jl:308-382,
 # gpu_dense.jl:86-138), so loading both packages is neither ambiguous nor type piracy (a type this module owns is in every
 # signature).  The native plans live in the solver object (which this module owns), built lazily from the kkt's own maps at
@@ -332,6 +335,109 @@ function MadNLP.mul!(y::CuVector{T}, kkt::B200DenseAugKKT{T}, x::CuVector{T}) wh
     N = size(kkt.aug_com, 1)
     check(ccall((:b2d_symv_lower, libb200kkt), Cint, (Int32, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
         N, stride(kkt.aug_com, 2), pointer(kkt.aug_com), pointer(x), pointer(y), one(T), zero(T), stream_ptr()), SolveException)
+    return y
+end
+
+# ---------------------------------------------------------------------------------------------------------------------
+# SparseUnreducedKKTSystem (src/KKT/Sparse/unreduced.jl) with B200Solver.  The analysis must know which rows are bound duals
+# (b2_options.kkt_n_dual), so create_kkt_system fills kkt_n_primal = n_tot and kkt_n_dual = m when they were left at 0 and then
+# runs the stock constructor.  Plans (transfer maps, SpMV plans, bounds) live beside the solver, as for the condensed type.
+# ---------------------------------------------------------------------------------------------------------------------
+const B200UnreducedKKT{T} = MadNLP.SparseUnreducedKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200Solver}
+
+function MadNLP.create_kkt_system(::Type{MadNLP.SparseUnreducedKKTSystem}, cb::MadNLP.SparseCallback, linear_solver::Type{<:B200Solver};
+                                  opt_linear_solver = default_options(linear_solver), kwargs...)
+    n_tot = cb.nvar + length(cb.ind_ineq)
+    opt_linear_solver.b200_kkt_n_primal == 0 && (opt_linear_solver.b200_kkt_n_primal = n_tot)
+    opt_linear_solver.b200_kkt_n_dual == 0 && (opt_linear_solver.b200_kkt_n_dual = cb.ncon)
+    return invoke(MadNLP.create_kkt_system, Tuple{Type{MadNLP.SparseUnreducedKKTSystem},MadNLP.SparseCallback,Type},
+                  MadNLP.SparseUnreducedKKTSystem, cb, linear_solver; opt_linear_solver = opt_linear_solver, kwargs...)
+end
+
+mutable struct UnreducedPlans
+    aug_plan::Ptr{Cvoid}; hess_plan::Ptr{Cvoid}; jac_plan::Ptr{Cvoid}   # b2_transfer_plan: aug_raw / hess_raw / jac_raw -> CSC
+    hess_spmv::Ptr{Cvoid}; jac_spmv::Ptr{Cvoid}                         # b2_spmv_plan of hess_com (n_tot x n_tot) / jac_com (m x n_tot)
+    bounds::Ptr{Cvoid}
+end
+const _uplans = IdDict{Any,UnreducedPlans}()
+
+function uplans(kkt::B200UnreducedKKT{T}) where T
+    get!(_uplans, kkt.linear_solver) do
+        h0(v) = Array(v) .- one(eltype(v))
+        tplan(map_d, nnz_csc) = begin
+            mp = Array(map_d) .- 1; h = Ref{Ptr{Cvoid}}(C_NULL)
+            check(ccall((:b2_transfer_plan_create, libb200kkt), Cint, (Int64, Int64, Ptr{Int64}, Ptr{Ptr{Cvoid}}),
+                length(mp), nnz_csc, mp, h), SymbolicException); h[]
+        end
+        splan(A) = begin
+            h = Ref{Ptr{Cvoid}}(C_NULL)
+            check(ccall((:b2_spmv_plan_create, libb200kkt), Cint, (Int32, Int32, Ptr{Int32}, Ptr{Int32}, Ptr{Ptr{Cvoid}}),
+                size(A, 1), size(A, 2), h0(A.colPtr), h0(A.rowVal), h), SymbolicException); h[]
+        end
+        lb = Array(kkt.ind_lb) .- 1; ub = Array(kkt.ind_ub) .- 1; b = Ref{Ptr{Cvoid}}(C_NULL)
+        check(ccall((:b2_bounds_create, libb200kkt), Cint, (Int64, Int64, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Ptr{Cvoid}}),
+            length(kkt.pr_diag), length(lb), length(ub), lb, ub, b), SymbolicException)
+        nz(A) = length(MadNLP.nzval(A))
+        UnreducedPlans(tplan(kkt.aug_csc_map, nz(kkt.aug_com)), tplan(kkt.hess_csc_map, nz(kkt.hess_com)),
+                       tplan(kkt.jac_csc_map, nz(kkt.jac_com)), splan(kkt.hess_com), splan(kkt.jac_com), b[])
+    end
+end
+
+_transfer(plan, dst, src) = check(ccall((:b2_transfer, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Ptr{Cvoid}),
+    plan, pointer(dst), pointer(src), stream_ptr()), FactorizationException)
+
+# build_kkt! (unreduced.jl:178-180) = transfer!(aug_com, aug_raw, aug_csc_map)
+MadNLP.build_kkt!(kkt::B200UnreducedKKT) = _transfer(uplans(kkt).aug_plan, MadNLP.nzval(kkt.aug_com), kkt.aug_raw.V)
+MadNLP.compress_hessian!(kkt::B200UnreducedKKT) = _transfer(uplans(kkt).hess_plan, MadNLP.nzval(kkt.hess_com), kkt.hess_raw.V)
+# compress_jacobian! (Sparse/utils.jl:36-40): slack entries -1, then transfer!
+function MadNLP.compress_jacobian!(kkt::B200UnreducedKKT{T}) where T
+    ns = length(kkt.ind_ineq)
+    ns > 0 && check(ccall((:b2_fill, libb200kkt), Cint, (Int64, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+        ns, -one(T), pointer(kkt.jac, length(kkt.jac) - ns + 1), stream_ptr()), FactorizationException)
+    _transfer(uplans(kkt).jac_plan, MadNLP.nzval(kkt.jac_com), kkt.jac_raw.V)
+end
+
+# _set_aug_diagonal!(::AbstractUnreducedKKTSystem) (src/IPM/kernels.jl:29-34): one launch
+function MadNLP._set_aug_diagonal!(kkt::B200UnreducedKKT{T}) where T
+    check(ccall((:b2_set_aug_diagonal_unreduced, libb200kkt), Cint,
+        (Int64, Int64, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        length(kkt.pr_diag), length(kkt.l_lower), length(kkt.u_lower), pointer(kkt.reg), pointer(kkt.l_lower), pointer(kkt.u_lower),
+        pointer(kkt.pr_diag), pointer(kkt.l_lower_aug), pointer(kkt.u_lower_aug), stream_ptr()), FactorizationException)
+    return
+end
+
+# solve_kkt! (src/IPM/factorization.jl:29-39): scale the bound-dual blocks -> b2_solve on full(w) -> scale back
+function MadNLP.solve_kkt!(kkt::B200UnreducedKKT{T}, w::MadNLP.AbstractKKTVector) where T
+    wv = MadNLP.full(w)
+    args = (length(kkt.pr_diag), length(kkt.du_diag), length(kkt.l_lower), length(kkt.u_lower))
+    sig = (Int64, Int64, Int64, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid})
+    check(ccall((:b2_unreduced_solve_pre, libb200kkt), Cint, sig, args..., pointer(kkt.l_lower_aug), pointer(kkt.u_lower_aug),
+        pointer(wv), stream_ptr()), SolveException)
+    solve_linear_system!(kkt.linear_solver, wv)
+    check(ccall((:b2_unreduced_solve_post, libb200kkt), Cint, sig, args..., pointer(kkt.l_lower_aug), pointer(kkt.u_lower_aug),
+        pointer(wv), stream_ptr()), SolveException)
+    return w
+end
+
+# mul! (src/IPM/factorization.jl:231-237): symmetric Hessian, J' y, J x, then _kktmul!
+function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200UnreducedKKT{T}, x::MadNLP.AbstractKKTVector, alpha = one(T), beta = zero(T)) where T
+    p = uplans(kkt); st = stream_ptr(); xv = MadNLP.full(x); wv = MadNLP.full(w)
+    spmv(name, plan, nz, xp, yp, b) = check(ccall((name, libb200kkt), Cint,
+        (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}), plan, pointer(nz), xp, yp, alpha, b, st), SolveException)
+    spmv(:b2_spmv_symlower, p.hess_spmv, MadNLP.nzval(kkt.hess_com), pointer(xv), pointer(wv), beta)
+    spmv(:b2_spmv_t, p.jac_spmv, MadNLP.nzval(kkt.jac_com), pointer(MadNLP.dual(x)), pointer(wv), one(T))
+    spmv(:b2_spmv_n, p.jac_spmv, MadNLP.nzval(kkt.jac_com), pointer(xv), pointer(MadNLP.dual(w)), beta)
+    check(ccall((:b2_kktmul, libb200kkt), Cint,
+        (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        p.bounds, length(kkt.du_diag), pointer(kkt.reg), pointer(kkt.du_diag), pointer(kkt.l_lower), pointer(kkt.u_lower),
+        pointer(kkt.l_diag), pointer(kkt.u_diag), alpha, beta, pointer(xv), pointer(wv), st), SolveException)
+    return w
+end
+
+# jtprod! (Sparse/utils.jl:28-30): y = jac_com' x
+function MadNLP.jtprod!(y::CuVector{T}, kkt::B200UnreducedKKT{T}, x::CuVector{T}) where T
+    check(ccall((:b2_spmv_t, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
+        uplans(kkt).jac_spmv, pointer(MadNLP.nzval(kkt.jac_com)), pointer(x), pointer(y), one(T), zero(T), stream_ptr()), SolveException)
     return y
 end
 

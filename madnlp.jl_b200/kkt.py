@@ -202,11 +202,12 @@ class _KKTBase:
 
 
 # ======================================================================================================
-class SparseKKTSystem(_KKTBase):
-    """src/KKT/Sparse/augmented.jl: augmented system as COO value vector
-    V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m)] (aliasing views) -> lower CSC."""
+class _SparseKKTBase(_KKTBase):
+    """What SparseKKTSystem and SparseUnreducedKKTSystem share (src/KKT/Sparse/utils.jl, src/IPM/factorization.jl:231-237): a COO
+    value vector V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m) | ...] with aliasing views, its lower CSC
+    aug_com, the separate jac_com / hess_com, and compress_*, get_*, mul and jtprod."""
 
-    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
+    def _build(self, cb, linear_solver, opt_linear_solver, unreduced):
         n, m = cb.nvar, cb.ncon
         ns = len(cb.ind_ineq)
         hI = np.array(cb.hess_I, dtype=np.int64); hJ = np.array(cb.hess_J, dtype=np.int64)
@@ -214,24 +215,37 @@ class SparseKKTSystem(_KKTBase):
         jI = np.asarray(cb.jac_I, dtype=np.int64); jJ = np.asarray(cb.jac_J, dtype=np.int64)
         n_jac, n_hess = len(jI), len(hI)
         n_tot = n + ns
+        nlb, nub = (len(cb.ind_lb), len(cb.ind_ub)) if unreduced else (0, 0)
         self.n, self.m, self.ns, self.n_tot = n, m, ns, n_tot
-        L = n_tot + m + n_hess + n_jac + ns                          # augmented.jl:75
-        o1 = n_tot; o2 = o1 + n_hess; o3 = o2 + n_jac; o4 = o3 + ns
+        L = n_tot + m + n_hess + n_jac + ns + 2 * nlb + 2 * nub      # augmented.jl:75, unreduced.jl:85
+        o1 = n_tot; o2 = o1 + n_hess; o3 = o2 + n_jac; o4 = o3 + ns; o5 = o4 + m
         I = np.empty(L, dtype=np.int64); J = np.empty(L, dtype=np.int64)
         ineq = np.asarray(cb.ind_ineq, dtype=np.int64)
         I[:o1] = np.arange(n_tot); J[:o1] = np.arange(n_tot)
         I[o1:o2] = hI; J[o1:o2] = hJ
         I[o2:o3] = jI + n_tot; J[o2:o3] = jJ
         I[o3:o4] = ineq + n_tot; J[o3:o4] = np.arange(n, n + ns)
-        I[o4:] = np.arange(n_tot, n_tot + m); J[o4:] = np.arange(n_tot, n_tot + m)
+        I[o4:o5] = np.arange(n_tot, n_tot + m); J[o4:o5] = np.arange(n_tot, n_tot + m)
         self.V = _dz(L)
         self.pr_diag = self.V[:o1]
         self.hess = self.V[o1:o2]
         self.jac = self.V[o2:o4]
         self.jac_callback = self.V[o2:o3]
-        self.du_diag = self.V[o4:]
-        self._init_common(cb, n_tot, m)
+        self.du_diag = self.V[o4:o5]
         N = n_tot + m
+        if unreduced:
+            # unreduced.jl:97-113: bound row k of zl is [sqrt(zl_k) in column ind_lb[k] | l_diag_k on the diagonal], then zu likewise
+            lb_rows = N + np.arange(nlb); ub_rows = N + nlb + np.arange(nub)
+            o6 = o5 + nlb; o7 = o6 + nlb; o8 = o7 + nub
+            I[o5:o6] = lb_rows; J[o5:o6] = lb_rows
+            I[o6:o7] = lb_rows; J[o6:o7] = np.asarray(cb.ind_lb, dtype=np.int64)
+            I[o7:o8] = ub_rows; J[o7:o8] = ub_rows
+            I[o8:] = ub_rows; J[o8:] = np.asarray(cb.ind_ub, dtype=np.int64)
+            N += nlb + nub
+        self._init_common(cb, n_tot, m)
+        if unreduced:                                                # views into V instead of _init_common's own vectors
+            self.l_diag, self.l_lower_aug = self.V[o5:o6], self.V[o6:o7]
+            self.u_diag, self.u_lower_aug = self.V[o7:o8], self.V[o8:]
         self.N = N
         cp, rv, mp = coo_to_csc(I, J, N, N)
         self.aug_com = DeviceCSC(N, N, cp, rv, _dz(len(rv)))
@@ -250,16 +264,12 @@ class SparseKKTSystem(_KKTBase):
             opt_linear_solver = linear_solver.default_options()
         if opt_linear_solver is not None and getattr(opt_linear_solver, "kkt_n_primal", None) == 0:
             opt_linear_solver.kkt_n_primal = n_tot     # zero (2,2) block: dual rows follow a primal neighbour
+        if unreduced and opt_linear_solver is not None and getattr(opt_linear_solver, "kkt_n_dual", None) == 0:
+            opt_linear_solver.kkt_n_dual = m           # rows from n_tot + m on are bound duals: each goes just before its variable
         self.linear_solver = linear_solver(self.aug_com, opt_linear_solver)
 
     def num_variables(self):
         return len(self.pr_diag)
-
-    def initialize(self):
-        """Sparse/utils.jl:52-62."""
-        self._initialize_common()
-        self.l_lower.zero_(); self.u_lower.zero_(); self.l_diag.fill_(1.0); self.u_diag.fill_(1.0)
-        self.hess_com.nzval.zero_()
 
     def get_jacobian(self):
         return self.jac_callback
@@ -278,18 +288,11 @@ class SparseKKTSystem(_KKTBase):
         check(lib.b2_transfer(self._hess_plan.h, ptr(self.hess_com.nzval), ptr(self.hess), _sp(self.stream)))
 
     def build_kkt(self):
-        """augmented.jl:146-148: transfer!(aug_com, aug_raw, aug_csc_map)."""
+        """augmented.jl:146-148 / unreduced.jl:178-180: transfer!(aug_com, aug_raw, aug_csc_map)."""
         check(lib.b2_transfer(self._aug_plan.h, ptr(self.aug_com.nzval), ptr(self.V), _sp(self.stream)))
 
-    def solve_kkt(self, w: UnreducedKKTVector):
-        """src/IPM/factorization.jl:41-46."""
-        self.reduce_rhs(w)
-        self.linear_solver.solve_linear_system(w.primal_dual())
-        self.finish_aug_solve(w)
-        return w
-
     def mul(self, w, x, alpha=1.0, beta=0.0):
-        """src/IPM/factorization.jl:231-237."""
+        """src/IPM/factorization.jl:231-237 (one method for both sparse types)."""
         sp = _sp(self.stream)
         check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(x.values), ptr(w.values), alpha, beta, sp))
         check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x.dual()), ptr(w.values), alpha, 1.0, sp))
@@ -300,6 +303,60 @@ class SparseKKTSystem(_KKTBase):
     def jtprod(self, y, x):
         """Sparse/utils.jl:28-30."""
         check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
+
+
+class SparseKKTSystem(_SparseKKTBase):
+    """src/KKT/Sparse/augmented.jl: augmented system as COO value vector
+    V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m)] (aliasing views) -> lower CSC."""
+
+    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
+        self._build(cb, linear_solver, opt_linear_solver, unreduced=False)
+
+    def initialize(self):
+        """Sparse/utils.jl:52-62."""
+        self._initialize_common()
+        self.l_lower.zero_(); self.u_lower.zero_(); self.l_diag.fill_(1.0); self.u_diag.fill_(1.0)
+        self.hess_com.nzval.zero_()
+
+    def solve_kkt(self, w: UnreducedKKTVector):
+        """src/IPM/factorization.jl:41-46."""
+        self.reduce_rhs(w)
+        self.linear_solver.solve_linear_system(w.primal_dual())
+        self.finish_aug_solve(w)
+        return w
+
+
+class SparseUnreducedKKTSystem(_SparseKKTBase):
+    """src/KKT/Sparse/unreduced.jl: the unreduced system of order N = n_tot + m + nlb + nub, COO value vector
+    V = [pr_diag | hess | jac | slack -1 (ns) | du_diag | l_diag | l_lower_aug | u_diag | u_lower_aug] (aliasing views) -> lower CSC.
+    Each bound row holds l_diag = xl - x (< 0) on the diagonal and sqrt(zl) in its variable's column; the analysis eliminates it
+    just before that variable (kkt_n_dual), so it contributes the reduced system's barrier term -zl / l_diag to that pivot.
+    Inertia at a correct iterate: (n_tot, 0, m + nlb + nub).  Quasi-Newton is not supported (factorization.jl:170-173)."""
+
+    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
+        self._build(cb, linear_solver, opt_linear_solver, unreduced=True)
+
+    def initialize(self):
+        """unreduced.jl:160-172."""
+        self._initialize_common()
+        self.l_lower.zero_(); self.u_lower.zero_(); self.l_diag.fill_(-1.0); self.u_diag.fill_(-1.0)
+        self.l_lower_aug.zero_(); self.u_lower_aug.zero_()
+        self.hess_com.nzval.zero_()
+
+    def set_aug_diagonal_(self):
+        """_set_aug_diagonal!(::AbstractUnreducedKKTSystem) (src/IPM/kernels.jl:29-34): pr_diag = reg, sqrt of the multipliers."""
+        check(lib.b2_set_aug_diagonal_unreduced(self._n_tot, len(self.l_lower), len(self.u_lower), ptr(self.reg), ptr(self.l_lower),
+                                                ptr(self.u_lower), ptr(self.pr_diag), ptr(self.l_lower_aug), ptr(self.u_lower_aug),
+                                                _sp(self.stream)))
+
+    def solve_kkt(self, w: UnreducedKKTVector):
+        """src/IPM/factorization.jl:29-39: scale the bound-dual blocks, solve the full system, scale back."""
+        args = (self._n_tot, self._m, len(self.l_lower), len(self.u_lower), ptr(self.l_lower_aug), ptr(self.u_lower_aug), ptr(w.values),
+                _sp(self.stream))
+        check(lib.b2_unreduced_solve_pre(*args))
+        self.linear_solver.solve_linear_system(w.full())
+        check(lib.b2_unreduced_solve_post(*args))
+        return w
 
 
 # ======================================================================================================
