@@ -423,6 +423,56 @@ int b2_get_sc(b2_bounds* b, const double* zl_d, const double* zu_d, double s_max
 int b2_set_aug_rhs(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* f_d,
                    const double* zl_d, const double* zu_d, const double* jacl_d, const double* c_d, double mu, double* p_d, void* stream);
 
+/* ------------------------------------------------------------------ compact L-BFGS (SparseKKTSystem, hessian_approximation = CompactLBFGS)
+ * src/quasi_newton.jl:212-437 and src/IPM/factorization.jl:76-139, 253-276.  B_k = sigma I - U U' + V V' on the n model variables
+ * (no slacks); S, Y are n x max_history, the memory p <= max_history.  max_history is limited to 32, so that
+ * T = P + E'C^{-1}E (2 max_history square) fits in one CTA's shared memory.  Every state value (counters, sigma, pairs, small
+ * matrices) is device memory: no entry point below synchronises except b2_lbfgs_state and the debug getters, and all can be
+ * captured in a CUDA graph.  Reductions are deterministic (fixed order).  Use a handle from one stream at a time.
+ * init_strategy: 1..4 = SCALAR1..SCALAR4 (src/enums.jl).  Bk_d is kkt.hess: the n diagonal values of B_k. */
+typedef struct b2_lbfgs b2_lbfgs;
+int b2_lbfgs_create(int64_t n, int32_t max_history, int32_t init_strategy, double init_value, double sigma_min, double sigma_max,
+                    b2_lbfgs** out);
+int b2_lbfgs_destroy(b2_lbfgs* h);
+/* p = current_mem, skipped = skipped_iter, sigma; synchronises `stream` (tests and tools) */
+int b2_lbfgs_state(b2_lbfgs* h, int64_t* p, int64_t* skipped, double* sigma, void* stream);
+/* init!: Bk .= 2 rho0 init_value (Gilbert-Lemarechal rule with norm_g0 = g0'g0); 2 launches */
+int b2_lbfgs_init(b2_lbfgs* h, double* Bk_d, const double* g0_d, double f0, void* stream);
+/* update!: skip (Bk untouched) when |s| < 100 eps, |y| < 100 eps or s'y < sqrt(eps)|s||y|, reset on the second skip since the
+ * last reset; otherwise store the pair (dropping the oldest when full), Bk .= sigma and recompute U, V.  2 launches */
+int b2_lbfgs_update(b2_lbfgs* h, double* Bk_d, const double* sk_d, const double* yk_d, void* stream);
+/* once per factorisation of C (the augmented matrix with Bk on its diagonal): H_d (N x 2 max_history, ld N = n_tot + m) = E, then
+ * b2_solve(s, H_d, 2 max_history), then T = P + E'H and its Bunch-Kaufman factorisation (dsytf2 'L').  Columns of E beyond the
+ * current p are zero, so their H columns are exactly zero and T carries unit pivots there. */
+/* n_tot_plus_m must equal the solver's order (B2_ERR_INVALID otherwise). */
+int b2_lbfgs_smw_prepare(b2_lbfgs* h, b2_solver* s, int64_t n_tot_plus_m, double* H_d, void* stream);
+/* after b2_solve of w (primal_dual, N entries): w -= H T^{-1} E'w; an exact no-op when p = 0.  2 launches.
+ * H and T belong to the state at the last b2_lbfgs_smw_prepare: a b2_lbfgs_update in between invalidates them until the next
+ * prepare (MadNLP's order is update!, then the factorisation, then the solves, src/IPM/solver.jl). */
+int b2_lbfgs_smw_apply(b2_lbfgs* h, int64_t n_tot_plus_m, const double* H_d, double* w_d, void* stream);
+/* mul!: w[0:n) += alpha (-U U'x + V V'x); issued between the Jacobian products and b2_kktmul.  2 launches */
+int b2_lbfgs_kkt_mul_lowrank(b2_lbfgs* h, double alpha, const double* x_d, double* w_d, void* stream);
+/* Debug/test: copy one state buffer to the host and return the ring slot of the oldest pair; synchronises.  Sizes (doubles):
+ * S, Y, U, V: n x max_history (S, Y in ring-slot order); SS, L, J, DL: max_history^2 (ld max_history); D: max_history;
+ * T, TF: (2 max_history)^2.  b2_lbfgs_debug_ipiv copies the 2 max_history pivots of TF (LAPACK convention, 1-based). */
+#define B2_LBFGS_BUF_S  0
+#define B2_LBFGS_BUF_Y  1
+#define B2_LBFGS_BUF_U  2
+#define B2_LBFGS_BUF_V  3
+#define B2_LBFGS_BUF_SS 4
+#define B2_LBFGS_BUF_L  5
+#define B2_LBFGS_BUF_D  6
+#define B2_LBFGS_BUF_J  7
+#define B2_LBFGS_BUF_DL 8
+#define B2_LBFGS_BUF_T  9
+#define B2_LBFGS_BUF_TF 10
+int b2_lbfgs_debug_get(b2_lbfgs* h, int32_t what, double* dst_h, int64_t* first, void* stream);
+int b2_lbfgs_debug_ipiv(b2_lbfgs* h, int32_t* ipiv_h, void* stream);
+/* Debug/test: the same Bunch-Kaufman kernels on a caller's N x N matrix (N <= 64, column-major, lower triangle; factor in place)
+ * and the dsytrs 'L' solve of one right-hand side. */
+int b2_debug_bk_factor(int32_t N, double* A_d, int32_t* ipiv_d, void* stream);
+int b2_debug_bk_solve(int32_t N, const double* F_d, const int32_t* ipiv_d, double* b_d, void* stream);
+
 
 #ifdef __cplusplus
 }

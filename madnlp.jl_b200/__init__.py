@@ -6,6 +6,7 @@ Only what the hot path needs lives here (SURVEY.md section 8):
   linear_solvers  mirror of MadNLP's AbstractLinearSolver surface (B200SparseSolver, B200DenseSolver)
   kkt             mirror of the AbstractKKTSystem surface (SparseKKTSystem, SparseUnreducedKKTSystem,
                   SparseCondensedKKTSystem, DenseCondensedKKTSystem, DenseKKTSystem, UnreducedKKTVector)
+  quasi_newton    ExactHessian / CompactLBFGS (the device L-BFGS state SparseKKTSystem uses)
   richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric
   workloads       synthetic generators for the configurations named in BASELINE.json
   julia/          the Julia shim a MadNLP.jl maintainer would add (cannot be run in this image)
@@ -20,6 +21,6 @@ def __getattr__(name):
     # torch-dependent modules are imported lazily so that CPU-only tooling (ABI checks, symbolic analysis)
     # does not pay for `import torch`.
     import importlib
-    if name in ("kkt", "linear_solvers", "richardson", "ipm", "parallel"):
+    if name in ("kkt", "linear_solvers", "quasi_newton", "richardson", "ipm", "parallel"):
         return importlib.import_module(f".{name}", __name__)
     raise AttributeError(name)

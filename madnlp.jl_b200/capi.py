@@ -183,6 +183,18 @@ PROTOTYPES = {
     "b2_axpy": (C.c_int, [_i64, _f64, _p, _p, _p]),
     "b2_copy": (C.c_int, [_i64, _p, _p, _p]),
     "b2_fill": (C.c_int, [_i64, _f64, _p, _p]),
+    "b2_lbfgs_create": (C.c_int, [_i64, _i32, _i32, _f64, _f64, _f64, _PP]),
+    "b2_lbfgs_destroy": (C.c_int, [_p]),
+    "b2_lbfgs_state": (C.c_int, [_p, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64), _p]),
+    "b2_lbfgs_init": (C.c_int, [_p, _p, _p, _f64, _p]),
+    "b2_lbfgs_update": (C.c_int, [_p, _p, _p, _p, _p]),
+    "b2_lbfgs_smw_prepare": (C.c_int, [_p, _p, _i64, _p, _p]),
+    "b2_lbfgs_smw_apply": (C.c_int, [_p, _i64, _p, _p, _p]),
+    "b2_lbfgs_kkt_mul_lowrank": (C.c_int, [_p, _f64, _p, _p, _p]),
+    "b2_lbfgs_debug_get": (C.c_int, [_p, _i32, _p, C.POINTER(_i64), _p]),
+    "b2_lbfgs_debug_ipiv": (C.c_int, [_p, _p, _p]),
+    "b2_debug_bk_factor": (C.c_int, [_i32, _p, _p, _p]),
+    "b2_debug_bk_solve": (C.c_int, [_i32, _p, _p, _p, _p]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

@@ -107,11 +107,11 @@ class IPMLinearAlgebra:
         k.compress_hessian()
         k.set_aug_diagonal_()
         k.build_kkt()
-        k.linear_solver.factorize()
+        k.factorize_kkt()
 
     def _factorize_wrapper(self):
         self.kkt.build_kkt()
-        self.kkt.linear_solver.factorize()
+        self.kkt.factorize_kkt()
         self.cnt["factorizations"] += 1
 
     def _solve_refine_wrapper(self):
@@ -120,7 +120,7 @@ class IPMLinearAlgebra:
             # improve!() changed a factorisation parameter (pivot threshold) that the captured prologue has baked in:
             # drop the captured graph so that every later step factorises with the new setting
             self._prologue_graph = None
-            self.kkt.linear_solver.factorize()
+            self.kkt.factorize_kkt()
             ok = self.iterator.solve_refine(self.d, self.p, self.w)
         self.cnt["backsolves"] += self.iterator.ir
         return ok

@@ -465,4 +465,102 @@ function inertia_fetch(M::B200Solver)
     return (Int(p[]), Int(z[]), Int(n[]))
 end
 
+# ---------------------------------------------------------------------------------------------------------------------
+# hessian_approximation = CompactLBFGS with SparseKKTSystem (src/quasi_newton.jl:212-437, src/IPM/factorization.jl:76-139,
+# 253-276).  Not executed here (no Julia in the build image).  The stock CompactLBFGS is CONSTRUCTED with its
+# `additional_buffers` slot already holding a B200LBFGSState (a type this module owns), so its fourth type parameter is
+# B200LBFGSState from the start: init!/update! dispatch on CompactLBFGS{T,VT,MT,<:B200LBFGSState} and the KKT overloads on
+# QN <: that type with LS <: B200Solver -- no type piracy.  The create_kkt_system overload below hands the generic constructor
+# the marker B200CompactLBFGS (a subtype of AbstractQuasiNewton, so build_hessian_structure takes the diagonal pattern,
+# Sparse/utils.jl:18-26), whose create_quasi_newton method builds that struct.  The state lives on the device; the host-side
+# counters of the stock struct are not maintained (b2_lbfgs_state reads them).
+# ---------------------------------------------------------------------------------------------------------------------
+mutable struct B200LBFGSState
+    handle::Ptr{Cvoid}
+    n::Int
+    max_mem::Int
+    H::CuMatrix{Float64}          # N x 2 max_history: E, then C^{-1} E after factorize_kkt!
+end
+
+function B200LBFGSState(n, N, opt::MadNLP.QuasiNewtonOptions)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:b2_lbfgs_create, libb200kkt), Cint, (Int64, Int32, Int32, Float64, Float64, Float64, Ptr{Ptr{Cvoid}}),
+                n, opt.max_history, Int32(opt.init_strategy), opt.init_value, opt.sigma_min, opt.sigma_max, h), SymbolicException)
+    st = B200LBFGSState(h[], n, opt.max_history, CUDA.zeros(Float64, N, 2 * opt.max_history))
+    finalizer(x -> ccall((:b2_lbfgs_destroy, libb200kkt), Cint, (Ptr{Cvoid},), x.handle), st)
+    return st
+end
+
+# marker passed as hessian_approximation to the generic constructor; never instantiated
+abstract type B200CompactLBFGS <: MadNLP.AbstractQuasiNewton{Float64, CuVector{Float64}} end
+
+# the stock struct, field for field as create_quasi_newton(::Type{CompactLBFGS}, ...) builds it (quasi_newton.jl:242-277),
+# except additional_buffers
+function MadNLP.create_quasi_newton(::Type{B200CompactLBFGS}, cb::MadNLP.AbstractCallback{T,VT}, n;
+        options = MadNLP.QuasiNewtonOptions{T}()) where {T, VT<:CuVector{T}}
+    N = cb.nvar + length(cb.ind_ineq) + cb.ncon                   # order of the augmented system
+    vec() = fill!(MadNLP.create_array(cb, n), zero(T))
+    mat(r, c) = fill!(MadNLP.create_array(cb, r, c), zero(T))
+    return MadNLP.CompactLBFGS(
+        options.init_strategy, vec(), vec(), vec(), vec(), vec(),
+        T(options.init_value), T(options.sigma_min), T(options.sigma_max), options.max_history, 0, 0,
+        mat(n, 0), mat(n, 0), mat(0, 0), mat(0, 0), mat(0, 0), mat(0, 0), mat(0, 0), mat(0, 0), mat(0, 0), mat(0, 0),
+        fill!(MadNLP.create_array(cb, 0), zero(T)), fill!(MadNLP.create_array(cb, 0), zero(T)),
+        fill!(MadNLP.create_array(cb, 0), zero(T)),
+        B200LBFGSState(n, N, options),
+        false,
+    )
+end
+
+const B200LBFGS{T,VT,MT} = MadNLP.CompactLBFGS{T,VT,MT,<:B200LBFGSState}
+const B200LBFGSKKT{T} = MadNLP.SparseKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN<:B200LBFGS,LS<:B200Solver}
+
+function MadNLP.create_kkt_system(::Type{MadNLP.SparseKKTSystem}, cb::MadNLP.SparseCallback{T,VT}, ::Type{LS};
+        opt_linear_solver = default_options(LS), hessian_approximation = MadNLP.ExactHessian,
+        qn_options = MadNLP.QuasiNewtonOptions()) where {T, VT<:CuVector{T}, LS<:B200Solver}
+    qn = hessian_approximation <: MadNLP.CompactLBFGS ? B200CompactLBFGS : hessian_approximation
+    return invoke(MadNLP.create_kkt_system, Tuple{Type{MadNLP.SparseKKTSystem}, MadNLP.SparseCallback{T,VT}, Type},
+                  MadNLP.SparseKKTSystem, cb, LS; opt_linear_solver, hessian_approximation = qn, qn_options)
+end
+
+MadNLP.init!(qn::B200LBFGS{T}, Bk::CuVector{T}, g0::CuVector{T}, f0::T) where T =
+    check(ccall((:b2_lbfgs_init, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, Float64, Ptr{Cvoid}),
+                qn.additional_buffers.handle, pointer(Bk), pointer(g0), f0, stream_ptr()), FactorizationException)
+
+function MadNLP.update!(qn::B200LBFGS{T}, Bk::CuVector{T}, sk::CuVector{T}, yk::CuVector{T}) where T
+    check(ccall((:b2_lbfgs_update, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                qn.additional_buffers.handle, pointer(Bk), pointer(sk), pointer(yk), stream_ptr()), FactorizationException)
+    return true          # whether the pair was kept is decided on the device (b2_lbfgs_state)
+end
+
+function MadNLP.factorize_kkt!(kkt::B200LBFGSKKT)
+    factorize!(kkt.linear_solver)
+    st = kkt.quasi_newton.additional_buffers
+    check(ccall((:b2_lbfgs_smw_prepare, libb200kkt), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, CuPtr{Float64}, Ptr{Cvoid}),
+                st.handle, kkt.linear_solver.handle, size(st.H, 1), pointer(st.H), stream_ptr()), FactorizationException)
+    return
+end
+
+function MadNLP.solve_kkt!(kkt::B200LBFGSKKT, w::MadNLP.AbstractKKTVector)
+    st = kkt.quasi_newton.additional_buffers
+    MadNLP.reduce_rhs!(kkt, w)
+    w_ = MadNLP.primal_dual(w)
+    solve_linear_system!(kkt.linear_solver, w_)
+    check(ccall((:b2_lbfgs_smw_apply, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{Float64}, CuPtr{Float64}, Ptr{Cvoid}),
+                st.handle, size(st.H, 1), pointer(st.H), pointer(w_), stream_ptr()), SolveException)
+    MadNLP.finish_aug_solve!(kkt, w)
+    return w
+end
+
+function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200LBFGSKKT, x::MadNLP.AbstractKKTVector, alpha = one(T), beta = zero(T)) where T
+    mul!(MadNLP.primal(w), Symmetric(kkt.hess_com, :L), MadNLP.primal(x), alpha, beta)
+    mul!(MadNLP.primal(w), kkt.jac_com', MadNLP.dual(x), alpha, one(T))
+    mul!(MadNLP.dual(w), kkt.jac_com, MadNLP.primal(x), alpha, beta)
+    check(ccall((:b2_lbfgs_kkt_mul_lowrank, libb200kkt), Cint, (Ptr{Cvoid}, Float64, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                kkt.quasi_newton.additional_buffers.handle, alpha, pointer(MadNLP.full(x)), pointer(MadNLP.full(w)), stream_ptr()),
+          SolveException)
+    MadNLP._kktmul!(w, x, kkt.reg, kkt.du_diag, kkt.l_lower, kkt.u_lower, kkt.l_diag, kkt.u_diag, alpha, beta)
+    return w
+end
+
 end # module

@@ -18,6 +18,7 @@ import torch
 from . import capi
 from .capi import lib, check, ptr
 from .linear_solvers import B200DenseSolver, B200SparseSolver, DeviceCSC
+from .quasi_newton import CompactLBFGS, ExactHessian
 
 _DEV = "cuda"
 
@@ -207,10 +208,13 @@ class _SparseKKTBase(_KKTBase):
     value vector V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m) | ...] with aliasing views, its lower CSC
     aug_com, the separate jac_com / hess_com, and compress_*, get_*, mul and jtprod."""
 
-    def _build(self, cb, linear_solver, opt_linear_solver, unreduced):
+    def _build(self, cb, linear_solver, opt_linear_solver, unreduced, diagonal_hessian=False):
         n, m = cb.nvar, cb.ncon
         ns = len(cb.ind_ineq)
-        hI = np.array(cb.hess_I, dtype=np.int64); hJ = np.array(cb.hess_J, dtype=np.int64)
+        if diagonal_hessian:                                         # quasi-Newton: only sigma I is stored (Sparse/utils.jl:18-26)
+            hI = np.arange(n, dtype=np.int64); hJ = np.arange(n, dtype=np.int64)
+        else:
+            hI = np.array(cb.hess_I, dtype=np.int64); hJ = np.array(cb.hess_J, dtype=np.int64)
         force_lower_triangular(hI, hJ)                               # augmented.jl:65
         jI = np.asarray(cb.jac_I, dtype=np.int64); jJ = np.asarray(cb.jac_J, dtype=np.int64)
         n_jac, n_hess = len(jI), len(hI)
@@ -297,8 +301,12 @@ class _SparseKKTBase(_KKTBase):
         check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(x.values), ptr(w.values), alpha, beta, sp))
         check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x.dual()), ptr(w.values), alpha, 1.0, sp))
         check(lib.b2_spmv_n(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x.values), ptr(w.dual()), alpha, beta, sp))
+        self._mul_lowrank(w, x, alpha)
         self._kktmul(w, x, alpha, beta)
         return w
+
+    def _mul_lowrank(self, w, x, alpha):
+        pass
 
     def jtprod(self, y, x):
         """Sparse/utils.jl:28-30."""
@@ -307,10 +315,40 @@ class _SparseKKTBase(_KKTBase):
 
 class SparseKKTSystem(_SparseKKTBase):
     """src/KKT/Sparse/augmented.jl: augmented system as COO value vector
-    V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m)] (aliasing views) -> lower CSC."""
+    V = [pr_diag(n_tot) | hess(nnzh) | jac(nnzj) | slack -1 (ns) | du_diag(m)] (aliasing views) -> lower CSC.
 
-    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
-        self._build(cb, linear_solver, opt_linear_solver, unreduced=False)
+    hessian_approximation=CompactLBFGS: `hess` holds the n diagonal values of B_k = sigma I - U U' + V V' (the model's Hessian
+    pattern is ignored), `quasi_newton` the device L-BFGS state.  The low-rank part enters by Sherman-Morrison-Woodbury:
+    factorize_kkt() also solves C H = E for the 2 max_history columns of E = [U V] and factors T = P + E'H; solve_kkt then applies
+    w -= H T^{-1} E'w after the sparse solve, and mul adds the low-rank product.  H is computed once per factorisation and reused
+    by every refinement step (the reference recomputes it in each solve_kkt!, with identical values)."""
+
+    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None, hessian_approximation=ExactHessian,
+                 qn_options=None):
+        lbfgs = hessian_approximation is CompactLBFGS
+        if not lbfgs and hessian_approximation is not ExactHessian:
+            raise ValueError(f"unsupported hessian_approximation {hessian_approximation!r}")
+        if lbfgs and opt_linear_solver is not None and getattr(opt_linear_solver, "n_parts", 1) > 1:
+            raise ValueError("CompactLBFGS is not supported with a sharded linear solver (n_parts > 1)")
+        self._build(cb, linear_solver, opt_linear_solver, unreduced=False, diagonal_hessian=lbfgs)
+        self.quasi_newton = CompactLBFGS(self.n, qn_options) if lbfgs else ExactHessian()
+        self._lbfgs = lbfgs
+        if lbfgs:
+            self.quasi_newton.stream = self.stream
+            # column-major N x 2 max_history: E, then C^{-1} E after factorize_kkt()
+            self.smw_H = torch.zeros((2 * self.quasi_newton.max_mem, self.N), dtype=torch.float64, device=_DEV)
+
+    def factorize_kkt(self):
+        """factorize!(linear_solver), plus the Woodbury prologue with an L-BFGS Hessian"""
+        self.linear_solver.factorize()
+        if self._lbfgs:
+            self.quasi_newton.smw_prepare(self.linear_solver, self.smw_H)
+        return self.linear_solver
+
+    def _mul_lowrank(self, w, x, alpha):
+        """factorization.jl:266-273: w[1:n] += alpha (-U U'x + V V'x), between the Jacobian products and _kktmul!"""
+        if self._lbfgs:
+            self.quasi_newton.mul_lowrank(alpha, x.values, w.values)
 
     def initialize(self):
         """Sparse/utils.jl:52-62."""
@@ -319,9 +357,11 @@ class SparseKKTSystem(_SparseKKTBase):
         self.hess_com.nzval.zero_()
 
     def solve_kkt(self, w: UnreducedKKTVector):
-        """src/IPM/factorization.jl:41-46."""
+        """src/IPM/factorization.jl:41-46; with CompactLBFGS :76-139 (H and T from factorize_kkt)."""
         self.reduce_rhs(w)
         self.linear_solver.solve_linear_system(w.primal_dual())
+        if self._lbfgs:
+            self.quasi_newton.smw_apply(self.smw_H, w.primal_dual())
         self.finish_aug_solve(w)
         return w
 
@@ -652,8 +692,19 @@ class DenseKKTSystem(_DenseKKTBase):
         return y
 
 
-def create_kkt_system(kkt_type, cb, linear_solver=None, opt_linear_solver=None):
-    """src/IPM/IPM.jl:157-165 -> create_kkt_system(::Type{K}, cb, linear_solver; opt_linear_solver)."""
+_QN_UNSUPPORTED = {SparseUnreducedKKTSystem: "SparseUnreducedKKTSystem", SparseCondensedKKTSystem: "SparseCondensedKKTSystem"}
+
+
+def create_kkt_system(kkt_type, cb, linear_solver=None, opt_linear_solver=None, hessian_approximation=ExactHessian,
+                      qn_options=None):
+    """src/IPM/IPM.jl:157-165 -> create_kkt_system(::Type{K}, cb, linear_solver; opt_linear_solver, hessian_approximation,
+    qn_options).  CompactLBFGS is supported by SparseKKTSystem only (src/IPM/factorization.jl:169-188)."""
     if linear_solver is None:
         linear_solver = B200DenseSolver if kkt_type in (DenseCondensedKKTSystem, DenseKKTSystem) else B200SparseSolver
+    if hessian_approximation is not ExactHessian:
+        if kkt_type is not SparseKKTSystem:
+            name = _QN_UNSUPPORTED.get(kkt_type, kkt_type.__name__)
+            raise ValueError(f"Quasi-Newton approximation of the Hessian is not supported by the KKT formulation {name}. "
+                             "Please use SparseKKTSystem instead.")
+        return kkt_type(cb, linear_solver, opt_linear_solver, hessian_approximation=hessian_approximation, qn_options=qn_options)
     return kkt_type(cb, linear_solver, opt_linear_solver)
