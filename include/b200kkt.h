@@ -473,6 +473,34 @@ int b2_lbfgs_debug_ipiv(b2_lbfgs* h, int32_t* ipiv_h, void* stream);
 int b2_debug_bk_factor(int32_t N, double* A_d, int32_t* ipiv_d, void* stream);
 int b2_debug_bk_solve(int32_t N, const double* F_d, const int32_t* ipiv_d, double* b_d, void* stream);
 
+/* ------------------------------------------------------------------ dense quasi-Newton (DenseKKTSystem / DenseCondensedKKTSystem,
+ * hessian_approximation = BFGS or DampedBFGS; src/quasi_newton.jl:71-201, 425-437).  Bk_d is the KKT system's `hess`: n x n,
+ * column-major, leading dimension n; only its lower triangle is read or written.  Every state value (is_instantiated, the last
+ * decision, the scalars, bsk = B s and r) is device memory: no entry point below synchronises except b2d_qn_state and the debug
+ * getter, each issues a fixed launch sequence, and all can be captured in a CUDA graph.  Reductions are deterministic (fixed
+ * order).  Use a handle from one stream at a time.  n <= 2^31 - 1; element offsets are 64-bit. */
+#define B2_QN_BFGS        1
+#define B2_QN_DAMPED_BFGS 2
+typedef struct b2d_qn b2d_qn;
+int b2d_qn_create(int64_t n, int32_t kind, b2d_qn** out);
+int b2d_qn_destroy(b2d_qn* h);
+/* init!: Bk[i, i] = 2 rho0 (Gilbert-Lemarechal rule with norm_g0 = g0'g0; f0 = +-0 takes the 1 / norm_g0 branch); the rest of Bk
+ * and is_instantiated are left alone.  2 launches */
+int b2d_qn_init(b2d_qn* h, double* Bk_d, const double* g0_d, double f0, void* stream);
+/* update!: BFGS skips (Bk bit-unchanged) when y's < 1e-8; DampedBFGS never skips.  The first accepted call sets the diagonal to
+ * y's / s's.  Then bsk = B s (b2d_symv_lower), alpha1 = 1 / s'bsk and, in one pass over the lower triangle, per element
+ * a = a + b_i ((-alpha1) b_j); a = a + v_i (alpha2 v_j) (no contraction), with v = y, alpha2 = 1 / y's (BFGS) or
+ * v = r = (0 + theta y) + (1 - theta) bsk, alpha2 = 1 / r's (DampedBFGS).  6 launches */
+int b2d_qn_update(b2d_qn* h, double* Bk_d, const double* sk_d, const double* yk_d, void* stream);
+/* the fused rank-2 pass of b2d_qn_update alone, with the decision, scalars and vectors of the last update (benchmarks); yk_d is
+ * read by BFGS only */
+int b2d_qn_rank2(b2d_qn* h, double* Bk_d, const double* yk_d, void* stream);
+/* is_instantiated, the last decision, and scalars[6] = {y's, s's, s'Bs, theta, alpha1, alpha2} of the last update (on a skipped
+ * BFGS call, the values the update would have used); synchronises `stream` */
+int b2d_qn_state(b2d_qn* h, int32_t* instantiated, int32_t* accepted, double* scalars, void* stream);
+/* Debug/test: host copies of bsk and r (n doubles each; r is written by DampedBFGS only); synchronises */
+int b2d_qn_debug_vectors(b2d_qn* h, double* bsk_h, double* rk_h, void* stream);
+
 
 #ifdef __cplusplus
 }

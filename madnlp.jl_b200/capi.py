@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libb200kkt.so")
 B2_OK = 0
 B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE, B2_ERR_NO_DEVICE = 1, 2, 3, 4, 5, 6
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
+QN_BFGS, QN_DAMPED_BFGS = 1, 2
 
 
 class B2Error(RuntimeError):
@@ -195,6 +196,13 @@ PROTOTYPES = {
     "b2_lbfgs_debug_ipiv": (C.c_int, [_p, _p, _p]),
     "b2_debug_bk_factor": (C.c_int, [_i32, _p, _p, _p]),
     "b2_debug_bk_solve": (C.c_int, [_i32, _p, _p, _p, _p]),
+    "b2d_qn_create": (C.c_int, [_i64, _i32, _PP]),
+    "b2d_qn_destroy": (C.c_int, [_p]),
+    "b2d_qn_init": (C.c_int, [_p, _p, _p, _f64, _p]),
+    "b2d_qn_update": (C.c_int, [_p, _p, _p, _p, _p]),
+    "b2d_qn_rank2": (C.c_int, [_p, _p, _p, _p]),
+    "b2d_qn_state": (C.c_int, [_p, C.POINTER(_i32), C.POINTER(_i32), _p, _p]),
+    "b2d_qn_debug_vectors": (C.c_int, [_p, _p, _p, _p]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

@@ -563,4 +563,59 @@ function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200LBFGSKKT, x::MadNL
     return w
 end
 
+# ---------------------------------------------------------------------------------------------------------------------
+# hessian_approximation = BFGS / DampedBFGS with DenseKKTSystem and DenseCondensedKKTSystem (src/quasi_newton.jl:71-201, 425-437).
+# Not executed here (no Julia in the build image).  The create_kkt_system overloads below swap the stock markers for
+# B200BFGS / B200DampedBFGS, types this module owns that hold a b2d_qn handle, and `invoke` the generic constructor, which calls
+# their create_quasi_newton methods.  They carry the fields eval_lag_hess_wrapper! reads (sk, yk, last_g, last_x, last_jv,
+# src/IPM/callbacks.jl:146-192); bsk, r, is_instantiated and the decision live on the device (b2d_qn_state reads them).  Bk is the
+# KKT system's `hess`, updated in place on its lower triangle, the only one the dense KKT kernels read.
+# ---------------------------------------------------------------------------------------------------------------------
+abstract type B200DenseQuasiNewton{T,VT} <: MadNLP.AbstractQuasiNewton{T,VT} end
+
+for (name, kind) in ((:B200BFGS, 1), (:B200DampedBFGS, 2))
+    @eval begin
+        mutable struct $name{T,VT<:CuVector{T}} <: B200DenseQuasiNewton{T,VT}
+            handle::Ptr{Cvoid}
+            init_strategy::MadNLP.BFGSInitStrategy      # stored and unused, as in the reference
+            sk::VT
+            yk::VT
+            last_g::VT
+            last_x::VT
+            last_jv::VT
+        end
+        function MadNLP.create_quasi_newton(::Type{$name}, cb::MadNLP.AbstractCallback{T,VT}, n;
+                options = MadNLP.QuasiNewtonOptions{T}()) where {T, VT<:CuVector{T}}
+            h = Ref{Ptr{Cvoid}}(C_NULL)
+            check(ccall((:b2d_qn_create, libb200kkt), Cint, (Int64, Int32, Ptr{Ptr{Cvoid}}), n, Int32($kind), h), SymbolicException)
+            vec() = fill!(MadNLP.create_array(cb, n), zero(T))
+            qn = $name{T,VT}(h[], options.init_strategy, vec(), vec(), vec(), vec(), vec())
+            finalizer(x -> ccall((:b2d_qn_destroy, libb200kkt), Cint, (Ptr{Cvoid},), x.handle), qn)
+            return qn
+        end
+    end
+end
+
+_b200_dense_qn(qn) = qn <: MadNLP.DampedBFGS ? B200DampedBFGS : qn <: MadNLP.BFGS ? B200BFGS : qn
+
+for KKT in (:DenseKKTSystem, :DenseCondensedKKTSystem)
+    @eval function MadNLP.create_kkt_system(::Type{MadNLP.$KKT}, cb::MadNLP.AbstractCallback{T,VT}, ::Type{LS};
+            opt_linear_solver = default_options(LS), hessian_approximation = MadNLP.ExactHessian,
+            qn_options = MadNLP.QuasiNewtonOptions()) where {T, VT<:CuVector{T}, LS<:B200DenseSolver}
+        return invoke(MadNLP.create_kkt_system, Tuple{Type{MadNLP.$KKT}, MadNLP.AbstractCallback{T,VT}, Type},
+                      MadNLP.$KKT, cb, LS; opt_linear_solver, hessian_approximation = _b200_dense_qn(hessian_approximation),
+                      qn_options)
+    end
+end
+
+MadNLP.init!(qn::B200DenseQuasiNewton{T}, Bk::CuMatrix{T}, g0::CuVector{T}, f0::T) where T =
+    check(ccall((:b2d_qn_init, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, Float64, Ptr{Cvoid}),
+                qn.handle, pointer(Bk), pointer(g0), f0, stream_ptr()), FactorizationException)
+
+function MadNLP.update!(qn::B200DenseQuasiNewton{T}, Bk::CuMatrix{T}, sk::CuVector{T}, yk::CuVector{T}) where T
+    check(ccall((:b2d_qn_update, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                qn.handle, pointer(Bk), pointer(sk), pointer(yk), stream_ptr()), FactorizationException)
+    return true          # whether BFGS skipped the pair is decided on the device (b2d_qn_state)
+end
+
 end # module

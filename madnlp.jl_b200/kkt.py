@@ -18,7 +18,7 @@ import torch
 from . import capi
 from .capi import lib, check, ptr
 from .linear_solvers import B200DenseSolver, B200SparseSolver, DeviceCSC
-from .quasi_newton import CompactLBFGS, ExactHessian
+from .quasi_newton import BFGS, CompactLBFGS, DampedBFGS, ExactHessian
 
 _DEV = "cuda"
 
@@ -518,7 +518,21 @@ class SparseCondensedKKTSystem(_KKTBase):
 class _DenseKKTBase(_KKTBase):
     """What both dense formulations share (AbstractDenseKKTSystem, src/KKT/Dense/utils.jl:3-29).  Dense matrices are
     torch tensors whose MEMORY is the column-major matrix (tensor[j, i] = M[i, j]), so pointers can be handed to the kernels
-    exactly as Julia would hand them."""
+    exactly as Julia would hand them.
+
+    hessian_approximation=BFGS or DampedBFGS: `quasi_newton` is the device state whose init / update rewrite the lower triangle
+    of `hess` in place (csrc/dense_qn.cu); every consumer of `hess` reads only that triangle, so nothing else changes."""
+
+    @staticmethod
+    def _check_hessian_approximation(hessian_approximation):
+        if hessian_approximation is not ExactHessian and hessian_approximation not in (BFGS, DampedBFGS):
+            raise ValueError(f"unsupported hessian_approximation {hessian_approximation!r}")
+
+    def _init_quasi_newton(self, hessian_approximation, qn_options):
+        if hessian_approximation is ExactHessian:
+            self.quasi_newton = ExactHessian()
+        else:
+            self.quasi_newton = hessian_approximation(self.n, qn_options, stream=self.stream)
 
     def get_jacobian(self):
         return self.jac
@@ -558,7 +572,9 @@ class _DenseKKTBase(_KKTBase):
 class DenseCondensedKKTSystem(_DenseKKTBase):
     """src/KKT/Dense/condensed.jl."""
 
-    def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None):
+    def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None, hessian_approximation=ExactHessian,
+                 qn_options=None):
+        self._check_hessian_approximation(hessian_approximation)
         n, m = cb.nvar, cb.ncon
         ind_ineq = np.asarray(cb.ind_ineq, dtype=np.int64)
         ind_eq = np.setdiff1d(np.arange(m), ind_ineq).astype(np.int64)
@@ -591,6 +607,7 @@ class DenseCondensedKKTSystem(_DenseKKTBase):
             check(lib.b2d_ozaki_plan_create(n, ns, C.byref(hz)))
             self._ozaki = _Plan(hz, lib.b2d_ozaki_plan_destroy)
         self.linear_solver = linear_solver(self.aug_com, opt_linear_solver)
+        self._init_quasi_newton(hessian_approximation, qn_options)
 
     def num_variables(self):
         return self.n
@@ -643,7 +660,9 @@ class DenseKKTSystem(_DenseKKTBase):
     """src/KKT/Dense/augmented.jl: the augmented system of order N = n + ns + m as one dense column-major matrix,
     factorised whole by the dense LDL^T (inertia (n + ns, 0, m) at a minimiser)."""
 
-    def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None):
+    def __init__(self, cb, linear_solver=B200DenseSolver, opt_linear_solver=None, hessian_approximation=ExactHessian,
+                 qn_options=None):
+        self._check_hessian_approximation(hessian_approximation)
         n, m = cb.nvar, cb.ncon
         ind_ineq = np.asarray(cb.ind_ineq, dtype=np.int64)
         ns = len(ind_ineq)
@@ -661,6 +680,7 @@ class DenseKKTSystem(_DenseKKTBase):
         check(lib.b2d_kkt_create(n, m, ns, ind_ineq.ctypes.data if ns else None, C.byref(h)))
         self._dk = _Plan(h, lib.b2d_kkt_destroy)
         self.linear_solver = linear_solver(self.aug_com, opt_linear_solver)
+        self._init_quasi_newton(hessian_approximation, qn_options)
 
     def num_variables(self):
         """augmented.jl:96."""
@@ -698,9 +718,16 @@ _QN_UNSUPPORTED = {SparseUnreducedKKTSystem: "SparseUnreducedKKTSystem", SparseC
 def create_kkt_system(kkt_type, cb, linear_solver=None, opt_linear_solver=None, hessian_approximation=ExactHessian,
                       qn_options=None):
     """src/IPM/IPM.jl:157-165 -> create_kkt_system(::Type{K}, cb, linear_solver; opt_linear_solver, hessian_approximation,
-    qn_options).  CompactLBFGS is supported by SparseKKTSystem only (src/IPM/factorization.jl:169-188)."""
+    qn_options).  CompactLBFGS is supported by SparseKKTSystem only (src/IPM/factorization.jl:169-188); BFGS and DampedBFGS by
+    the dense systems only (check_option_sanity, src/IPM/options.jl:232-241), checked before anything is allocated."""
+    dense = kkt_type in (DenseCondensedKKTSystem, DenseKKTSystem)
     if linear_solver is None:
-        linear_solver = B200DenseSolver if kkt_type in (DenseCondensedKKTSystem, DenseKKTSystem) else B200SparseSolver
+        linear_solver = B200DenseSolver if dense else B200SparseSolver
+    if hessian_approximation in (BFGS, DampedBFGS):
+        if not dense:
+            raise ValueError("[options] DENSE_BFGS and DENSE_DAMPED_BFGS quasi-Newton approximations\n"
+                             "require a dense KKT system (DENSE_KKT_SYSTEM or DENSE_CONDENSED_KKT_SYSTEM).")
+        return kkt_type(cb, linear_solver, opt_linear_solver, hessian_approximation=hessian_approximation, qn_options=qn_options)
     if hessian_approximation is not ExactHessian:
         if kkt_type is not SparseKKTSystem:
             name = _QN_UNSUPPORTED.get(kkt_type, kkt_type.__name__)

@@ -1,9 +1,11 @@
-"""Host mirror of MadNLP's Hessian sources (src/quasi_newton.jl): the `ExactHessian` and `CompactLBFGS` markers passed as
-`hessian_approximation`, `QuasiNewtonOptions`, and the device-resident compact L-BFGS state of SparseKKTSystem.
+"""Host mirror of MadNLP's Hessian sources (src/quasi_newton.jl): the `ExactHessian`, `CompactLBFGS`, `BFGS` and `DampedBFGS`
+markers passed as `hessian_approximation`, `QuasiNewtonOptions`, the device-resident compact L-BFGS state of SparseKKTSystem and
+the device-resident dense BFGS / DampedBFGS states of the dense KKT systems.
 
-B_k = sigma I - U U' + V V' on the n model variables.  Every numeric operation is a C-ABI call into csrc/lbfgs.cu and every state
-value stays on the device, so `init`, `update` and the KKT calls built on them never block the host and can be captured in a CUDA
-graph; only `size()` synchronises.
+Compact L-BFGS: B_k = sigma I - U U' + V V' on the n model variables (csrc/lbfgs.cu).  BFGS / DampedBFGS: B_k is the dense KKT
+system's n x n `hess`, updated in place on its lower triangle (csrc/dense_qn.cu).  Every numeric operation is a C-ABI call and
+every state value stays on the device, so `init`, `update` and the KKT calls built on them never block the host and can be
+captured in a CUDA graph; only `size()` / `state()` and the debug getters synchronise.
 """
 from __future__ import annotations
 
@@ -129,3 +131,77 @@ class CompactLBFGS:
         ip = np.zeros(2 * self.max_mem, dtype=np.int32)
         check(lib.b2_lbfgs_debug_ipiv(self._h, ip.ctypes.data, self._sp()))
         return ip
+
+
+class _DenseQuasiNewton:
+    """What BFGS and DampedBFGS share: the device state of csrc/dense_qn.cu.  `sk`, `yk`, `last_g`, `last_x`, `last_jv` are device
+    vectors of length n the caller fills (callbacks.jl:146-192); `init(Bk, g0, f0)` and `update(Bk, sk, yk)` restate init! and
+    update!, with Bk the dense KKT system's `hess` (n x n, column-major, lower triangle only).  `init_strategy` is stored and not
+    used, as in the reference."""
+
+    KIND = 0
+
+    def __init__(self, n, options: QuasiNewtonOptions | None = None, stream=None):
+        capi.require_device()
+        opt = options if options is not None else QuasiNewtonOptions()
+        self.options = opt
+        self.init_strategy = opt.init_strategy
+        self.n = int(n)
+        self.stream = stream
+        z = lambda: torch.zeros(self.n, dtype=torch.float64, device="cuda")
+        self.sk, self.yk, self.last_g, self.last_x, self.last_jv = z(), z(), z(), z(), z()
+        h = C.c_void_p()
+        check(lib.b2d_qn_create(self.n, self.KIND, C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h and lib is not None:
+            lib.b2d_qn_destroy(h)
+            self._h = None
+
+    @property
+    def handle(self):
+        return self._h
+
+    def _sp(self):
+        return capi.stream_ptr(self.stream)
+
+    def init(self, Bk, g0, f0):
+        """init! (quasi_newton.jl:425-437): the diagonal of Bk = 2 rho0; nothing else changes."""
+        check(lib.b2d_qn_init(self._h, ptr(Bk), ptr(g0), float(f0), self._sp()))
+
+    def update(self, Bk, sk=None, yk=None):
+        """update!.  Whether the pair was used is decided on the device; `state()` tells."""
+        sk = self.sk if sk is None else sk
+        yk = self.yk if yk is None else yk
+        check(lib.b2d_qn_update(self._h, ptr(Bk), ptr(sk), ptr(yk), self._sp()))
+
+    def rank2(self, Bk, yk=None):
+        """the fused rank-2 pass of the last update alone, applied again to Bk (benchmarks)"""
+        yk = self.yk if yk is None else yk
+        check(lib.b2d_qn_rank2(self._h, ptr(Bk), ptr(yk), self._sp()))
+
+    def state(self):
+        """dict(instantiated, accepted, ys, ss, sBs, theta, alpha1, alpha2) of the last update; synchronises"""
+        inst, acc = C.c_int32(), C.c_int32()
+        sc = np.zeros(6)
+        check(lib.b2d_qn_state(self._h, C.byref(inst), C.byref(acc), sc.ctypes.data, self._sp()))
+        return dict(instantiated=bool(inst.value), accepted=bool(acc.value),
+                    **dict(zip(("ys", "ss", "sBs", "theta", "alpha1", "alpha2"), sc.tolist())))
+
+    def debug_vectors(self):
+        """host copies of (bsk, r) of the last update; synchronises"""
+        b, r = np.zeros(self.n), np.zeros(self.n)
+        check(lib.b2d_qn_debug_vectors(self._h, b.ctypes.data, r.ctypes.data, self._sp()))
+        return b, r
+
+
+class BFGS(_DenseQuasiNewton):
+    """BFGS (quasi_newton.jl:71-129) on the device: B+ = B - (Bs)(Bs)'/(s'Bs) + yy'/(y's), skipped when y's < 1e-8."""
+    KIND = capi.QN_BFGS
+
+
+class DampedBFGS(_DenseQuasiNewton):
+    """DampedBFGS (quasi_newton.jl:131-201) on the device: Powell's damping (Nocedal & Wright, Procedure 18.2), never skipped."""
+    KIND = capi.QN_DAMPED_BFGS
