@@ -423,6 +423,31 @@ int b2_get_sc(b2_bounds* b, const double* zl_d, const double* zu_d, double s_max
 int b2_set_aug_rhs(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* f_d,
                    const double* zl_d, const double* zu_d, const double* jacl_d, const double* c_d, double mu, double* p_d, void* stream);
 
+/* ------------------------------------------------------------------ inertia-free regularisation (inertia_correction_method = InertiaFree)
+ * src/IPM/solver.jl:672-737, 785-788; src/IPM/kernels.jl:233-248; src/IPM/factorization.jl:326-350.  One elementwise launch each;
+ * outputs are bit-identical to the reference's broadcasts (left-to-right, no contraction; +-0, +-Inf and NaN as in IEEE). */
+/* set_g_ifr!: g = f - mu ./ (x - xl) + mu ./ (xu - x) + jacl over n entries (n_tot; an infinite bound contributes mu / Inf = 0) */
+int b2_set_g_ifr(int64_t n, const double* f_d, const double* x_d, const double* xl_d, const double* xu_d, const double* jacl_d, double mu,
+                 double* g_d, void* stream);
+/* set_aug_rhs_ifr!: p0 = [0 (n_tot) | -c (m) | 0 (nlb) | 0 (nub)] */
+int b2_set_aug_rhs_ifr(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* c_d, double* p0_d, void* stream);
+/* mul_hess_blk! after the Hessian product: wx[0:n_h) holds Symmetric(H, :L) t[0:n_h) (b2_spmv_symlower on hess_com, or b2d_symv_lower on
+ * the dense hess); this pass sets wx[n_h:n_tot) = 0, then wx .+= t .* pr_diag and, with unreduced = 1, wx[ind_lb] .-= t[ind_lb] .*
+ * (l_lower ./ l_diag) followed by the same for ub (n_tot, ind_lb, ind_ub from `b`).  With result_d = NULL that is all (n_d, g_d and tol
+ * are ignored).  With result_d (B2_CURV_RESULT_LEN device doubles) the same launch also forms wx't, wx'n, g'n and t't as fixed-order
+ * block partials and writes them, lhs = wx't + max(wx'n - g'n, 0) - tol t't (NaN-propagating max) and pass = (lhs >= 0) as 1.0 / 0.0.
+ * Deterministic, never synchronises, graph-capturable.  The partials live in `b`: one test at a time per b2_bounds object. */
+#define B2_CURV_WXT  0
+#define B2_CURV_WXN  1
+#define B2_CURV_GN   2
+#define B2_CURV_TT   3
+#define B2_CURV_LHS  4
+#define B2_CURV_PASS 5
+#define B2_CURV_RESULT_LEN 6
+int b2_mul_hess_blk_tail(b2_bounds* b, int64_t n_h, int32_t unreduced, const double* pr_diag_d, const double* l_lower_d,
+                         const double* l_diag_d, const double* u_lower_d, const double* u_diag_d, const double* t_d, double* wx_d,
+                         const double* n_d, const double* g_d, double tol, double* result_d, void* stream);
+
 /* ------------------------------------------------------------------ compact L-BFGS (SparseKKTSystem, hessian_approximation = CompactLBFGS)
  * src/quasi_newton.jl:212-437 and src/IPM/factorization.jl:76-139, 253-276.  B_k = sigma I - U U' + V V' on the n model variables
  * (no slacks); S, Y are n x max_history, the memory p <= max_history.  max_history is limited to 32, so that

@@ -8,7 +8,8 @@ Only what the hot path needs lives here (SURVEY.md section 8):
                   SparseCondensedKKTSystem, DenseCondensedKKTSystem, DenseKKTSystem, UnreducedKKTVector)
   quasi_newton    ExactHessian / CompactLBFGS (the device L-BFGS state SparseKKTSystem uses) / BFGS / DampedBFGS (the
                   device dense quasi-Newton states of DenseKKTSystem and DenseCondensedKKTSystem)
-  richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric
+  richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric, with the
+                  InertiaBased (default), InertiaFree and InertiaIgnore regularisations
   workloads       synthetic generators for the configurations named in BASELINE.json
   julia/          the Julia shim a MadNLP.jl maintainer would add (cannot be run in this image)
 

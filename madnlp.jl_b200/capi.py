@@ -16,6 +16,8 @@ B2_OK = 0
 B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE, B2_ERR_NO_DEVICE = 1, 2, 3, 4, 5, 6
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
+# layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
+CURV_WXT, CURV_WXN, CURV_GN, CURV_TT, CURV_LHS, CURV_PASS, CURV_RESULT_LEN = 0, 1, 2, 3, 4, 5, 6
 
 
 class B2Error(RuntimeError):
@@ -177,6 +179,9 @@ PROTOTYPES = {
     "b2_get_sd": (C.c_int, [_p, _i64, _p, _p, _p, _f64, _p, _p]),
     "b2_get_sc": (C.c_int, [_p, _p, _p, _f64, _p, _p]),
     "b2_set_aug_rhs": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _f64, _p, _p]),
+    "b2_set_g_ifr": (C.c_int, [_i64, _p, _p, _p, _p, _p, _f64, _p, _p]),
+    "b2_set_aug_rhs_ifr": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p]),
+    "b2_mul_hess_blk_tail": (C.c_int, [_p, _i64, _i32] + [_p] * 9 + [_f64, _p, _p]),
     "b2_richardson_begin": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_richardson_update": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_copy_many": (C.c_int, [_i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(_i64), _p]),

@@ -11,4 +11,6 @@ struct b2_bounds {
     b2::DevBuf<int32_t> lbpos, ubpos;      // [n_tot] position in ind_lb / ind_ub or -1
     b2::DevBuf<double> red_part;           // [B2_RED_BLOCKS] per-CTA partial results
     b2::DevBuf<unsigned> red_ticket;       // [1] arrival counter (reset by the last CTA)
+    b2::DevBuf<double> curv_part;          // [4 * B2_RED_BLOCKS] partials of the curvature test (inertia_free.cu)
+    b2::DevBuf<unsigned> curv_ticket;      // [1] its arrival counter
 };

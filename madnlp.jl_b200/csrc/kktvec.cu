@@ -33,7 +33,9 @@ extern "C" int b2_bounds_create(int64_t n_tot, int64_t nlb, int64_t nub, const i
     if (b->ind_lb.upload(ind_lb_h, nlb) != cudaSuccess || b->ind_ub.upload(ind_ub_h, nub) != cudaSuccess ||
         b->lbpos.upload(lp.data(), lp.size()) != cudaSuccess || b->ubpos.upload(up.data(), up.size()) != cudaSuccess ||
         b->red_part.alloc(B2_RED_BLOCKS) != cudaSuccess || b->red_ticket.alloc(1) != cudaSuccess ||
-        cudaMemset(b->red_ticket.p, 0, sizeof(unsigned)) != cudaSuccess) {
+        cudaMemset(b->red_ticket.p, 0, sizeof(unsigned)) != cudaSuccess ||
+        b->curv_part.alloc(4 * B2_RED_BLOCKS) != cudaSuccess || b->curv_ticket.alloc(1) != cudaSuccess ||
+        cudaMemset(b->curv_ticket.p, 0, sizeof(unsigned)) != cudaSuccess) {
         delete b;
         return cuda_fail(cudaGetLastError(), "bounds upload", __FILE__, __LINE__);
     }

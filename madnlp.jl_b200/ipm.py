@@ -7,6 +7,10 @@
         factorize_wrapper! = build_kkt! + factorize!   ; inertia ; is_inertia_correct
         solve_refine_wrapper! (Richardson)             ; on failure improve! and retry (factorization.jl:1-19)
         while !ok: regularize_diagonal!(dw, dc) ; factorize_wrapper! ; inertia ; solve_refine
+    or, with inertia_correction_method = InertiaFree (src/IPM/solver.jl:672-737):
+        set_g_ifr! ; set_aug_rhs_ifr! ; factorize_wrapper! ; solve_refine (d0, p0) && solve_refine (d, p) ; t = dx - n
+        while !curv_test || !ok: regularize_diagonal!(dw, dc) ; factorize_wrapper! ; the two solves ; t = dx - n
+    (InertiaIgnore, :739-783: the same loop with the d solve only and no test)
 
 The model callbacks themselves are out of scope (SURVEY.md 8a A0): an iterate supplies their outputs.
 """
@@ -33,10 +37,72 @@ class InertiaOptions:
     jacobian_regularization_exponent: float = 0.25
 
 
-class IPMLinearAlgebra:
-    """Owns the work vectors of MadNLPSolver that the hot path touches (d, p, _w4) and drives one iteration."""
+INERTIA_CORRECTION_METHODS = ("InertiaAuto", "InertiaBased", "InertiaIgnore", "InertiaFree")
 
-    def __init__(self, kkt, tol=1e-8, use_cuda_graph=True, speculate=True):
+
+def resolve_inertia_correction_method(method, linear_solver):
+    """src/IPM/IPM.jl:203-207: InertiaAuto is InertiaBased when the linear solver reports inertia, InertiaFree otherwise"""
+    if method not in INERTIA_CORRECTION_METHODS:
+        raise ValueError(f"inertia_correction_method must be one of {', '.join(INERTIA_CORRECTION_METHODS)}; got {method!r}")
+    if method == "InertiaAuto":
+        return "InertiaBased" if linear_solver.is_inertia() else "InertiaFree"
+    return method
+
+
+class InertiaFreeCorrector:
+    """The InertiaFree corrector (src/IPM/inertiacorrector.jl:7-17): p0, d0, t, wx, g, plus the solver vectors set_g_ifr! and
+    set_aug_rhs_ifr! read (f, x, xl, xu, jacl: n_tot, +-Inf for an absent bound; c: m), which IPMLinearAlgebra.load_ifr_inputs
+    fills, and _w3, the work vector of the d0 solve."""
+
+    def __init__(self, kkt):
+        from . import capi
+        self.p0 = UnreducedKKTVector.for_kkt(kkt)
+        self.d0 = UnreducedKKTVector.for_kkt(kkt)
+        self.w3 = UnreducedKKTVector.for_kkt(kkt)
+        n_tot, m = self.p0.n, self.p0.m
+        z = lambda k: torch.zeros(k, dtype=torch.float64, device=self.p0.values.device)
+        self.t, self.wx, self.g = z(n_tot), z(n_tot), z(n_tot)
+        self.f, self.x, self.xl, self.xu, self.jacl = (z(n_tot) for _ in range(5))
+        self.c = z(m)
+        self.result_h = torch.zeros(capi.CURV_RESULT_LEN, dtype=torch.float64).pin_memory()
+        self.last_result = None
+
+    def set_rhs(self, kkt, mu):
+        """set_g_ifr! (src/IPM/kernels.jl:242-248) and set_aug_rhs_ifr! (:233-240)"""
+        from .capi import lib, check, ptr, stream_ptr
+        sp = stream_ptr(getattr(kkt, "stream", None))
+        p0 = self.p0
+        check(lib.b2_set_g_ifr(p0.n, ptr(self.f), ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.jacl), float(mu), ptr(self.g), sp))
+        check(lib.b2_set_aug_rhs_ifr(p0.n, p0.m, p0.nlb, p0.nub, ptr(self.c), ptr(p0.values), sp))
+
+    def direction_difference(self, kkt, d):
+        """t = dx - n with n = primal(d0): copyto! then axpy!(-1, n, t), exact"""
+        from .capi import lib, check, ptr, stream_ptr
+        sp = stream_ptr(getattr(kkt, "stream", None))
+        check(lib.b2_copy(self.p0.n, ptr(d.primal()), ptr(self.t), sp))
+        check(lib.b2_axpy(self.p0.n, -1.0, ptr(self.d0.primal()), ptr(self.t), sp))
+
+    def curvature_ok(self, kkt, tol):
+        """curv_test (src/IPM/solver.jl:785-788) on the device; the host reads its result with one pinned copy"""
+        res = kkt.curv_test(self.t, self.d0.primal(), self.g, self.wx, tol)
+        self.result_h.copy_(res, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        self.last_result = tuple(float(v) for v in self.result_h)
+        from .capi import CURV_PASS
+        return self.last_result[CURV_PASS] == 1.0
+
+
+class IPMLinearAlgebra:
+    """Owns the work vectors of MadNLPSolver that the hot path touches (d, p, _w4) and drives one iteration.
+
+    inertia_correction_method (MadNLP's option of the same name): "InertiaBased" (the default), "InertiaFree" (the curvature test
+    of Chiang & Zavala; its inputs come from load_ifr_inputs), "InertiaIgnore", or "InertiaAuto" (InertiaBased with every
+    solver of this package, since each reports inertia).  inertia_free_tol is the curvature test's tolerance (default 0)."""
+
+    def __init__(self, kkt, tol=1e-8, use_cuda_graph=True, speculate=True, inertia_correction_method="InertiaBased",
+                 inertia_free_tol=0.0):
+        self.inertia_correction_method = resolve_inertia_correction_method(inertia_correction_method, kkt.linear_solver)
+        self.inertia_free_tol = float(inertia_free_tol)
         self.kkt = kkt
         self.use_cuda_graph = use_cuda_graph
         self.speculate = speculate     # first refinement step queued before the inertia is known (see step())
@@ -45,9 +111,21 @@ class IPMLinearAlgebra:
         self.d = UnreducedKKTVector.for_kkt(kkt)
         self.p = UnreducedKKTVector.for_kkt(kkt)
         self.w = UnreducedKKTVector.for_kkt(kkt)
+        self.ifr = InertiaFreeCorrector(kkt) if self.inertia_correction_method == "InertiaFree" else None
         self.opt = InertiaOptions()
         self.del_w_last = 0.0
         self.cnt = dict(factorizations=0, backsolves=0, regularized=0, failed=0)
+
+    def load_ifr_inputs(self, f, x, xl, xu, jacl, c, non_blocking=True):
+        """Copy the solver vectors the inertia-free test reads (f, x, xl, xu, jacl: n_tot; c: m) into the corrector's buffers"""
+        if self.ifr is None:
+            raise ValueError("load_ifr_inputs needs inertia_correction_method = InertiaFree")
+        r = self.ifr
+        for dst, src in ((r.f, f), (r.x, x), (r.xl, xl), (r.xu, xu), (r.jacl, jacl), (r.c, c)):
+            src = torch.as_tensor(src, dtype=torch.float64)
+            if src.numel() != dst.numel():
+                raise ValueError(f"load_ifr_inputs: expected {dst.numel()} entries, got {src.numel()}")
+            dst.copy_(src, non_blocking=non_blocking)
 
     def load_iterate(self, it, non_blocking=True):
         """Copy one iterate's callback outputs / diagonal inputs into the KKT buffers (H2D when `it` holds pinned
@@ -114,14 +192,17 @@ class IPMLinearAlgebra:
         self.kkt.factorize_kkt()
         self.cnt["factorizations"] += 1
 
-    def _solve_refine_wrapper(self):
-        ok = self.iterator.solve_refine(self.d, self.p, self.w)
+    def _solve_refine_wrapper(self, x=None, b=None, w=None):
+        """solve_refine_wrapper!(x, solver, b, w); (d, p, _w4) by default"""
+        if x is None:
+            x, b, w = self.d, self.p, self.w
+        ok = self.iterator.solve_refine(x, b, w)
         if not ok and self.kkt.linear_solver.improve():
             # improve!() changed a factorisation parameter (pivot threshold) that the captured prologue has baked in:
             # drop the captured graph so that every later step factorises with the new setting
             self._prologue_graph = None
             self.kkt.factorize_kkt()
-            ok = self.iterator.solve_refine(self.d, self.p, self.w)
+            ok = self.iterator.solve_refine(x, b, w)
         self.cnt["backsolves"] += self.iterator.ir
         return ok
 
@@ -131,6 +212,8 @@ class IPMLinearAlgebra:
         inertia: host-side work placed there (e.g. queueing the next iterate's H2D copies, HostIteratePipeline) is hidden
         behind ~0.2 ms of device work instead of sitting between two steps."""
         k = self.kkt
+        if self.ifr is not None:
+            self.ifr.set_rhs(k, mu)
         # compress_* + set_aug_diagonal! + the first factorize_wrapper! of inertia_correction!: fixed launch sequence,
         # replayed as one CUDA graph from the third step on (eager, capture, replay)
         if not self.use_cuda_graph or self._prologue_graph is None:
@@ -150,6 +233,8 @@ class IPMLinearAlgebra:
         self._wait_rhs()
         if after_prologue is not None:
             after_prologue()
+        if self.inertia_correction_method != "InertiaBased":
+            return self._inertia_correction_without_inertia(mu)
         # inertia_correction!(InertiaBased)
         o = self.opt
         n_trial = 0
@@ -190,6 +275,54 @@ class IPMLinearAlgebra:
         if del_w != 0.0:
             self.del_w_last = del_w
         self.last_inertia = inertia
+        return True
+
+    def _trial_solves(self):
+        """InertiaFree: the d0 solve and, only if it succeeded, the d solve (the reference's `&&`), then t = dx - n.
+        InertiaIgnore: the d solve."""
+        r = self.ifr
+        if r is None:
+            return self._solve_refine_wrapper()
+        ok = self._solve_refine_wrapper(r.d0, r.p0, r.w3) and self._solve_refine_wrapper()
+        r.direction_difference(self.kkt, self.d)
+        return ok
+
+    def _trial_accepted(self, ok):
+        # the reference evaluates curv_test first (`!curv_test(...) || !solve_status`); when a solve failed its value cannot change
+        # the outcome, so the test only runs after successful solves
+        if not ok:
+            return False
+        return self.ifr is None or self.ifr.curvature_ok(self.kkt, self.inertia_free_tol)
+
+    def _inertia_correction_without_inertia(self, mu):
+        """inertia_correction!(::InertiaFree) (src/IPM/solver.jl:672-737) and (::InertiaIgnore) (:739-783), after the first
+        factorisation: the inertia is never read, and del_c is set on every trial.  `last_del_w` lists the del_w of each trial."""
+        k = self.kkt
+        o = self.opt
+        n_trial = 0
+        del_w = del_c = del_w_prev = del_c_prev = 0.0
+        self.last_del_w = []
+        self.last_inertia = None
+        ok = self._trial_solves()
+        while not self._trial_accepted(ok):
+            if n_trial == 0:
+                del_w = o.first_hessian_perturbation if self.del_w_last == 0.0 else max(
+                    o.min_hessian_perturbation, o.perturb_dec_fact * self.del_w_last)
+            else:
+                del_w *= o.perturb_inc_fact_first if self.del_w_last == 0.0 else o.perturb_inc_fact
+                if del_w > o.max_hessian_perturbation:
+                    self.cnt["failed"] += 1
+                    return False
+            del_c = o.jacobian_regularization_value * mu ** o.jacobian_regularization_exponent
+            k.regularize_diagonal(del_w - del_w_prev, del_c - del_c_prev)
+            del_w_prev, del_c_prev = del_w, del_c
+            self.last_del_w.append(del_w)
+            self._factorize_wrapper()
+            ok = self._trial_solves()
+            n_trial += 1
+            self.cnt["regularized"] += 1
+        if del_w != 0.0:
+            self.del_w_last = del_w
         return True
 
 class HostIteratePipeline:

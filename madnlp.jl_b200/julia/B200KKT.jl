@@ -618,4 +618,70 @@ function MadNLP.update!(qn::B200DenseQuasiNewton{T}, Bk::CuMatrix{T}, sk::CuVect
     return true          # whether BFGS skipped the pair is decided on the device (b2d_qn_state)
 end
 
+# ---------------------------------------------------------------- inertia_correction_method = InertiaFree
+# mul_hess_blk! (src/IPM/factorization.jl:326-350) and curv_test (src/IPM/solver.jl:785-788) for every KKT type above, dispatched on
+# the KKT's linear solver (B200Solver / B200DenseSolver, owned here): the Hessian product (b2_spmv_symlower on hess_com, b2d_symv_lower
+# on hess), then b2_mul_hess_blk_tail, which with a result buffer also reduces the four dot products and takes the decision on the
+# device.  curv_test reads the 6-double result with one copy.  set_g_ifr! and set_aug_rhs_ifr! stay MadNLP's broadcasts on the
+# solver's own vectors; b2_set_g_ifr / b2_set_aug_rhs_ifr are their one-launch equivalents.  Like the rest of this file, NOT RUN.
+const B200SparseAugKKT{T} = MadNLP.SparseKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200Solver}
+const B200IFRKKT{T} = Union{B200SparseAugKKT{T},B200UnreducedKKT{T},B200CondensedKKT{T},B200AnyDenseKKT{T}}
+
+mutable struct IFRPlans
+    hess_spmv::Ptr{Cvoid}        # b2_spmv_plan of hess_com (C_NULL for the dense types)
+    bounds::Ptr{Cvoid}           # b2_bounds over n_tot (its curvature-test scratch is used)
+    result::CuVector{Float64}    # B2_CURV_RESULT_LEN = 6: wx't, wx'n, g'n, t't, lhs, pass
+    result_h::Vector{Float64}
+end
+const _ifr_plans = IdDict{Any,IFRPlans}()      # linear solver -> plans
+
+function ifr_plans(kkt::B200IFRKKT)
+    get!(_ifr_plans, kkt.linear_solver) do
+        sp = C_NULL
+        if !(kkt isa B200AnyDenseKKT)
+            H = kkt.hess_com
+            cp = Int32.(Array(H.colPtr) .- 1); rv = Int32.(Array(H.rowVal) .- 1)
+            h = Ref{Ptr{Cvoid}}(C_NULL)
+            check(ccall((:b2_spmv_plan_create, libb200kkt), Cint, (Int32, Int32, Ptr{Int32}, Ptr{Int32}, Ptr{Ptr{Cvoid}}),
+                        size(H, 1), size(H, 2), cp, rv, h), SymbolicException)
+            sp = h[]
+        end
+        lb = Int64.(Array(kkt.ind_lb) .- 1); ub = Int64.(Array(kkt.ind_ub) .- 1)
+        b = Ref{Ptr{Cvoid}}(C_NULL)
+        check(ccall((:b2_bounds_create, libb200kkt), Cint, (Int64, Int64, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Ptr{Cvoid}}),
+                    length(kkt.pr_diag), length(lb), length(ub), lb, ub, b), SymbolicException)
+        IFRPlans(sp, b[], CUDA.zeros(Float64, 6), zeros(Float64, 6))
+    end
+end
+
+function _hess_blk!(wx::CuVector{T}, kkt::B200IFRKKT{T}, t::CuVector{T}, n, g, tol, result) where T
+    p = ifr_plans(kkt)
+    if kkt isa B200AnyDenseKKT
+        nh = size(kkt.hess, 1)
+        check(ccall((:b2d_symv_lower, libb200kkt), Cint, (Int32, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
+                    nh, nh, pointer(kkt.hess), pointer(t), pointer(wx), one(T), zero(T), stream_ptr()), SolveException)
+    else
+        nh = size(kkt.hess_com, 1)
+        check(ccall((:b2_spmv_symlower, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
+                    p.hess_spmv, pointer(MadNLP.nzval(kkt.hess_com)), pointer(t), pointer(wx), one(T), zero(T), stream_ptr()), SolveException)
+    end
+    ptr_or_null(v) = v === nothing ? CuPtr{T}(0) : pointer(v)
+    check(ccall((:b2_mul_hess_blk_tail, libb200kkt), Cint,
+                (Ptr{Cvoid}, Int64, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T},
+                 Cdouble, CuPtr{T}, Ptr{Cvoid}),
+                p.bounds, nh, Int32(kkt isa B200UnreducedKKT), pointer(kkt.pr_diag), pointer(kkt.l_lower), pointer(kkt.l_diag),
+                pointer(kkt.u_lower), pointer(kkt.u_diag), pointer(t), pointer(wx), ptr_or_null(n), ptr_or_null(g), Float64(tol),
+                ptr_or_null(result), stream_ptr()), SolveException)
+    return wx
+end
+
+MadNLP.mul_hess_blk!(wx::CuVector{T}, kkt::B200IFRKKT{T}, t::CuVector{T}) where T = _hess_blk!(wx, kkt, t, nothing, nothing, 0.0, nothing)
+
+function MadNLP.curv_test(t::CuVector{T}, n::CuVector{T}, g::CuVector{T}, kkt::B200IFRKKT{T}, wx::CuVector{T}, inertia_free_tol) where T
+    p = ifr_plans(kkt)
+    _hess_blk!(wx, kkt, t, n, g, inertia_free_tol, p.result)
+    copyto!(p.result_h, p.result)                  # the one synchronising read of the test
+    return p.result_h[6] == 1.0
+end
+
 end # module

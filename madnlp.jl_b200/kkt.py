@@ -201,6 +201,38 @@ class _KKTBase:
     def _initialize_common(self):
         self.reg.fill_(1.0); self.pr_diag.fill_(1.0); self.du_diag.zero_(); self.hess.zero_()
 
+    # ---- inertia-free regularisation (src/IPM/factorization.jl:326-350, src/IPM/solver.jl:785-788) ----
+    _unreduced = 0          # 1: mul_hess_blk! puts the barrier terms back (pr_diag holds reg only)
+    _curv = None
+
+    def _hess_mul(self, wx, t):
+        """wx[0:n_h) = Symmetric(H, :L) t[0:n_h) with the type's own product; returns n_h = size(hess, 1)"""
+        raise NotImplementedError
+
+    def _hess_blk(self, wx, t, n=None, g=None, tol=0.0, result=None):
+        for v in (wx, t) + ((n, g) if result is not None else ()):
+            if v.numel() != self._n_tot:
+                raise ValueError(f"mul_hess_blk: vectors must have n_tot = {self._n_tot} entries, got {v.numel()}")
+        n_h = self._hess_mul(wx, t)
+        check(lib.b2_mul_hess_blk_tail(self._bounds.h, n_h, self._unreduced, ptr(self.pr_diag), ptr(self.l_lower), ptr(self.l_diag),
+                                       ptr(self.u_lower), ptr(self.u_diag), ptr(t), ptr(wx), ptr(n), ptr(g), float(tol), ptr(result),
+                                       _sp(self.stream)))
+
+    def mul_hess_blk(self, wx, t):
+        """mul_hess_blk!(wx, kkt, t): wx = [Symmetric(H, :L) t[0:n_h) | 0] + t .* pr_diag (the unreduced system also subtracts
+        t .* l_lower ./ l_diag on ind_lb, then the same on ind_ub); wx, t of length n_tot.  Two launches, no synchronisation."""
+        self._hess_blk(wx, t)
+        return wx
+
+    def curv_test(self, t, n, g, wx, tol=0.0):
+        """curv_test(t, n, g, kkt, wx, inertia_free_tol): mul_hess_blk!(wx, kkt, t), then
+        dot(wx,t) + max(dot(wx,n) - dot(g,n), 0) - tol dot(t,t) >= 0.  Returns the device result (capi.CURV_* layout: the four
+        dots, lhs, pass as 1.0 / 0.0) without synchronising; the tensor is reused by the next call."""
+        if self._curv is None:
+            self._curv = _dz(capi.CURV_RESULT_LEN)
+        self._hess_blk(wx, t, n, g, tol, self._curv)
+        return self._curv
+
 
 # ======================================================================================================
 class _SparseKKTBase(_KKTBase):
@@ -308,6 +340,10 @@ class _SparseKKTBase(_KKTBase):
     def _mul_lowrank(self, w, x, alpha):
         pass
 
+    def _hess_mul(self, wx, t):
+        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        return self.hess_com.n
+
     def jtprod(self, y, x):
         """Sparse/utils.jl:28-30."""
         check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
@@ -321,7 +357,8 @@ class SparseKKTSystem(_SparseKKTBase):
     pattern is ignored), `quasi_newton` the device L-BFGS state.  The low-rank part enters by Sherman-Morrison-Woodbury:
     factorize_kkt() also solves C H = E for the 2 max_history columns of E = [U V] and factors T = P + E'H; solve_kkt then applies
     w -= H T^{-1} E'w after the sparse solve, and mul adds the low-rank product.  H is computed once per factorisation and reused
-    by every refinement step (the reference recomputes it in each solve_kkt!, with identical values)."""
+    by every refinement step (the reference recomputes it in each solve_kkt!, with identical values).  mul_hess_blk (the
+    inertia-free curvature test) uses hess_com alone, i.e. sigma I without the low-rank term, as the reference does."""
 
     def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None, hessian_approximation=ExactHessian,
                  qn_options=None):
@@ -372,6 +409,7 @@ class SparseUnreducedKKTSystem(_SparseKKTBase):
     Each bound row holds l_diag = xl - x (< 0) on the diagonal and sqrt(zl) in its variable's column; the analysis eliminates it
     just before that variable (kkt_n_dual), so it contributes the reduced system's barrier term -zl / l_diag to that pivot.
     Inertia at a correct iterate: (n_tot, 0, m + nlb + nub).  Quasi-Newton is not supported (factorization.jl:170-173)."""
+    _unreduced = 1
 
     def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
         self._build(cb, linear_solver, opt_linear_solver, unreduced=True)
@@ -508,6 +546,10 @@ class SparseCondensedKKTSystem(_KKTBase):
                                             float(alpha), float(beta), ptr(x.values), ptr(w.values), ptr(norm_out), _sp(self.stream)))
         return w
 
+    def _hess_mul(self, wx, t):
+        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        return self.n
+
     def jtprod(self, y, x):
         """condensed.jl:150-156."""
         check(lib.b2_spmv_n(self._jt_spmv.h, ptr(self.jt_csc.nzval), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
@@ -561,6 +603,10 @@ class _DenseKKTBase(_KKTBase):
                               ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta),
                               ptr(x.values), ptr(w.values), _sp(self.stream)))
         return w
+
+    def _hess_mul(self, wx, t):
+        check(lib.b2d_symv_lower(self.n, self.n, ptr(self.hess), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        return self.n
 
     def jtprod(self, y, x):
         """src/KKT/Dense/utils.jl:12-23: y[1:n] = jac' x ; y[n + k] = -x[ind_ineq[k]] (not on the per-iteration solve path)."""

@@ -385,6 +385,19 @@ def ipm_iterates(model: ACOPF, st: NLPStructure, n_iter: int, seed: int = 0, y_s
     return out
 
 
+def ifr_inputs(n_tot: int, m: int, ind_lb, ind_ub, l_diag, u_diag, seed: int = 0):
+    """The solver vectors the inertia-free test reads besides the KKT system (set_g_ifr!, set_aug_rhs_ifr!), consistent with an
+    iterate's bound distances: x standard normal, xl = x + l_diag on ind_lb (l_diag = xl - x), xu = x - u_diag on ind_ub
+    (u_diag = x - xu), +-Inf elsewhere; f and jacl standard normal (n_tot), c = 0.01 standard normal (m).  Its own RNG stream."""
+    rng = np.random.default_rng(seed)
+    x = rng.standard_normal(n_tot)
+    xl = np.full(n_tot, -np.inf); xu = np.full(n_tot, np.inf)
+    ind_lb = np.asarray(ind_lb, dtype=np.int64); ind_ub = np.asarray(ind_ub, dtype=np.int64)
+    xl[ind_lb] = x[ind_lb] + np.asarray(l_diag)
+    xu[ind_ub] = x[ind_ub] - np.asarray(u_diag)
+    return dict(f=rng.standard_normal(n_tot), x=x, xl=xl, xu=xu, jacl=rng.standard_normal(n_tot), c=0.01 * rng.standard_normal(m))
+
+
 def acopf_case(name: str = "case10000_goc", seed: int = 0, relax_equality: bool = True):
     nbus, nbranch, ngen = PGLIB_COUNTS[name]
     net = synthetic_network(nbus, nbranch, ngen, seed)
