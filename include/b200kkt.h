@@ -353,7 +353,8 @@ int b2_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const double* du_dia
               const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
               double alpha, double beta, const double* x_d, double* w_d, void* stream);
 
-/* solve_kkt!(::SparseCondensedKKTSystem) pre/post stages around b2_solve (IPM/factorization.jl:143-167), n = nvar, m = ncon:
+/* solve_kkt!(::SparseCondensedKKTSystem) pre/post stages around b2_solve (IPM/factorization.jl:143-167), n = nvar, m = ncon,
+ * pre in two launches, post in one:
  *   pre : reduce_rhs!; buffer = D.*(wz + ws./Ss); wx += Jt*buffer
  *   post: buffer2 = Jt'*wx; wz = -buffer + D.*buffer2; ws = (ws+wz)./Ss; finish_aug_solve! */
 int b2_condensed_solve_pre(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m,
@@ -363,6 +364,19 @@ int b2_condensed_solve_post(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m
                             const double* jt_nz_d, const double* pr_diag_d, const double* diag_buffer_d,
                             const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
                             const double* buffer_d, double* w_d, void* stream);
+/* One Richardson step (src/LinearSolvers/backsolve.jl:45-52) of the condensed system in five launches:
+ *   b2_condensed_refine_pre        (= b2_condensed_solve_pre; also norms_d[0] = norms_d[1] = 0)
+ *   b2_solve on w[0:n)
+ *   b2_condensed_solve_post_update (= b2_condensed_solve_post; also x += w and norms_d[1] = ||x||_inf)
+ *   b2_condensed_kkt_mul_norm_y    with alpha = -1, beta = 1, y = b: w = b - K x, norms_d[0] = ||w||_inf
+ * bit-identical to solve_pre -> b2_solve -> solve_post -> b2_richardson_update -> b2_condensed_kkt_mul_norm */
+int b2_condensed_refine_pre(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m,
+                            const double* jt_nz_d, const double* pr_diag_d, const double* diag_buffer_d,
+                            const double* l_diag_d, const double* u_diag_d, double* buffer_d, double* w_d, double* norms_d, void* stream);
+int b2_condensed_solve_post_update(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m,
+                                   const double* jt_nz_d, const double* pr_diag_d, const double* diag_buffer_d,
+                                   const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
+                                   const double* buffer_d, double* w_d, double* x_d, double* norms_d, void* stream);
 /* mul!(w, ::SparseCondensedKKTSystem, x, alpha, beta)  (IPM/factorization.jl:303-324) incl. _kktmul! */
 int b2_condensed_kkt_mul(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
                          const double* hess_nz_d, const double* jt_nz_d,
@@ -376,6 +390,12 @@ int b2_condensed_kkt_mul_norm(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt
                          const double* reg_d, const double* du_diag_d, const double* l_lower_d, const double* u_lower_d,
                          const double* l_diag_d, const double* u_diag_d, double alpha, double beta,
                          const double* x_d, double* w_d, double* norm_inf_d, void* stream);
+/* the same with the beta term read from y (a vector other than w): w = alpha*K*x + beta*y ; ||w||_inf into *norm_inf_d */
+int b2_condensed_kkt_mul_norm_y(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
+                           const double* hess_nz_d, const double* jt_nz_d,
+                           const double* reg_d, const double* du_diag_d, const double* l_lower_d, const double* u_lower_d,
+                           const double* l_diag_d, const double* u_diag_d, double alpha, double beta,
+                           const double* x_d, const double* y_d, double* w_d, double* norm_inf_d, void* stream);
 
 /* infinity norm of a device vector into a device scalar (no host sync) */
 /* start of solve_refine! (src/LinearSolvers/backsolve.jl:36-44) in one pass: *norm_b_d = ||b||_inf ; x = 0 ; w = b */

@@ -167,6 +167,9 @@ PROTOTYPES = {
     "b2_condensed_solve_post": (C.c_int, [_p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b2_condensed_kkt_mul": (C.c_int, [_p, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _f64, _f64, _p, _p, _p]),
     "b2_condensed_kkt_mul_norm": (C.c_int, [_p, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _f64, _f64, _p, _p, _p, _p]),
+    "b2_condensed_refine_pre": (C.c_int, [_p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b2_condensed_solve_post_update": (C.c_int, [_p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b2_condensed_kkt_mul_norm_y": (C.c_int, [_p, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _f64, _f64, _p, _p, _p, _p, _p]),
     "b2_get_alpha_max": (C.c_int, [_p, _p, _p, _p, _p, _f64, _p, _p]),
     "b2_get_alpha_z": (C.c_int, [_p, _p, _p, _p, _p, _f64, _p, _p]),
     "b2_get_varphi": (C.c_int, [_p, _f64, _p, _p, _p, _f64, _p, _p]),

@@ -249,24 +249,24 @@ __device__ __forceinline__ double col_dot(const int32_t* __restrict__ colptr, co
     }
     return s;
 }
-template <bool STRICT>
+template <bool STRICT, int B = GB>
 __device__ __forceinline__ double row_dot_t(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
                                             const int32_t* __restrict__ valmap, const double* __restrict__ nz,
                                             const double* __restrict__ x, int64_t i) {
     double s = 0.0;
     const int a = rowptr[i], b = rowptr[i + 1];
-    for (int q0 = a; q0 < b; q0 += GB) {
-        int ci[GB], vi[GB]; double nv[GB], xv[GB];
+    for (int q0 = a; q0 < b; q0 += B) {
+        int ci[B], vi[B]; double nv[B], xv[B];
 #pragma unroll
-        for (int u = 0; u < GB; ++u) {
+        for (int u = 0; u < B; ++u) {
             const bool ok = q0 + u < b;
             ci[u] = ok ? colidx[q0 + u] : -1; vi[u] = ok ? valmap[q0 + u] : 0;
             if (STRICT && ci[u] == (int)i) ci[u] = -1;                 // skip the diagonal entry
         }
 #pragma unroll
-        for (int u = 0; u < GB; ++u) { nv[u] = (ci[u] >= 0) ? nz[vi[u]] : 0.0; xv[u] = (ci[u] >= 0) ? x[ci[u]] : 0.0; }
+        for (int u = 0; u < B; ++u) { nv[u] = (ci[u] >= 0) ? nz[vi[u]] : 0.0; xv[u] = (ci[u] >= 0) ? x[ci[u]] : 0.0; }
 #pragma unroll
-        for (int u = 0; u < GB; ++u) if (ci[u] >= 0) s = fma(nv[u], xv[u], s);
+        for (int u = 0; u < B; ++u) if (ci[u] >= 0) s = fma(nv[u], xv[u], s);
     }
     return s;
 }
@@ -382,63 +382,156 @@ extern "C" int b2_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const dou
 // ---------------------------------------------------------------------------------------------------------
 // solve_kkt!(::SparseCondensedKKTSystem) pre / post  (IPM/factorization.jl:143-167)
 // ---------------------------------------------------------------------------------------------------------
-__global__ void k_cond_pre1(int64_t n, int64_t m, int64_t nlb, const int32_t* __restrict__ lbpos, const int32_t* __restrict__ ubpos,
-                            const double* __restrict__ ld, const double* __restrict__ ud, const double* __restrict__ pr,
-                            const double* __restrict__ D, double* __restrict__ buffer, double* __restrict__ w) {
+__device__ __forceinline__ void norm_inf_commit(double mx, unsigned long long* out) {   // NaN-propagating max of non-negative doubles
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const double t = __shfl_xor_sync(0xffffffffu, mx, o); if (t > mx || t != t) mx = t; }
+    if ((threadIdx.x & 31) == 0) atomicMax(out, (unsigned long long)__double_as_longlong(mx));
+}
+
+struct CondArgs {
+    int64_t n, m, nlb;
+    const int32_t *lbpos, *ubpos;
+    const double *ld, *ud, *pr, *D;        // l_diag, u_diag, pr_diag, diag_buffer
+};
+// pre, two launches.  The row products of the second need every buffer entry; recomputing them per row from w instead costs
+// more than the launch it saves (rows of Jt hold up to 40 entries at OPF-10k, each a chain of dependent gathers).
+// pre1: reduce_rhs! (IPM/kernels.jl:182-195) on (x, s) and buffer_j = D_j (wz_j + ws_j / Ss_j).
+// `norms` (refinement variant): norms[0] = norms[1] = 0 for the atomicMax accumulations of the post and mul passes that follow.
+__global__ void k_cond_pre1(CondArgs a, double* __restrict__ buffer, double* __restrict__ w, double* __restrict__ norms) {
     pdl_sync();
-    const int64_t n_tot = n + m;
-    const double* wzl = w + n_tot + m;
-    const double* wzu = wzl + nlb;
+    if (norms && blockIdx.x == 0 && threadIdx.x == 0) { norms[0] = 0.0; norms[1] = 0.0; }
+    const int64_t n_tot = a.n + a.m;
+    const double* wzl = w + n_tot + a.m;
+    const double* wzu = wzl + a.nlb;
     GRID_STRIDE(i, n_tot) {
         double v = w[i];
-        const int p = lbpos[i], q = ubpos[i];
-        if (p >= 0) v = __dsub_rn(v, __ddiv_rn(wzl[p], ld[p]));
-        if (q >= 0) v = __dsub_rn(v, __ddiv_rn(wzu[q], ud[q]));
+        const int p = a.lbpos[i], q = a.ubpos[i];
+        if (p >= 0) v = __dsub_rn(v, __ddiv_rn(wzl[p], a.ld[p]));
+        if (q >= 0) v = __dsub_rn(v, __ddiv_rn(wzu[q], a.ud[q]));
         if (p >= 0 || q >= 0) w[i] = v;
-        if (i >= n) {
-            const int64_t j = i - n;
-            buffer[j] = D[j] * (w[n_tot + j] + v / pr[i]);
+        if (i >= a.n) {
+            const int64_t j = i - a.n;
+            buffer[j] = a.D[j] * (w[n_tot + j] + v / a.pr[i]);
         }
     }
 }
+// pre2: wx += Jt * buffer
 __global__ void k_cond_pre2(int64_t n, const int32_t* rowptr, const int32_t* colidx, const int32_t* valmap, const double* __restrict__ nz,
                             const double* __restrict__ buffer, double* w) {
     pdl_sync();
-    GRID_STRIDE(i, n) w[i] += row_dot(rowptr, colidx, valmap, nz, buffer, i);
+    GRID_STRIDE(i, n) w[i] += row_dot_t<false, 2 * GB>(rowptr, colidx, valmap, nz, buffer, i);   // Jt rows reach 40 entries
 }
-__global__ void k_cond_post1(int64_t n, int64_t m, const int32_t* colptr, const int32_t* rowval, const double* __restrict__ nz,
-                             const double* __restrict__ pr, const double* __restrict__ D, const double* __restrict__ buffer,
-                             double* w) {
+
+// post + finish_aug_solve! (IPM/kernels.jl:198-204) in one launch, one thread per constraint j (then one per primal index i):
+// constraint j writes wz_j = -buffer_j + D_j (Jt' wx)_j, ws_j = (ws_j + wz_j) / Ss_j and the bound duals of slack n + j; primal i
+// the bound duals of x_i.  Every entry has one writer and nobody writes wx, which the column gathers read.
+// UPDATE (Richardson step, backsolve.jl:45-48): also x += w and ||x||_inf -> *norm_x over every entry the thread owns.
+template <bool UPDATE>
+__global__ void k_cond_post(CondArgs a, const int32_t* __restrict__ colptr, const int32_t* __restrict__ rowval, const double* __restrict__ nz,
+                            const double* __restrict__ ll, const double* __restrict__ ul, const double* __restrict__ buffer, double* w,
+                            double* __restrict__ x, unsigned long long* norm_x) {
     pdl_sync();
-    GRID_STRIDE(j, m) {
-        const double b2v = col_dot(colptr, rowval, nz, w, j);      // (Jt' * wx)_j ; wx = w[0:n]
-        const double wz = -buffer[j] + D[j] * b2v;
-        w[n + m + j] = wz;
-        w[n + j] = (w[n + j] + wz) / pr[n + j];
+    const int64_t n = a.n, m = a.m, n_tot = n + m;
+    double* dlb = w + n_tot + m;
+    double* dub = dlb + a.nlb;
+    double mx = 0.0;
+    auto add_x = [&](int64_t t, double wt) {
+        if (UPDATE) {
+            const double xt = x[t] + wt;
+            x[t] = xt;
+            const double v = fabs(xt);
+            if (v > mx || v != v) mx = v;
+        }
+    };
+    GRID_STRIDE(t, m + n) {
+        const int64_t i = t < m ? n + t : t - m;
+        const int p = a.lbpos[i], q = a.ubpos[i];
+        double wi;
+        if (t < m) {
+            const int64_t j = t;
+            const double b2v = col_dot(colptr, rowval, nz, w, j);      // (Jt' * wx)_j ; wx = w[0:n]
+            const double wz = fma(a.D[j], b2v, -buffer[j]);
+            wi = __ddiv_rn(__dadd_rn(w[i], wz), a.pr[i]);
+            w[n_tot + j] = wz;
+            w[i] = wi;
+            add_x(n_tot + j, wz);
+        } else {
+            wi = w[i];
+        }
+        add_x(i, wi);
+        if (p >= 0) {
+            const double d = __ddiv_rn(__dadd_rn(-dlb[p], __dmul_rn(ll[p], wi)), a.ld[p]);
+            dlb[p] = d;
+            add_x(n_tot + m + p, d);
+        }
+        if (q >= 0) {
+            const double d = __ddiv_rn(__dsub_rn(dub[q], __dmul_rn(ul[q], wi)), a.ud[q]);
+            dub[q] = d;
+            add_x(n_tot + m + a.nlb + q, d);
+        }
     }
+    if (UPDATE) norm_inf_commit(mx, norm_x);
+}
+
+static CondArgs make_cond(b2_bounds* b, int64_t n, int64_t m, const double* l_diag, const double* u_diag, const double* pr,
+                          const double* D) {
+    CondArgs a;
+    a.n = n; a.m = m; a.nlb = b->nlb; a.lbpos = b->lbpos.p; a.ubpos = b->ubpos.p;
+    a.ld = l_diag; a.ud = u_diag; a.pr = pr; a.D = D;
+    return a;
+}
+static int cond_pre(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d, const double* pr_diag_d,
+                    const double* diag_buffer_d, const double* l_diag_d, const double* u_diag_d, double* buffer_d, double* w_d,
+                    double* norms_d, void* stream) {
+    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m || jt->nrow != n || jt->ncol != m) {
+        set_error(std::string(name) + ": invalid argument");
+        return B2_ERR_INVALID;
+    }
+    cudaStream_t st = as_stream(stream);
+    launch_pdl(k_cond_pre1, dim3(grid_for(n + m)), dim3(256), 0, st, make_cond(b, n, m, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d), buffer_d, w_d,
+               norms_d);
+    launch_pdl(k_cond_pre2, dim3(grid_for(n)), dim3(256), 0, st, n, jt->rowptr.p, jt->colidx.p, jt->valmap.p, jt_nz_d, buffer_d, w_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+template <bool UPDATE>
+static int cond_post(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d, const double* pr_diag_d,
+                     const double* diag_buffer_d, const double* l_lower_d, const double* u_lower_d, const double* l_diag_d,
+                     const double* u_diag_d, const double* buffer_d, double* w_d, double* x_d, double* norms_d, void* stream) {
+    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m || jt->nrow != n || jt->ncol != m || (UPDATE && (!x_d || !norms_d))) {
+        set_error(std::string(name) + ": invalid argument");
+        return B2_ERR_INVALID;
+    }
+    launch_pdl(k_cond_post<UPDATE>, dim3(grid_for(n + m)), dim3(256), 0, as_stream(stream),
+               make_cond(b, n, m, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d), jt->colptr.p, jt->rowval.p, jt_nz_d, l_lower_d, u_lower_d,
+               buffer_d, w_d, x_d, (unsigned long long*)(UPDATE ? norms_d + 1 : nullptr));
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
 }
 extern "C" int b2_condensed_solve_pre(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d,
                                       const double* pr_diag_d, const double* diag_buffer_d, const double* l_diag_d,
                                       const double* u_diag_d, double* buffer_d, double* w_d, void* stream) {
-    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m || jt->nrow != n || jt->ncol != m) {
-        set_error("b2_condensed_solve_pre: invalid argument");
-        return B2_ERR_INVALID;
-    }
-    cudaStream_t st = as_stream(stream);
-    launch_pdl(k_cond_pre1, dim3(grid_for(n + m)), dim3(256), 0, st, n, m, b->nlb, b->lbpos.p, b->ubpos.p, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d, buffer_d, w_d);
-    launch_pdl(k_cond_pre2, dim3(grid_for(n)), dim3(256), 0, st, n, jt->rowptr.p, jt->colidx.p, jt->valmap.p, jt_nz_d, buffer_d, w_d);
-    B2_CUDA(cudaGetLastError());
-    return B2_OK;
+    return cond_pre("b2_condensed_solve_pre", b, jt, n, m, jt_nz_d, pr_diag_d, diag_buffer_d, l_diag_d, u_diag_d, buffer_d, w_d, nullptr, stream);
+}
+extern "C" int b2_condensed_refine_pre(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d,
+                                       const double* pr_diag_d, const double* diag_buffer_d, const double* l_diag_d,
+                                       const double* u_diag_d, double* buffer_d, double* w_d, double* norms_d, void* stream) {
+    if (!norms_d) { set_error("b2_condensed_refine_pre: invalid argument"); return B2_ERR_INVALID; }
+    return cond_pre("b2_condensed_refine_pre", b, jt, n, m, jt_nz_d, pr_diag_d, diag_buffer_d, l_diag_d, u_diag_d, buffer_d, w_d, norms_d, stream);
 }
 extern "C" int b2_condensed_solve_post(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d,
                                        const double* pr_diag_d, const double* diag_buffer_d, const double* l_lower_d,
                                        const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
                                        const double* buffer_d, double* w_d, void* stream) {
-    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m) { set_error("b2_condensed_solve_post: invalid argument"); return B2_ERR_INVALID; }
-    cudaStream_t st = as_stream(stream);
-    if (m > 0) launch_pdl(k_cond_post1, dim3(grid_for(m)), dim3(256), 0, st, n, m, jt->colptr.p, jt->rowval.p, jt_nz_d, pr_diag_d, diag_buffer_d, buffer_d, w_d);
-    B2_CUDA(cudaGetLastError());
-    return b2_finish_aug_solve(b, m, l_lower_d, u_lower_d, l_diag_d, u_diag_d, w_d, stream);
+    return cond_post<false>("b2_condensed_solve_post", b, jt, n, m, jt_nz_d, pr_diag_d, diag_buffer_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d,
+                            buffer_d, w_d, nullptr, nullptr, stream);
+}
+extern "C" int b2_condensed_solve_post_update(b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d,
+                                              const double* pr_diag_d, const double* diag_buffer_d, const double* l_lower_d,
+                                              const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
+                                              const double* buffer_d, double* w_d, double* x_d, double* norms_d, void* stream) {
+    return cond_post<true>("b2_condensed_solve_post_update", b, jt, n, m, jt_nz_d, pr_diag_d, diag_buffer_d, l_lower_d, u_lower_d, l_diag_d,
+                           u_diag_d, buffer_d, w_d, x_d, norms_d, stream);
 }
 
 // mul!(w, ::SparseCondensedKKTSystem, x, alpha, beta) in one pass (IPM/factorization.jl:303-324 + _kktmul!)
@@ -448,22 +541,20 @@ struct CondMulArgs {
     const int32_t *j_colptr, *j_rowval, *j_rowptr, *j_colidx, *j_valmap;
     const double *h_nz, *j_nz;
 };
-__device__ __forceinline__ void norm_inf_commit(double mx, unsigned long long* out) {   // NaN-propagating max of non-negative doubles
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { const double t = __shfl_xor_sync(0xffffffffu, mx, o); if (t > mx || t != t) mx = t; }
-    if ((threadIdx.x & 31) == 0) atomicMax(out, (unsigned long long)__double_as_longlong(mx));
-}
-__global__ void k_cond_mul(CondMulArgs c, KktMulArgs a, const double* __restrict__ x, double* __restrict__ w, unsigned long long* norm_out) {
+// Y_IN: the beta term reads y instead of w (w = alpha K x + beta y), so a Richardson step needs no w = b copy before it
+template <bool Y_IN>
+__global__ void k_cond_mul(CondMulArgs c, KktMulArgs a, const double* __restrict__ x, const double* __restrict__ y, double* __restrict__ w,
+                           unsigned long long* norm_out) {
     pdl_sync();
     const int64_t n = c.n, m = c.m;
     double mx = 0.0;
     const double* xs = x + n;
     const double* xz = x + n + m;
     GRID_STRIDE(t, a.n_tot + a.m + a.nlb + a.nub) {
-        double wt = w[t];
+        double wt = Y_IN ? y[t] : w[t];
         if (t < n) {
             const double hx = col_dot(c.h_colptr, c.h_rowval, c.h_nz, x, t) + row_dot_strict(c.h_rowptr, c.h_colidx, c.h_valmap, c.h_nz, x, t);
-            const double jz = row_dot(c.j_rowptr, c.j_colidx, c.j_valmap, c.j_nz, xz, t);
+            const double jz = row_dot_t<false, 2 * GB>(c.j_rowptr, c.j_colidx, c.j_valmap, c.j_nz, xz, t);   // Jt rows reach 40 entries
             wt = a.alpha * hx + scl(a.beta, wt) + a.alpha * jz;
         } else if (t < n + m) {
             wt = scl(a.beta, wt) - a.alpha * xz[t - n];
@@ -478,10 +569,10 @@ __global__ void k_cond_mul(CondMulArgs c, KktMulArgs a, const double* __restrict
     }
     if (norm_out) norm_inf_commit(mx, norm_out);
 }
-extern "C" int b2_condensed_kkt_mul_norm(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
-                                    const double* hess_nz_d, const double* jt_nz_d, const double* reg_d, const double* du_diag_d,
-                                    const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
-                                    double alpha, double beta, const double* x_d, double* w_d, double* norm_inf_d, void* stream) {
+static int cond_mul(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m, const double* hess_nz_d, const double* jt_nz_d,
+                    const double* reg_d, const double* du_diag_d, const double* l_lower_d, const double* u_lower_d, const double* l_diag_d,
+                    const double* u_diag_d, double alpha, double beta, const double* x_d, const double* y_d, double* w_d, double* norm_inf_d,
+                    void* stream) {
     if (!b || !hess || !jt || !x_d || !w_d || b->n_tot != n + m || hess->nrow != n || jt->nrow != n || jt->ncol != m) {
         set_error("b2_condensed_kkt_mul: invalid argument");
         return B2_ERR_INVALID;
@@ -493,9 +584,26 @@ extern "C" int b2_condensed_kkt_mul_norm(b2_bounds* b, b2_spmv_plan* hess, b2_sp
     c.h_nz = hess_nz_d; c.j_nz = jt_nz_d;
     KktMulArgs a = make_kktmul(b, m, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta);
     const int64_t tot = a.n_tot + a.m + a.nlb + a.nub;
-    launch_pdl(k_cond_mul, dim3(grid_for(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, w_d, (unsigned long long*)norm_inf_d);
+    if (y_d) launch_pdl(k_cond_mul<true>, dim3(grid_for(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
+    else launch_pdl(k_cond_mul<false>, dim3(grid_for(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
+}
+extern "C" int b2_condensed_kkt_mul_norm(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
+                                    const double* hess_nz_d, const double* jt_nz_d, const double* reg_d, const double* du_diag_d,
+                                    const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
+                                    double alpha, double beta, const double* x_d, double* w_d, double* norm_inf_d, void* stream) {
+    return cond_mul(b, hess, jt, n, m, hess_nz_d, jt_nz_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta, x_d,
+                    nullptr, w_d, norm_inf_d, stream);
+}
+extern "C" int b2_condensed_kkt_mul_norm_y(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
+                                      const double* hess_nz_d, const double* jt_nz_d, const double* reg_d, const double* du_diag_d,
+                                      const double* l_lower_d, const double* u_lower_d, const double* l_diag_d, const double* u_diag_d,
+                                      double alpha, double beta, const double* x_d, const double* y_d, double* w_d, double* norm_inf_d,
+                                      void* stream) {
+    if (!y_d || y_d == w_d) { set_error("b2_condensed_kkt_mul_norm_y: invalid argument (y must be a vector other than w)"); return B2_ERR_INVALID; }
+    return cond_mul(b, hess, jt, n, m, hess_nz_d, jt_nz_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta, x_d,
+                    y_d, w_d, norm_inf_d, stream);
 }
 extern "C" int b2_condensed_kkt_mul(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t n, int64_t m,
                                     const double* hess_nz_d, const double* jt_nz_d, const double* reg_d, const double* du_diag_d,

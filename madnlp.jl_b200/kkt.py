@@ -518,32 +518,43 @@ class SparseCondensedKKTSystem(_KKTBase):
     def should_regularize_dual(self, num_pos, num_zero, num_neg):
         return True                                                    # condensed.jl:141
 
+    def _pre_args(self):
+        return (self._bounds.h, self._jt_spmv.h, self.n, self.m, ptr(self.jt_csc.nzval), ptr(self.pr_diag), ptr(self.diag_buffer))
+
+    def _post_args(self):
+        return self._pre_args() + (ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer))
+
+    def _mul_args(self):
+        return (self._bounds.h, self._hess_spmv.h, self._jt_spmv.h, self.n, self.m, ptr(self.hess_com.nzval), ptr(self.jt_csc.nzval),
+                ptr(self.reg), ptr(self.du_diag), ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag))
+
     def solve_kkt(self, w: UnreducedKKTVector):
-        """src/IPM/factorization.jl:143-167."""
+        """src/IPM/factorization.jl:143-167: pre (two launches), solve, post (one)."""
         sp = _sp(self.stream)
-        check(lib.b2_condensed_solve_pre(self._bounds.h, self._jt_spmv.h, self.n, self.m, ptr(self.jt_csc.nzval),
-                                         ptr(self.pr_diag), ptr(self.diag_buffer), ptr(self.l_diag), ptr(self.u_diag),
-                                         ptr(self.buffer), ptr(w.values), sp))
+        check(lib.b2_condensed_solve_pre(*self._pre_args(), ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(w.values), sp))
         self.linear_solver.solve_linear_system(w.values[: self.n])
-        check(lib.b2_condensed_solve_post(self._bounds.h, self._jt_spmv.h, self.n, self.m, ptr(self.jt_csc.nzval),
-                                          ptr(self.pr_diag), ptr(self.diag_buffer), ptr(self.l_lower), ptr(self.u_lower),
-                                          ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(w.values), sp))
+        check(lib.b2_condensed_solve_post(*self._post_args(), ptr(w.values), sp))
         return w
+
+    def refine_step(self, x, b, w, norms):
+        """One Richardson step (src/LinearSolvers/backsolve.jl:45-52) in five launches: solve_kkt!(w); x += w; w = b - K x;
+        norms[0] = ||w||_inf, norms[1] = ||x||_inf (device).  Same values as solve_kkt, b2_richardson_update and mul_norm."""
+        sp = _sp(self.stream)
+        check(lib.b2_condensed_refine_pre(*self._pre_args(), ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(w.values),
+                                          ptr(norms), sp))
+        self.linear_solver.solve_linear_system(w.values[: self.n])
+        check(lib.b2_condensed_solve_post_update(*self._post_args(), ptr(w.values), ptr(x.values), ptr(norms), sp))
+        check(lib.b2_condensed_kkt_mul_norm_y(*self._mul_args(), -1.0, 1.0, ptr(x.values), ptr(b.values), ptr(w.values), ptr(norms), sp))
 
     def mul(self, w, x, alpha=1.0, beta=0.0):
         """src/IPM/factorization.jl:303-324."""
-        check(lib.b2_condensed_kkt_mul(self._bounds.h, self._hess_spmv.h, self._jt_spmv.h, self.n, self.m,
-                                       ptr(self.hess_com.nzval), ptr(self.jt_csc.nzval), ptr(self.reg), ptr(self.du_diag),
-                                       ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag),
-                                       float(alpha), float(beta), ptr(x.values), ptr(w.values), _sp(self.stream)))
+        check(lib.b2_condensed_kkt_mul(*self._mul_args(), float(alpha), float(beta), ptr(x.values), ptr(w.values), _sp(self.stream)))
         return w
 
     def mul_norm(self, w, x, alpha, beta, norm_out):
         """mul! that also accumulates ||w||_inf of the result into the (zeroed) device scalar `norm_out`"""
-        check(lib.b2_condensed_kkt_mul_norm(self._bounds.h, self._hess_spmv.h, self._jt_spmv.h, self.n, self.m,
-                                            ptr(self.hess_com.nzval), ptr(self.jt_csc.nzval), ptr(self.reg), ptr(self.du_diag),
-                                            ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag),
-                                            float(alpha), float(beta), ptr(x.values), ptr(w.values), ptr(norm_out), _sp(self.stream)))
+        check(lib.b2_condensed_kkt_mul_norm(*self._mul_args(), float(alpha), float(beta), ptr(x.values), ptr(w.values), ptr(norm_out),
+                                            _sp(self.stream)))
         return w
 
     def _hess_mul(self, wx, t):

@@ -33,6 +33,9 @@ class RichardsonIterator:
     def _body(self, x, b, w):
         """solve_kkt!(w); x += w; w = b; w -= K x; norms of w and x on the device (backsolve.jl:45-52)"""
         kkt = self.kkt
+        if hasattr(kkt, "refine_step"):          # the same step fused into fewer launches (SparseCondensedKKTSystem)
+            kkt.refine_step(x, b, w, self._norms)
+            return
         stream = capi.stream_ptr(getattr(kkt, "stream", None))
         n = b.values.numel()
         kkt.solve_kkt(w)
