@@ -468,6 +468,70 @@ int b2_mul_hess_blk_tail(b2_bounds* b, int64_t n_h, int32_t unreduced, const dou
                          const double* l_diag_d, const double* u_lower_d, const double* u_diag_d, const double* t_d, double* wx_d,
                          const double* n_d, const double* g_d, double tol, double* result_d, void* stream);
 
+/* ------------------------------------------------------------------ feasibility restoration (robust!, src/IPM/solver.jl:413-540)
+ * The restorer's state (src/IPM/types.jl:1-32) and the solver vectors as device arrays: x, xl, xu, zl, zu, f, jacl, x_ref, D_R, f_R and
+ * dx of length n_tot (zl / zu FULL length, +-Inf for an absent bound; the _r views go through ind_lb / ind_ub of `b`); c, y, pp, nn,
+ * zp, zn and their steps of length m; dzl / dzu compressed (nlb / nub).  Elementwise kernels: one launch each, outputs bit-identical to
+ * the reference's broadcasts (left-to-right, no contraction, x^2 = x*x, Julia's NaN-propagating min / max).  Reductions: as the IPM
+ * reductions above (one device double at out_d, deterministic, min / max exact, sums up to association); the m-length segments
+ * follow the n_tot or bound segments.  Nothing synchronises; everything can be captured in a CUDA graph.  The reference's _RR / _R
+ * suffixes are spelled _rr / _r here (every exported symbol is lowercase). */
+/* initialize_robust_restorer! after its two norms (src/IPM/restoration.jl:45-67; the host forms mu_R = max(mu, ||c||_inf)):
+ * x_ref = x; D_R = min(1, 1 ./ |x_ref|); f_R = 0; nn by populate_RR_nn! (kernels.jl:825-829) with mu_R; pp = c + nn; zp = mu_R ./ pp;
+ * zn = mu_R ./ nn; y = 0; zl_r = min(rho, zl_r); zu_r = min(rho, zu_r) */
+int b2_rr_init(b2_bounds* b, int64_t m, const double* x_d, const double* c_d, double mu_R, double rho, double* x_ref_d, double* D_R_d,
+               double* f_R_d, double* pp_d, double* nn_d, double* zp_d, double* zn_d, double* y_d, double* zl_d, double* zu_d, void* stream);
+/* set_aug_RR! (kernels.jl:72-84) before the KKT type's own _set_aug_diagonal!: reg = del_w + zeta D_R^2 (n_tot);
+ * du_diag = -del_c - pp ./ zp - nn ./ zn (m); l_lower = zl_r, l_diag = xl_r - x_lr (nlb); u_lower = zu_r, u_diag = x_ur - xu_r (nub).
+ * del_w / del_c: default_primal_regularization / default_dual_regularization */
+int b2_set_aug_rr(b2_bounds* b, int64_t m, double del_w, double del_c, double zeta, const double* D_R_d, const double* pp_d,
+                  const double* nn_d, const double* zp_d, const double* zn_d, const double* x_d, const double* xl_d, const double* xu_d,
+                  const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d, double* u_lower_d,
+                  double* l_diag_d, double* u_diag_d, void* stream);
+/* set_aug_rhs_RR! (:133-158): p = [ -f_R + zl - zu - jacl | -c + pp - nn + (mu_R - (rho - y) pp) ./ zp - (mu_R - (rho + y) nn) ./ zn |
+ *                                  (xl_r - x_lr) zl_r + mu_R | (xu_r - x_ur) zu_r - mu_R ] */
+int b2_set_aug_rhs_rr(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d,
+                      const double* zu_d, const double* jacl_d, const double* f_R_d, const double* c_d, const double* y_d, const double* pp_d,
+                      const double* nn_d, const double* zp_d, const double* zn_d, double mu_R, double rho, double* p_d, void* stream);
+/* finish_aug_solve_RR! (:251-257) with l = y, dl = dual(d): dzp = rho - l - dl - zp; dzn = rho + l + dl - zn;
+ * dpp = -pp + mu_R ./ zp - (pp ./ zp) dzp; dnn = -nn + mu_R ./ zn - (nn ./ zn) dzn */
+int b2_finish_aug_solve_rr(int64_t m, const double* l_d, const double* dl_d, const double* pp_d, const double* nn_d, const double* zp_d,
+                           const double* zn_d, double mu_R, double rho, double* dpp_d, double* dnn_d, double* dzp_d, double* dzn_d,
+                           void* stream);
+/* set_f_RR! (:106-110): f_R = zeta D_R^2 (x - x_ref) over n entries */
+int b2_set_f_rr(int64_t n, double zeta, const double* D_R_d, const double* x_d, const double* x_ref_d, double* f_R_d, void* stream);
+/* reset_bound_dual! (:775-800).  One-vector form (zp with pp, zn with nn): z = max(min(z, (ks mu) ./ x), (mu / ks) ./ x) over n.
+ * Two-vector form on the bounded entries: zl_r with x_lr - xl_r and zu_r with xu_r - x_ur, one launch; the other entries of zl / zu
+ * are left as they are (the reference maps them too: a zero multiplier against an infinite bound stays zero) */
+int b2_reset_bound_dual(int64_t n, double* z_d, const double* x_d, double mu, double kappa_sigma, void* stream);
+int b2_reset_bound_dual_lu(b2_bounds* b, double* zl_d, double* zu_d, const double* x_d, const double* xl_d, const double* xu_d, double mu,
+                           double kappa_sigma, void* stream);
+/* adjust_boundary! (:656-673): with c1 = eps mu, c2 = eps^(3/4): xl_r = x_lr - xl_r < c1 ? xl_r - c2 max(1, |x_lr|) : xl_r, and
+ * xu_r = xu_r - x_ur < c1 ? xu_r + c2 max(1, |x_ur|) : xu_r */
+int b2_adjust_boundary(b2_bounds* b, const double* x_d, double* xl_d, double* xu_d, double mu, void* stream);
+/* the restoration line search's reductions (kernels.jl:390-636) and get_theta (:409, ||c||_1 over m; ||c||_inf is b2_norm_inf) */
+int b2_get_theta(b2_bounds* b, int64_t m, const double* c_d, double* out_d, void* stream);
+int b2_get_theta_r(b2_bounds* b, int64_t m, const double* c_d, const double* pp_d, const double* nn_d, double* out_d, void* stream);  /* :411-421 */
+int b2_get_inf_pr_r(b2_bounds* b, int64_t m, const double* c_d, const double* pp_d, const double* nn_d, double* out_d, void* stream); /* :423-433 */
+int b2_get_obj_val_r(b2_bounds* b, int64_t m, const double* pp_d, const double* nn_d, const double* D_R_d, const double* x_d,
+                     const double* x_ref_d, double rho, double zeta, double* out_d, void* stream);                         /* :390-407 */
+int b2_get_inf_du_r(b2_bounds* b, int64_t m, const double* f_R_d, const double* l_d, const double* zl_d, const double* zu_d,
+                    const double* jacl_d, const double* zp_d, const double* zn_d, double rho, double sd, double* out_d, void* stream); /* :435-454 */
+int b2_get_inf_compl_r(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d,
+                       const double* zu_d, const double* pp_d, const double* zp_d, const double* nn_d, const double* zn_d, double mu_R,
+                       double sc, double* out_d, void* stream);                                                          /* :456-484 */
+int b2_get_alpha_max_r(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* dx_d,
+                       const double* pp_d, const double* dpp_d, const double* nn_d, const double* dnn_d, double tau_R, double* out_d,
+                       void* stream);                                                                                    /* :486-515 */
+int b2_get_alpha_z_r(b2_bounds* b, int64_t m, const double* zl_d, const double* zu_d, const double* dzl_d, const double* dzu_d,
+                     const double* zp_d, const double* dzp_d, const double* zn_d, const double* dzn_d, double tau_R, double* out_d,
+                     void* stream);                                                                                      /* :517-542 */
+int b2_get_varphi_r(b2_bounds* b, int64_t m, double obj_val, const double* x_d, const double* xl_d, const double* xu_d, const double* pp_d,
+                    const double* nn_d, double mu_R, double* out_d, void* stream);                                       /* :544-570 */
+int b2_get_varphi_d_r(b2_bounds* b, int64_t m, const double* f_R_d, const double* x_d, const double* xl_d, const double* xu_d,
+                      const double* dx_d, const double* pp_d, const double* nn_d, const double* dpp_d, const double* dnn_d, double mu_R,
+                      double rho, double* out_d, void* stream);                                                          /* :612-636 */
+
 /* ------------------------------------------------------------------ compact L-BFGS (SparseKKTSystem, hessian_approximation = CompactLBFGS)
  * src/quasi_newton.jl:212-437 and src/IPM/factorization.jl:76-139, 253-276.  B_k = sigma I - U U' + V V' on the n model variables
  * (no slacks); S, Y are n x max_history, the memory p <= max_history.  max_history is limited to 32, so that

@@ -185,6 +185,24 @@ PROTOTYPES = {
     "b2_set_g_ifr": (C.c_int, [_i64, _p, _p, _p, _p, _p, _f64, _p, _p]),
     "b2_set_aug_rhs_ifr": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p]),
     "b2_mul_hess_blk_tail": (C.c_int, [_p, _i64, _i32] + [_p] * 9 + [_f64, _p, _p]),
+    "b2_rr_init": (C.c_int, [_p, _i64, _p, _p, _f64, _f64] + [_p] * 10 + [_p]),
+    "b2_set_aug_rr": (C.c_int, [_p, _i64, _f64, _f64, _f64] + [_p] * 16 + [_p]),
+    "b2_set_aug_rhs_rr": (C.c_int, [_p, _i64] + [_p] * 13 + [_f64, _f64, _p, _p]),
+    "b2_finish_aug_solve_rr": (C.c_int, [_i64] + [_p] * 6 + [_f64, _f64] + [_p] * 4 + [_p]),
+    "b2_set_f_rr": (C.c_int, [_i64, _f64, _p, _p, _p, _p, _p]),
+    "b2_reset_bound_dual": (C.c_int, [_i64, _p, _p, _f64, _f64, _p]),
+    "b2_reset_bound_dual_lu": (C.c_int, [_p] + [_p] * 5 + [_f64, _f64, _p]),
+    "b2_adjust_boundary": (C.c_int, [_p, _p, _p, _p, _f64, _p]),
+    "b2_get_theta": (C.c_int, [_p, _i64, _p, _p, _p]),
+    "b2_get_theta_r": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
+    "b2_get_inf_pr_r": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
+    "b2_get_obj_val_r": (C.c_int, [_p, _i64] + [_p] * 5 + [_f64, _f64, _p, _p]),
+    "b2_get_inf_du_r": (C.c_int, [_p, _i64] + [_p] * 7 + [_f64, _f64, _p, _p]),
+    "b2_get_inf_compl_r": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _p, _p]),
+    "b2_get_alpha_max_r": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64, _p, _p]),
+    "b2_get_alpha_z_r": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64, _p, _p]),
+    "b2_get_varphi_r": (C.c_int, [_p, _i64, _f64] + [_p] * 5 + [_f64, _p, _p]),
+    "b2_get_varphi_d_r": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _p, _p]),
     "b2_richardson_begin": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_richardson_update": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_copy_many": (C.c_int, [_i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(_i64), _p]),

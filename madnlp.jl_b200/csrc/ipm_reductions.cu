@@ -163,6 +163,121 @@ struct ScaleSum {
     }
 };
 
+// ---- the restoration phase (robust!, src/IPM/solver.jl:413-540; kernels.jl:390-636).  Every term is written with __d*_rn in the
+// reference's left-to-right order (no contraction), so min / max results are exact and sums differ from the scalar loops only by
+// association.  The m-length segments (pp, nn, zp, zn, y) follow the n_tot or bound segments in the term index.
+__device__ __forceinline__ double dmax(double a, double b) { return comb<R_MAX>(a, b); }
+
+// get_theta (:409): ||c||_1
+struct Theta {
+    const double* c;
+    __device__ double term(int64_t i) const { return fabs(c[i]); }
+    __device__ double finish(double r) const { return r; }
+};
+// get_theta_R (:411-421) as a sum, get_inf_pr_R (:423-433) as a max: |c - p + n|
+struct ThetaR {
+    const double *c, *p, *nn;
+    __device__ double term(int64_t i) const { return fabs(__dadd_rn(__dsub_rn(c[i], p[i]), nn[i])); }
+    __device__ double finish(double r) const { return r; }
+};
+// get_obj_val_R (:390-407): [n_tot: zeta/2 D_R^2 (x - x_ref)^2 | m: rho (p + n)]
+struct ObjValR {
+    int64_t n_tot; const double *p, *nn, *D, *x, *xr; double rho, zeta;
+    __device__ double term(int64_t i) const {
+        if (i < n_tot) {
+            const double d = D[i], e = __dsub_rn(x[i], xr[i]);
+            return __dmul_rn(__dmul_rn(__ddiv_rn(zeta, 2.0), __dmul_rn(d, d)), __dmul_rn(e, e));
+        }
+        const int64_t j = i - n_tot;
+        return __dmul_rn(rho, __dadd_rn(p[j], nn[j]));
+    }
+    __device__ double finish(double r) const { return r; }
+};
+// get_inf_du_R (:435-454): [n_tot: |f_R - zl + zu + jacl| | m: max(|rho - l - zp|, |rho + l - zn|)] / sd
+struct InfDuR {
+    int64_t n_tot; const double *f, *zl, *zu, *jacl, *l, *zp, *zn; double rho, sd;
+    __device__ double term(int64_t i) const {
+        if (i < n_tot) return fabs(__dadd_rn(__dadd_rn(__dsub_rn(f[i], zl[i]), zu[i]), jacl[i]));
+        const int64_t j = i - n_tot;
+        const double lj = l[j];
+        return dmax(fabs(__dsub_rn(__dsub_rn(rho, lj), zp[j])), fabs(__dsub_rn(__dadd_rn(rho, lj), zn[j])));
+    }
+    __device__ double finish(double r) const { return r / sd; }
+};
+// get_inf_compl_R (:456-484): [nlb: |(x_lr - xl_r) zl_r - mu| | nub: |(xu_r - x_ur) zu_r - mu| | m: |pp zp - mu| | m: |nn zn - mu|] / sc
+struct InfComplR {
+    const int64_t *ind_lb, *ind_ub; int64_t nlb, nub, m; const double *x, *xl, *xu, *zl, *zu, *pp, *zp, *nn, *zn; double mu, sc;
+    __device__ double term(int64_t i) const {
+        double v;
+        if (i < nlb) { const int64_t k = ind_lb[i]; v = __dmul_rn(__dsub_rn(x[k], xl[k]), zl[k]); }
+        else if (i < nlb + nub) { const int64_t k = ind_ub[i - nlb]; v = __dmul_rn(__dsub_rn(xu[k], x[k]), zu[k]); }
+        else if (i < nlb + nub + m) { const int64_t j = i - nlb - nub; v = __dmul_rn(pp[j], zp[j]); }
+        else { const int64_t j = i - nlb - nub - m; v = __dmul_rn(nn[j], zn[j]); }
+        return fabs(__dsub_rn(v, mu));
+    }
+    __device__ double finish(double r) const { return r / sc; }
+};
+// the step-length term of a positive variable: d < 0 ? -v tau / d : Inf
+__device__ __forceinline__ double step_to_zero(double v, double d, double tau) {
+    return d < 0.0 ? __ddiv_rn(__dmul_rn(-v, tau), d) : dinf();
+}
+// get_alpha_max_R (:486-515): [n_tot: (bound - x) tau / dx toward the bound dx points to, Inf for dx = 0 | m: pp | m: nn]
+struct AlphaMaxR {
+    int64_t n_tot, m; const double *x, *xl, *xu, *dx, *pp, *dpp, *nn, *dnn; double tau;
+    __device__ double term(int64_t i) const {
+        if (i < n_tot) {
+            const double d = dx[i];
+            if (d < 0.0) return __ddiv_rn(__dmul_rn(__dadd_rn(-x[i], xl[i]), tau), d);
+            if (d > 0.0) return __ddiv_rn(__dmul_rn(__dadd_rn(-x[i], xu[i]), tau), d);
+            return dinf();
+        }
+        if (i < n_tot + m) { const int64_t j = i - n_tot; return step_to_zero(pp[j], dpp[j], tau); }
+        const int64_t j = i - n_tot - m;
+        return step_to_zero(nn[j], dnn[j], tau);
+    }
+    __device__ double finish(double r) const { return r; }
+};
+// get_alpha_z_R (:517-542): [nlb: zl_r | nub: zu_r | m: zp | m: zn]
+struct AlphaZR {
+    const int64_t *ind_lb, *ind_ub; int64_t nlb, nub, m; const double *zl, *zu, *dzl, *dzu, *zp, *dzp, *zn, *dzn; double tau;
+    __device__ double term(int64_t i) const {
+        if (i < nlb) return step_to_zero(zl[ind_lb[i]], dzl[i], tau);
+        if (i < nlb + nub) { const int64_t j = i - nlb; return step_to_zero(zu[ind_ub[j]], dzu[j], tau); }
+        if (i < nlb + nub + m) { const int64_t j = i - nlb - nub; return step_to_zero(zp[j], dzp[j], tau); }
+        const int64_t j = i - nlb - nub - m;
+        return step_to_zero(zn[j], dzn[j], tau);
+    }
+    __device__ double finish(double r) const { return r; }
+};
+// get_varphi_R (:544-570): obj_val minus, over [nlb: x_lr - xl_r | nub: xu_r - x_ur | m: pp | m: nn], (d < 0 ? Inf : mu log d)
+struct VarphiR {
+    const int64_t *ind_lb, *ind_ub; int64_t nlb, nub, m; const double *x, *xl, *xu, *pp, *nn; double mu, obj_val;
+    __device__ double term(int64_t i) const {
+        double d;
+        if (i < nlb) { const int64_t k = ind_lb[i]; d = __dsub_rn(x[k], xl[k]); }
+        else if (i < nlb + nub) { const int64_t k = ind_ub[i - nlb]; d = __dsub_rn(xu[k], x[k]); }
+        else if (i < nlb + nub + m) d = pp[i - nlb - nub];
+        else d = nn[i - nlb - nub - m];
+        return d < 0.0 ? -dinf() : -__dmul_rn(mu, log(d));
+    }
+    __device__ double finish(double r) const { return obj_val + r; }
+};
+// get_varphi_d_R (:612-636): [n_tot: (f_R - mu / (x - xl) + mu / (xu - x)) dx | m: (rho - mu / pp) dpp | m: (rho - mu / nn) dnn]
+struct VarphiDR {
+    int64_t n_tot, m; const double *f, *x, *xl, *xu, *dx, *pp, *nn, *dpp, *dnn; double mu, rho;
+    __device__ double term(int64_t i) const {
+        if (i < n_tot) {
+            const double xi = x[i];
+            const double g = __dadd_rn(__dsub_rn(f[i], __ddiv_rn(mu, __dsub_rn(xi, xl[i]))), __ddiv_rn(mu, __dsub_rn(xu[i], xi)));
+            return __dmul_rn(g, dx[i]);
+        }
+        if (i < n_tot + m) { const int64_t j = i - n_tot; return __dmul_rn(__dsub_rn(rho, __ddiv_rn(mu, pp[j])), dpp[j]); }
+        const int64_t j = i - n_tot - m;
+        return __dmul_rn(__dsub_rn(rho, __ddiv_rn(mu, nn[j])), dnn[j]);
+    }
+    __device__ double finish(double r) const { return r; }
+};
+
 // ---- set_aug_rhs! (:113-130): px = -f + zl - zu - jacl ; py = -c ; pzl = (xl_r - x_lr) zl_r + mu ; pzu = (xu_r - x_ur) zu_r - mu
 __global__ void k_set_aug_rhs(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const int64_t* __restrict__ ind_lb,
                               const int64_t* __restrict__ ind_ub, const double* __restrict__ x, const double* __restrict__ xl,
@@ -272,6 +387,80 @@ int b2_set_aug_rhs(b2_bounds* b, int64_t m, const double* x_d, const double* xl_
                                x_d, xl_d, xu_d, f_d, zl_d, zu_d, jacl_d, c_d, mu, p_d);
     if (e != cudaSuccess) return cuda_fail(e, "b2_set_aug_rhs", __FILE__, __LINE__);
     return B2_OK;
+}
+
+// ---- the restoration phase
+int b2_get_theta(b2_bounds* b, int64_t m, const double* c_d, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (m == 0 || c_d), "b2_get_theta");
+    return run_reduce<R_SUM>(b, m, Theta{c_d}, 0.0, out_d, stream, "b2_get_theta");
+}
+
+int b2_get_theta_r(b2_bounds* b, int64_t m, const double* c_d, const double* pp_d, const double* nn_d, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (m == 0 || (c_d && pp_d && nn_d)), "b2_get_theta_r");
+    return run_reduce<R_SUM>(b, m, ThetaR{c_d, pp_d, nn_d}, 0.0, out_d, stream, "b2_get_theta_r");
+}
+
+int b2_get_inf_pr_r(b2_bounds* b, int64_t m, const double* c_d, const double* pp_d, const double* nn_d, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (m == 0 || (c_d && pp_d && nn_d)), "b2_get_inf_pr_r");
+    return run_reduce<R_MAX>(b, m, ThetaR{c_d, pp_d, nn_d}, 0.0, out_d, stream, "b2_get_inf_pr_r");
+}
+
+int b2_get_obj_val_r(b2_bounds* b, int64_t m, const double* pp_d, const double* nn_d, const double* D_R_d, const double* x_d,
+                     const double* x_ref_d, double rho, double zeta, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (m == 0 || (pp_d && nn_d)) && (b->n_tot == 0 || (D_R_d && x_d && x_ref_d)), "b2_get_obj_val_r");
+    ObjValR f{b->n_tot, pp_d, nn_d, D_R_d, x_d, x_ref_d, rho, zeta};
+    return run_reduce<R_SUM>(b, b->n_tot + m, f, 0.0, out_d, stream, "b2_get_obj_val_r");
+}
+
+int b2_get_inf_du_r(b2_bounds* b, int64_t m, const double* f_R_d, const double* l_d, const double* zl_d, const double* zu_d,
+                    const double* jacl_d, const double* zp_d, const double* zn_d, double rho, double sd, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (b->n_tot == 0 || (f_R_d && zl_d && zu_d && jacl_d)) && (m == 0 || (l_d && zp_d && zn_d)), "b2_get_inf_du_r");
+    InfDuR f{b->n_tot, f_R_d, zl_d, zu_d, jacl_d, l_d, zp_d, zn_d, rho, sd};
+    return run_reduce<R_MAX>(b, b->n_tot + m, f, 0.0, out_d, stream, "b2_get_inf_du_r");
+}
+
+int b2_get_inf_compl_r(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d,
+                       const double* zu_d, const double* pp_d, const double* zp_d, const double* nn_d, const double* zn_d, double mu_R,
+                       double sc, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (b->nlb + b->nub == 0 || x_d) && (b->nlb == 0 || (xl_d && zl_d)) && (b->nub == 0 || (xu_d && zu_d)) &&
+                (m == 0 || (pp_d && zp_d && nn_d && zn_d)), "b2_get_inf_compl_r");
+    InfComplR f{b->ind_lb.p, b->ind_ub.p, b->nlb, b->nub, m, x_d, xl_d, xu_d, zl_d, zu_d, pp_d, zp_d, nn_d, zn_d, mu_R, sc};
+    return run_reduce<R_MAX>(b, b->nlb + b->nub + 2 * m, f, 0.0, out_d, stream, "b2_get_inf_compl_r");
+}
+
+int b2_get_alpha_max_r(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* dx_d,
+                       const double* pp_d, const double* dpp_d, const double* nn_d, const double* dnn_d, double tau_R, double* out_d,
+                       void* stream) {
+    B2_NEED(b && m >= 0 && (b->n_tot == 0 || (x_d && xl_d && xu_d && dx_d)) && (m == 0 || (pp_d && dpp_d && nn_d && dnn_d)),
+            "b2_get_alpha_max_r");
+    AlphaMaxR f{b->n_tot, m, x_d, xl_d, xu_d, dx_d, pp_d, dpp_d, nn_d, dnn_d, tau_R};
+    return run_reduce<R_MIN>(b, b->n_tot + 2 * m, f, 1.0, out_d, stream, "b2_get_alpha_max_r");
+}
+
+int b2_get_alpha_z_r(b2_bounds* b, int64_t m, const double* zl_d, const double* zu_d, const double* dzl_d, const double* dzu_d,
+                     const double* zp_d, const double* dzp_d, const double* zn_d, const double* dzn_d, double tau_R, double* out_d,
+                     void* stream) {
+    B2_NEED(b && m >= 0 && (b->nlb == 0 || (zl_d && dzl_d)) && (b->nub == 0 || (zu_d && dzu_d)) &&
+                (m == 0 || (zp_d && dzp_d && zn_d && dzn_d)), "b2_get_alpha_z_r");
+    AlphaZR f{b->ind_lb.p, b->ind_ub.p, b->nlb, b->nub, m, zl_d, zu_d, dzl_d, dzu_d, zp_d, dzp_d, zn_d, dzn_d, tau_R};
+    return run_reduce<R_MIN>(b, b->nlb + b->nub + 2 * m, f, 1.0, out_d, stream, "b2_get_alpha_z_r");
+}
+
+int b2_get_varphi_r(b2_bounds* b, int64_t m, double obj_val, const double* x_d, const double* xl_d, const double* xu_d, const double* pp_d,
+                    const double* nn_d, double mu_R, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (b->nlb + b->nub == 0 || x_d) && (b->nlb == 0 || xl_d) && (b->nub == 0 || xu_d) && (m == 0 || (pp_d && nn_d)),
+            "b2_get_varphi_r");
+    VarphiR f{b->ind_lb.p, b->ind_ub.p, b->nlb, b->nub, m, x_d, xl_d, xu_d, pp_d, nn_d, mu_R, obj_val};
+    return run_reduce<R_SUM>(b, b->nlb + b->nub + 2 * m, f, 0.0, out_d, stream, "b2_get_varphi_r");
+}
+
+int b2_get_varphi_d_r(b2_bounds* b, int64_t m, const double* f_R_d, const double* x_d, const double* xl_d, const double* xu_d,
+                      const double* dx_d, const double* pp_d, const double* nn_d, const double* dpp_d, const double* dnn_d, double mu_R,
+                      double rho, double* out_d, void* stream) {
+    B2_NEED(b && m >= 0 && (b->n_tot == 0 || (f_R_d && x_d && xl_d && xu_d && dx_d)) && (m == 0 || (pp_d && nn_d && dpp_d && dnn_d)),
+            "b2_get_varphi_d_r");
+    VarphiDR f{b->n_tot, m, f_R_d, x_d, xl_d, xu_d, dx_d, pp_d, nn_d, dpp_d, dnn_d, mu_R, rho};
+    return run_reduce<R_SUM>(b, b->n_tot + 2 * m, f, 0.0, out_d, stream, "b2_get_varphi_d_r");
 }
 
 }  // extern "C"

@@ -12,6 +12,10 @@
         while !curv_test || !ok: regularize_diagonal!(dw, dc) ; factorize_wrapper! ; the two solves ; t = dx - n
     (InertiaIgnore, :739-783: the same loop with the d solve only and no test)
 
+restoration_step replays a restoration iteration of robust! (src/IPM/solver.jl:458-466) through the same inertia_correction! loop:
+    compress_* ; set_aug_RR! + _set_aug_diagonal! ; factorize_wrapper! ; set_aug_rhs_RR! ; inertia_correction! ; finish_aug_solve_RR!
+(the restorer's state and kernels: restoration.py).
+
 The model callbacks themselves are out of scope (SURVEY.md 8a A0): an iterate supplies their outputs.
 """
 from __future__ import annotations
@@ -107,6 +111,7 @@ class IPMLinearAlgebra:
         self.use_cuda_graph = use_cuda_graph
         self.speculate = speculate     # first refinement step queued before the inertia is known (see step())
         self._prologue_graph = None
+        self._rr_graph = self._rr_graph_key = None      # restoration_step's prologue graph and what it was captured for
         self.iterator = RichardsonIterator(kkt, tol=tol, use_cuda_graph=use_cuda_graph)
         self.d = UnreducedKKTVector.for_kkt(kkt)
         self.p = UnreducedKKTVector.for_kkt(kkt)
@@ -201,6 +206,7 @@ class IPMLinearAlgebra:
             # improve!() changed a factorisation parameter (pivot threshold) that the captured prologue has baked in:
             # drop the captured graph so that every later step factorises with the new setting
             self._prologue_graph = None
+            self._rr_graph = None
             self.kkt.factorize_kkt()
             ok = self.iterator.solve_refine(x, b, w)
         self.cnt["backsolves"] += self.iterator.ir
@@ -233,12 +239,83 @@ class IPMLinearAlgebra:
         self._wait_rhs()
         if after_prologue is not None:
             after_prologue()
+        return self._inertia_correction(mu)
+
+    def restoration_step(self, rr, rho=1000.0, mu=1e-2, primal_regularization=0.0, dual_regularization=0.0):
+        """The linear algebra of one restoration iteration of robust! (src/IPM/solver.jl:458-466), after the caller's
+        _update_monotone_RR! and the Hessian at obj_weight = 0 (is_resto = true) in kkt.hess:
+
+            compress_* ; set_aug_RR! + _set_aug_diagonal! ; factorize_wrapper!    (one CUDA graph, as step()'s prologue)
+            set_aug_rhs_RR! ; inertia_correction! (the method of this object, with the solver's mu) ; finish_aug_solve_RR!
+
+        rr: a RobustRestorer of this KKT system after rr.initialize; rho is MadNLP's option of that name, the regularisations its
+        default_primal_regularization / default_dual_regularization.  Returns what inertia_correction! returns (False sends robust!
+        to RESTORATION_FAILED); the direction is in d and rr.dpp, rr.dnn, rr.dzp, rr.dzn.  Under InertiaFree the curvature test reads
+        rr's f, x, xl, xu, jacl and c, as the reference's set_g_ifr! reads the solver's.  A quasi-Newton Hessian is refused."""
+        from .quasi_newton import ExactHessian
+        k = self.kkt
+        if not isinstance(getattr(k, "quasi_newton", ExactHessian()), ExactHessian):
+            raise ValueError("restoration_step: the restoration phase with a quasi-Newton Hessian is not supported")
+        if rr.kkt is not k:
+            raise ValueError("restoration_step: the RobustRestorer belongs to another KKT system")
+        if self.ifr is not None:
+            self._load_ifr_from(rr)
+            self.ifr.set_rhs(k, mu)
+        # the graph bakes in the restorer's buffers and the scalars of set_aug_RR!: capture again when either changes (the key holds
+        # the restorer itself, so its buffers stay alive as long as a graph may replay them)
+        key = (rr, rr.zeta, float(primal_regularization), float(dual_regularization))
+
+        def prologue():
+            k.compress_jacobian()
+            k.compress_hessian()
+            rr.set_aug_RR(k, primal_regularization, dual_regularization)
+            k.build_kkt()
+            k.factorize_kkt()
+        old = self._rr_graph_key
+        if old is None or old[0] is not rr or old[1:] != key[1:]:
+            self._rr_graph, self._rr_graph_key = None, key
+        if not self.use_cuda_graph or self._rr_graph is None:
+            prologue()
+            if self.use_cuda_graph:
+                self._rr_graph = False
+        elif self._rr_graph is False:
+            g = torch.cuda.CUDAGraph()
+            torch.cuda.synchronize()
+            with torch.cuda.graph(g):
+                prologue()
+            self._rr_graph = g
+            g.replay()
+        else:
+            self._rr_graph.replay()
+        self.cnt["factorizations"] += 1
+        rr.set_aug_rhs_RR(self.p, rho)
+        ok = self._inertia_correction(mu)
+        if ok:
+            rr.finish_aug_solve_RR(self.d, rho)
+        return ok
+
+    def _load_ifr_from(self, rr):
+        """the curvature test's inputs from the restorer's solver vectors (one launch)"""
+        import ctypes as C
+        from .capi import lib, check, stream_ptr
+        r = self.ifr
+        pairs = ((r.f, rr.f), (r.x, rr.x), (r.xl, rr.xl), (r.xu, rr.xu), (r.jacl, rr.jacl), (r.c, rr.c))
+        cnt = len(pairs)
+        src = (C.c_void_p * cnt)(*[s_.data_ptr() for _, s_ in pairs])
+        dst = (C.c_void_p * cnt)(*[d_.data_ptr() for d_, _ in pairs])
+        ns = (C.c_int64 * cnt)(*[d_.numel() for d_, _ in pairs])
+        check(lib.b2_copy_many(cnt, src, dst, ns, stream_ptr(getattr(self.kkt, "stream", None))))
+
+    def _inertia_correction(self, mu):
+        """inertia_correction! after its first factorize_wrapper! (src/IPM/solver.jl:611-783), for the method of this object"""
+        k = self.kkt
         if self.inertia_correction_method != "InertiaBased":
             return self._inertia_correction_without_inertia(mu)
         # inertia_correction!(InertiaBased)
         o = self.opt
         n_trial = 0
         del_w = del_c = del_w_prev = del_c_prev = 0.0
+        self.last_del_w = []
         ls = k.linear_solver
         if self.speculate and hasattr(ls, "inertia_enqueue"):
             # queue the inertia read AND the first refinement step behind the factorisation, block once for both
@@ -267,6 +344,7 @@ class IPMLinearAlgebra:
                      if k.should_regularize_dual(*inertia) else 0.0)
             k.regularize_diagonal(del_w - del_w_prev, del_c - del_c_prev)
             del_w_prev, del_c_prev = del_w, del_c
+            self.last_del_w.append(del_w)
             self._factorize_wrapper()
             inertia = k.linear_solver.inertia()
             ok = self._solve_refine_wrapper() if k.is_inertia_correct(*inertia) else False

@@ -17,6 +17,7 @@ import MadNLP: AbstractLinearSolver, AbstractOptions, MadNLPLogger, SymbolicExce
     SolveException, factorize!, solve_linear_system!, is_inertia, inertia, improve!, introduce, input_type,
     default_options, is_supported, is_async
 using CUDA, CUDA.CUSPARSE
+import Libdl
 # (nothing here extends a method on types this module does not own without one of ITS types in the signature)
 
 const libb200kkt = get(ENV, "B200KKT_LIB", "libb200kkt.so")
@@ -683,5 +684,118 @@ function MadNLP.curv_test(t::CuVector{T}, n::CuVector{T}, g::CuVector{T}, kkt::B
     copyto!(p.result_h, p.result)                  # the one synchronising read of the test
     return p.result_h[6] == 1.0
 end
+
+# ---------------------------------------------------------------- feasibility restoration (robust!, src/IPM/solver.jl:413-540)
+# set_aug_RR!, set_aug_rhs_RR! and set_f_RR! / initialize_robust_restorer! dispatch on a KKT system with our linear solver (directly, or
+# through the KKTSystem parameter of MadNLPSolver).  finish_aug_solve_RR! and the _R reductions take plain vectors in the reference, so
+# they cannot be overloaded without type piracy: they are this module's functions with the KKT system as first argument, and robust! /
+# filter_line_search_RR! call them instead (one line per call site, INTEGRATION.md).  The b2_bounds object and a result slot come from
+# ifr_plans.  Every vector is the solver's own full vector (zl / zu via full(...), +-Inf bounds); indices 0-based on the device side.
+# Like the rest of this file, NOT RUN.
+const B200RRSolver{T} = MadNLP.MadNLPSolver{T,VT,VI,KKT} where {VT,VI,KKT<:B200IFRKKT{T}}
+_ptr(v) = pointer(v)
+_sp() = stream_ptr()
+
+function MadNLP.set_aug_RR!(kkt::B200IFRKKT{T}, solver::MadNLP.AbstractMadNLPSolver, RR::MadNLP.RobustRestorer) where T
+    p, o = ifr_plans(kkt), MadNLP.get_opt(solver)
+    x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
+    zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
+    check(ccall((:b2_set_aug_rr, libb200kkt), Cint,
+                (Ptr{Cvoid}, Int64, Cdouble, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 16)..., Ptr{Cvoid}),
+                p.bounds, length(RR.pp), o.default_primal_regularization, o.default_dual_regularization, RR.zeta, _ptr(RR.D_R),
+                _ptr(RR.pp), _ptr(RR.nn), _ptr(RR.zp), _ptr(RR.zn), _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl), _ptr(zu), _ptr(kkt.reg),
+                _ptr(kkt.du_diag), _ptr(kkt.l_lower), _ptr(kkt.u_lower), _ptr(kkt.l_diag), _ptr(kkt.u_diag), _sp()), SolveException)
+    MadNLP._set_aug_diagonal!(kkt)                 # each type's own (the unreduced one takes the square roots)
+    return
+end
+
+function MadNLP.set_aug_rhs_RR!(solver::MadNLP.AbstractMadNLPSolver, kkt::B200IFRKKT{T}, RR::MadNLP.RobustRestorer, rho) where T
+    pl = ifr_plans(kkt)
+    x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
+    zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
+    check(ccall((:b2_set_aug_rhs_rr, libb200kkt), Cint, (Ptr{Cvoid}, Int64, ntuple(_ -> CuPtr{T}, 13)..., Cdouble, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+                pl.bounds, length(RR.pp), _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl), _ptr(zu), _ptr(MadNLP.get_jacl(solver)), _ptr(RR.f_R),
+                _ptr(MadNLP.get_c(solver)), _ptr(MadNLP.get_y(solver)), _ptr(RR.pp), _ptr(RR.nn), _ptr(RR.zp), _ptr(RR.zn), RR.mu_R,
+                Float64(rho), _ptr(MadNLP.full(MadNLP.get_p(solver))), _sp()), SolveException)
+    return
+end
+
+function MadNLP.set_f_RR!(solver::B200RRSolver{T}, RR::MadNLP.RobustRestorer) where T
+    x = MadNLP.full(MadNLP.get_x(solver))
+    check(ccall((:b2_set_f_rr, libb200kkt), Cint, (Int64, Cdouble, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                length(x), RR.zeta, _ptr(RR.D_R), _ptr(x), _ptr(RR.x_ref), _ptr(RR.f_R), _sp()), SolveException)
+    return
+end
+
+# initialize_robust_restorer! (src/IPM/restoration.jl:39-75): the two norms of c in one read, then one launch (b2_rr_init) and the
+# obj_val_R reduction
+function MadNLP.initialize_robust_restorer!(solver::B200RRSolver{T}) where T
+    MadNLP.get_RR(solver) === nothing && MadNLP.set_RR!(solver, MadNLP.RobustRestorer(solver))
+    RR::MadNLP.RobustRestorer = MadNLP.get_RR(solver)
+    kkt, o, c = MadNLP.get_kkt(solver), MadNLP.get_opt(solver), MadNLP.get_c(solver)
+    pl = ifr_plans(kkt)
+    r = CUDA.zeros(T, 2)
+    check(ccall((:b2_get_theta, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), pl.bounds, length(c), _ptr(c),
+                _ptr(r), _sp()), SolveException)
+    check(ccall((:b2_norm_inf, libb200kkt), Cint, (Int64, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), length(c), _ptr(c), _ptr(r) + sizeof(T), _sp()),
+          SolveException)
+    rh = Array(r)
+    RR.theta_ref = rh[1]
+    RR.mu_R = max(MadNLP.get_mu(solver), rh[2])
+    RR.tau_R = max(o.tau_min, 1 - RR.mu_R)
+    RR.zeta = sqrt(RR.mu_R)
+    x = MadNLP.full(MadNLP.get_x(solver))
+    zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
+    check(ccall((:b2_rr_init, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 10)..., Ptr{Cvoid}),
+                pl.bounds, length(c), _ptr(x), _ptr(c), RR.mu_R, o.rho, _ptr(RR.x_ref), _ptr(RR.D_R), _ptr(RR.f_R), _ptr(RR.pp),
+                _ptr(RR.nn), _ptr(RR.zp), _ptr(RR.zn), _ptr(MadNLP.get_y(solver)), _ptr(zl), _ptr(zu), _sp()), SolveException)
+    RR.obj_val_R = get_obj_val_R(kkt, RR.pp, RR.nn, RR.D_R, x, RR.x_ref, o.rho, RR.zeta)
+    empty!(RR.filter)
+    push!(RR.filter, (MadNLP.get_theta_max(solver), -Inf))
+    MadNLP.get_cnt(solver).t = 0
+    MadNLP.set_del_w!(solver, zero(T))
+end
+
+# finish_aug_solve_RR!(dpp, dnn, dzp, dzn, l, dl, pp, nn, zp, zn, mu_R, rho) (src/IPM/kernels.jl:251-257)
+function finish_aug_solve_RR!(kkt::B200IFRKKT{T}, dpp, dnn, dzp, dzn, l, dl, pp, nn, zp, zn, mu_R, rho) where T
+    check(ccall((:b2_finish_aug_solve_rr, libb200kkt), Cint, (Int64, ntuple(_ -> CuPtr{T}, 6)..., Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 4)...,
+                Ptr{Cvoid}), length(l), _ptr(l), _ptr(dl), _ptr(pp), _ptr(nn), _ptr(zp), _ptr(zn), mu_R, rho, _ptr(dpp), _ptr(dnn),
+                _ptr(dzp), _ptr(dzn), _sp()), SolveException)
+    return
+end
+
+# the reductions (kernels.jl:390-636): one launch each into the plans' result slot, then one read.  Arguments as in the reference
+# (vectors full length: x, xl, xu, zl, zu, f_R, jacl, dx n_tot; c, l, pp, nn, zp, zn and steps m; dzl / dzu compressed).
+function _reduce(kkt::B200IFRKKT{T}, sym::Symbol, argt::Tuple, args...) where T
+    pl = ifr_plans(kkt)
+    check(ccall(Libdl.dlsym(Libdl.dlopen(libb200kkt), sym), Cint, (Ptr{Cvoid}, argt..., CuPtr{T}, Ptr{Cvoid}), pl.bounds, args...,
+                _ptr(pl.result), _sp()), SolveException)
+    return Array(view(pl.result, 1:1))[1]
+end
+const _V = CuPtr{Float64}
+get_theta(kkt::B200IFRKKT, c) = _reduce(kkt, :b2_get_theta, (Int64, _V), length(c), _ptr(c))
+get_theta_R(kkt::B200IFRKKT, c, p, n) = _reduce(kkt, :b2_get_theta_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
+get_inf_pr_R(kkt::B200IFRKKT, c, p, n) = _reduce(kkt, :b2_get_inf_pr_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
+get_obj_val_R(kkt::B200IFRKKT, p, n, D_R, x, x_ref, rho, zeta) =
+    _reduce(kkt, :b2_get_obj_val_r, (Int64, _V, _V, _V, _V, _V, Cdouble, Cdouble), length(p), _ptr(p), _ptr(n), _ptr(D_R), _ptr(x),
+            _ptr(x_ref), rho, zeta)
+get_inf_du_R(kkt::B200IFRKKT, f_R, l, zl, zu, jacl, zp, zn, rho, sd) =
+    _reduce(kkt, :b2_get_inf_du_r, (Int64, ntuple(_ -> _V, 7)..., Cdouble, Cdouble), length(l), _ptr(f_R), _ptr(l), _ptr(zl), _ptr(zu),
+            _ptr(jacl), _ptr(zp), _ptr(zn), rho, sd)
+get_inf_compl_R(kkt::B200IFRKKT, x, xl, xu, zl, zu, pp, zp, nn, zn, mu_R, sc) =
+    _reduce(kkt, :b2_get_inf_compl_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl),
+            _ptr(zu), _ptr(pp), _ptr(zp), _ptr(nn), _ptr(zn), mu_R, sc)
+get_alpha_max_R(kkt::B200IFRKKT, x, xl, xu, dx, pp, dpp, nn, dnn, tau_R) =
+    _reduce(kkt, :b2_get_alpha_max_r, (Int64, ntuple(_ -> _V, 8)..., Cdouble), length(pp), _ptr(x), _ptr(xl), _ptr(xu), _ptr(dx), _ptr(pp),
+            _ptr(dpp), _ptr(nn), _ptr(dnn), tau_R)
+get_alpha_z_R(kkt::B200IFRKKT, zl, zu, dzl, dzu, zp, dzp, zn, dzn, tau_R) =
+    _reduce(kkt, :b2_get_alpha_z_r, (Int64, ntuple(_ -> _V, 8)..., Cdouble), length(zp), _ptr(zl), _ptr(zu), _ptr(dzl), _ptr(dzu), _ptr(zp),
+            _ptr(dzp), _ptr(zn), _ptr(dzn), tau_R)
+get_varphi_R(kkt::B200IFRKKT, obj_val, x, xl, xu, pp, nn, mu_R) =
+    _reduce(kkt, :b2_get_varphi_r, (Int64, Cdouble, ntuple(_ -> _V, 5)..., Cdouble), length(pp), obj_val, _ptr(x), _ptr(xl), _ptr(xu),
+            _ptr(pp), _ptr(nn), mu_R)
+get_varphi_d_R(kkt::B200IFRKKT, f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho) =
+    _reduce(kkt, :b2_get_varphi_d_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(f_R), _ptr(x), _ptr(xl), _ptr(xu),
+            _ptr(dx), _ptr(pp), _ptr(nn), _ptr(dpp), _ptr(dnn), mu_R, rho)
 
 end # module

@@ -398,6 +398,50 @@ def ifr_inputs(n_tot: int, m: int, ind_lb, ind_ub, l_diag, u_diag, seed: int = 0
     return dict(f=rng.standard_normal(n_tot), x=x, xl=xl, xu=xu, jacl=rng.standard_normal(n_tot), c=0.01 * rng.standard_normal(m))
 
 
+def restoration_inputs(model, st=None, seed: int = 0, mu: float = 1e-1):
+    """A seeded entry into the feasibility restoration phase (robust!) for an ACOPF `model` with its NLPStructure `st`, or for a
+    DenseQP `model`: what the restoration kernels read besides the restorer's own state.
+
+    x: the model's sample point (ACOPF) or uniform in (0, 1) (QP), slacks standard normal; bound distances log-uniform in
+    [1e-4, 1] on ind_lb / ind_ub (xl = x - dl, xu = x + du, +-Inf elsewhere); zl, zu = mu / distance with 30 % log-normal spread
+    (full length, zero off the index sets); y = 0.1 standard normal; f the objective gradient (standard normal on the model
+    variables, zero on the slacks); jacl = J'y with the slack columns -I; c infeasible, |c_i| up to 10 (so ||c||_inf is of order
+    1-10).  jac / hess: the Jacobian values and the Lagrangian Hessian at obj_weight = 0 (is_resto = true) with this y -- COO
+    values for ACOPF, dense m x n and n x n matrices for the QP (whose Hessian is then zero).  Its own RNG stream; the regular-phase
+    generators are unchanged."""
+    rng = np.random.default_rng(seed)
+    if isinstance(model, DenseQP):
+        n, m = model.n, model.m
+        ind_ineq, ind_lb, ind_ub = model.ind_ineq, model.ind_lb, model.ind_ub
+        x0 = rng.uniform(0.05, 0.95, n)
+        y = 0.1 * rng.standard_normal(m)
+        jac = np.asfortranarray(model.A.copy())
+        hess = np.zeros((n, n), order="F")
+        jty = model.A.T @ y
+    else:
+        n, m = st.nvar, st.ncon
+        ind_ineq, ind_lb, ind_ub = st.ind_ineq, st.ind_lb, st.ind_ub
+        x0 = model.sample_point(rng)
+        y = 0.1 * rng.standard_normal(m)
+        jac = model.jac_coord(x0)
+        hess = model.hess_coord(x0, y, obj_weight=0.0)
+        jty = np.zeros(n)
+        np.add.at(jty, st.jac_J, jac * y[st.jac_I])
+    ns = len(ind_ineq)
+    n_tot = n + ns
+    x = np.concatenate([x0, rng.standard_normal(ns)])
+    dl = np.exp(rng.uniform(np.log(1e-4), 0.0, len(ind_lb))); du = np.exp(rng.uniform(np.log(1e-4), 0.0, len(ind_ub)))
+    xl = np.full(n_tot, -np.inf); xu = np.full(n_tot, np.inf)
+    xl[ind_lb] = x[ind_lb] - dl; xu[ind_ub] = x[ind_ub] + du
+    zl = np.zeros(n_tot); zu = np.zeros(n_tot)
+    zl[ind_lb] = mu / dl * np.exp(0.3 * rng.standard_normal(len(ind_lb)))
+    zu[ind_ub] = mu / du * np.exp(0.3 * rng.standard_normal(len(ind_ub)))
+    f = np.concatenate([rng.standard_normal(n), np.zeros(ns)])
+    jacl = np.concatenate([jty, -y[ind_ineq]])
+    c = rng.uniform(-1.0, 1.0, m) * 10.0 ** rng.uniform(0.0, 1.0, m)
+    return dict(jac=jac, hess=hess, x=x, xl=xl, xu=xu, zl=zl, zu=zu, y=y, f=f, jacl=jacl, c=c, mu=mu)
+
+
 def acopf_case(name: str = "case10000_goc", seed: int = 0, relax_equality: bool = True):
     nbus, nbranch, ngen = PGLIB_COUNTS[name]
     net = synthetic_network(nbus, nbranch, ngen, seed)
