@@ -532,6 +532,47 @@ int b2_get_varphi_d_r(b2_bounds* b, int64_t m, const double* f_R_d, const double
                       const double* dx_d, const double* pp_d, const double* nn_d, const double* dpp_d, const double* dnn_d, double mu_R,
                       double rho, double* out_d, void* stream);                                                          /* :612-636 */
 
+/* ------------------------------------------------------------------ adaptive barrier (barrier = QualityFunctionUpdate, src/IPM/barrier.jl:150-302)
+ * The device half of get_adaptive_mu(solver, ::QualityFunctionUpdate): the new mu is computed on the device, and the free / monotone mode
+ * switch and the filter stay with the caller (barrier.jl:121-148).  Vectors as in the IPM reductions above (x, xl, xu, zl, zu: n_tot, zl / zu
+ * full length, +-Inf for an absent bound); aff_d, cen_d, p_d: UnreducedKKTVector buffers [x (n_tot) | y (m) | zl (nlb) | zu (nub)].
+ * The per-iteration scalars live in a small device array scal_d, so that a captured graph stays valid when they change: */
+#define B2_QF_TAU         0   /* tau (written by the caller) */
+#define B2_QF_NRM_PRIMAL  1   /* norm(primal(p)) of the affine right-hand side (b2_primal_dual_norm2) */
+#define B2_QF_NRM_DUAL    2   /* norm(dual(p)) */
+#define B2_QF_MU_AVG      3   /* get_average_complementarity (b2_get_average_complementarity) */
+#define B2_QF_SCAL_LEN    4
+/* result_d of b2_qf_search: sigma_opt, the new mu, the number of evaluations of the quality function, the golden-section iterations run, 1.0
+ * when the sigma_tol exit was taken (else 0.0), then one (sigma, phi, alpha_pr, alpha_du) row per evaluation in evaluation order */
+#define B2_QF_SIGMA       0
+#define B2_QF_MU          1
+#define B2_QF_N_EVAL      2
+#define B2_QF_N_GS_ITER   3
+#define B2_QF_TOL_EXIT    4
+#define B2_QF_TRACE       8
+#define B2_QF_MAX_GS_ITER 64
+#define B2_QF_RESULT_LEN(max_gs_iter) (B2_QF_TRACE + 4 * (6 + (max_gs_iter)))
+/* out_d[0] = ||p[0:n_tot)||_2, out_d[1] = ||p[n_tot:n_tot+m)||_2 in one deterministic launch (the two norms of barrier.jl:270-271;
+ * pass out_d = scal_d + B2_QF_NRM_PRIMAL) */
+int b2_primal_dual_norm2(b2_bounds* b, int64_t m, const double* p_d, double* out_d, void* stream);
+/* set_centering_aug_rhs! (barrier.jl:248-258) then dual_inf_perturbation! (kernels.jl:818-823) in one launch, with mu = *mu_d (device):
+ * p = [0 | 0 | mu | -mu]; px[ind_llb] -= mu kappa_d; px[ind_uub] += mu kappa_d.  ind_llb / ind_uub (src/Callbacks/nlpmodels.jl:391-392):
+ * device index arrays, ascending (findall order), over the model variables that have only a lower / only an upper bound */
+int b2_set_centering_aug_rhs(b2_bounds* b, int64_t m, int64_t nllb, const int64_t* ind_llb_d, int64_t nuub, const int64_t* ind_uub_d,
+                             const double* mu_d, double kappa_d, double* p_d, void* stream);
+/* The quality-function search of get_adaptive_mu (barrier.jl:276-301, with _evaluate_quality_function :152-201 and _run_golden_search!
+ * :205-246) for the affine and centering steps aff_d, cen_d: phi at sigma = 1 and 1 - 1e-4, the interval, the golden-section search,
+ * clamp(sigma_opt mu, mu_min, mu_max).  A fixed sequence of 2 (2 + max_gs_iter) launches that never synchronises (graph-capturable); the
+ * launches after the sigma_tol exit return at once.  Each evaluation forms aff + sigma cen on the fly: one pass for alpha_pr and alpha_du,
+ * one for the complementarity sums; the last CTA of the second finishes phi and moves the search on.  Kept as the reference has them: the
+ * infeasibility norms enter swapped (phi = (1 - alpha_du)^2 ||dual(p)||^2 / n_tot + (1 - alpha_pr)^2 ||primal(p)||^2 / m + compl), and the
+ * else branch of the search sets phi_mid2 = phi_mid1 after phi_mid1 has been recomputed.  Requires nlb + nub > 0 (the reference returns
+ * mu_min before any of this) and 0 <= max_gs_iter <= B2_QF_MAX_GS_ITER; result_d holds B2_QF_RESULT_LEN(max_gs_iter) doubles.
+ * One search at a time per b2_bounds object (its qf scratch). */
+int b2_qf_search(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d, const double* zu_d,
+                 const double* aff_d, const double* cen_d, const double* scal_d, double sigma_min, double sigma_max, double mu_min,
+                 double mu_max, double sigma_tol, int32_t max_gs_iter, double* result_d, void* stream);
+
 /* ------------------------------------------------------------------ compact L-BFGS (SparseKKTSystem, hessian_approximation = CompactLBFGS)
  * src/quasi_newton.jl:212-437 and src/IPM/factorization.jl:76-139, 253-276.  B_k = sigma I - U U' + V V' on the n model variables
  * (no slacks); S, Y are n x max_history, the memory p <= max_history.  max_history is limited to 32, so that

@@ -11,6 +11,7 @@ Only what the hot path needs lives here (SURVEY.md section 8):
   richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric, with the
                   InertiaBased (default), InertiaFree and InertiaIgnore regularisations
   restoration     RobustRestorer: the feasibility restoration phase's state, kernels and reductions on the device
+  barrier         the barrier update rules; AdaptiveBarrier: the quality-function and LOQO rules' new mu on the device
   workloads       synthetic generators for the configurations named in BASELINE.json
   julia/          the Julia shim a MadNLP.jl maintainer would add (cannot be run in this image)
 
@@ -24,6 +25,6 @@ def __getattr__(name):
     # torch-dependent modules are imported lazily so that CPU-only tooling (ABI checks, symbolic analysis)
     # does not pay for `import torch`.
     import importlib
-    if name in ("kkt", "linear_solvers", "quasi_newton", "richardson", "ipm", "parallel", "restoration"):
+    if name in ("kkt", "linear_solvers", "quasi_newton", "richardson", "ipm", "parallel", "restoration", "barrier"):
         return importlib.import_module(f".{name}", __name__)
     raise AttributeError(name)

@@ -18,6 +18,13 @@ ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
 # layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
 CURV_WXT, CURV_WXN, CURV_GN, CURV_TT, CURV_LHS, CURV_PASS, CURV_RESULT_LEN = 0, 1, 2, 3, 4, 5, 6
+# the adaptive barrier's scalar array and b2_qf_search's result (B2_QF_* in include/b200kkt.h)
+QF_TAU, QF_NRM_PRIMAL, QF_NRM_DUAL, QF_MU_AVG, QF_SCAL_LEN = 0, 1, 2, 3, 4
+QF_SIGMA, QF_MU, QF_N_EVAL, QF_N_GS_ITER, QF_TOL_EXIT, QF_TRACE, QF_MAX_GS_ITER = 0, 1, 2, 3, 4, 8, 64
+
+
+def qf_result_len(max_gs_iter):
+    return QF_TRACE + 4 * (6 + max_gs_iter)
 
 
 class B2Error(RuntimeError):
@@ -203,6 +210,9 @@ PROTOTYPES = {
     "b2_get_alpha_z_r": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64, _p, _p]),
     "b2_get_varphi_r": (C.c_int, [_p, _i64, _f64] + [_p] * 5 + [_f64, _p, _p]),
     "b2_get_varphi_d_r": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _p, _p]),
+    "b2_primal_dual_norm2": (C.c_int, [_p, _i64, _p, _p, _p]),
+    "b2_set_centering_aug_rhs": (C.c_int, [_p, _i64, _i64, _p, _i64, _p, _p, _f64, _p, _p]),
+    "b2_qf_search": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64] * 5 + [_i32, _p, _p]),
     "b2_richardson_begin": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_richardson_update": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_copy_many": (C.c_int, [_i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(_i64), _p]),

@@ -13,4 +13,9 @@ struct b2_bounds {
     b2::DevBuf<unsigned> red_ticket;       // [1] arrival counter (reset by the last CTA)
     b2::DevBuf<double> curv_part;          // [4 * B2_RED_BLOCKS] partials of the curvature test (inertia_free.cu)
     b2::DevBuf<unsigned> curv_ticket;      // [1] its arrival counter
+    b2::DevBuf<double> qf_part;            // [8 * B2_RED_BLOCKS] partials of the adaptive-barrier passes (barrier.cu)
+    b2::DevBuf<unsigned> qf_ticket;        // [1] their arrival counter
+    b2::DevBuf<double> qf_state;           // [B2_QF_STATE_DOUBLES] the quality-function search between its launches
 };
+
+constexpr int B2_QF_STATE_DOUBLES = 64;

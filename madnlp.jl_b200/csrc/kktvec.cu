@@ -35,7 +35,10 @@ extern "C" int b2_bounds_create(int64_t n_tot, int64_t nlb, int64_t nub, const i
         b->red_part.alloc(B2_RED_BLOCKS) != cudaSuccess || b->red_ticket.alloc(1) != cudaSuccess ||
         cudaMemset(b->red_ticket.p, 0, sizeof(unsigned)) != cudaSuccess ||
         b->curv_part.alloc(4 * B2_RED_BLOCKS) != cudaSuccess || b->curv_ticket.alloc(1) != cudaSuccess ||
-        cudaMemset(b->curv_ticket.p, 0, sizeof(unsigned)) != cudaSuccess) {
+        cudaMemset(b->curv_ticket.p, 0, sizeof(unsigned)) != cudaSuccess ||
+        b->qf_part.alloc(8 * B2_RED_BLOCKS) != cudaSuccess || b->qf_ticket.alloc(1) != cudaSuccess ||
+        cudaMemset(b->qf_ticket.p, 0, sizeof(unsigned)) != cudaSuccess || b->qf_state.alloc(B2_QF_STATE_DOUBLES) != cudaSuccess ||
+        cudaMemset(b->qf_state.p, 0, B2_QF_STATE_DOUBLES * sizeof(double)) != cudaSuccess) {
         delete b;
         return cuda_fail(cudaGetLastError(), "bounds upload", __FILE__, __LINE__);
     }

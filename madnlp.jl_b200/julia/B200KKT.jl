@@ -798,4 +798,53 @@ get_varphi_d_R(kkt::B200IFRKKT, f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho)
     _reduce(kkt, :b2_get_varphi_d_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(f_R), _ptr(x), _ptr(xl), _ptr(xu),
             _ptr(dx), _ptr(pp), _ptr(nn), _ptr(dpp), _ptr(dnn), mu_R, rho)
 
+# ---- the adaptive barrier rules (get_adaptive_mu, src/IPM/barrier.jl:260-316) for the solvers this module owns.  The quality-function
+# rule keeps the reference's sequence (set_aug_rhs! with mu = 0, the two solves into _w3 / _w4 without refinement, on the factor the
+# solver holds) and moves the norms, the average complementarity, the centering right-hand side and the whole search to the device:
+# the host reads mu once.  _check_progress, the mode switch and _update_monotone! stay MadNLP's.  Like the rest of this file, NOT RUN.
+const B2_QF_TRACE = 8
+function MadNLP.get_adaptive_mu(solver::B200RRSolver{T}, barrier::MadNLP.QualityFunctionUpdate{T}) where T
+    MadNLP.get_nlb(solver) + MadNLP.get_nub(solver) == 0 && return barrier.mu_min
+    kkt, o = MadNLP.get_kkt(solver), MadNLP.get_opt(solver)
+    pl = ifr_plans(kkt)
+    x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
+    zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
+    p, m = MadNLP.get_p(solver), length(MadNLP.get_c(solver))
+    step_aff, step_cen = MadNLP.get__w3(solver), MadNLP.get__w4(solver)
+    scal = CuVector{T}([MadNLP.get_tau(solver), zero(T), zero(T), zero(T)])   # B2_QF_TAU, _NRM_PRIMAL, _NRM_DUAL, _MU_AVG
+    MadNLP.set_aug_rhs!(solver, kkt, MadNLP.get_c(solver), zero(T))
+    check(ccall((:b2_primal_dual_norm2, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), pl.bounds, m,
+                _ptr(MadNLP.full(p)), _ptr(scal) + sizeof(T), _sp()), SolveException)
+    copyto!(MadNLP.full(step_aff), MadNLP.full(p))
+    MadNLP.solve_kkt!(kkt, step_aff)
+    check(ccall((:b2_get_average_complementarity, libb200kkt), Cint, (Ptr{Cvoid}, ntuple(_ -> CuPtr{T}, 6)..., Ptr{Cvoid}), pl.bounds,
+                _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl), _ptr(zu), _ptr(scal) + 3 * sizeof(T), _sp()), SolveException)
+    llb = CuVector{Int64}(MadNLP.get_ind_llb(solver) .- 1); uub = CuVector{Int64}(MadNLP.get_ind_uub(solver) .- 1)
+    check(ccall((:b2_set_centering_aug_rhs, libb200kkt), Cint,
+                (Ptr{Cvoid}, Int64, Int64, CuPtr{Int64}, Int64, CuPtr{Int64}, CuPtr{T}, Cdouble, CuPtr{T}, Ptr{Cvoid}), pl.bounds, m,
+                length(llb), _ptr(llb), length(uub), _ptr(uub), _ptr(scal) + 3 * sizeof(T), o.kappa_d, _ptr(MadNLP.full(p)), _sp()),
+          SolveException)
+    copyto!(MadNLP.full(step_cen), MadNLP.full(p))
+    MadNLP.solve_kkt!(kkt, step_cen)
+    res = CUDA.zeros(T, B2_QF_TRACE + 4 * (6 + barrier.max_gs_iter))
+    check(ccall((:b2_qf_search, libb200kkt), Cint,
+                (Ptr{Cvoid}, Int64, ntuple(_ -> CuPtr{T}, 8)..., Cdouble, Cdouble, Cdouble, Cdouble, Cdouble, Int32, CuPtr{T}, Ptr{Cvoid}),
+                pl.bounds, m, _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl), _ptr(zu), _ptr(MadNLP.full(step_aff)), _ptr(MadNLP.full(step_cen)),
+                _ptr(scal), barrier.sigma_min, barrier.sigma_max, barrier.mu_min, barrier.mu_max, barrier.sigma_tol,
+                Int32(barrier.max_gs_iter), _ptr(res), _sp()), SolveException)
+    barrier.n_update += 1
+    return Array(view(res, 2:2))[1]                    # B2_QF_MU
+end
+
+function MadNLP.get_adaptive_mu(solver::B200RRSolver{T}, barrier::MadNLP.LOQOUpdate{T}) where T
+    MadNLP.get_nlb(solver) + MadNLP.get_nub(solver) == 0 && return barrier.mu_min
+    kkt = MadNLP.get_kkt(solver)
+    v = map(MadNLP.full, (MadNLP.get_x(solver), MadNLP.get_xl(solver), MadNLP.get_xu(solver), MadNLP.get_zl(solver), MadNLP.get_zu(solver)))
+    mu = _reduce(kkt, :b2_get_average_complementarity, ntuple(_ -> _V, 5), map(_ptr, v)...)
+    min_cc = _reduce(kkt, :b2_get_min_complementarity, ntuple(_ -> _V, 5), map(_ptr, v)...)
+    xi = min_cc / mu
+    sigma = barrier.gamma * min((1 - barrier.r) * ((1 - xi) / xi), 2)^3
+    return clamp(sigma * mu, barrier.mu_min, barrier.mu_max)
+end
+
 end # module
