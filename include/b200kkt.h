@@ -84,8 +84,17 @@ typedef struct b2_options {
                                 one off-diagonal entry, in a primal column.  The ordering places each bound row immediately before
                                 its primal neighbour, so that it is eliminated first and adds its barrier term to that variable's
                                 pivot.  0 (default): every non-primal row is a constraint dual.  Ignored with B2_ORDER_USER. */
-    int32_t reserved[3];
+    int32_t dense_pivoting;  /* dense solver (b2d_*) only, B2_DENSE_PIVOT_*: STATIC (default) eliminates in natural order with
+                                |d| < pivot_eps -> +-pivot_eps; BUNCH_KAUFMAN uses LAPACK dsytrf('L')'s pivot sequence (1x1 and
+                                2x2 pivots, symmetric interchanges) and exact inertia (MadNLP's lapack_algorithm = BUNCHKAUFMAN).
+                                The sparse solver (b2_create*) rejects any value but STATIC.  BUNCH_KAUFMAN needs
+                                N <= 128 * (number of SMs of the device), 16,896 on an H100 SXM: its solve is one launch
+                                with one resident CTA per 128 rows; b2d_create rejects a larger N (B2_ERR_INVALID).      */
+    int32_t reserved[2];
 } b2_options;
+
+#define B2_DENSE_PIVOT_STATIC        0
+#define B2_DENSE_PIVOT_BUNCH_KAUFMAN 1
 
 int b2_options_default(b2_options* opt);
 
@@ -197,6 +206,11 @@ int b2d_inertia(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num
 int b2d_inertia_enqueue(b2d_solver* s, void* stream);
 int b2d_inertia_fetch(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg);
 int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream);
+/* Test/debug export of a Bunch-Kaufman factor (opt.dense_pivoting = B2_DENSE_PIVOT_BUNCH_KAUFMAN) in LAPACK's convention, N entries
+ * each on the host: ipiv_h 1-based (a 1x1 pivot interchanged row k with ipiv[k]; -kp on both rows of a 2x2 block), d_h D's diagonal,
+ * e_h D's subdiagonal (0 for a 1x1 pivot, d21 at the first index of a 2x2 block).  A zero column is reported with its perturbed
+ * pivot +-pivot_eps.  Synchronises the device; B2_ERR_INVALID on a static-pivoting handle. */
+int b2d_get_pivots(b2d_solver* s, int32_t* ipiv_h, double* d_h, double* e_h);
 
 /* ------------------------------------------------------------------ assembly: COO -> CSC */
 /* Host, one-time: CSC pattern of a COO matrix with duplicate merging and the COO->CSC map

@@ -16,6 +16,7 @@ B2_OK = 0
 B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE, B2_ERR_NO_DEVICE = 1, 2, 3, 4, 5, 6
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
+B2_DENSE_PIVOT_STATIC, B2_DENSE_PIVOT_BUNCH_KAUFMAN = 0, 1
 # layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
 CURV_WXT, CURV_WXN, CURV_GN, CURV_TT, CURV_LHS, CURV_PASS, CURV_RESULT_LEN = 0, 1, 2, 3, 4, 5, 6
 # the adaptive barrier's scalar array and b2_qf_search's result (B2_QF_* in include/b200kkt.h)
@@ -50,11 +51,20 @@ class InertiaException(RuntimeError):
     pass
 
 
+class _OptionsTail(C.Union):
+    """the three int32 after kkt_n_dual: `dense_pivoting` took the first (include/b200kkt.h).  `reserved` keeps the view of all
+    three at the offset it always had, so that code which reads `Options.reserved` still finds it there; the header's
+    `reserved[2]` (and the Julia shim's) is `reserved[1:]` here, and `reserved[0]` is `dense_pivoting`."""
+    _fields_ = [("dense_pivoting", C.c_int32), ("reserved", C.c_int32 * 3)]
+
+
 class Options(C.Structure):
+    _anonymous_ = ("_tail",)
     _fields_ = [
         ("ordering", C.c_int32), ("nemin", C.c_int32), ("relax_zeros", C.c_double), ("pivot_eps", C.c_double),
         ("use_cuda_graph", C.c_int32), ("small_front_max", C.c_int32), ("n_parts", C.c_int32), ("part_rank", C.c_int32),
-        ("kkt_n_primal", C.c_int32), ("fuse_max_fronts", C.c_int32), ("dep_schedule", C.c_int32), ("chain_merge_f", C.c_int32), ("kkt_n_dual", C.c_int32), ("reserved", C.c_int32 * 3),
+        ("kkt_n_primal", C.c_int32), ("fuse_max_fronts", C.c_int32), ("dep_schedule", C.c_int32), ("chain_merge_f", C.c_int32), ("kkt_n_dual", C.c_int32),
+        ("_tail", _OptionsTail),
     ]
 
 
@@ -129,6 +139,7 @@ PROTOTYPES = {
     "b2d_inertia_enqueue": (C.c_int, [_p, _p]),
     "b2d_inertia_fetch": (C.c_int, [_p, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "b2d_solve": (C.c_int, [_p, _p, _i32, _p]),
+    "b2d_get_pivots": (C.c_int, [_p, _p, _p, _p]),
     "b2_condensed_symbolic_device": (C.c_int, [_i32, _i32, _p, _p, _p, _p, _PP, C.POINTER(_i64), _p]),
     "b2_coo_to_csc_device": (C.c_int, [_i32, _i32, _i64, _p, _p, _p, _p, _p, C.POINTER(_i64), _p]),
     "b2d_ozaki_plan_create": (C.c_int, [_i32, _i32, _PP]),

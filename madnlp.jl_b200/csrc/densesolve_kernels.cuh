@@ -42,9 +42,15 @@ __device__ __forceinline__ double ds_poll(const double* p, int* err) {
 constexpr int DS_LDI = BS + 1;
 constexpr size_t DS_SMEM = (size_t)(BS * DS_LDI + 2 * BS + 2 * 8 * BS + BS) * sizeof(double);
 
+// BK (Bunch-Kaufman factor, dense_bk.cu): L is the unit-lower factor of A(perm, perm), so x is gathered through perm on entry and
+// scattered through it on exit, and D is block diagonal: evec[i] != 0 marks a 2 x 2 block on rows (i, i+1), which may straddle two
+// 128-row blocks -- its partner value is then polled from ybuf like any other hand-off (the block after publishes it once its own
+// forward sweep, which needs only this block's y, is done).  The 2 x 2 solve is dsytrs's.
+template <bool BK>
 __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const double* __restrict__ L, const double* __restrict__ Linv,
                                                               const double* __restrict__ dvec, double* __restrict__ x,
-                                                              double* ybuf, double* xbuf, int* err) {
+                                                              double* ybuf, double* xbuf, int* err,
+                                                              const int32_t* __restrict__ perm, const double* __restrict__ evec) {
     extern __shared__ __align__(16) double ds_sm[];
     double* Ls = ds_sm;                                   // [BS][DS_LDI]: Ls[c*DS_LDI + r] = Linv_k(r, c)
     double (*vec)[BS] = (double (*)[BS])(Ls + BS * DS_LDI);                  // [2][BS] the block vector being applied
@@ -60,7 +66,7 @@ __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const doub
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     // ---------------- forward
-    double t = (g == 0 && r < nb) ? x[kb + r] : 0.0;                         // group 0 carries the accumulator
+    double t = (g == 0 && r < nb) ? x[BK ? perm[kb + r] : kb + r] : 0.0;     // group 0 carries the accumulator
     double v[16];
     for (int c = 0; c < k; ++c) {
         {                                                                     // L(kb + r, c*BS + g*16 + q), issued before the poll
@@ -104,6 +110,17 @@ __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const doub
     // s_k(j) -= sum_i L(cb + i, kb + j) x_c(i): a warp owns 4 columns j, its lanes stride the rows i (each load instruction reads
     // 32 consecutive rows of one column: coalesced), column sums meet through shuffles; `sacc` lives in the threads tid < BS
     double s = (g == 0 && r < nb) ? yk / dvec[kb + r] : 0.0;
+    if constexpr (BK) {
+        const int i = kb + r;
+        const bool first = g == 0 && r < nb && evec[i] != 0.0, second = g == 0 && r < nb && i > 0 && evec[i - 1] != 0.0;
+        if (first || second) {
+            const int i0 = first ? i : i - 1;
+            const double y0 = first ? yk : ds_poll(ybuf + i0, err), y1 = first ? ds_poll(ybuf + i0 + 1, err) : yk;
+            const double akm1k = evec[i0], akm1 = dvec[i0] / akm1k, ak = dvec[i0 + 1] / akm1k;
+            const double denom = akm1 * ak - 1.0, bkm1 = y0 / akm1k, bk = y1 / akm1k;
+            s = first ? (ak * bkm1 - bk) / denom : (akm1 * bk - bkm1) / denom;
+        }
+    }
     const int warp = tid >> 5, lane = tid & 31;
     for (int c = nblk - 1; c > k; --c) {
         const int cb = c * BS, ncb = min(BS, N - cb);
@@ -145,7 +162,7 @@ __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const doub
         for (int u = 0; u < 8; ++u) xk += part[1][u][r];
         if (r >= nb) xk = 0.0;
         xbuf[(size_t)k * BS + r] = xk;                                        // publish x_k (consumers: the block columns before)
-        if (r < nb) x[kb + r] = xk;
+        if (r < nb) x[BK ? perm[kb + r] : kb + r] = xk;
     }
 }
 

@@ -15,6 +15,7 @@
 #include "warp_kernels.cuh"
 #include "bigsolve_kernels.cuh"
 #include "densesolve_kernels.cuh"
+#include "dense_bk.cuh"
 
 using namespace b2;
 
@@ -543,6 +544,10 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
                   const b2_options* opt, const int32_t* user_perm_h, bool symbolic_only, b2_solver** out) {
     if (!out || !colptr_h || !rowval_h || n <= 0) { set_error("b2_create: invalid argument"); return B2_ERR_INVALID; }
     if (colptr_h[n] != nnz) { set_error("b2_create: colptr[n] != nnz"); return B2_ERR_INVALID; }
+    if (opt && opt->dense_pivoting != B2_DENSE_PIVOT_STATIC) {
+        set_error("b2_create: dense_pivoting applies to the dense solver (b2d_create) only; the sparse solver pivots statically");
+        return B2_ERR_INVALID;
+    }
     if (opt && opt->kkt_n_dual != 0) {
         const std::string bad = check_kkt_rows(n, colptr_h, rowval_h, opt->kkt_n_primal, opt->kkt_n_dual);
         if (!bad.empty()) { set_error("b2_create: " + bad); return B2_ERR_INVALID; }
@@ -1087,6 +1092,8 @@ struct b2d_solver {
     cudaGraphExec_t g_factor = nullptr;
     cudaStream_t cap_stream = nullptr;
     bool factorized = false;
+    bool bunch_kaufman = false;                      // opt.dense_pivoting == B2_DENSE_PIVOT_BUNCH_KAUFMAN (dense_bk.cu)
+    DenseBK bk;
     ~b2d_solver() {
         if (g_factor) cudaGraphExecDestroy(g_factor);
         for (auto e : ev_pool) cudaEventDestroy(e);
@@ -1205,6 +1212,10 @@ void enqueue_dense_factor_lookahead(b2d_solver* s, cudaStream_t S1) {
 }
 
 void enqueue_dense_factor(b2d_solver* s, cudaStream_t st) {
+    if (s->bunch_kaufman) {
+        bk_enqueue_factor(s->bk, s->lda, s->A_d, s->fact.p, s->linv.p, s->dvec.p, s->counters.p, s->opt.pivot_eps, st);
+        return;
+    }
     if (s->N > 4 * DB) { enqueue_dense_factor_lookahead(s, st); return; }
     FactorArgs a;
     a.desc = s->desc.p; a.child_idx = nullptr; a.rel = nullptr; a.amap_src = nullptr; a.amap_dst = nullptr;
@@ -1220,15 +1231,24 @@ extern "C" {
 
 int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt, b2d_solver** out) {
     if (!out || N <= 0 || lda < N || !A_d) { set_error("b2d_create: invalid argument"); return B2_ERR_INVALID; }
+    if (opt && opt->dense_pivoting != B2_DENSE_PIVOT_STATIC && opt->dense_pivoting != B2_DENSE_PIVOT_BUNCH_KAUFMAN) {
+        set_error("b2d_create: dense_pivoting must be B2_DENSE_PIVOT_STATIC (0) or B2_DENSE_PIVOT_BUNCH_KAUFMAN (1)");
+        return B2_ERR_INVALID;
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
         set_error("b2d_create: no CUDA device (this library has no CPU fallback)");
         return B2_ERR_NO_DEVICE;
     }
+    if (opt && opt->dense_pivoting == B2_DENSE_PIVOT_BUNCH_KAUFMAN && (N + BS - 1) / BS > sm_count()) {
+        set_error("b2d_create: the Bunch-Kaufman solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
+        return B2_ERR_INVALID;
+    }
     auto* s = new b2d_solver();
     s->N = N; s->lda = lda; s->A_d = A_d;
     if (opt) s->opt = *opt; else b2_options_default(&s->opt);
+    s->bunch_kaufman = s->opt.dense_pivoting == B2_DENSE_PIVOT_BUNCH_KAUFMAN;
     FrontDesc d;
     std::memset(&d, 0, sizeof(d));
     d.col0 = 0; d.w = N; d.f = N;
@@ -1244,7 +1264,8 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
         cudaStreamCreateWithFlags(&s->side_stream, cudaStreamNonBlocking) != cudaSuccess ||
         s->tilecnt.alloc((size_t)((N + DB - 1) / DB)) != cudaSuccess ||
         (getenv("B2_DENSE_TRACE") && atoi(getenv("B2_DENSE_TRACE")) && s->trace.alloc((size_t)16 * ((N + DB - 1) / DB)) != cudaSuccess) ||
-        cudaMemset(s->fact.p, 0, s->fact.bytes()) != cudaSuccess || cudaMemset(s->counters.p, 0, 4 * sizeof(int32_t)) != cudaSuccess) {
+        cudaMemset(s->fact.p, 0, s->fact.bytes()) != cudaSuccess || cudaMemset(s->counters.p, 0, 4 * sizeof(int32_t)) != cudaSuccess ||
+        (s->bunch_kaufman && bk_alloc(s->bk, N) != cudaSuccess)) {
         delete s;
         return cuda_fail(cudaGetLastError(), "b2d_create allocation", __FILE__, __LINE__);
     }
@@ -1295,7 +1316,7 @@ int b2d_inertia_enqueue(b2d_solver* s, void* stream) {
 
 int b2d_inertia_fetch(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg) {
     if (!s || !s->factorized) { set_error("b2d_inertia: not factorized"); return B2_ERR_FACTORIZATION; }
-    if (s->h_counters[2]) { set_error("b2d: a hand-off wait timed out inside the single-launch solve"); return B2_ERR_SOLVE; }
+    if (s->h_counters[2]) { set_error("b2d: a device-wide wait timed out (single-launch solve or Bunch-Kaufman panel)"); return B2_ERR_SOLVE; }
     const int64_t neg = s->h_counters[0], zero = s->h_counters[1];
     if (num_neg) *num_neg = neg;
     if (num_zero) *num_zero = zero;
@@ -1317,14 +1338,26 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream) {
     const int N = s->N;
     const int nblk = (N + BS - 1) / BS;
     static const bool flow_ok =         // every CTA of the dataflow kernel must be resident: one per SM
-        cudaFuncSetAttribute(k_dense_solve_flow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
+        cudaFuncSetAttribute(k_dense_solve_flow<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
+    static const bool flow_bk_ok =
+        cudaFuncSetAttribute(k_dense_solve_flow<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
+    if (s->bunch_kaufman && !(flow_bk_ok && nblk <= sm_count())) {
+        set_error("b2d_solve: the Bunch-Kaufman solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
+        return B2_ERR_INVALID;
+    }
     for (int c = 0; c < nrhs; ++c) {
         double* x = x_d + (size_t)c * N;
+        if (s->bunch_kaufman) {
+            B2_CUDA(cudaMemsetAsync(s->flow.p, 0xFF, s->flow.bytes(), st));
+            k_dense_solve_flow<true><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
+                                                                  s->counters.p + 2, s->bk.perm.p, s->bk.evec.p);
+            continue;
+        }
         if (flow_ok && nblk <= sm_count()) {
             // ONE launch: block row / block column k is owned by CTA k, hand-off through sentinel-initialised vectors
             B2_CUDA(cudaMemsetAsync(s->flow.p, 0xFF, s->flow.bytes(), st));
-            k_dense_solve_flow<<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
-                                                            s->counters.p + 2);
+            k_dense_solve_flow<false><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
+                                                                   s->counters.p + 2, nullptr, nullptr);
             continue;
         }
         BigSolveArgs bs;
@@ -1343,6 +1376,17 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream) {
         k_bs_bwd_finish<<<dim3((N + 255) / 256, 1), 256, 0, st>>>(bs, s->list.p);
     }
     B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+int b2d_get_pivots(b2d_solver* s, int32_t* ipiv_h, double* d_h, double* e_h) {
+    if (!s || !ipiv_h || !d_h || !e_h) { set_error("b2d_get_pivots: invalid argument"); return B2_ERR_INVALID; }
+    if (!s->bunch_kaufman) { set_error("b2d_get_pivots: the handle pivots statically (opt.dense_pivoting = 0)"); return B2_ERR_INVALID; }
+    if (!s->factorized) { set_error("b2d_get_pivots: not factorized"); return B2_ERR_FACTORIZATION; }
+    B2_CUDA(cudaDeviceSynchronize());
+    B2_CUDA(cudaMemcpy(ipiv_h, s->bk.ipiv.p, s->bk.ipiv.bytes(), cudaMemcpyDeviceToHost));
+    B2_CUDA(cudaMemcpy(d_h, s->dvec.p, (size_t)s->N * sizeof(double), cudaMemcpyDeviceToHost));
+    B2_CUDA(cudaMemcpy(e_h, s->bk.evec.p, s->bk.evec.bytes(), cudaMemcpyDeviceToHost));
     return B2_OK;
 }
 

@@ -149,7 +149,17 @@ class B200DenseSolver:
         return np.dtype(dtype) == np.float64
 
     def introduce(self) -> str:
+        if self.opt.dense_pivoting == capi.B2_DENSE_PIVOT_BUNCH_KAUFMAN:
+            return f"b200kkt dense LDL^T (Bunch-Kaufman pivoting) v{lib.b2_version()}"
         return f"b200kkt dense LDL^T (DMMA) v{lib.b2_version()}"
+
+    def pivots(self):
+        """LAPACK-convention (ipiv, D diagonal, D subdiagonal) of a Bunch-Kaufman factor (b2d_get_pivots); synchronises."""
+        ipiv = np.empty(self.n, dtype=np.int32)
+        d = np.empty(self.n, dtype=np.float64)
+        e = np.empty(self.n, dtype=np.float64)
+        check(lib.b2d_get_pivots(self._h, ipiv.ctypes.data, d.ctypes.data, e.ctypes.data))
+        return ipiv, d, e
 
     def is_async(self) -> bool:
         return True

@@ -499,6 +499,30 @@ def dense_qp_iterate(qp: DenseQP, mu: float, seed: int = 2):
                 du_diag=np.zeros(qp.m), rhs=rng.standard_normal(n_tot + qp.m + nlb + nub))
 
 
+def dense_free_qp(n: int = 200, m: int = 80, n_free: int = 50, n_eq: int = 80, seed: int = 5):
+    """A QP whose first `n_free` variables are unbounded with zero curvature (the free columns of an LP), the others bounded in
+    [0, 1] with a diagonal Hessian, and an iterate for it: bound terms whose sum Sigma is log-uniform in [1e-3, 1e3], no primal
+    regularisation, a zero (2,2) block.  Its KKT matrix is nonsingular with n_free zero diagonal entries in front: a pivot-free
+    LDL^T meets them as zero pivots, Bunch-Kaufman pivots them with the constraint rows.  Returns (DenseQP, iterate dict)."""
+    if not (0 <= n_free <= n and 0 <= n_eq <= m and n_free <= m):
+        raise ValueError("dense_free_qp needs 0 <= n_free <= min(n, m) and 0 <= n_eq <= m")
+    rng = np.random.default_rng(seed)
+    bounded = np.arange(n_free, n, dtype=np.int64)
+    P = np.zeros((n, n))
+    P[bounded, bounded] = np.exp(rng.uniform(np.log(1e-2), np.log(1.0), n - n_free))
+    A = rng.standard_normal((m, n)) / np.sqrt(n)
+    q = rng.standard_normal(n)
+    ns = m - n_eq
+    ind = np.concatenate([bounded, np.arange(n, n + ns, dtype=np.int64)])        # bounded variables and every slack
+    qp = DenseQP(n, m, np.asfortranarray(P), np.asfortranarray(A), q, np.arange(n_eq, dtype=np.int64),
+                 np.arange(n_eq, m, dtype=np.int64), ind, ind.copy())
+    sigma = np.exp(rng.uniform(np.log(1e-3), np.log(1e3), len(ind)))
+    n_tot = n + ns
+    it = dict(l_diag=-np.ones(len(ind)), u_diag=-np.ones(len(ind)), l_lower=sigma / 2, u_lower=sigma / 2, reg=np.zeros(n_tot),
+              du_diag=np.zeros(m), rhs=rng.standard_normal(n_tot + m + 2 * len(ind)))
+    return qp, it
+
+
 # --------------------------------------------------------------------------------------------
 # Large sparse indefinite system of BASELINE.json configs[4] (SparseKKTSystem-style augmented matrix)
 # --------------------------------------------------------------------------------------------
