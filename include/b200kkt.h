@@ -582,7 +582,7 @@ int b2_set_centering_aug_rhs(b2_bounds* b, int64_t m, int64_t nllb, const int64_
  * infeasibility norms enter swapped (phi = (1 - alpha_du)^2 ||dual(p)||^2 / n_tot + (1 - alpha_pr)^2 ||primal(p)||^2 / m + compl), and the
  * else branch of the search sets phi_mid2 = phi_mid1 after phi_mid1 has been recomputed.  Requires nlb + nub > 0 (the reference returns
  * mu_min before any of this) and 0 <= max_gs_iter <= B2_QF_MAX_GS_ITER; result_d holds B2_QF_RESULT_LEN(max_gs_iter) doubles.
- * One search at a time per b2_bounds object (its qf scratch). */
+ * One search at a time per b2_bounds object, from the stream its other reductions use (they share one scratch). */
 int b2_qf_search(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d, const double* zu_d,
                  const double* aff_d, const double* cen_d, const double* scal_d, double sigma_min, double sigma_max, double mu_min,
                  double mu_max, double sigma_tol, int32_t max_gs_iter, double* result_d, void* stream);

@@ -9,100 +9,17 @@
 // Rounding: every elementwise formula is written with __dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn in the reference's left-to-right
 // order, so aff + sigma cen, the alpha terms and the complementarity terms are bit-identical to the broadcasts; t^2 is t*t.  min is exact,
 // so alpha_pr and alpha_du equal the scalar loops; the sums differ from mapreduce only by association (fixed tree: deterministic).
-#include <algorithm>
 #include <cmath>
 
 #include "bounds.cuh"
 #include "common.cuh"
+#include "grid_reduce.cuh"
 
 using namespace b2;
 
 namespace {
 
-inline int grid_elem(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-inline int grid_red(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, B2_RED_BLOCKS)); }
-
-__device__ __forceinline__ double dinf() { return __longlong_as_double(0x7ff0000000000000LL); }
-__device__ __forceinline__ double neg(double v) { return __longlong_as_double(__double_as_longlong(v) ^ (long long)0x8000000000000000ULL); }
 __device__ __forceinline__ double sq(double v) { return __dmul_rn(v, v); }
-
-// Julia's min / max on Float64 (base/math.jl): a NaN operand returns x - y, otherwise the sign of x - y decides
-__device__ __forceinline__ double jl_min(double x, double y) {
-    const double d = __dsub_rn(x, y);
-    if (x != x || y != y) return d;
-    return signbit(d) ? x : y;
-}
-__device__ __forceinline__ double jl_max(double x, double y) {
-    const double d = __dsub_rn(x, y);
-    if (x != x || y != y) return d;
-    return signbit(d) ? y : x;
-}
-// Julia's clamp(x, lo, hi) = x > hi ? hi : (x < lo ? lo : x)
-__device__ __forceinline__ double jl_clamp(double x, double lo, double hi) { return x > hi ? hi : (x < lo ? lo : x); }
-
-enum { R_SUM = 0, R_MIN = 1 };
-
-template <int KIND>
-__device__ __forceinline__ double comb(double a, double b) {
-    if (KIND == R_SUM) return __dadd_rn(a, b);
-    if (a != a || b != b) return __dadd_rn(a, b);       // NaN in, NaN out (Julia's min)
-    return a < b ? a : b;
-}
-
-// K reductions over the grid in a fixed order: thread (grid-stride) -> warp (xor tree) -> CTA (warps in order) -> part[j * B2_RED_BLOCKS
-// + cta]; the CTA that arrives last (ticket) combines the partials in index order with the same tree.  Returns true in that CTA only,
-// where thread 0 holds the K results in out; the caller resets the ticket.
-template <int KIND, int K>
-__device__ __forceinline__ bool grid_reduce(double (&v)[K], double identity, double* __restrict__ part, unsigned* ticket, double (&out)[K]) {
-    __shared__ double sm[K][8];
-    __shared__ bool last;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-        for (int j = 0; j < K; ++j) v[j] = comb<KIND>(v[j], __shfl_xor_sync(0xffffffffu, v[j], o));
-    if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int j = 0; j < K; ++j) sm[j][threadIdx.x >> 5] = v[j];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int j = 0; j < K; ++j) {
-            double r = sm[j][0];
-#pragma unroll
-            for (int w = 1; w < 8; ++w) r = comb<KIND>(r, sm[j][w]);
-            part[j * B2_RED_BLOCKS + blockIdx.x] = r;
-        }
-        __threadfence();
-        last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!last) return false;
-    __threadfence();
-    double r[K];
-#pragma unroll
-    for (int j = 0; j < K; ++j) r[j] = identity;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += 256)
-#pragma unroll
-        for (int j = 0; j < K; ++j) r[j] = comb<KIND>(r[j], __ldcg(part + j * B2_RED_BLOCKS + k));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-        for (int j = 0; j < K; ++j) r[j] = comb<KIND>(r[j], __shfl_xor_sync(0xffffffffu, r[j], o));
-    __syncthreads();                                    // every thread has read sm above: it may be reused
-    if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int j = 0; j < K; ++j) sm[j][threadIdx.x >> 5] = r[j];
-    __syncthreads();
-    if (threadIdx.x == 0)
-#pragma unroll
-        for (int j = 0; j < K; ++j) {
-            double t = sm[j][0];
-#pragma unroll
-            for (int w = 1; w < 8; ++w) t = comb<KIND>(t, sm[j][w]);
-            out[j] = t;
-        }
-    return true;
-}
 
 // ---- the two norms of barrier.jl:270-271: out = [||p[0:n_tot)||_2, ||p[n_tot:n_tot+m)||_2]
 __global__ void __launch_bounds__(256) k_pd_norm2(int64_t n_tot, int64_t m, const double* __restrict__ p, double* __restrict__ part,
@@ -119,7 +36,6 @@ __global__ void __launch_bounds__(256) k_pd_norm2(int64_t n_tot, int64_t m, cons
     if (threadIdx.x == 0) {
         out[0] = __dsqrt_rn(r[0]);
         out[1] = __dsqrt_rn(r[1]);
-        *ticket = 0;
     }
 }
 
@@ -144,7 +60,7 @@ __global__ void k_centering_rhs(int64_t n_tot, int64_t m, int64_t nlb, int64_t n
     const double mu = *mu_d;
     const double v = __dmul_rn(mu, kappa_d);
     const int64_t tot = n_tot + m + nlb + nub;
-    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < tot; t += (int64_t)gridDim.x * blockDim.x) {
+    GRID_STRIDE(t, tot) {
         double r;
         if (t < n_tot) {
             r = 0.0;
@@ -239,7 +155,6 @@ __global__ void __launch_bounds__(256) k_qf_alpha(QF a, int first) {
         }
 #pragma unroll
         for (int j = 0; j < 4; ++j) { st->apr[j] = r[j]; st->adu[j] = r[4 + j]; }
-        *a.ticket = 0;
     }
 }
 
@@ -371,19 +286,16 @@ __global__ void __launch_bounds__(256) k_qf_compl(QF a) {
     }
     a.res[B2_QF_N_EVAL] = (double)st->n_eval;
     qf_advance(a, st, phi);
-    *a.ticket = 0;
 }
 
 }  // namespace
-
-#define B2_NEED(cond, who) do { if (!(cond)) { set_error(who ": invalid argument"); return B2_ERR_INVALID; } } while (0)
 
 extern "C" {
 
 int b2_primal_dual_norm2(b2_bounds* b, int64_t m, const double* p_d, double* out_d, void* stream) {
     B2_NEED(b && m >= 0 && out_d && (b->n_tot + m == 0 || p_d), "b2_primal_dual_norm2");
-    cudaError_t e = launch_pdl(k_pd_norm2, dim3(grid_red(b->n_tot + m)), dim3(256), 0, as_stream(stream), b->n_tot, m, p_d, b->qf_part.p,
-                               b->qf_ticket.p, out_d);
+    cudaError_t e = launch_pdl(k_pd_norm2, dim3(grid_red(b->n_tot + m)), dim3(256), 0, as_stream(stream), b->n_tot, m, p_d, b->red_part.p,
+                               b->red_ticket.p, out_d);
     if (e != cudaSuccess) return cuda_fail(e, "b2_primal_dual_norm2", __FILE__, __LINE__);
     return B2_OK;
 }
@@ -407,7 +319,7 @@ int b2_qf_search(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d,
     B2_NEED(b && m >= 0 && b->nlb + b->nub > 0 && max_gs_iter >= 0 && max_gs_iter <= B2_QF_MAX_GS_ITER, "b2_qf_search");
     B2_NEED(x_d && xl_d && xu_d && zl_d && zu_d && aff_d && cen_d && scal_d && result_d, "b2_qf_search");
     QF a{b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, x_d, xl_d, xu_d, zl_d, zu_d, aff_d, cen_d, scal_d, sigma_min, sigma_max,
-         mu_min, mu_max, sigma_tol, (int)max_gs_iter, b->qf_part.p, b->qf_ticket.p, reinterpret_cast<QFState*>(b->qf_state.p), result_d};
+         mu_min, mu_max, sigma_tol, (int)max_gs_iter, b->red_part.p, b->red_ticket.p, reinterpret_cast<QFState*>(b->qf_state.p), result_d};
     const dim3 ga(grid_red(b->n_tot + b->nlb + b->nub)), gc(grid_red(b->nlb + b->nub));
     cudaStream_t st = as_stream(stream);
     // {1, 1 - 1e-4}, then {lb, ub, mid1, mid2}, then one sigma per golden step

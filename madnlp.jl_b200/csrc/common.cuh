@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <string>
@@ -53,6 +54,35 @@ inline cudaStream_t as_stream(void* s) { return (cudaStream_t)s; }
 
 // number of SMs of the current device (cached)
 int sm_count();
+
+// grid of a grid-stride elementwise kernel of 256-thread CTAs over n entries
+inline int grid_elem(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
+
+// argument check of a C entry point: on failure, records "<who>: invalid argument" and returns B2_ERR_INVALID
+#define B2_NEED(cond, who) do { if (!(cond)) { ::b2::set_error(who ": invalid argument"); return B2_ERR_INVALID; } } while (0)
+
+#ifdef __CUDACC__
+#define GRID_STRIDE(i, n) for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
+
+__device__ __forceinline__ double dinf() { return __longlong_as_double(0x7ff0000000000000LL); }
+// sign flip as Julia's unary minus does it, NaN payload and sign included (neg.f64 returns the canonical NaN)
+__device__ __forceinline__ double neg(double v) { return __longlong_as_double(__double_as_longlong(v) ^ (long long)0x8000000000000000ULL); }
+
+// Julia's min / max on Float64 (base/math.jl): diff = x - y; a NaN operand returns diff, otherwise the sign of diff decides
+// (so -0.0 is below +0.0)
+__device__ __forceinline__ double jl_min(double x, double y) {
+    const double d = __dsub_rn(x, y);
+    if (x != x || y != y) return d;
+    return signbit(d) ? x : y;
+}
+__device__ __forceinline__ double jl_max(double x, double y) {
+    const double d = __dsub_rn(x, y);
+    if (x != x || y != y) return d;
+    return signbit(d) ? y : x;
+}
+// Julia's clamp(x, lo, hi) = x > hi ? hi : (x < lo ? lo : x)
+__device__ __forceinline__ double jl_clamp(double x, double lo, double hi) { return x > hi ? hi : (x < lo ? lo : x); }
+#endif
 
 // ---- programmatic dependent launch (PDL).  A kernel launched through launch_pdl() may be scheduled while its predecessor
 // in the stream is still running; it must not touch anything the predecessor produces before pdl_wait() returns (and must

@@ -4,21 +4,21 @@
 // Bk is the dense KKT system's `hess`: n x n, column-major, leading dimension n; only its lower triangle is read or written, as
 // the reference's _symv!('L') / _syr!('L') do.  Every state value (is_instantiated, the last accept decision, the scalars) lives in
 // device memory, and every entry point issues a fixed launch sequence with no host branch on data, so it can be captured in a CUDA
-// graph.  The n-wide dot products are block partials summed by the last block to finish (a ticket), both in a fixed order, as in
-// lbfgs.cu: replays are bit-identical.  update = [s'y, s's; decision] -> [diagonal on the first accepted call] -> b2d_symv_lower
-// (bsk = B s) -> [s'bsk, theta, r, r's, alpha1, alpha2] -> one fused read-modify-write pass over the lower triangle that applies
-// both rank-1 terms (the reference's symv + syr + syr read the half matrix five times; this reads it three times).
+// graph.  The n-wide dot products are grid_sums (grid_reduce.cuh), as in lbfgs.cu: replays are bit-identical.
+// update = [s'y, s's; decision] -> [diagonal on the first accepted call] -> b2d_symv_lower (bsk = B s) -> [s'bsk, theta, r, r's,
+// alpha1, alpha2] -> one fused read-modify-write pass over the lower triangle that applies both rank-1 terms (the reference's
+// symv + syr + syr read the half matrix five times; this reads it three times).
 // Concurrent calls on one handle from two streams are not supported (one ticket per handle).
 #include <algorithm>
 #include <cmath>
 
 #include "common.cuh"
+#include "grid_reduce.cuh"
 
 using namespace b2;
 
 namespace {
 constexpr int QN_T = 256;          // threads of the reduction kernels
-constexpr int QN_MAX_BLOCKS = 256;
 constexpr int QN_TILE = 64;        // the rank-2 pass works on 64 x 64 tiles of the lower triangle
 constexpr int QN_RANK2_T = 256;    // 4 threads per tile row: each updates 16 columns of its row
 constexpr int QN_COLS = QN_TILE * QN_TILE / QN_RANK2_T;
@@ -32,65 +32,12 @@ struct QnState {
     unsigned ticket;
 };
 
-int qn_blocks(int64_t n) { return (int)std::min<int64_t>(QN_MAX_BLOCKS, std::max<int64_t>(1, (n + 2047) / 2048)); }
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// sum of one value per thread over the block, in a fixed order; valid in thread 0
-__device__ __forceinline__ double block_sum(double v) {
-    __shared__ double sh[QN_T / 32];
-    v = warp_sum(v);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double a = 0.0;
-    if (threadIdx.x == 0)
-        for (int k = 0; k < (int)(blockDim.x >> 5); ++k) a += sh[k];
-    __syncthreads();
-    return a;
-}
-
-// out[q] = sum_{r < n} f(q, r) for q < NQ over the whole grid in a fixed order (thread, warp, block, then blocks in order by
-// the last block to arrive, which re-arms the ticket).  Returns true in the last block only, with out[] valid in thread 0.
-template <int NQ, class F>
-__device__ __forceinline__ bool grid_sums(int64_t n, F f, double* part, unsigned* ticket, double* out) {
-    __shared__ bool s_last;
-    double acc[NQ];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) acc[q] = 0.0;
-    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x)
-#pragma unroll
-        for (int q = 0; q < NQ; ++q) acc[q] += f(q, r);
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) {
-        const double b = block_sum(acc[q]);
-        if (threadIdx.x == 0) part[(int64_t)blockIdx.x * NQ + q] = b;
-    }
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (!s_last) return false;
-    __threadfence();
-    if (threadIdx.x == 0) {
-        *ticket = 0;
-        for (int q = 0; q < NQ; ++q) {
-            double a = 0.0;
-            for (int b = 0; b < (int)gridDim.x; ++b) a += __ldcg(part + (int64_t)b * NQ + q);
-            out[q] = a;
-        }
-    }
-    return true;
-}
-
 // init! (quasi_newton.jl:425-437): norm_g0 = g0'g0; the last block stores 2 rho0.  `f0 ≈ 0` with isapprox's default tolerances
 // holds for exactly +-0 only.
 __global__ void __launch_bounds__(QN_T) k_qn_init(int64_t n, const double* __restrict__ g0, double f0, QnState* st, double* part) {
-    double out[1];
+    __shared__ double out[1];
     auto f = [&](int, int64_t r) { return g0[r] * g0[r]; };
-    if (!grid_sums<1>(n, f, part, &st->ticket, out) || threadIdx.x != 0) return;
+    if (!grid_sums<1>(n, 1, f, part, &st->ticket, out) || threadIdx.x != 0) return;
     const double norm_g0 = out[0];
     const double rho0 = norm_g0 < sqrt(2.220446049250313e-16) ? 1.0 : (f0 == 0.0 ? 1.0 / norm_g0 : fabs(f0) / norm_g0);
     st->init_diag = 2.0 * rho0;
@@ -108,9 +55,9 @@ __global__ void k_qn_diag(int64_t n, int init, const QnState* __restrict__ st, d
 // writes it, so a NaN is not skipped); DampedBFGS never skips.  The first accepted call rewrites the diagonal (k_qn_diag).
 __global__ void __launch_bounds__(QN_T) k_qn_pre(int64_t n, int kind, const double* __restrict__ s, const double* __restrict__ y,
                                                 QnState* st, double* part) {
-    double out[2];
+    __shared__ double out[2];
     auto f = [&](int q, int64_t r) { return q == 0 ? s[r] * y[r] : s[r] * s[r]; };
-    if (!grid_sums<2>(n, f, part, &st->ticket, out) || threadIdx.x != 0) return;
+    if (!grid_sums<2>(n, 2, f, part, &st->ticket, out) || threadIdx.x != 0) return;
     const double ys = out[0], ss = out[1];
     const int acc = kind == 1 ? !(ys < 1e-8) : 1;
     st->ys = ys;
@@ -127,9 +74,9 @@ __global__ void __launch_bounds__(QN_T) k_qn_pre(int64_t n, int kind, const doub
 __global__ void __launch_bounds__(QN_T) k_qn_post(int64_t n, int kind, const double* __restrict__ s, const double* __restrict__ y,
                                                  const double* __restrict__ bsk, double* __restrict__ rk, QnState* st, double* part) {
     __shared__ double s_theta;
-    double out[1];
+    __shared__ double out[1];
     auto f = [&](int, int64_t r) { return s[r] * bsk[r]; };
-    if (!grid_sums<1>(n, f, part, &st->ticket, out)) return;
+    if (!grid_sums<1>(n, 1, f, part, &st->ticket, out)) return;
     if (threadIdx.x == 0) {
         const double sBs = out[0], ys = st->ys;
         st->sBs = sBs;
@@ -201,8 +148,6 @@ __global__ void __launch_bounds__(QN_RANK2_T) k_qn_rank2(int64_t n, const QnStat
     }
 }
 
-int grid_stride_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-
 }  // namespace
 
 struct b2d_qn {
@@ -220,7 +165,7 @@ extern "C" int b2d_qn_create(int64_t n, int32_t kind, b2d_qn** out) {
         return B2_ERR_INVALID;
     }
     auto* h = new b2d_qn();
-    h->n = n; h->kind = kind; h->nb = qn_blocks(n);
+    h->n = n; h->kind = kind; h->nb = grid_sums_blocks(n);
     cudaError_t e = cudaSuccess;
     auto A = [&](auto& buf, size_t cnt) { if (e == cudaSuccess) e = buf.alloc(cnt); if (e == cudaSuccess) e = cudaMemset(buf.p, 0, buf.bytes()); };
     A(h->st, 1); A(h->bsk, (size_t)n); A(h->rk, (size_t)n); A(h->part, (size_t)h->nb * 2);
@@ -235,7 +180,7 @@ extern "C" int b2d_qn_init(b2d_qn* h, double* Bk_d, const double* g0_d, double f
     if (!h || !Bk_d || !g0_d) { set_error("b2d_qn_init: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     k_qn_init<<<h->nb, QN_T, 0, st>>>(h->n, g0_d, f0, h->st.p, h->part.p);
-    k_qn_diag<<<grid_stride_blocks(h->n), 256, 0, st>>>(h->n, 1, h->st.p, Bk_d);
+    k_qn_diag<<<grid_elem(h->n), 256, 0, st>>>(h->n, 1, h->st.p, Bk_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -245,7 +190,7 @@ extern "C" int b2d_qn_update(b2d_qn* h, double* Bk_d, const double* sk_d, const 
     cudaStream_t st = as_stream(stream);
     const int64_t n = h->n;
     k_qn_pre<<<h->nb, QN_T, 0, st>>>(n, h->kind, sk_d, yk_d, h->st.p, h->part.p);
-    k_qn_diag<<<grid_stride_blocks(n), 256, 0, st>>>(n, 0, h->st.p, Bk_d);
+    k_qn_diag<<<grid_elem(n), 256, 0, st>>>(n, 0, h->st.p, Bk_d);
     B2_CUDA(cudaGetLastError());
     const int rc = b2d_symv_lower((int32_t)n, (int32_t)n, Bk_d, sk_d, h->bsk.p, 1.0, 0.0, stream);
     if (rc != B2_OK) return rc;

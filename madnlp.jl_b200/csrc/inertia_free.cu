@@ -4,28 +4,24 @@
 //
 // mul_hess_blk! = [b2_spmv_symlower on hess_com | b2d_symv_lower on hess] (wx[0:n_h) = H t) ; k_hess_blk_tail.  The tail writes
 // wx[n_h:n_tot) = 0, adds t .* pr_diag and, for the unreduced system, the lb then ub barrier terms through the inverse maps of
-// b2_bounds (one thread per variable: no atomics).  Given a result pointer, the same pass reduces wx't, wx'n, g'n and t't as fixed-order
-// block partials (the ticket pattern of ipm_reductions.cu, with its own scratch) and the last CTA evaluates the test.
+// b2_bounds (one thread per variable: no atomics).  Given a result pointer, the same pass reduces wx't, wx'n, g'n and t't with
+// grid_reduce (grid_reduce.cuh) and the last CTA evaluates the test.
 //
 // Rounding: every elementwise formula is written with __dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn in the reference's left-to-right
 // order, so no contraction can happen and the outputs are bit-identical to the numpy broadcast.
-#include <algorithm>
-
 #include "bounds.cuh"
 #include "common.cuh"
+#include "grid_reduce.cuh"
 
 using namespace b2;
 
 namespace {
 
-inline int grid_elem(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-inline int grid_red(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, B2_RED_BLOCKS)); }
-
 // ---- set_g_ifr! (kernels.jl:242-248): g = f - mu ./ (x - xl) + mu ./ (xu - x) + jacl
 __global__ void k_set_g_ifr(int64_t n, const double* __restrict__ f, const double* __restrict__ x, const double* __restrict__ xl,
                             const double* __restrict__ xu, const double* __restrict__ jacl, double mu, double* __restrict__ g) {
     pdl_sync();
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    GRID_STRIDE(i, n) {
         const double xi = x[i];
         double v = __dsub_rn(f[i], __ddiv_rn(mu, __dsub_rn(xi, xl[i])));
         v = __dadd_rn(v, __ddiv_rn(mu, __dsub_rn(xu[i], xi)));
@@ -33,14 +29,10 @@ __global__ void k_set_g_ifr(int64_t n, const double* __restrict__ f, const doubl
     }
 }
 
-// sign flip as Julia's unary minus does it, NaN payload and sign included (neg.f64 returns the canonical NaN)
-__device__ __forceinline__ double neg(double v) { return __longlong_as_double(__double_as_longlong(v) ^ (long long)0x8000000000000000ULL); }
-
 // ---- set_aug_rhs_ifr! (kernels.jl:233-240): p0 = [0 | -c | 0 | 0]
 __global__ void k_set_aug_rhs_ifr(int64_t n_tot, int64_t m, int64_t tot, const double* __restrict__ c, double* __restrict__ p0) {
     pdl_sync();
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < tot; i += (int64_t)gridDim.x * blockDim.x)
-        p0[i] = (i >= n_tot && i < n_tot + m) ? neg(c[i - n_tot]) : 0.0;
+    GRID_STRIDE(i, tot) p0[i] = (i >= n_tot && i < n_tot + m) ? neg(c[i - n_tot]) : 0.0;
 }
 
 struct Tail {
@@ -71,75 +63,28 @@ __global__ void __launch_bounds__(256) k_hess_blk_tail(Tail a) {
     for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < a.n_tot; i += stride) a.entry(i);
 }
 
-__device__ __forceinline__ void warp_sum4(double (&v)[4]) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
-}
-
-// the tail plus curv_test: part[j * B2_RED_BLOCKS + cta] holds the CTA's partial of dot j; res = B2_CURV_* layout
+// the tail plus curv_test: res = B2_CURV_* layout
 __global__ void __launch_bounds__(256) k_hess_blk_curv(Tail a, const double* __restrict__ nv, const double* __restrict__ g, double tol,
                                                        double* __restrict__ part, unsigned* ticket, double* __restrict__ res) {
-    __shared__ double sm[4][8];
-    __shared__ bool last;
     pdl_sync();
     double acc[4] = {0.0, 0.0, 0.0, 0.0};              // wx't, wx'n, g'n, t't
     for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < a.n_tot; i += (int64_t)gridDim.x * 256) {
         const double w = a.entry(i), ti = a.t[i], ni = nv[i];
         acc[0] += w * ti; acc[1] += w * ni; acc[2] += g[i] * ni; acc[3] += ti * ti;
     }
-    warp_sum4(acc);
-    if ((threadIdx.x & 31) == 0)
+    double d[4];
+    if (!grid_reduce<R_SUM, 4>(acc, 0.0, part, ticket, d) || threadIdx.x != 0) return;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) sm[j][threadIdx.x >> 5] = acc[j];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            double r = sm[j][0];
-#pragma unroll
-            for (int w = 1; w < 8; ++w) r += sm[j][w];
-            part[j * B2_RED_BLOCKS + blockIdx.x] = r;
-        }
-        __threadfence();
-        last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    // the last CTA: partials in index order (thread t owns partials t, t + 256, ...; then the same tree as above)
-    double r[4] = {0.0, 0.0, 0.0, 0.0};
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += 256)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) r[j] += __ldcg(part + j * B2_RED_BLOCKS + k);
-    warp_sum4(r);
-    if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) sm[j][threadIdx.x >> 5] = r[j];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double d[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            d[j] = sm[j][0];
-#pragma unroll
-            for (int w = 1; w < 8; ++w) d[j] += sm[j][w];
-            res[j] = d[j];
-        }
-        // dot(wx,t) + max(dot(wx,n) - dot(g,n), 0) - tol*dot(t,t) >= 0, with Julia's NaN-propagating max
-        const double e = __dsub_rn(d[1], d[2]);
-        const double mx = (e != e) ? e : (e > 0.0 ? e : 0.0);
-        const double lhs = __dsub_rn(__dadd_rn(d[0], mx), __dmul_rn(tol, d[3]));
-        res[B2_CURV_LHS] = lhs;
-        res[B2_CURV_PASS] = (lhs >= 0.0) ? 1.0 : 0.0;   // NaN fails
-        *ticket = 0;                                     // ready for the next test on this stream
-    }
+    for (int j = 0; j < 4; ++j) res[j] = d[j];
+    // dot(wx,t) + max(dot(wx,n) - dot(g,n), 0) - tol*dot(t,t) >= 0, with Julia's NaN-propagating max
+    const double e = __dsub_rn(d[1], d[2]);
+    const double mx = (e != e) ? e : (e > 0.0 ? e : 0.0);
+    const double lhs = __dsub_rn(__dadd_rn(d[0], mx), __dmul_rn(tol, d[3]));
+    res[B2_CURV_LHS] = lhs;
+    res[B2_CURV_PASS] = (lhs >= 0.0) ? 1.0 : 0.0;       // NaN fails
 }
 
 }  // namespace
-
-#define B2_NEED(cond, who) do { if (!(cond)) { set_error(who ": invalid argument"); return B2_ERR_INVALID; } } while (0)
 
 extern "C" {
 
@@ -174,8 +119,8 @@ int b2_mul_hess_blk_tail(b2_bounds* b, int64_t n_h, int32_t unreduced, const dou
            t_d, wx_d};
     cudaError_t e = cudaSuccess;
     if (result_d) {
-        e = launch_pdl(k_hess_blk_curv, dim3(grid_red(n)), dim3(256), 0, as_stream(stream), a, n_d, g_d, tol, b->curv_part.p,
-                       b->curv_ticket.p, result_d);
+        e = launch_pdl(k_hess_blk_curv, dim3(grid_red(n)), dim3(256), 0, as_stream(stream), a, n_d, g_d, tol, b->red_part.p,
+                       b->red_ticket.p, result_d);
     } else {
         if (n == 0) return B2_OK;
         e = launch_pdl(k_hess_blk_tail, dim3(grid_elem(n)), dim3(256), 0, as_stream(stream), a);

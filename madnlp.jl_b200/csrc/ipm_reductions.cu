@@ -4,79 +4,38 @@
 // The reference computes them with scalar loops on the CPU (src/IPM/kernels.jl:263-388,675-695) and, on the GPU, with
 // allocating mapreduce calls (lib/MadNLPGPU/src/IPM/kernels.jl).
 //
-// Determinism: a fixed grid of B2_RED_BLOCKS CTAs; every CTA reduces its grid-stride slice in a fixed order and writes one
-// partial; the CTA that arrives last (atomic ticket) combines the partials in index order and applies the final scaling.
-// min / max propagate NaN like Julia's `min` / `max`.
-#include <algorithm>
+// Determinism: a fixed grid of up to B2_RED_BLOCKS CTAs reduces in grid_reduce's fixed order (grid_reduce.cuh); the last CTA
+// applies the final scaling.  min / max propagate NaN like Julia's `min` / `max`.
 #include <cmath>
 
 #include "bounds.cuh"
 #include "common.cuh"
+#include "grid_reduce.cuh"
 
 using namespace b2;
 
 namespace {
-
-enum { R_SUM = 0, R_MIN = 1, R_MAX = 2 };
-
-template <int KIND>
-__device__ __forceinline__ double comb(double a, double b) {
-    if (KIND == R_SUM) return a + b;
-    if (a != a || b != b) return a + b;                 // NaN in, NaN out
-    return (KIND == R_MIN) ? (a < b ? a : b) : (a > b ? a : b);
-}
 
 // F: struct with `__device__ double term(int64_t i) const` over i in [0, n), `double init` semantics via identity(),
 // and `__device__ double finish(double r) const` applied once to the reduced value.
 template <int KIND, class F>
 __global__ void __launch_bounds__(256) k_reduce(int64_t n, F f, double identity, double* __restrict__ part, unsigned* ticket,
                                                 double* __restrict__ out) {
-    __shared__ double sm[8];
-    __shared__ bool last;
     pdl_sync();
-    double acc = identity;
-    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) acc = comb<KIND>(acc, f.term(i));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc = comb<KIND>(acc, __shfl_xor_sync(0xffffffffu, acc, o));
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double r = sm[0];
-#pragma unroll
-        for (int w = 1; w < 8; ++w) r = comb<KIND>(r, sm[w]);
-        part[blockIdx.x] = r;
-        __threadfence();
-        last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    // the last CTA: partials in index order (thread t owns partials t, t+256, ...; then the same tree as above)
-    double r = identity;
-    for (int k = threadIdx.x; k < (int)gridDim.x; k += 256) r = comb<KIND>(r, __ldcg(part + k));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) r = comb<KIND>(r, __shfl_xor_sync(0xffffffffu, r, o));
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = r;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = sm[0];
-#pragma unroll
-        for (int w = 1; w < 8; ++w) t = comb<KIND>(t, sm[w]);
-        out[0] = f.finish(t);
-        *ticket = 0;                                    // ready for the next reduction on this stream
-    }
+    double acc[1] = {identity};
+    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) acc[0] = comb<KIND>(acc[0], f.term(i));
+    double r[1];
+    if (grid_reduce<KIND, 1>(acc, identity, part, ticket, r) && threadIdx.x == 0) out[0] = f.finish(r[0]);
 }
 
 template <int KIND, class F>
 int run_reduce(b2_bounds* b, int64_t n, const F& f, double identity, double* out_d, void* stream, const char* who) {
     if (!b || !out_d || n < 0) { set_error(std::string(who) + ": invalid argument"); return B2_ERR_INVALID; }
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, B2_RED_BLOCKS));
-    cudaError_t e = launch_pdl(k_reduce<KIND, F>, dim3(grid), dim3(256), 0, as_stream(stream), n, f, identity, b->red_part.p, b->red_ticket.p, out_d);
+    cudaError_t e = launch_pdl(k_reduce<KIND, F>, dim3(grid_red(n)), dim3(256), 0, as_stream(stream), n, f, identity, b->red_part.p,
+                               b->red_ticket.p, out_d);
     if (e != cudaSuccess) return cuda_fail(e, who, __FILE__, __LINE__);
     return B2_OK;
 }
-
-__device__ __forceinline__ double dinf() { return __longlong_as_double(0x7ff0000000000000LL); }
 
 // ---- get_alpha_max (src/IPM/kernels.jl:356-371)
 struct AlphaMax {
@@ -286,7 +245,7 @@ __global__ void k_set_aug_rhs(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub
                               double* __restrict__ p) {
     pdl_sync();
     const int64_t tot = n_tot + m + nlb + nub;
-    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < tot; t += (int64_t)gridDim.x * blockDim.x) {
+    GRID_STRIDE(t, tot) {
         double v;
         if (t < n_tot) v = -f[t] + zl[t] - zu[t] - jacl[t];
         else if (t < n_tot + m) v = -c[t - n_tot];
@@ -297,8 +256,6 @@ __global__ void k_set_aug_rhs(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub
 }
 
 }  // namespace
-
-#define B2_NEED(cond, who) do { if (!(cond)) { set_error(who ": invalid argument"); return B2_ERR_INVALID; } } while (0)
 
 extern "C" {
 
@@ -382,8 +339,7 @@ int b2_set_aug_rhs(b2_bounds* b, int64_t m, const double* x_d, const double* xl_
     const int64_t tot = b->n_tot + m + b->nlb + b->nub;
     if (tot == 0) return B2_OK;
     B2_NEED(p_d && (b->n_tot == 0 || (x_d && xl_d && xu_d && f_d && zl_d && zu_d && jacl_d)) && (m == 0 || c_d), "b2_set_aug_rhs");
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((tot + 255) / 256, 8 * sm_count()));
-    cudaError_t e = launch_pdl(k_set_aug_rhs, dim3(grid), dim3(256), 0, as_stream(stream), b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p,
+    cudaError_t e = launch_pdl(k_set_aug_rhs, dim3(grid_elem(tot)), dim3(256), 0, as_stream(stream), b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p,
                                x_d, xl_d, xu_d, f_d, zl_d, zu_d, jacl_d, c_d, mu, p_d);
     if (e != cudaSuccess) return cuda_fail(e, "b2_set_aug_rhs", __FILE__, __LINE__);
     return B2_OK;

@@ -32,12 +32,8 @@ extern "C" int b2_bounds_create(int64_t n_tot, int64_t nlb, int64_t nub, const i
     b->n_tot = n_tot; b->nlb = nlb; b->nub = nub;
     if (b->ind_lb.upload(ind_lb_h, nlb) != cudaSuccess || b->ind_ub.upload(ind_ub_h, nub) != cudaSuccess ||
         b->lbpos.upload(lp.data(), lp.size()) != cudaSuccess || b->ubpos.upload(up.data(), up.size()) != cudaSuccess ||
-        b->red_part.alloc(B2_RED_BLOCKS) != cudaSuccess || b->red_ticket.alloc(1) != cudaSuccess ||
-        cudaMemset(b->red_ticket.p, 0, sizeof(unsigned)) != cudaSuccess ||
-        b->curv_part.alloc(4 * B2_RED_BLOCKS) != cudaSuccess || b->curv_ticket.alloc(1) != cudaSuccess ||
-        cudaMemset(b->curv_ticket.p, 0, sizeof(unsigned)) != cudaSuccess ||
-        b->qf_part.alloc(8 * B2_RED_BLOCKS) != cudaSuccess || b->qf_ticket.alloc(1) != cudaSuccess ||
-        cudaMemset(b->qf_ticket.p, 0, sizeof(unsigned)) != cudaSuccess || b->qf_state.alloc(B2_QF_STATE_DOUBLES) != cudaSuccess ||
+        b->red_part.alloc(8 * B2_RED_BLOCKS) != cudaSuccess || b->red_ticket.alloc(1) != cudaSuccess ||
+        cudaMemset(b->red_ticket.p, 0, sizeof(unsigned)) != cudaSuccess || b->qf_state.alloc(B2_QF_STATE_DOUBLES) != cudaSuccess ||
         cudaMemset(b->qf_state.p, 0, B2_QF_STATE_DOUBLES * sizeof(double)) != cudaSuccess) {
         delete b;
         return cuda_fail(cudaGetLastError(), "bounds upload", __FILE__, __LINE__);
@@ -46,9 +42,6 @@ extern "C" int b2_bounds_create(int64_t n_tot, int64_t nlb, int64_t nub, const i
     return B2_OK;
 }
 extern "C" int b2_bounds_destroy(b2_bounds* b) { delete b; return B2_OK; }
-
-static inline int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-#define GRID_STRIDE(i, n) for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
 
 // ---------------------------------------------------------------------------------------------------------
 __global__ void k_set_aug_diagonal(int64_t n_tot, const int32_t* __restrict__ lbpos, const int32_t* __restrict__ ubpos,
@@ -67,7 +60,7 @@ extern "C" int b2_set_aug_diagonal(b2_bounds* b, const double* reg_d, const doub
                                    const double* u_lower_d, const double* u_diag_d, double* pr_diag_d, void* stream) {
     if (!b || !reg_d || !pr_diag_d) { set_error("b2_set_aug_diagonal: invalid argument"); return B2_ERR_INVALID; }
     if (b->n_tot == 0) return B2_OK;
-    launch_pdl(k_set_aug_diagonal, dim3(grid_for(b->n_tot)), dim3(256), 0, as_stream(stream), b->n_tot, b->lbpos.p, b->ubpos.p, reg_d, l_lower_d, l_diag_d,
+    launch_pdl(k_set_aug_diagonal, dim3(grid_elem(b->n_tot)), dim3(256), 0, as_stream(stream), b->n_tot, b->lbpos.p, b->ubpos.p, reg_d, l_lower_d, l_diag_d,
                                                                          u_lower_d, u_diag_d, pr_diag_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
@@ -94,7 +87,7 @@ extern "C" int b2_set_aug_diagonal_unreduced(int64_t n_tot, int64_t nlb, int64_t
     }
     const int64_t tot = n_tot + nlb + nub;
     if (tot == 0) return B2_OK;
-    k_set_aug_diagonal_unreduced<<<grid_for(tot), 256, 0, as_stream(stream)>>>(n_tot, nlb, nub, reg_d, l_lower_d, u_lower_d, pr_diag_d,
+    k_set_aug_diagonal_unreduced<<<grid_elem(tot), 256, 0, as_stream(stream)>>>(n_tot, nlb, nub, reg_d, l_lower_d, u_lower_d, pr_diag_d,
                                                                                l_lower_aug_d, u_lower_aug_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
@@ -121,7 +114,7 @@ static int unreduced_scale(const char* name, int64_t n_tot, int64_t m, int64_t n
         return B2_ERR_INVALID;
     }
     if (nlb + nub == 0) return B2_OK;
-    k_unreduced_scale<POST><<<grid_for(nlb + nub), 256, 0, as_stream(stream)>>>(nlb, nub, sl, su, w + n_tot + m);
+    k_unreduced_scale<POST><<<grid_elem(nlb + nub), 256, 0, as_stream(stream)>>>(nlb, nub, sl, su, w + n_tot + m);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -145,7 +138,7 @@ extern "C" int b2_regularize_diagonal(int64_t n_tot, int64_t m, double dw, doubl
                                       double* du_diag_d, void* stream) {
     if (n_tot < 0 || m < 0 || !reg_d || !pr_diag_d || (m && !du_diag_d)) { set_error("b2_regularize_diagonal: invalid argument"); return B2_ERR_INVALID; }
     if (n_tot + m == 0) return B2_OK;
-    k_regularize<<<grid_for(n_tot + m), 256, 0, as_stream(stream)>>>(n_tot, m, dw, dc, reg_d, pr_diag_d, du_diag_d);
+    k_regularize<<<grid_elem(n_tot + m), 256, 0, as_stream(stream)>>>(n_tot, m, dw, dc, reg_d, pr_diag_d, du_diag_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -166,7 +159,7 @@ __global__ void k_reduce_rhs(int64_t n_tot, int64_t m, int64_t nlb, const int32_
 extern "C" int b2_reduce_rhs(b2_bounds* b, int64_t m, const double* l_diag_d, const double* u_diag_d, double* w_d, void* stream) {
     if (!b || !w_d) { set_error("b2_reduce_rhs: invalid argument"); return B2_ERR_INVALID; }
     if (b->n_tot == 0) return B2_OK;
-    k_reduce_rhs<<<grid_for(b->n_tot), 256, 0, as_stream(stream)>>>(b->n_tot, m, b->nlb, b->lbpos.p, b->ubpos.p, l_diag_d, u_diag_d, w_d);
+    k_reduce_rhs<<<grid_elem(b->n_tot), 256, 0, as_stream(stream)>>>(b->n_tot, m, b->nlb, b->lbpos.p, b->ubpos.p, l_diag_d, u_diag_d, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -189,7 +182,7 @@ extern "C" int b2_finish_aug_solve(b2_bounds* b, int64_t m, const double* l_lowe
                                    const double* l_diag_d, const double* u_diag_d, double* w_d, void* stream) {
     if (!b || !w_d) { set_error("b2_finish_aug_solve: invalid argument"); return B2_ERR_INVALID; }
     if (b->nlb + b->nub == 0) return B2_OK;
-    launch_pdl(k_finish_aug_solve, dim3(grid_for(b->nlb + b->nub)), dim3(256), 0, as_stream(stream), b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p,
+    launch_pdl(k_finish_aug_solve, dim3(grid_elem(b->nlb + b->nub)), dim3(256), 0, as_stream(stream), b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p,
                                                                                l_lower_d, u_lower_d, l_diag_d, u_diag_d, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
@@ -309,21 +302,21 @@ __global__ void k_spmv_sym(int64_t n, const int32_t* colptr, const int32_t* rowv
 extern "C" int b2_spmv_n(b2_spmv_plan* p, const double* nz_d, const double* x_d, double* y_d, double alpha, double beta, void* stream) {
     if (!p || !x_d || !y_d) { set_error("b2_spmv_n: invalid argument"); return B2_ERR_INVALID; }
     if (p->nrow == 0) return B2_OK;
-    k_spmv_n<<<grid_for(p->nrow), 256, 0, as_stream(stream)>>>(p->nrow, p->rowptr.p, p->colidx.p, p->valmap.p, nz_d, x_d, y_d, alpha, beta);
+    k_spmv_n<<<grid_elem(p->nrow), 256, 0, as_stream(stream)>>>(p->nrow, p->rowptr.p, p->colidx.p, p->valmap.p, nz_d, x_d, y_d, alpha, beta);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
 extern "C" int b2_spmv_t(b2_spmv_plan* p, const double* nz_d, const double* x_d, double* y_d, double alpha, double beta, void* stream) {
     if (!p || !x_d || !y_d) { set_error("b2_spmv_t: invalid argument"); return B2_ERR_INVALID; }
     if (p->ncol == 0) return B2_OK;
-    k_spmv_t<<<grid_for(p->ncol), 256, 0, as_stream(stream)>>>(p->ncol, p->colptr.p, p->rowval.p, nz_d, x_d, y_d, alpha, beta);
+    k_spmv_t<<<grid_elem(p->ncol), 256, 0, as_stream(stream)>>>(p->ncol, p->colptr.p, p->rowval.p, nz_d, x_d, y_d, alpha, beta);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
 extern "C" int b2_spmv_symlower(b2_spmv_plan* p, const double* nz_d, const double* x_d, double* y_d, double alpha, double beta, void* stream) {
     if (!p || !x_d || !y_d || p->nrow != p->ncol) { set_error("b2_spmv_symlower: invalid argument"); return B2_ERR_INVALID; }
     if (p->nrow == 0) return B2_OK;
-    k_spmv_sym<<<grid_for(p->nrow), 256, 0, as_stream(stream)>>>(p->nrow, p->colptr.p, p->rowval.p, p->rowptr.p, p->colidx.p, p->valmap.p,
+    k_spmv_sym<<<grid_elem(p->nrow), 256, 0, as_stream(stream)>>>(p->nrow, p->colptr.p, p->rowval.p, p->rowptr.p, p->colidx.p, p->valmap.p,
                                                                  nz_d, x_d, y_d, alpha, beta);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
@@ -377,7 +370,7 @@ extern "C" int b2_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const dou
     KktMulArgs a = make_kktmul(b, m, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta);
     const int64_t tot = a.n_tot + a.m + a.nlb + a.nub;
     if (tot == 0) return B2_OK;
-    k_kktmul<<<grid_for(tot), 256, 0, as_stream(stream)>>>(a, x_d, w_d);
+    k_kktmul<<<grid_elem(tot), 256, 0, as_stream(stream)>>>(a, x_d, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -491,9 +484,9 @@ static int cond_pre(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n,
         return B2_ERR_INVALID;
     }
     cudaStream_t st = as_stream(stream);
-    launch_pdl(k_cond_pre1, dim3(grid_for(n + m)), dim3(256), 0, st, make_cond(b, n, m, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d), buffer_d, w_d,
+    launch_pdl(k_cond_pre1, dim3(grid_elem(n + m)), dim3(256), 0, st, make_cond(b, n, m, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d), buffer_d, w_d,
                norms_d);
-    launch_pdl(k_cond_pre2, dim3(grid_for(n)), dim3(256), 0, st, n, jt->rowptr.p, jt->colidx.p, jt->valmap.p, jt_nz_d, buffer_d, w_d);
+    launch_pdl(k_cond_pre2, dim3(grid_elem(n)), dim3(256), 0, st, n, jt->rowptr.p, jt->colidx.p, jt->valmap.p, jt_nz_d, buffer_d, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -505,7 +498,7 @@ static int cond_post(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n
         set_error(std::string(name) + ": invalid argument");
         return B2_ERR_INVALID;
     }
-    launch_pdl(k_cond_post<UPDATE>, dim3(grid_for(n + m)), dim3(256), 0, as_stream(stream),
+    launch_pdl(k_cond_post<UPDATE>, dim3(grid_elem(n + m)), dim3(256), 0, as_stream(stream),
                make_cond(b, n, m, l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d), jt->colptr.p, jt->rowval.p, jt_nz_d, l_lower_d, u_lower_d,
                buffer_d, w_d, x_d, (unsigned long long*)(UPDATE ? norms_d + 1 : nullptr));
     B2_CUDA(cudaGetLastError());
@@ -587,8 +580,8 @@ static int cond_mul(b2_bounds* b, b2_spmv_plan* hess, b2_spmv_plan* jt, int64_t 
     c.h_nz = hess_nz_d; c.j_nz = jt_nz_d;
     KktMulArgs a = make_kktmul(b, m, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta);
     const int64_t tot = a.n_tot + a.m + a.nlb + a.nub;
-    if (y_d) launch_pdl(k_cond_mul<true>, dim3(grid_for(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
-    else launch_pdl(k_cond_mul<false>, dim3(grid_for(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
+    if (y_d) launch_pdl(k_cond_mul<true>, dim3(grid_elem(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
+    else launch_pdl(k_cond_mul<false>, dim3(grid_elem(tot)), dim3(256), 0, as_stream(stream), c, a, x_d, y_d, w_d, (unsigned long long*)norm_inf_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -656,7 +649,7 @@ extern "C" int b2_richardson_begin(int64_t n, const double* b_d, double* w_d, do
     if (n < 0 || !norm_b_d || (n && (!b_d || !w_d || !x_d))) { set_error("b2_richardson_begin: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     B2_CUDA(cudaMemsetAsync(norm_b_d, 0, sizeof(double), st));
-    if (n) k_richardson_begin<<<grid_for(n), 256, 0, st>>>(n, b_d, w_d, x_d, (unsigned long long*)norm_b_d);
+    if (n) k_richardson_begin<<<grid_elem(n), 256, 0, st>>>(n, b_d, w_d, x_d, (unsigned long long*)norm_b_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -664,7 +657,7 @@ extern "C" int b2_richardson_update(int64_t n, const double* b_d, double* w_d, d
     if (n < 0 || !norms_d || (n && (!b_d || !w_d || !x_d))) { set_error("b2_richardson_update: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     B2_CUDA(cudaMemsetAsync(norms_d, 0, 2 * sizeof(double), st));
-    if (n) launch_pdl(k_richardson_update, dim3(grid_for(n)), dim3(256), 0, st, n, b_d, w_d, x_d, (unsigned long long*)(norms_d + 1));
+    if (n) launch_pdl(k_richardson_update, dim3(grid_elem(n)), dim3(256), 0, st, n, b_d, w_d, x_d, (unsigned long long*)(norms_d + 1));
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -672,7 +665,7 @@ extern "C" int b2_norm_inf(int64_t n, const double* x_d, double* out_d, void* st
     if (n < 0 || !out_d || (n && !x_d)) { set_error("b2_norm_inf: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     B2_CUDA(cudaMemsetAsync(out_d, 0, sizeof(double), st));
-    if (n) k_norm_inf<<<grid_for(n), 256, 0, st>>>(n, x_d, (unsigned long long*)out_d);
+    if (n) k_norm_inf<<<grid_elem(n), 256, 0, st>>>(n, x_d, (unsigned long long*)out_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -681,13 +674,13 @@ __global__ void k_copy(int64_t n, const double* __restrict__ x, double* __restri
 __global__ void k_fill(int64_t n, double v, double* __restrict__ x) { GRID_STRIDE(i, n) x[i] = v; }
 extern "C" int b2_axpy(int64_t n, double a, const double* x_d, double* y_d, void* stream) {
     if (n < 0 || (n && (!x_d || !y_d))) return B2_ERR_INVALID;
-    if (n) k_axpy<<<grid_for(n), 256, 0, as_stream(stream)>>>(n, a, x_d, y_d);
+    if (n) k_axpy<<<grid_elem(n), 256, 0, as_stream(stream)>>>(n, a, x_d, y_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
 extern "C" int b2_copy(int64_t n, const double* x_d, double* y_d, void* stream) {
     if (n < 0 || (n && (!x_d || !y_d))) return B2_ERR_INVALID;
-    if (n) k_copy<<<grid_for(n), 256, 0, as_stream(stream)>>>(n, x_d, y_d);
+    if (n) k_copy<<<grid_elem(n), 256, 0, as_stream(stream)>>>(n, x_d, y_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -718,7 +711,7 @@ extern "C" int b2_copy_many(int32_t count, const double* const* src_d, double* c
 }
 extern "C" int b2_fill(int64_t n, double v, double* x_d, void* stream) {
     if (n < 0 || (n && !x_d)) return B2_ERR_INVALID;
-    if (n) k_fill<<<grid_for(n), 256, 0, as_stream(stream)>>>(n, v, x_d);
+    if (n) k_fill<<<grid_elem(n), 256, 0, as_stream(stream)>>>(n, v, x_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -967,7 +960,7 @@ extern "C" int b2d_kkt_solve_pre(b2d_kkt* k, b2_bounds* b, const double* jac_d, 
     cudaStream_t st = as_stream(stream);
     const int64_t tot = b->n_tot + k->n_eq;
     if (tot == 0) return B2_OK;
-    k_dcond_pre<<<grid_for(tot), 256, 0, st>>>(k->n, k->m, k->ns, k->n_eq, b->nlb, b->lbpos.p, b->ubpos.p, k->ind_ineq.p, k->ind_eq.p,
+    k_dcond_pre<<<grid_elem(tot), 256, 0, st>>>(k->n, k->m, k->ns, k->n_eq, b->nlb, b->lbpos.p, b->ubpos.p, k->ind_ineq.p, k->ind_eq.p,
                                               l_diag_d, u_diag_d, pr_diag_d, diag_buffer_d, buffer_d, pd_buffer_d, w_d);
     if (k->m > 0 && k->n > 0)
         k_gemv_t<<<(k->n + 7) / 8, 256, 0, st>>>(k->m, k->n, k->m, jac_d, buffer_d, pd_buffer_d, 1.0, 1.0);
@@ -984,7 +977,7 @@ extern "C" int b2d_kkt_solve_post(b2d_kkt* k, b2_bounds* b, const double* jac_d,
     if (tot == 0) return B2_OK;
     if (k->m > 0)
         k_gemv_n<<<(k->m + GEMV_ROWS - 1) / GEMV_ROWS, 256, 0, st>>>(k->m, k->n, k->m, jac_d, pd_buffer_d, w_d + b->n_tot, 1.0, 0.0);    // dual(w) = jac * xx
-    k_dcond_post<<<grid_for(tot), 256, 0, st>>>(k->n, k->m, k->ns, k->n_eq, k->ind_ineq.p, k->ind_eq.p, pr_diag_d, diag_buffer_d, buffer_d,
+    k_dcond_post<<<grid_elem(tot), 256, 0, st>>>(k->n, k->m, k->ns, k->n_eq, k->ind_ineq.p, k->ind_eq.p, pr_diag_d, diag_buffer_d, buffer_d,
                                                pd_buffer_d, w_d);
     B2_CUDA(cudaGetLastError());
     return b2_finish_aug_solve(b, k->m, l_lower_d, u_lower_d, l_diag_d, u_diag_d, w_d, stream);
@@ -1003,7 +996,7 @@ extern "C" int b2d_kkt_mul(b2d_kkt* k, b2_bounds* b, const double* hess_d, const
     }
     KktMulArgs a = make_kktmul(b, m, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta);
     const int64_t tot = a.n_tot + a.m + a.nlb + a.nub;
-    if (tot) k_dcond_mul_tail<<<grid_for(tot), 256, 0, st>>>(a, n, k->ineq_pos.p, k->ind_ineq.p, x_d, w_d);
+    if (tot) k_dcond_mul_tail<<<grid_elem(tot), 256, 0, st>>>(a, n, k->ineq_pos.p, k->ind_ineq.p, x_d, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }

@@ -3,14 +3,15 @@
 //
 // B_k = sigma I - U U' + V V' on the n model variables.  Every state value (counters, sigma, the pairs, the small matrices) lives in
 // device memory, so no entry point synchronises the host and every one can be captured in a CUDA graph.  The n-wide reductions are
-// block partials summed by the last block to finish (a ticket), both in a fixed order: replays are bit-identical.  The small dense
-// algebra (Cholesky of M, Bunch-Kaufman of T, its solve) runs in that last block.  Concurrent calls on one handle from two
-// streams are not supported (one ticket per handle).
+// grid_sums (grid_reduce.cuh): block partials summed in a fixed order by the last block to finish, so replays are bit-identical.
+// The small dense algebra (Cholesky of M, Bunch-Kaufman of T, its solve) runs in that last block.  Concurrent calls on one handle
+// from two streams are not supported (one ticket per handle).
 #include <algorithm>
 #include <cmath>
 #include <vector>
 
 #include "common.cuh"
+#include "grid_reduce.cuh"
 
 using namespace b2;
 
@@ -18,7 +19,6 @@ namespace {
 constexpr int LB_MAXP = 32;              // max_history bound: T is at most 64 x 64 and fits in one CTA's shared memory
 constexpr int LB_T = 256;                // threads of the reduction kernels
 constexpr int LB_ROW_T = 64;             // threads of the row kernels
-constexpr int LB_MAX_BLOCKS = 256;
 constexpr int LB_TILE = 32;              // rows per shared-memory tile of the E'H reduction
 constexpr int LB_NQ_MAX = 3 + 2 * LB_MAXP;
 constexpr int LB_NT_MAX = (2 * LB_MAXP) * (2 * LB_MAXP + 1) / 2;
@@ -35,8 +35,6 @@ struct LbState {
     unsigned ticket;
 };
 
-// number of blocks of every n-wide reduction: a function of n only, so that the summation order never changes
-int lb_blocks(int64_t n) { return (int)std::min<int64_t>(LB_MAX_BLOCKS, std::max<int64_t>(1, (n + 2047) / 2048)); }
 int lb_rows_grid(int64_t n) { return (int)std::max<int64_t>(1, (n + LB_ROW_T - 1) / LB_ROW_T); }
 }  // namespace
 
@@ -54,55 +52,6 @@ struct b2_lbfgs {
 
 // ---------------------------------------------------------------------------------------------------------------- device helpers
 namespace {
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// Last-block election: every block has written its partials; returns true in all threads of the last block to arrive, which
-// may then read every partial.  The last block re-arms the ticket for the next launch.
-__device__ __forceinline__ bool last_block(unsigned* ticket) {
-    __shared__ bool s_last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (!s_last) return false;
-    __threadfence();
-    if (threadIdx.x == 0) *ticket = 0;
-    return true;
-}
-
-// out[q] = sum_{r < n} f(q, r), q < nq, for the whole grid in a fixed order: each thread sums its rows (grid stride), warps
-// reduce by shuffles, warps are summed in order into this block's partials, and the last block sums the blocks in order.  Returns
-// true (with out[] in shared memory, valid after the call) in the last block only.
-template <class F>
-__device__ __forceinline__ bool grid_sums(int64_t n, int nq, F f, double* part, unsigned* ticket, double* out) {
-    __shared__ double sh[LB_NQ_MAX * (LB_T / 32)];
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-    for (int q = 0; q < nq; ++q) {
-        double acc = 0.0;
-        for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x)
-            acc += f(q, r);
-        acc = warp_sum(acc);
-        if (lane == 0) sh[q * nw + w] = acc;
-    }
-    __syncthreads();
-    for (int q = threadIdx.x; q < nq; q += blockDim.x) {
-        double a = 0.0;
-        for (int k = 0; k < nw; ++k) a += sh[q * nw + k];
-        part[(int64_t)blockIdx.x * nq + q] = a;
-    }
-    if (!last_block(ticket)) return false;
-    for (int q = threadIdx.x; q < nq; q += blockDim.x) {
-        double a = 0.0;
-        for (int b = 0; b < (int)gridDim.x; ++b) a += __ldcg(part + (int64_t)b * nq + q);
-        out[q] = a;
-    }
-    __syncthreads();
-    return true;
-}
 
 // Unblocked Bunch-Kaufman of the symmetric N x N matrix A (column-major, ld N, lower triangle) in shared memory, in place,
 // by the whole block: LAPACK dsytf2 'L' (same alpha = (1 + sqrt 17) / 8, same first-maximum pivot search, same update
@@ -265,7 +214,7 @@ __global__ void __launch_bounds__(LB_T) k_lb_init(int64_t n, const double* __res
                                                  LbState* st, double* part) {
     __shared__ double out[1];
     auto f = [&](int, int64_t r) { return g0[r] * g0[r]; };
-    if (!grid_sums(n, 1, f, part, &st->ticket, out)) return;
+    if (!grid_sums<LB_NQ_MAX>(n, 1, f, part, &st->ticket, out)) return;
     if (threadIdx.x == 0) {
         const double norm_g0 = out[0];
         const double rho0 = norm_g0 < sqrt(2.220446049250313e-16) ? 1.0 : (f0 == 0.0 ? 1.0 / norm_g0 : fabs(f0) / norm_g0);
@@ -301,7 +250,7 @@ __global__ void __launch_bounds__(LB_T) k_lb_update_small(int64_t n, int pbar, i
         if (j >= p_old) return 0.0;
         return (q < 3 + pbar ? S : Y)[r + (int64_t)j * n] * sr;
     };
-    if (!grid_sums(n, nq, f, part, &st->ticket, tot)) return;
+    if (!grid_sums<LB_NQ_MAX>(n, nq, f, part, &st->ticket, tot)) return;
     const int t = threadIdx.x, nt = blockDim.x;
     if (t == 0) {
         const double eps = 2.220446049250313e-16;
@@ -542,7 +491,7 @@ __global__ void __launch_bounds__(LB_T, 2) k_lb_apply_xr(int64_t n, int pbar, Lb
     const int p = (int)st->p;
     if (p == 0) return;                                           // nothing to correct: w keeps its bits
     auto f = [&](int c, int64_t r) { return e_val(U, V, n, p, c, r) * w[r]; };
-    if (!grid_sums(n, 2 * p, f, part, &st->ticket, xr)) return;
+    if (!grid_sums<LB_NQ_MAX>(n, 2 * p, f, part, &st->ticket, xr)) return;
     const int N2 = 2 * pbar;
     if (threadIdx.x < N2 && threadIdx.x >= 2 * p) xr[threadIdx.x] = 0.0;
     __syncthreads();
@@ -570,7 +519,7 @@ __global__ void __launch_bounds__(LB_T) k_lb_mul_vx(int64_t n, LbState* st, cons
     const int p = (int)st->p;
     if (p == 0) return;
     auto f = [&](int c, int64_t r) { return e_val(U, V, n, p, c, r) * x[r]; };
-    if (!grid_sums(n, 2 * p, f, part, &st->ticket, vx)) return;
+    if (!grid_sums<LB_NQ_MAX>(n, 2 * p, f, part, &st->ticket, vx)) return;
     if (threadIdx.x < 2 * p) gvx[threadIdx.x] = threadIdx.x < p ? -vx[threadIdx.x] : vx[threadIdx.x];
 }
 
@@ -604,8 +553,6 @@ __global__ void k_bk_solve_debug(int N, const double* F, const int32_t* ipiv, do
     for (int i = threadIdx.x; i < N; i += 32) b[i] = sb[i];
 }
 
-int grid_stride_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------------- C ABI
@@ -619,7 +566,7 @@ extern "C" int b2_lbfgs_create(int64_t n, int32_t max_history, int32_t init_stra
     auto* h = new b2_lbfgs();
     const int pb = max_history;
     h->n = n; h->pbar = pb; h->strategy = init_strategy; h->init_value = init_value; h->sigma_min = sigma_min; h->sigma_max = sigma_max;
-    h->nb = lb_blocks(n);
+    h->nb = grid_sums_blocks(n);
     const size_t np = (size_t)n * pb, pp = (size_t)pb * pb, tt = (size_t)4 * pb * pb;
     const size_t npart = (size_t)h->nb * std::max(LB_NQ_MAX, LB_NT_MAX);
     cudaError_t e = cudaSuccess;
@@ -652,7 +599,7 @@ extern "C" int b2_lbfgs_init(b2_lbfgs* h, double* Bk_d, const double* g0_d, doub
     if (!h || !Bk_d || !g0_d) { set_error("b2_lbfgs_init: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     k_lb_init<<<h->nb, LB_T, 0, st>>>(h->n, g0_d, f0, h->init_value, h->st.p, h->part.p);
-    k_lb_fill<<<grid_stride_blocks(h->n), 256, 0, st>>>(h->n, h->st.p, Bk_d);
+    k_lb_fill<<<grid_elem(h->n), 256, 0, st>>>(h->n, h->st.p, Bk_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -682,7 +629,7 @@ extern "C" int b2_lbfgs_smw_prepare(b2_lbfgs* h, b2_solver* s, int64_t n_tot_plu
     }
     cudaStream_t st = as_stream(stream);
     const int64_t N = n_tot_plus_m;
-    k_lb_fill_e<<<grid_stride_blocks(N * 2 * h->pbar), 256, 0, st>>>(h->n, N, h->pbar, h->st.p, h->U.p, h->V.p, H_d);
+    k_lb_fill_e<<<grid_elem(N * 2 * h->pbar), 256, 0, st>>>(h->n, N, h->pbar, h->st.p, h->U.p, h->V.p, H_d);
     B2_CUDA(cudaGetLastError());
     const int rc = b2_solve(s, H_d, 2 * h->pbar, stream);      // H = C^{-1} E; padding columns stay exactly zero
     if (rc != B2_OK) return rc;
@@ -695,7 +642,7 @@ extern "C" int b2_lbfgs_smw_apply(b2_lbfgs* h, int64_t n_tot_plus_m, const doubl
     if (!h || !H_d || !w_d || n_tot_plus_m < h->n) { set_error("b2_lbfgs_smw_apply: invalid argument (n_tot_plus_m >= n)"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     k_lb_apply_xr<<<h->nb, LB_T, 0, st>>>(h->n, h->pbar, h->st.p, h->U.p, h->V.p, w_d, h->part.p, h->Tf.p, h->ipiv.p, h->xr.p);
-    k_lb_apply_w<<<grid_stride_blocks(n_tot_plus_m), 256, 0, st>>>(n_tot_plus_m, h->st.p, H_d, h->xr.p, w_d);
+    k_lb_apply_w<<<grid_elem(n_tot_plus_m), 256, 0, st>>>(n_tot_plus_m, h->st.p, H_d, h->xr.p, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }
@@ -704,7 +651,7 @@ extern "C" int b2_lbfgs_kkt_mul_lowrank(b2_lbfgs* h, double alpha, const double*
     if (!h || !x_d || !w_d) { set_error("b2_lbfgs_kkt_mul_lowrank: invalid argument"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     k_lb_mul_vx<<<h->nb, LB_T, 0, st>>>(h->n, h->st.p, h->U.p, h->V.p, x_d, h->part.p, h->vx.p);
-    k_lb_mul_w<<<grid_stride_blocks(h->n), 256, 0, st>>>(h->n, alpha, h->st.p, h->U.p, h->V.p, h->vx.p, w_d);
+    k_lb_mul_w<<<grid_elem(h->n), 256, 0, st>>>(h->n, alpha, h->st.p, h->U.p, h->V.p, h->vx.p, w_d);
     B2_CUDA(cudaGetLastError());
     return B2_OK;
 }

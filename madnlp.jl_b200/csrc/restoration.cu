@@ -8,7 +8,6 @@
 // Rounding: every formula is written with __dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn / __dsqrt_rn in the reference's left-to-right
 // order, so no contraction can happen and the outputs are bit-identical to the broadcasts; x^2 is x*x (Julia lowers a literal square
 // so); min / max are Julia's (NaN in, NaN out; -0.0 below +0.0).
-#include <algorithm>
 #include <cmath>
 
 #include "bounds.cuh"
@@ -17,25 +16,6 @@
 using namespace b2;
 
 namespace {
-
-inline int grid_elem(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 8 * sm_count())); }
-
-// Julia's min / max on Float64 (base/math.jl): diff = x - y; a NaN operand returns diff, otherwise the sign of diff decides
-__device__ __forceinline__ double jl_min(double x, double y) {
-    const double d = __dsub_rn(x, y);
-    if (x != x || y != y) return d;
-    return signbit(d) ? x : y;
-}
-__device__ __forceinline__ double jl_max(double x, double y) {
-    const double d = __dsub_rn(x, y);
-    if (x != x || y != y) return d;
-    return signbit(d) ? y : x;
-}
-
-// sign flip as Julia's unary minus does it (NaN payload and sign included)
-__device__ __forceinline__ double neg(double v) { return __longlong_as_double(__double_as_longlong(v) ^ (long long)0x8000000000000000ULL); }
-
-#define B2_GRID_STRIDE(t, tot) for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < (tot); t += (int64_t)gridDim.x * blockDim.x)
 
 // ---- initialize_robust_restorer! after theta_ref and mu_R (restoration.jl:45-67), segments [n_tot | m | nlb | nub]:
 //   x_ref = x ; D_R = min(1, 1 / |x_ref|) ; f_R = 0
@@ -49,7 +29,7 @@ __global__ void k_rr_init(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, co
     pdl_sync();
     const int64_t tot = n_tot + m + nlb + nub;
     const double two_rho = __dmul_rn(2.0, rho);
-    B2_GRID_STRIDE(t, tot) {
+    GRID_STRIDE(t, tot) {
         if (t < n_tot) {
             const double xi = x[t];
             x_ref[t] = xi;
@@ -85,7 +65,7 @@ __global__ void k_set_aug_RR(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub,
                              double* __restrict__ u_lower, double* __restrict__ l_diag, double* __restrict__ u_diag) {
     pdl_sync();
     const int64_t tot = n_tot + m + nlb + nub;
-    B2_GRID_STRIDE(t, tot) {
+    GRID_STRIDE(t, tot) {
         if (t < n_tot) {
             const double d = D_R[t];
             reg[t] = __dadd_rn(del_w, __dmul_rn(zeta, __dmul_rn(d, d)));
@@ -116,7 +96,7 @@ __global__ void k_set_aug_rhs_RR(int64_t n_tot, int64_t m, int64_t nlb, int64_t 
                                  double* __restrict__ p) {
     pdl_sync();
     const int64_t tot = n_tot + m + nlb + nub;
-    B2_GRID_STRIDE(t, tot) {
+    GRID_STRIDE(t, tot) {
         double v;
         if (t < n_tot) {
             v = __dsub_rn(__dsub_rn(__dadd_rn(neg(f_R[t]), zl[t]), zu[t]), jacl[t]);
@@ -144,7 +124,7 @@ __global__ void k_finish_aug_solve_RR(int64_t m, const double* __restrict__ l, c
                                       double mu, double rho, double* __restrict__ dpp, double* __restrict__ dnn, double* __restrict__ dzp,
                                       double* __restrict__ dzn) {
     pdl_sync();
-    B2_GRID_STRIDE(j, m) {
+    GRID_STRIDE(j, m) {
         const double lj = l[j], dlj = dl[j], pj = pp[j], nj = nn[j], zpj = zp[j], znj = zn[j];
         const double a = __dsub_rn(__dsub_rn(__dsub_rn(rho, lj), dlj), zpj);
         const double b = __dsub_rn(__dadd_rn(__dadd_rn(rho, lj), dlj), znj);
@@ -158,7 +138,7 @@ __global__ void k_finish_aug_solve_RR(int64_t m, const double* __restrict__ l, c
 __global__ void k_set_f_RR(int64_t n, double zeta, const double* __restrict__ D_R, const double* __restrict__ x,
                            const double* __restrict__ x_ref, double* __restrict__ f_R) {
     pdl_sync();
-    B2_GRID_STRIDE(i, n) {
+    GRID_STRIDE(i, n) {
         const double d = D_R[i];
         f_R[i] = __dmul_rn(__dmul_rn(zeta, __dmul_rn(d, d)), __dsub_rn(x[i], x_ref[i]));
     }
@@ -171,7 +151,7 @@ __device__ __forceinline__ double reset_dual(double z, double s, double mu, doub
 // ---- reset_bound_dual! (kernels.jl:775-786), one-vector form: z = max(min(z, (ks mu) / x), (mu / ks) / x)
 __global__ void k_reset_bound_dual(int64_t n, double* __restrict__ z, const double* __restrict__ x, double mu, double ks) {
     pdl_sync();
-    B2_GRID_STRIDE(i, n) z[i] = reset_dual(z[i], x[i], mu, ks);
+    GRID_STRIDE(i, n) z[i] = reset_dual(z[i], x[i], mu, ks);
 }
 
 // ---- reset_bound_dual! (:788-800), two-vector form on the bounded entries, segments [nlb | nub]:
@@ -180,7 +160,7 @@ __global__ void k_reset_bound_dual_lu(int64_t nlb, int64_t nub, const int64_t* _
                                       double* __restrict__ zl, double* __restrict__ zu, const double* __restrict__ x,
                                       const double* __restrict__ xl, const double* __restrict__ xu, double mu, double ks) {
     pdl_sync();
-    B2_GRID_STRIDE(t, nlb + nub) {
+    GRID_STRIDE(t, nlb + nub) {
         if (t < nlb) {
             const int64_t k = ind_lb[t];
             zl[k] = reset_dual(zl[k], __dsub_rn(x[k], xl[k]), mu, ks);
@@ -196,7 +176,7 @@ __global__ void k_reset_bound_dual_lu(int64_t nlb, int64_t nub, const int64_t* _
 __global__ void k_adjust_boundary(int64_t nlb, int64_t nub, const int64_t* __restrict__ ind_lb, const int64_t* __restrict__ ind_ub,
                                   const double* __restrict__ x, double* __restrict__ xl, double* __restrict__ xu, double c1, double c2) {
     pdl_sync();
-    B2_GRID_STRIDE(t, nlb + nub) {
+    GRID_STRIDE(t, nlb + nub) {
         if (t < nlb) {
             const int64_t k = ind_lb[t];
             const double xk = x[k], lk = xl[k];
@@ -211,7 +191,6 @@ __global__ void k_adjust_boundary(int64_t nlb, int64_t nub, const int64_t* __res
 
 }  // namespace
 
-#define B2_NEED(cond, who) do { if (!(cond)) { set_error(who ": invalid argument"); return B2_ERR_INVALID; } } while (0)
 #define B2_LAUNCH(who, kern, tot, ...) do {                                                                                        \
         if ((tot) == 0) return B2_OK;                                                                                              \
         cudaError_t e__ = launch_pdl(kern, dim3(grid_elem(tot)), dim3(256), 0, as_stream(stream), __VA_ARGS__);                    \
