@@ -14,6 +14,7 @@
 // the near-diagonal kernels below.  Pivoting is static (front_kernels.cuh): |d| < eps is replaced by sign(d)*eps and counted.
 #pragma once
 #include "front_kernels.cuh"
+#include "ptx.cuh"
 
 namespace b2 {
 
@@ -40,23 +41,6 @@ struct Diag128Smem {
     double tb[32 * 36];                   // phase I: one 32 x 32 product of the blocked inversion (column-major, ld 36)
     unsigned long long bar[4];            // [0..1] phase F (2..3 unused)
 };
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, int parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "MBAR_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra MBAR_DONE;\n"
-        "bra MBAR_WAIT;\n"
-        "MBAR_DONE:\n"
-        "}\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(parity) : "memory");
-}
 
 // Phase I of the diagonal-block kernel: on entry sm.Lc[k*DB_LDS + i] = l(i,k) for i > k and
 // 0 for i <= k; on exit the unit-lower inverse is in sm.Lc and has been stored to `out` (column-major, ld DB, zero outside nb x nb).
@@ -170,7 +154,7 @@ __global__ void __launch_bounds__(256, 1) k_big_diag128(FactorArgs a, const int3
         if (j <= i) cp_async8_zfill(stage + j * DB_LDS + i, Lp + (size_t)(kb + j) * f + kb + min(i, nb - 1), i < nb);
     }
     cp_async_commit_group();
-    cp_async_wait_group_n<0>();
+    cp_async_wait_group<0>();
     __syncthreads();
     if (nb < DB) {                                                 // identity padding
         if (tid < DB && tid >= nb) stage[tid * DB_LDS + tid] = 1.0;
@@ -212,7 +196,7 @@ __global__ void __launch_bounds__(256, 1) k_big_diag128(FactorArgs a, const int3
             if (have_next && !own_next) mbar_arrive(&sm.bar[(k + 1) & 1]);     // (this column has been read)
             if (!(fabs(dk) >= a.eps)) { dk = (dk < 0.0) ? -a.eps : a.eps; ++npert; }
             else if (dk < 0.0) ++nneg;
-            const double rk = fast_rcp_d(dk);
+            const double rk = fast_rcp(dk);
             double li[8];
 #pragma unroll
             for (int ia = 0; ia < 8; ++ia) li[ia] = -ur[ia] * rk;
@@ -323,7 +307,7 @@ __global__ void __launch_bounds__(256, 2) k_big_trsm(FactorArgs a, const int32_t
 #pragma unroll
         for (int y = 0; y < 4; ++y) c[x][y][0] = c[x][y][1] = 0.0;
     for (int ch = 0; ch < nchunk; ++ch) {
-        cp_async_wait_group_n<GU_STAGES - 2>();
+        cp_async_wait_group<GU_STAGES - 2>();
         __syncthreads();
         if (ch + GU_STAGES - 1 < nchunk) issue(ch + GU_STAGES - 1);
         cp_async_commit_group();
@@ -347,7 +331,7 @@ __global__ void __launch_bounds__(256, 2) k_big_trsm(FactorArgs a, const int32_t
         }
     }
     // epilogue: Ut -> shared memory as Cs[i][c], then coalesced stores of L21(i, c) = Ut(c, i) / d_c  (i fastest)
-    cp_async_wait_group_n<0>();
+    cp_async_wait_group<0>();
     __syncthreads();
     double* Cs = gu_sm;                                               // [TR_ROWS][GU_LDC]
 #pragma unroll
@@ -381,10 +365,6 @@ constexpr int NT_ROWS = 8;                       // rows per CTA of k_near_trsm
 constexpr int NT_LDA = 12;                       // A strip: As[k*12 + i]  (12 q + g covers every 16-bank residue exactly twice)
 constexpr int NT_LDB = DB + 4;                   // Linv:    Bs[k*132 + c]
 constexpr size_t NT_SMEM = (size_t)(DB * NT_LDA + DB * NT_LDB + DB) * sizeof(double);
-__device__ __forceinline__ void cp_async16_l2(void* smem_dst, const void* gsrc) {
-    const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gsrc) : "memory");
-}
 __global__ void __launch_bounds__(256, 1) k_near_trsm(FactorArgs a, const int32_t* __restrict__ list, int kb,
                                                       const double* __restrict__ Linv, const int64_t* __restrict__ linv_off) {
     const int s = list[0];
@@ -408,11 +388,11 @@ __global__ void __launch_bounds__(256, 1) k_near_trsm(FactorArgs a, const int32_
     // Linv(c, k) at Li[k*DB + c]: row k is needed for the 16-column groups that contain or follow k (pairs of columns, 16 bytes)
     for (int e = tid; e < DB * (DB / 2); e += 256) {
         const int p = e & (DB / 2 - 1), k = e >> 6;
-        if (k < 16 * (p / 8 + 1)) cp_async16_l2(Bs + k * NT_LDB + 2 * p, Li + (size_t)k * DB + 2 * p);
+        if (k < 16 * (p / 8 + 1)) cp_async16_cg(Bs + k * NT_LDB + 2 * p, Li + (size_t)k * DB + 2 * p);
     }
     cp_async_commit_group();
     if (tid < DB) dinv[tid] = 1.0 / a.dvec[d.col0 + kb + tid];
-    cp_async_wait_group_n<0>();
+    cp_async_wait_group<0>();
     __syncthreads();
     double c[2][2];
     const int t0 = warp, t1 = 15 - warp;                               // this warp's two 8-column tiles
@@ -469,7 +449,7 @@ __global__ void __launch_bounds__(256, 2) k_near_syrk(FactorArgs a, const int32_
     }
     cp_async_commit_group();
     if (tid < DB) dneg[tid] = -a.dvec[d.col0 + kb + tid];
-    cp_async_wait_group_n<0>();
+    cp_async_wait_group<0>();
     __syncthreads();
     const int mb = (warp & 1) * 16, nb = (warp >> 1) * 8;              // warp tile: 16 rows (two m8 fragments) x 8 columns
     double c[2][2] = {{0.0, 0.0}, {0.0, 0.0}};

@@ -9,6 +9,9 @@
 #include <utility>
 
 #include "../../include/b200kkt.h"
+#ifdef __CUDACC__
+#include "ptx.cuh"
+#endif
 
 namespace b2 {
 
@@ -84,14 +87,9 @@ __device__ __forceinline__ double jl_max(double x, double y) {
 __device__ __forceinline__ double jl_clamp(double x, double lo, double hi) { return x > hi ? hi : (x < lo ? lo : x); }
 #endif
 
-// ---- programmatic dependent launch (PDL).  A kernel launched through launch_pdl() may be scheduled while its predecessor
-// in the stream is still running; it must not touch anything the predecessor produces before pdl_wait() returns (and must
-// pass pdl_wait() before it exits, so that ITS completion implies the predecessor's).  Kernels with nothing to prefetch
-// simply start with pdl_sync(): what overlaps is the launch latency.
+// ---- programmatic dependent launch (PDL): the launch side.  The kernel side (pdl_trigger / pdl_wait / pdl_sync) and its rules
+// are in ptx.cuh.
 #ifdef __CUDACC__
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_sync() { pdl_trigger(); pdl_wait(); }
 template <typename... P, typename... A>
 inline cudaError_t launch_pdl(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
     cudaLaunchConfig_t cfg = {};

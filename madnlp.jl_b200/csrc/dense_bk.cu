@@ -20,6 +20,7 @@
 #include <climits>
 
 #include "dense_bk.cuh"
+#include "ptx.cuh"
 
 namespace b2 {
 namespace {
@@ -38,37 +39,27 @@ struct BkProg {
     uint32_t bar_count, bar_gen;
 };
 
-__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-
-__device__ __forceinline__ int ld_relaxed_s32(const int* p) {
-    int v;
-    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-
 // Sense-reversing grid barrier over the resident CTAs of one launch (grid <= number of SMs).  The count returns to zero at every
 // barrier, so consecutive launches share the state.  A wait is bounded; on time-out it sets *err and goes on.  Once *err is set the
 // barrier count is no longer aligned with the CTAs, so every later barrier of the factorisation returns at once instead of timing
 // out again (the next factorisation starts by clearing the flag and the count): the results are then garbage, and b2d_inertia
 // reports the error.
+constexpr unsigned BK_SPIN_MAX = 1u << 24;
 __device__ __forceinline__ void grid_sync(BkProg* pg, int* err) {
     __syncthreads();
-    if (threadIdx.x == 0 && !ld_relaxed_s32(err)) {
-        const uint32_t g0 = ld_acquire_u32(&pg->bar_gen);
+    if (threadIdx.x == 0 && !ld_relaxed(err)) {
+        const uint32_t g0 = ld_acquire(&pg->bar_gen);
         __threadfence();
         if (atomicAdd(&pg->bar_count, 1u) == gridDim.x - 1) {
             atomicExch(&pg->bar_count, 0u);
             __threadfence();
             atomicExch(&pg->bar_gen, g0 + 1);
         } else {
+            // (not bounded_spin: with the early exit below, that gives this kernel different instructions)
             unsigned it = 0;
-            while (ld_acquire_u32(&pg->bar_gen) == g0) {
-                if (++it == (1u << 24)) { atomicExch(err, 1); break; }
-                if ((it & 255u) == 0 && ld_relaxed_s32(err)) break;           // another CTA's wait timed out
+            while (ld_acquire(&pg->bar_gen) == g0) {
+                if (++it == BK_SPIN_MAX) { atomicExch(err, 1); break; }
+                if ((it & 255u) == 0 && ld_relaxed(err)) break;           // another CTA's wait timed out
             }
         }
         __threadfence();
@@ -76,16 +67,10 @@ __device__ __forceinline__ void grid_sync(BkProg* pg, int* err) {
     __syncthreads();
 }
 
-// 1 / b and a / b from the hardware reciprocal with Newton corrections (as fast_rcp_d in front_kernels.cuh): inline, so the panel
-// loop keeps its registers (the IEEE division's slow path is a call that spills them); within an ulp for normal operands
-__device__ __forceinline__ double rcp(double b) {
-    double r;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(b));
-    r = fma(r, fma(-b, r, 1.0), r);
-    return fma(r, fma(-b, r, 1.0), r);
-}
+// a / b from fast_rcp and one more correction: inline, so the panel loop keeps its registers (the IEEE division's slow path is a
+// call that spills them); within an ulp for normal operands
 __device__ __forceinline__ double ddiv(double a, double b) {
-    const double r = rcp(b), q = a * r;
+    const double r = fast_rcp(b), q = a * r;
     return fma(fma(-b, q, a), r, q);
 }
 
@@ -256,7 +241,7 @@ __global__ void __launch_bounds__(BK_NT) k_bk_panel(PanelArgs a) {
             const double d = __ldcg(&Wa(kc, j));
             const bool tiny = !(fabs(d) >= a.eps);
             const double dp = tiny ? ((d < 0.0) ? -a.eps : a.eps) : d;
-            const double r1v = rcp(dp);
+            const double r1v = fast_rcp(dp);
             for (int i = max(r0, kc + 1) + tid; i < r1; i += BK_NT) Fa(i, kc) = __ldcg(&Wa(i, j)) * r1v;
             if (b == 0 && tid == 0) {
                 Fa(kc, kc) = dp; a.dvec[kc] = dp; a.evec[kc] = 0.0; a.ipiv[kc] = kp + 1;
@@ -266,7 +251,7 @@ __global__ void __launch_bounds__(BK_NT) k_bk_panel(PanelArgs a) {
         } else {
             const double w11 = __ldcg(&Wa(kc, j)), w21 = __ldcg(&Wa(kc + 1, j)), w22 = __ldcg(&Wa(kc + 1, j + 1));
             const double d11 = ddiv(w22, w21), d22 = ddiv(w11, w21);
-            const double t = rcp(d11 * d22 - 1.0);
+            const double t = fast_rcp(d11 * d22 - 1.0);
             const double d21 = ddiv(t, w21);
             for (int i = max(r0, kc + 2) + tid; i < r1; i += BK_NT) {
                 const double x = __ldcg(&Wa(i, j)), y = __ldcg(&Wa(i, j + 1));

@@ -7,8 +7,8 @@
 //   diagonal:  z_k = y_k ./ d_k
 //   backward:  s_k = z_k - sum_{c>k} L(c,k)' x_c  accumulated as the x_c become available,  x_k = Linv_k' s_k
 //
-// Hand-off between CTAs goes through two small global vectors (ybuf, xbuf) whose entries start as a SENTINEL bit pattern
-// (all ones: a NaN no arithmetic produces) -- a consumer polls the 128 values themselves, so a block costs ONE L2 round trip
+// Hand-off between CTAs goes through two small global vectors (ybuf, xbuf) whose entries start as SLOT_EMPTY
+// (ptx.cuh: all ones, a NaN no arithmetic produces) -- a consumer polls the 128 values themselves, so a block costs ONE L2 round trip
 // on the critical path instead of flag + data, and needs no fence (8-byte stores are single-copy atomic).  The factor block a
 // CTA needs next is loaded into registers BEFORE it polls, so the chain per block is: poll -> 16 FMAs + shared-memory reduction
 // (off-diagonal block) -> 16 FMAs + reduction (inverted diagonal block) -> 128 stores.  Every CTA of the grid must be
@@ -16,25 +16,21 @@
 // Deterministic: fixed summation order, no atomics.
 #pragma once
 #include "bigsolve_kernels.cuh"
+#include "ptx.cuh"
 
 namespace b2 {
 
-constexpr unsigned long long DS_SENTINEL = 0xFFFFFFFFFFFFFFFFull;
 constexpr int DS_NT = 1024;
+constexpr unsigned DS_SPIN_MAX = 1u << 22;
 
 __device__ __forceinline__ double ds_poll(const double* p, int* err) {
-    unsigned long long v = DS_SENTINEL;
-    unsigned it = 0;
-    do {
-        asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-        if (v != DS_SENTINEL) break;
-    } while (++it < (1u << 22));
-    if (v == DS_SENTINEL) { atomicExch(err, 1); return 0.0; }
+    unsigned long long v;
+    if (!bounded_spin<DS_SPIN_MAX, 0>(err, [&](unsigned) { return (v = ld_relaxed_b64(p)) != SLOT_EMPTY; })) return 0.0;
     return __longlong_as_double((long long)v);
 }
 
 // L: N x N column-major factor (unit lower, D on the diagonal), Linv: inverted 128 x 128 diagonal blocks (ld 128),
-// dvec: D, x: right-hand side in / solution out, ybuf/xbuf: [nblk*128] hand-off vectors preset to the sentinel.
+// dvec: D, x: right-hand side in / solution out, ybuf/xbuf: [nblk*128] hand-off vectors preset to SLOT_EMPTY.
 // Registers hold ONE 128 x 128 block of L (16 doubles per thread, 1024 threads); its load is issued BEFORE the poll of the
 // vector it multiplies, so on the critical path (the newest y_c / x_c) the block is already there.  The CTA's own inverted
 // diagonal block sits in shared memory (cp.async at kernel start, padded rows: both the plain and the transposed apply are
@@ -63,7 +59,7 @@ __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const doub
     {
         const double* Li = Linv + (size_t)k * BS * BS;
         for (int e = tid; e < BS * BS; e += DS_NT) cp_async8(Ls + (e >> 7) * DS_LDI + (e & (BS - 1)), Li + e);
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit_group();
     }
     // ---------------- forward
     double t = (g == 0 && r < nb) ? x[BK ? perm[kb + r] : kb + r] : 0.0;     // group 0 carries the accumulator
@@ -89,7 +85,7 @@ __global__ void __launch_bounds__(DS_NT, 1) k_dense_solve_flow(int N, const doub
             t -= sum;
         }
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");
+    cp_async_wait_all();
     if (g == 0) tk[r] = t;
     __syncthreads();
     {                                                                         // y_k = Linv_k t_k   (Linv(r, c) = 0 for c > r)

@@ -16,6 +16,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ptx.cuh"
+
 namespace b2 {
 
 struct FrontDesc {
@@ -44,7 +46,6 @@ struct FactorArgs {
 
 // Timeline stamps of the dense look-ahead schedule (b2d_debug_trace): slot = 8 * block column + kernel kind
 enum { TR_DIAG = 0, TR_NEAR1 = 1, TR_NEAR2 = 2, TR_TRSM = 3, TR_COL = 4, TR_BULK = 5 };
-__device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void trace_enter(const FactorArgs& a, int slot) {
     if (a.trace && threadIdx.x == 0) atomicMin(a.trace + 2 * slot, global_ns());
 }
@@ -236,14 +237,6 @@ __global__ void k_big_extend_add(FactorArgs a, const int32_t* __restrict__ list,
     }
 }
 
-__device__ __forceinline__ double fast_rcp_d(double x) {
-    double r;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
-    r = fma(r, fma(-x, r, 1.0), r);
-    r = fma(r, fma(-x, r, 1.0), r);
-    return r;
-}
-
 // ----------------------------------------------------------------------------------------------------------
 // Trailing update of the blocked factorisation (> 95 % of the flops of a big front; see bigfactor_kernels.cuh):
 //   C(i,j) -= sum_{k in [kb0, kb0+kcount)} L(i,k) d_k L(j,k),  i >= j, jlo <= j < jhi
@@ -257,20 +250,11 @@ constexpr int GU_M = 128, GU_N = 64, GU_K = 16, GU_STAGES = 4;
 constexpr int GU_LDA = GU_M + 4, GU_LDB = GU_N + 4, GU_LDC = GU_M + 2;
 constexpr size_t GU_SMEM = (size_t)(GU_STAGES * GU_K * (GU_LDA + GU_LDB) + 128) * sizeof(double);
 
-__device__ __forceinline__ void cp_async8_zfill(void* smem_dst, const void* gsrc, bool valid) {
-    const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-    const int sz = valid ? 8 : 0;
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(sa), "l"(gsrc), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit_group() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait_group_n() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // one 128 x 64 tile (bx, by) of the update; `gu_sm` is the CTA's dynamic shared memory (GU_SMEM bytes).  Returns without work for
 // tiles above the diagonal / outside the column range.  All threads of the CTA must call it together.
 template <bool NAMED>
 __device__ __forceinline__ void gu_sync() {           // NAMED: only the 256 consumer threads of a 288-thread CTA (barrier id 1)
-    if (NAMED) asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (NAMED) bar_sync<1, 256>();
     else __syncthreads();
 }
 template <bool NAMED = false>
@@ -325,7 +309,7 @@ __device__ __forceinline__ void big_update_tile(const FactorArgs& a, const Front
 #pragma unroll
         for (int y = 0; y < 4; ++y) c[x][y][0] = c[x][y][1] = 0.0;
     for (int ch = 0; ch < nchunk; ++ch) {
-        cp_async_wait_group_n<GU_STAGES - 2>();
+        cp_async_wait_group<GU_STAGES - 2>();
         gu_sync<NAMED>();                                              // slice ch landed; slice ch-1 fully consumed
         if (ch + GU_STAGES - 1 < nchunk) issue(ch + GU_STAGES - 1);
         cp_async_commit_group();
@@ -350,7 +334,7 @@ __device__ __forceinline__ void big_update_tile(const FactorArgs& a, const Front
     }
     // epilogue: accumulators -> shared memory (column-major tile), then a coalesced read-modify-write of C with all of
     // a thread's loads in flight at once (the fragment layout would make it 32 dependent 8-byte round trips per thread)
-    cp_async_wait_group_n<0>();
+    cp_async_wait_group<0>();
     gu_sync<NAMED>();
     double* Cs = gu_sm;                                               // [GU_N][GU_LDC]
 #pragma unroll
@@ -420,31 +404,6 @@ __global__ void __launch_bounds__(256, 2) k_big_update_rows(FactorArgs a, const 
 // ----------------------------------------------------------------------------------------------------------
 constexpr int GU_NT_BULK = 288;
 constexpr size_t GU_SMEM_BULK = GU_SMEM + 2 * GU_STAGES * sizeof(unsigned long long);
-__device__ __forceinline__ unsigned gu_s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void gu_mbar_init(unsigned long long* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(gu_s32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void gu_mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(gu_s32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void gu_mbar_arrive(unsigned long long* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(gu_s32(bar)) : "memory");
-}
-__device__ __forceinline__ void gu_mbar_wait(unsigned long long* bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "GU_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra GU_DONE;\n"
-        "bra GU_WAIT;\n"
-        "GU_DONE:\n"
-        "}\n" ::"r"(gu_s32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void gu_bulk_g2s(void* smem_dst, const void* gsrc, unsigned bytes, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(gu_s32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(gu_s32(bar)) : "memory");
-}
 
 // All 288 threads of the CTA call this together; the caller separates consecutive tiles by a CTA-wide barrier.
 __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const FrontDesc& d, int kb0, int kmax, int jlo_rel, int jhi_rel,
@@ -476,18 +435,18 @@ __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const 
         const int na = min(GU_M, f - i0), nb_ = min(GU_N, f - j0);
         for (int ch = 0; ch < nchunk; ++ch) {
             const unsigned g = it0 + ch, st = g % GU_STAGES;
-            if (g >= GU_STAGES) gu_mbar_wait(&empty[st], ((g / GU_STAGES) - 1) & 1);   // every consumer warp has left the stage's previous slice
+            if (g >= GU_STAGES) mbar_wait(&empty[st], ((g / GU_STAGES) - 1) & 1);   // every consumer warp has left the stage's previous slice
             // row `lane` of the slice: absolute element index of its first entry, rounded down to a 16-byte boundary
             const size_t eA = (size_t)d.lp_off + (size_t)(kb0 + ch * GU_K + (lane & (GU_K - 1))) * f + i0;
             const size_t eB = eA - i0 + j0;
             const unsigned pA = (unsigned)(eA & 1), pB = (unsigned)(eB & 1);
             const unsigned bytesA = 8u * ((na + pA + 1u) & ~1u), bytesB = 8u * ((nb_ + pB + 1u) & ~1u);
             const unsigned total = __reduce_add_sync(0xffffffffu, lane < GU_K ? bytesA + bytesB : 0u);
-            if (lane == 0) gu_mbar_expect_tx(&full[st], total);
+            if (lane == 0) mbar_expect_tx(&full[st], total);
             __syncwarp();
             if (lane < GU_K) {
-                gu_bulk_g2s(As + ((size_t)st * GU_K + lane) * GU_LDA, a.L + (eA - pA), bytesA, &full[st]);
-                gu_bulk_g2s(Bs + ((size_t)st * GU_K + lane) * GU_LDB, a.L + (eB - pB), bytesB, &full[st]);
+                bulk_g2s(As + ((size_t)st * GU_K + lane) * GU_LDA, a.L + (eA - pA), bytesA, &full[st]);
+                bulk_g2s(Bs + ((size_t)st * GU_K + lane) * GU_LDB, a.L + (eB - pB), bytesB, &full[st]);
             }
         }
         return;
@@ -506,7 +465,7 @@ __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const 
         for (int y = 0; y < 4; ++y) c[x][y][0] = c[x][y][1] = 0.0;
     for (int ch = 0; ch < nchunk; ++ch) {
         const unsigned gi = it0 + ch, st = gi % GU_STAGES;
-        gu_mbar_wait(&full[st], (gi / GU_STAGES) & 1);
+        mbar_wait(&full[st], (gi / GU_STAGES) & 1);
         const double* Ab = As + (size_t)st * GU_K * GU_LDA + shA;
         const double* Bb = Bs + (size_t)st * GU_K * GU_LDB + shB;
 #pragma unroll
@@ -526,7 +485,7 @@ __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const 
                                  : "d"(af[x]), "d"(af[x + 1]), "d"(bf[y]));
         }
         __syncwarp();
-        if (lane == 0) gu_mbar_arrive(&empty[st]);
+        if (lane == 0) mbar_arrive(&empty[st]);
     }
     // epilogue (as in big_update_tile): every consumer has passed its last `full` wait, so all copies have landed; the producer
     // cannot touch the ring again before the caller's CTA-wide barrier
@@ -569,10 +528,10 @@ __device__ __forceinline__ void big_update_tile_bulk(const FactorArgs& a, const 
 __device__ __forceinline__ void gu_bulk_setup(double* gu_sm) {
     unsigned long long* full = reinterpret_cast<unsigned long long*>(gu_sm + GU_STAGES * GU_K * (GU_LDA + GU_LDB) + 128);
     if (threadIdx.x < GU_STAGES) {
-        gu_mbar_init(&full[threadIdx.x], 1);
-        gu_mbar_init(&full[GU_STAGES + threadIdx.x], 8);
+        mbar_init(&full[threadIdx.x], 1);
+        mbar_init(&full[GU_STAGES + threadIdx.x], 8);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_fence_init();
     __syncthreads();
 }
 
@@ -597,7 +556,6 @@ __global__ void __launch_bounds__(GU_NT_BULK, 2) k_big_update_pipe_bulk(FactorAr
 // CTAs that land on the first `n_reserved` SMs exit at once, so those SMs stay free for the next panel's diagonal-block kernel
 // (one CTA that needs a whole SM) while this kernel works through the trailing update on all the others.  Tiles are handed out
 // by an atomic counter (`*tile_counter`, zeroed by the host before the launch), so it does not matter which CTAs left.
-__device__ __forceinline__ unsigned smid() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
 __global__ void __launch_bounds__(GU_NT_BULK, 2) k_big_update_dyn_bulk(FactorArgs a, const int32_t* __restrict__ list, int kb0, int kmax,
                                                                       int jlo_rel, int jhi_rel, int clip_jlo, int nbx, int nby, int* tile_counter,
                                                                       int n_reserved) {

@@ -21,6 +21,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "ptx.cuh"
+
 namespace ozk {
 
 constexpr int S = 8;             // digits
@@ -34,7 +36,7 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;             // + alignme
 constexpr int NTHREADS = 288;
 constexpr int GLD = BM + 4;                                         // int32 row stride of the parked accumulators (no bank conflicts)
 static_assert(S * BN * GLD * 4 <= STAGES * STAGE_BYTES, "the parked accumulators reuse the operand ring");
-constexpr uint32_t SPIN_MAX = 1u << 22;
+constexpr uint32_t SPIN_MAX = 1u << 22;                             // tries of a bounded mbarrier wait
 
 // ------------------------------------------------------------------------------------------------ digit split
 // one CTA per column m of the operand A (K x M): a(i, m) = (scale ? sqrt(scale[i]) : 1) * src[m*lds + (rows ? rows[i] : i)];
@@ -71,33 +73,11 @@ __global__ void __launch_bounds__(256) k_ozaki_split(int K, int Kpad, int Mpad, 
 }
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* err) {     // bounded: never hang the device
-    uint32_t done = 0;
-    for (uint32_t it = 0; it < SPIN_MAX; ++it) {
-        asm volatile(
-            "{\n.reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n}\n"
-            : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (done) return true;
-    }
-    atomicExch(err, 1);
-    return false;
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
+// (mbarriers, the shared-window address and the named barrier: ptx.cuh)
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, unsigned long long* bar, int c0, int c1, int c2) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+        ::"r"(b2::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(b2::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 // wgmma shared-memory descriptor of a K-major operand tile with 64-byte swizzle: rows of 64 bytes, 8-row groups 512 bytes
 // apart (stride byte offset), leading byte offset unused (1), layout type 2 = SWIZZLE_64B
@@ -125,7 +105,6 @@ __device__ __forceinline__ void wgmma_s8(int (&d)[32], uint64_t adesc, uint64_t 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // warps 0..7 only
 
 // 2^e for |e| <= 1022 (exponent field only)
 __device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(min(max(e, -1022), 1023) + 1023) << 52); }
@@ -156,15 +135,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
                                                             const double* __restrict__ pr, int lower_only, int* err) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
+    __shared__ unsigned long long full_bar[STAGES], empty_bar[STAGES];
     // warp index through a shuffle: the compiler then knows it is warp-uniform and does not serialise the wgmma sequence
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int bm = tiles[blockIdx.x].x, bn = tiles[blockIdx.x].y;
     const int nkb = K / BKB;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int s = 0; s < STAGES; ++s) { b2::mbar_init(&full_bar[s], 1); b2::mbar_init(&empty_bar[s], 2); }
+        b2::mbar_fence_init();
     }
     __syncthreads();
 
@@ -173,10 +152,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
         if (lane == 0) {
             for (int kb = 0; kb < nkb; ++kb) {
                 const int st = kb % STAGES;
-                if (kb >= STAGES && !mbar_wait(&empty_bar[st], ((kb / STAGES) - 1) & 1, err)) break;
+                if (kb >= STAGES && !b2::mbar_wait_bounded<SPIN_MAX>(&empty_bar[st], ((kb / STAGES) - 1) & 1, err)) break;
                 uint8_t* sa = smem + (size_t)st * STAGE_BYTES;
                 uint8_t* sb = sa + S * A_TILE;
-                mbar_expect_tx(&full_bar[st], STAGE_BYTES);
+                b2::mbar_expect_tx(&full_bar[st], STAGE_BYTES);
                 tma_load_3d(sa, &mapQ, &full_bar[st], kb * BKB, bm * BM, 0);      // box (64 B of K, 64 rows, 8 digits)
                 tma_load_3d(sb, &mapQ, &full_bar[st], kb * BKB, bn * BN, 0);
             }
@@ -194,21 +173,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
     bool ok = true;
     for (int kb = 0; kb < nkb; ++kb) {
         const int st = kb % STAGES;
-        ok = __all_sync(0xffffffffu, mbar_wait(&full_bar[st], (kb / STAGES) & 1, err));
+        ok = __all_sync(0xffffffffu, b2::mbar_wait_bounded<SPIN_MAX>(&full_bar[st], (kb / STAGES) & 1, err));
         if (!ok) break;
-        const uint32_t sa = smem_u32(smem + (size_t)st * STAGE_BYTES);
+        const uint32_t sa = b2::smem_u32(smem + (size_t)st * STAGE_BYTES);
         const uint64_t ad0 = gmma_desc_k_sw64(sa), bd0 = gmma_desc_k_sw64(sa + S * A_TILE);
         wgmma_fence();
         if (g == 0) mma_kblock<0>(acc, ad0, bd0);
         else mma_kblock<1>(acc, ad0, bd0);
         wgmma_commit();
         wgmma_wait_all();
-        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[st]);    // this warpgroup has read the stage
+        if ((threadIdx.x & 127) == 0) b2::mbar_arrive(&empty_bar[st]);    // this warpgroup has read the stage
     }
     wgmma_wait_all();
 
     // ---------------- epilogue: park G_d(m, n) at Gs[d][n][m] (over the operand ring, which every wgmma has finished reading)
-    consumers_sync();
+    b2::bar_sync<1, 256>();                               // warps 0..7 only
     int32_t* Gs = reinterpret_cast<int32_t*>(smem);
     {
         const int w = warp & 3;
@@ -223,7 +202,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
             }
         }
     }
-    consumers_sync();
+    b2::bar_sync<1, 256>();                               // warps 0..7 only
     if (!ok) return;
     const int ml = threadIdx.x & (BM - 1);
     const int m = bm * BM + ml;

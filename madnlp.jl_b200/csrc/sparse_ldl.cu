@@ -697,7 +697,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             P.sol_grid = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
             P.n_solve_launches = 1;
             B2_CUDA_THROW(s->d_slots.alloc((size_t)(2 * s->cbv_off[ns] + n)));
-            B2_CUDA_THROW(cudaMemset(s->d_slots.p, 0xff, s->d_slots.bytes()));     // every slot SLOT_EMPTY
+            B2_CUDA_THROW(cudaMemset(s->d_slots.p, SLOT_EMPTY_BYTE, s->d_slots.bytes()));     // every slot SLOT_EMPTY
         }
     } catch (std::exception&) {
         delete s;
@@ -1348,14 +1348,14 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream) {
     for (int c = 0; c < nrhs; ++c) {
         double* x = x_d + (size_t)c * N;
         if (s->bunch_kaufman) {
-            B2_CUDA(cudaMemsetAsync(s->flow.p, 0xFF, s->flow.bytes(), st));
+            B2_CUDA(cudaMemsetAsync(s->flow.p, SLOT_EMPTY_BYTE, s->flow.bytes(), st));
             k_dense_solve_flow<true><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
                                                                   s->counters.p + 2, s->bk.perm.p, s->bk.evec.p);
             continue;
         }
         if (flow_ok && nblk <= sm_count()) {
             // ONE launch: block row / block column k is owned by CTA k, hand-off through sentinel-initialised vectors
-            B2_CUDA(cudaMemsetAsync(s->flow.p, 0xFF, s->flow.bytes(), st));
+            B2_CUDA(cudaMemsetAsync(s->flow.p, SLOT_EMPTY_BYTE, s->flow.bytes(), st));
             k_dense_solve_flow<false><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
                                                                    s->counters.p + 2, nullptr, nullptr);
             continue;

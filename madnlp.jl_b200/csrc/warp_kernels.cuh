@@ -14,6 +14,7 @@
 #pragma once
 #include "common.cuh"
 #include "front_kernels.cuh"
+#include "ptx.cuh"
 #include "solve_kernels.cuh"
 
 namespace b2 {
@@ -35,14 +36,6 @@ struct WarpSched {
     const int32_t* stage_cnt;   // [nstage]
     const int32_t* list;        // supernode ids
 };
-
-__device__ __forceinline__ double fast_rcp(double x) {
-    double r;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
-    r = fma(r, fma(-x, r, 1.0), r);
-    r = fma(r, fma(-x, r, 1.0), r);
-    return r;
-}
 
 // ------------------------------------------------------------------------------------------------ factor
 // A front is owned by a TEAM of NW warps (NW = 1: order <= 32, NW = 2: order <= 64); thread `tid` of the team owns
@@ -86,55 +79,19 @@ struct TeamSmem {
     }
 };
 
-__device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async4(void* smem_dst, const void* gsrc) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async16_cg(void* smem_dst, const void* gsrc) {      // L2-only: data written by other CTAs
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
-}
 // dependency flags of the single-launch factorisation (k_factor_dep): zeroed before the launch, a flag is ready when it holds `want`
+// (stored with st_release by the front that finishes)
+constexpr unsigned DEP_SPIN_MAX = 1u << 24, DEP_SPIN_SLEEP_NS = 32;
 __device__ __forceinline__ void flag_wait(const int* flag, int* err, int want = 1) {
-    int v = 0;
-    unsigned it = 0;
-    do {
-        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
-        if (v == want) break;
-        __nanosleep(32);
-    } while (++it < (1u << 24));
-    if (v != want) {                     // bounded spin: never hang the device, report instead
-        atomicExch(err, 1);
-        __threadfence();
-    }
+    if (!bounded_spin<DEP_SPIN_MAX, DEP_SPIN_SLEEP_NS>(err, [&](unsigned) { return ld_acquire(flag) == want; })) __threadfence();
 }
-__device__ __forceinline__ void flag_set(int* flag, int v = 1) {
-    asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(v) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// Hand-off slots of the single-launch solve: the value is its own flag.  A slot holds SLOT_EMPTY until its one producer stores the
-// value; its one consumer polls the value itself (no flag, no release fence, one L2 round trip per hand-off) and stores SLOT_EMPTY
-// back once it has it, which arms the slot for the next launch.  SLOT_EMPTY is all-ones -- a negative NaN with a full payload, which
-// a byte-wise cudaMemset(0xff) writes and fp64 arithmetic never produces; a producer stores a value with that bit pattern (a NaN
-// from the caller's right-hand side) as the canonical NaN instead.
-constexpr unsigned long long SLOT_EMPTY = ~0ull;
-constexpr unsigned long long CANON_NAN = 0x7ff8000000000000ull;
-__device__ __forceinline__ unsigned long long slot_ld(const double* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(v) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ void slot_st(double* p, unsigned long long v) {
-    asm volatile("st.relaxed.gpu.global.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
+// Hand-off slots of the single-launch solve: the value is its own flag.  A slot holds SLOT_EMPTY (ptx.cuh) until its one producer
+// stores the value; its one consumer polls the value itself (no flag, no release fence, one L2 round trip per hand-off) and stores
+// SLOT_EMPTY back once it has it, which arms the slot for the next launch.
 __device__ __forceinline__ void slot_put(double* p, double v) {
     const unsigned long long b = (unsigned long long)__double_as_longlong(v);
-    slot_st(p, b == SLOT_EMPTY ? CANON_NAN : b);
+    st_relaxed_b64(p, b == SLOT_EMPTY ? CANON_NAN : b);
 }
 // take the slots p[c] with bit c of `need` set: poll them all at once until none is empty, then re-arm each.  Bounded like flag_wait:
 // a slot still empty at the time-out sets *err (the solve then writes NaN into x) and reads as NaN.
@@ -142,25 +99,25 @@ template <int K>
 __device__ __forceinline__ void slot_take(double* const (&p)[K], unsigned need, double (&v)[K], int* err) {
     unsigned long long b[K];
 #pragma unroll
-    for (int c = 0; c < K; ++c) b[c] = (need >> c & 1u) ? slot_ld(p[c]) : 0ull;
+    for (int c = 0; c < K; ++c) b[c] = (need >> c & 1u) ? ld_relaxed_b64(p[c]) : 0ull;
     unsigned it = 0;
     for (;;) {
         unsigned pend = 0;
 #pragma unroll
         for (int c = 0; c < K; ++c) pend |= ((need >> c & 1u) && b[c] == SLOT_EMPTY) ? 1u << c : 0u;
         if (!pend) break;
-        if (++it >= (1u << 24)) {            // never hang the device, report instead
+        if (++it >= DEP_SPIN_MAX) {          // never hang the device, report instead
             atomicExch(err, 1);
             break;
         }
-        __nanosleep(32);
+        __nanosleep(DEP_SPIN_SLEEP_NS);
 #pragma unroll
-        for (int c = 0; c < K; ++c) if (pend >> c & 1u) b[c] = slot_ld(p[c]);
+        for (int c = 0; c < K; ++c) if (pend >> c & 1u) b[c] = ld_relaxed_b64(p[c]);
     }
 #pragma unroll
     for (int c = 0; c < K; ++c) {
         v[c] = __longlong_as_double((long long)b[c]);
-        if ((need >> c & 1u) && b[c] != SLOT_EMPTY) slot_st(p[c], SLOT_EMPTY);
+        if ((need >> c & 1u) && b[c] != SLOT_EMPTY) st_relaxed_b64(p[c], SLOT_EMPTY);
     }
 }
 
@@ -216,7 +173,7 @@ __device__ __forceinline__ void pivot_iter(double (&av)[32 * NW + 1], double& lp
         if (c.tid > c.k) *dst = nx;
     } else {
         asm volatile("{\n\t.reg .pred p;\n\tsetp.gt.s32 p, %2, %3;\n\t@p st.shared.f64 [%0], %1;\n\tbar.arrive %4, 64;\n\t}"
-                     ::"r"((unsigned)__cvta_generic_to_shared(dst)), "d"(nx), "r"(c.tid), "r"(c.k),
+                     ::"r"(smem_u32(dst)), "d"(nx), "r"(c.tid), "r"(c.k),
                        "r"(3 + c.team * 4 + (c.tid >> 5) * 2 + ((c.k + 1) & 1)));
     }
     if (c.tid < c.f) c.Fk[c.tid] = (c.tid == c.k) ? dk : l;   // finished column k of the panel (rows < k: scratch)
@@ -284,7 +241,7 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
                 if (tid == 0) flag_wait(done + recs[ro].sn, err);          // child front finished (its update block is in L2)
                 __syncwarp();
                 int v = (tid == 0) ? 1 : 0;
-                if (tid > 0 && tid < nrec) asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(done + recs[ro + tid].sn) : "memory");
+                if (tid > 0 && tid < nrec) v = ld_acquire(done + recs[ro + tid].sn);
                 const unsigned m = __ballot_sync(0xffffffffu, v != 0);
                 if (tid == 0) *nready_sh = __ffs(~m) - 1;                  // length of the finished prefix (>= 1)
             }
@@ -403,7 +360,7 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
     // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed.  The same
     // barrier completes the pivot loop's writes of the panel columns into F.
     team_sync<NW>(team);
-    if (DEP && tid == 0) flag_set(done + s);
+    if (DEP && tid == 0) st_release(done + s, 1);
     if (a.ftrace && tid == 0) a.ftrace[3 * (size_t)s + 2] = global_ns();
     B2_STAMP(6);
     // panel, off the tree's critical path: column-major (forward solve, parent-independent) and row-major copy (backward solve)
@@ -454,7 +411,7 @@ __global__ void __launch_bounds__(TeamsPerCta<NW>::value * NW * 32) k_factor_war
 // Programmatic dependent launch: a level's kernel is launched while the previous level still runs.  Everything that is
 // CONSTANT during a solve (descriptors, index lists, the factor panels) is fetched before pdl_wait(); only the values the
 // previous levels produce (xp, cbv) are read after it.  Both calls are no-ops for a launch without the attribute.
-// (pdl_trigger / pdl_wait: common.cuh)
+// (pdl_trigger / pdl_wait: ptx.cuh)
 
 // A front's solve is three memory round trips, whatever its number of children or pivots:
 //   (1) descriptor;  (2) child records + the whole panel (cp.async into shared memory, in flight while (3) runs) + own
@@ -862,7 +819,7 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRe
     __syncthreads();
     if (bad_sh) {
         for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
-        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) slot_st(slots + i, SLOT_EMPTY);
+        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
     }
 }
 
