@@ -546,6 +546,59 @@ int b2_get_varphi_d_r(b2_bounds* b, int64_t m, const double* f_R_d, const double
                       const double* dx_d, const double* pp_d, const double* nn_d, const double* dpp_d, const double* dnn_d, double mu_R,
                       double rho, double* out_d, void* stream);                                                          /* :612-636 */
 
+/* ------------------------------------------------------------------ the other solve sites of the IPM (src/IPM/solver.jl)
+ * The least-squares dual initialisation (initialize_dual(solver, DualInitializeLeastSquares), :86-97), robust!'s return to the regular
+ * phase (:518-530), the second-order correction (second_order_correction, :547-608) and the soft restoration (restore!, :300-411).
+ * Vectors as in the IPM reductions above: x, xl, xu, f, zl, zu, jacl, dx, wx, x_trial of length n_tot (zl / zu FULL length, +-Inf for
+ * an absent bound; the _r views go through ind_lb / ind_ub of `b`); c, c_trial, y, dy of length m; dzl / dzu compressed (nlb / nub);
+ * p: an UnreducedKKTVector buffer [x (n_tot) | y (m) | zl (nlb) | zu (nub)].  Elementwise outputs are bit-identical to the reference's
+ * broadcasts (left-to-right, no contraction, unary minus a sign flip, Julia's min).  axpy! on a Julia vector goes to BLAS, which may
+ * fuse the multiply and the add; these kernels form y + (a x) with two roundings and can differ from a fused BLAS by one rounding.
+ * Reductions are deterministic (one device double, or the result array below).  Nothing synchronises; everything can be captured in
+ * a CUDA graph; the step lengths are read from device scalars, never by the host. */
+/* set_aug_diagonal!(kkt, solver) (src/IPM/kernels.jl:4-20) before the KKT type's own _set_aug_diagonal! (b2_set_aug_diagonal or
+ * b2_set_aug_diagonal_unreduced): reg = del_w (n_tot); du_diag = -del_c (m); l_lower = zl_r, l_diag = xl_r - x_lr (nlb);
+ * u_lower = zu_r, u_diag = x_ur - xu_r (nub).  del_w / del_c: default_primal_regularization / default_dual_regularization */
+int b2_set_aug_diagonal_iterate(b2_bounds* b, int64_t m, double del_w, double del_c, const double* x_d, const double* xl_d, const double* xu_d,
+                                const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d,
+                                double* u_lower_d, double* l_diag_d, double* u_diag_d, void* stream);
+/* set_aug_rhs!(solver, kkt, w, mu) (:113-130) then dual_inf_perturbation!(px, ind_llb, ind_uub, mu, kappa_d) (:818-823) in one launch,
+ * bit-identical to b2_set_aug_rhs followed by the perturbation: p = [-f + zl - zu - jacl | -w | (xl_r - x_lr) zl_r + mu | (xu_r - x_ur) zu_r
+ * - mu], then px[ind_llb] -= mu kappa_d, px[ind_uub] += mu kappa_d (mu kappa_d formed once).  w = c when c_trial_d is NULL, else
+ * w = c_trial + alpha c (the second-order correction's first right-hand side, copyto!(wy, c_trial); axpy!(alpha, c, wy), formed on the
+ * fly).  ind_llb / ind_uub as for b2_set_centering_aug_rhs: ascending device index arrays */
+int b2_set_aug_rhs_perturbed(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* f_d,
+                             const double* zl_d, const double* zu_d, const double* jacl_d, const double* c_d, const double* c_trial_d,
+                             double alpha, double mu, double kappa_d, int64_t nllb, const int64_t* ind_llb_d, int64_t nuub,
+                             const int64_t* ind_uub_d, double* p_d, void* stream);
+/* set_initial_rhs! (:220-230): p = [(-f + zl) - zu | 0 | 0 | 0] */
+int b2_set_initial_rhs(b2_bounds* b, int64_t m, const double* f_d, const double* zl_d, const double* zu_d, double* p_d, void* stream);
+/* The y rule of initialize_dual (solver.jl:92-96) and of robust!'s exit (:526-530), decided on the device in two launches:
+ * result_d[B2_DUAL_INIT_NORM] = ||dy||_inf (NaN-propagating, as b2_norm_inf), result_d[B2_DUAL_INIT_COPY] = 1.0 when
+ * solved && !(norm > constr_mult_init_max), else 0.0; then y = dy where that is 1.0, else y = +0.0.  A NaN norm compares false and
+ * dy is copied, as in Julia.  robust!'s exit passes solved = 1: it does not check its solve.  Uses the reduction scratch of `b`. */
+#define B2_DUAL_INIT_NORM       0
+#define B2_DUAL_INIT_COPY       1
+#define B2_DUAL_INIT_RESULT_LEN 2
+int b2_dual_init_select(b2_bounds* b, int64_t m, const double* dy_d, int32_t solved, double constr_mult_init_max, double* y_d,
+                        double* result_d, void* stream);
+/* get_F (:572-610) into one device double: F1 + F2 + F3 + F4 in that order, with F1 = sum |c|, F2 = sum |f - zl + zu + jacl| (n_tot),
+ * F3 = sum over ind_lb of (x_lr >= xl_r && zl_r >= 0 ? |(x_lr - xl_r) zl_r - mu| : Inf), and F4 = sum over ind_ub of
+ * (xu_r >= x_ur && zu_r >= 0 ? |(xu_r - xu_r) zu_r - mu| : Inf).  F4 keeps the reference's (xu_r - xu_r) (:606) where xu_r - x_ur is
+ * meant: that factor is 0 for a finite bound (NaN at an infinite one), so a feasible upper-bounded entry contributes |mu| whatever its
+ * complementarity.  Each sum is deterministic and differs from the scalar loop only by association. */
+int b2_get_pd_error(b2_bounds* b, int64_t m, const double* c_d, const double* f_d, const double* zl_d, const double* zu_d,
+                    const double* jacl_d, const double* x_d, const double* xl_d, const double* xu_d, double mu, double* out_d, void* stream);
+/* restore!'s step (solver.jl:324-339) in one launch: alpha = min(*alpha_max_d, *alpha_z_d) (Julia's min; the two scalars that
+ * b2_get_alpha_max and b2_get_alpha_z wrote) is written to *alpha_d, then x += alpha dx (n_tot), y += alpha dy (m),
+ * zl_r += alpha dzl (nlb), zu_r += alpha dzu (nub).  alpha_d must not alias either input scalar. */
+int b2_restore_update(b2_bounds* b, int64_t m, const double* alpha_max_d, const double* alpha_z_d, double* alpha_d, const double* dx_d,
+                      const double* dy_d, const double* dzl_d, const double* dzu_d, double* x_d, double* y_d, double* zl_d, double* zu_d,
+                      void* stream);
+/* x_trial = x + alpha wx over n entries with alpha = *alpha_d (the second-order correction's trial point after b2_get_alpha_max,
+ * solver.jl:567-575; the line search's trial point, line_search.jl:39-40) */
+int b2_soc_trial(int64_t n, const double* alpha_d, const double* x_d, const double* wx_d, double* x_trial_d, void* stream);
+
 /* ------------------------------------------------------------------ adaptive barrier (barrier = QualityFunctionUpdate, src/IPM/barrier.jl:150-302)
  * The device half of get_adaptive_mu(solver, ::QualityFunctionUpdate): the new mu is computed on the device, and the free / monotone mode
  * switch and the filter stay with the caller (barrier.jl:121-148).  Vectors as in the IPM reductions above (x, xl, xu, zl, zu: n_tot, zl / zu

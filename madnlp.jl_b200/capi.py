@@ -19,6 +19,8 @@ QN_BFGS, QN_DAMPED_BFGS = 1, 2
 B2_DENSE_PIVOT_STATIC, B2_DENSE_PIVOT_BUNCH_KAUFMAN = 0, 1
 # layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
 CURV_WXT, CURV_WXN, CURV_GN, CURV_TT, CURV_LHS, CURV_PASS, CURV_RESULT_LEN = 0, 1, 2, 3, 4, 5, 6
+# layout of b2_dual_init_select's result (B2_DUAL_INIT_* in include/b200kkt.h)
+DUAL_INIT_NORM, DUAL_INIT_COPY, DUAL_INIT_RESULT_LEN = 0, 1, 2
 # the adaptive barrier's scalar array and b2_qf_search's result (B2_QF_* in include/b200kkt.h)
 QF_TAU, QF_NRM_PRIMAL, QF_NRM_DUAL, QF_MU_AVG, QF_SCAL_LEN = 0, 1, 2, 3, 4
 QF_SIGMA, QF_MU, QF_N_EVAL, QF_N_GS_ITER, QF_TOL_EXIT, QF_TRACE, QF_MAX_GS_ITER = 0, 1, 2, 3, 4, 8, 64
@@ -221,6 +223,13 @@ PROTOTYPES = {
     "b2_get_alpha_z_r": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64, _p, _p]),
     "b2_get_varphi_r": (C.c_int, [_p, _i64, _f64] + [_p] * 5 + [_f64, _p, _p]),
     "b2_get_varphi_d_r": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _p, _p]),
+    "b2_set_aug_diagonal_iterate": (C.c_int, [_p, _i64, _f64, _f64] + [_p] * 11 + [_p]),
+    "b2_set_aug_rhs_perturbed": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _f64, _i64, _p, _i64, _p, _p, _p]),
+    "b2_set_initial_rhs": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
+    "b2_dual_init_select": (C.c_int, [_p, _i64, _p, _i32, _f64, _p, _p, _p]),
+    "b2_get_pd_error": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64, _p, _p]),
+    "b2_restore_update": (C.c_int, [_p, _i64] + [_p] * 11 + [_p]),
+    "b2_soc_trial": (C.c_int, [_i64, _p, _p, _p, _p, _p]),
     "b2_primal_dual_norm2": (C.c_int, [_p, _i64, _p, _p, _p]),
     "b2_set_centering_aug_rhs": (C.c_int, [_p, _i64, _i64, _p, _i64, _p, _p, _f64, _p, _p]),
     "b2_qf_search": (C.c_int, [_p, _i64] + [_p] * 8 + [_f64] * 5 + [_i32, _p, _p]),

@@ -39,18 +39,6 @@ __global__ void __launch_bounds__(256) k_pd_norm2(int64_t n_tot, int64_t m, cons
     }
 }
 
-// is key in the ascending index array a[0:n)?
-__device__ __forceinline__ bool contains(const int64_t* __restrict__ a, int64_t n, int64_t key) {
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        const int64_t v = a[mid];
-        if (v == key) return true;
-        if (v < key) lo = mid + 1; else hi = mid;
-    }
-    return false;
-}
-
 // ---- set_centering_aug_rhs! then dual_inf_perturbation!, one thread per entry of p = [px (n_tot) | py (m) | pzl (nlb) | pzu (nub)]:
 //   px = 0, then px[ind_llb] -= mu kappa_d, then px[ind_uub] += mu kappa_d ; py = 0 ; pzl = mu ; pzu = -mu
 __global__ void k_centering_rhs(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, int64_t nllb, const int64_t* __restrict__ ind_llb,

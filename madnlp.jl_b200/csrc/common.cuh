@@ -85,6 +85,26 @@ __device__ __forceinline__ double jl_max(double x, double y) {
 }
 // Julia's clamp(x, lo, hi) = x > hi ? hi : (x < lo ? lo : x)
 __device__ __forceinline__ double jl_clamp(double x, double lo, double hi) { return x > hi ? hi : (x < lo ? lo : x); }
+
+// is key in the ascending index array a[0:n)?  (ind_llb / ind_uub membership of dual_inf_perturbation!)
+__device__ __forceinline__ bool contains(const int64_t* __restrict__ a, int64_t n, int64_t key) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        const int64_t v = a[mid];
+        if (v == key) return true;
+        if (v < key) lo = mid + 1; else hi = mid;
+    }
+    return false;
+}
+
+// body of a C entry point that launches one grid-stride elementwise kernel over tot entries (nothing when tot = 0)
+#define B2_LAUNCH(who, kern, tot, ...) do {                                                                                        \
+        if ((tot) == 0) return B2_OK;                                                                                              \
+        cudaError_t e__ = ::b2::launch_pdl(kern, dim3(::b2::grid_elem(tot)), dim3(256), 0, ::b2::as_stream(stream), __VA_ARGS__);  \
+        if (e__ != cudaSuccess) return ::b2::cuda_fail(e__, who, __FILE__, __LINE__);                                             \
+        return B2_OK;                                                                                                              \
+    } while (0)
 #endif
 
 // ---- programmatic dependent launch (PDL): the launch side.  The kernel side (pdl_trigger / pdl_wait / pdl_sync) and its rules

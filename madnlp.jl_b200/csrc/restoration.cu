@@ -191,13 +191,6 @@ __global__ void k_adjust_boundary(int64_t nlb, int64_t nub, const int64_t* __res
 
 }  // namespace
 
-#define B2_LAUNCH(who, kern, tot, ...) do {                                                                                        \
-        if ((tot) == 0) return B2_OK;                                                                                              \
-        cudaError_t e__ = launch_pdl(kern, dim3(grid_elem(tot)), dim3(256), 0, as_stream(stream), __VA_ARGS__);                    \
-        if (e__ != cudaSuccess) return cuda_fail(e__, who, __FILE__, __LINE__);                                                    \
-        return B2_OK;                                                                                                              \
-    } while (0)
-
 extern "C" {
 
 int b2_rr_init(b2_bounds* b, int64_t m, const double* x_d, const double* c_d, double mu_R, double rho, double* x_ref_d, double* D_R_d,

@@ -16,6 +16,12 @@ restoration_step replays a restoration iteration of robust! (src/IPM/solver.jl:4
     compress_* ; set_aug_RR! + _set_aug_diagonal! ; factorize_wrapper! ; set_aug_rhs_RR! ; inertia_correction! ; finish_aug_solve_RR!
 (the restorer's state and kernels: restoration.py).
 
+The other call sites of src/IPM that factorise or solve, over the solver vectors in `solver_vectors` (restoration.SolverVectors):
+    initialize_dual               initialize_dual(solver, DualInitializeLeastSquares)  (solver.jl:86-97)
+    reinitialize_dual             robust!'s return to the regular phase               (solver.jl:518-530)
+    second_order_correction_step  one pass of second_order_correction's loop          (solver.jl:547-608)
+    restore_direction             the direction at the end of a restore! iteration    (solver.jl:390-402; restoration.SoftRestorer)
+
 The model callbacks themselves are out of scope (SURVEY.md 8a A0): an iterate supplies their outputs.
 """
 from __future__ import annotations
@@ -293,6 +299,128 @@ class IPMLinearAlgebra:
         if ok:
             rr.finish_aug_solve_RR(self.d, rho)
         return ok
+
+    # ------------------------------------------------------------------------------------------- the other solve sites
+    @property
+    def solver_vectors(self):
+        """the solver vectors (restoration.SolverVectors) the solve sites below read and write, and the work vectors _w1, _w2 of
+        MadNLPSolver; allocated on first use"""
+        if getattr(self, "_sv", None) is None:
+            from .restoration import SolverVectors
+            self._sv = SolverVectors(self.kkt)
+            self._w1 = UnreducedKKTVector.for_kkt(self.kkt)
+            self._w2 = UnreducedKKTVector.for_kkt(self.kkt)
+            self._sites = torch.zeros(4, dtype=torch.float64, device=self.d.values.device)     # DUAL_INIT_NORM, DUAL_INIT_COPY, alpha_soc
+            self._sites_h = torch.zeros(2, dtype=torch.float64).pin_memory()
+            self._llb_uub_d = None
+        return self._sv
+
+    def _sp(self):
+        from .capi import stream_ptr
+        return stream_ptr(getattr(self.kkt, "stream", None))
+
+    def _refuse_quasi_newton(self, who):
+        from .quasi_newton import ExactHessian
+        if not isinstance(getattr(self.kkt, "quasi_newton", ExactHessian()), ExactHessian):
+            raise ValueError(f"{who}: not supported with a quasi-Newton Hessian (as the restoration phase)")
+
+    def _llb_uub(self):
+        """ind_llb / ind_uub (src/Callbacks/nlpmodels.jl:391-392) on the device, the model variables being n_tot minus the slacks"""
+        if self._llb_uub_d is None:
+            from .barrier import llb_uub
+            k = self.kkt
+            dev = self.d.values.device
+            self._llb_uub_d = tuple(torch.from_numpy(a).to(dev) for a in llb_uub(k.ind_lb, k.ind_ub, len(k.pr_diag) - len(k.ind_ineq)))
+        return self._llb_uub_d
+
+    def _set_initial_rhs(self):
+        from .capi import lib, check, ptr
+        v = self.solver_vectors
+        check(lib.b2_set_initial_rhs(self.kkt._bounds.h, v.m, ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(self.p.values), self._sp()))
+
+    def _set_aug_rhs_perturbed(self, c, c_trial, alpha, mu, kappa_d):
+        from .capi import lib, check, ptr
+        v = self.solver_vectors
+        llb, uub = self._llb_uub()
+        check(lib.b2_set_aug_rhs_perturbed(self.kkt._bounds.h, v.m, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.f), ptr(v.zl), ptr(v.zu),
+                                           ptr(v.jacl), ptr(c), None if c_trial is None else ptr(c_trial), float(alpha), float(mu),
+                                           float(kappa_d), llb.numel(), ptr(llb) if llb.numel() else None, uub.numel(),
+                                           ptr(uub) if uub.numel() else None, ptr(self.p.values), self._sp()))
+
+    def _dual_init_select(self, solved, constr_mult_init_max):
+        """the y rule on the device, then one read of (norm, decision): returns (solved, ||dual(d)||_inf, y was copied)"""
+        from .capi import lib, check, ptr
+        v = self.solver_vectors
+        check(lib.b2_dual_init_select(self.kkt._bounds.h, v.m, ptr(self.d.dual()), int(bool(solved)), float(constr_mult_init_max),
+                                      ptr(v.y), ptr(self._sites), self._sp()))
+        self._sites_h.copy_(self._sites[:2], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return bool(solved), float(self._sites_h[0]), float(self._sites_h[1]) == 1.0
+
+    def initialize_dual(self, constr_mult_init_max=1e3):
+        """initialize_dual(solver, DualInitializeLeastSquares) (solver.jl:86-97) after the caller's kkt.initialize() and Jacobian values
+        (MadNLP's initialize!, solver.jl:52-62): compress_jacobian! (the tail of eval_jac_wrapper!), set_initial_rhs!,
+        factorize_wrapper!, solve_refine_wrapper! (with its improve! retry) and the y rule, which writes solver_vectors.y.  The inertia
+        is not read.  With [[I, J'], [J, 0]] factorised, dual(d) is the least-squares multiplier of J'y = -f + zl - zu.
+        Returns (solved, ||dual(d)||_inf, y copied): y = dual(d) when solved and the norm is not above constr_mult_init_max, else 0."""
+        self.kkt.compress_jacobian()
+        self._set_initial_rhs()
+        self._factorize_wrapper()
+        ok = self._solve_refine_wrapper()
+        return self._dual_init_select(ok, constr_mult_init_max)
+
+    def reinitialize_dual(self, constr_mult_init_max=1e3):
+        """robust!'s return to the regular phase (solver.jl:518-530), in the reference's order: set_initial_rhs!, kkt.initialize(),
+        factorize_wrapper!, solve_refine_wrapper!, the y rule with the solve taken as successful (the reference does not check it).
+        There is no compress_hessian! in between, so DenseKKTSystem factorises with the diag_hess of the last compress_hessian! on its
+        diagonal (Dense/augmented.jl:120), as the reference does.  Returns what initialize_dual returns.  Exact Hessian only."""
+        self._refuse_quasi_newton("reinitialize_dual")
+        self._set_initial_rhs()
+        self.kkt.initialize()
+        self._factorize_wrapper()
+        self._solve_refine_wrapper()
+        return self._dual_init_select(True, constr_mult_init_max)
+
+    def second_order_correction_step(self, p, alpha_max, mu, kappa_d=1e-5, tau=0.99):
+        """Pass p (1-based) of second_order_correction's loop (solver.jl:556-575) on the current factor: set_aug_rhs! with wy and
+        dual_inf_perturbation!, the refined solve into _w1, alpha_soc = get_alpha_max(x, xl, xu, primal(_w1), tau), and
+        x_trial = x + alpha_soc primal(_w1).  At p = 1, wy = c_trial + alpha_max c.  From p = 2 on, wy is dual(_w1) as the reference
+        has it: the solve overwrote _w1, so wy is the dual part of the previous correction (Ipopt would use alpha_soc c_soc + c(x_soc)).
+        The filter tests, the kappa_soc break and the callbacks stay with the caller, which evaluates c_trial at x_trial.  Returns
+        (solved, the one-element device tensor holding alpha_soc)."""
+        from .capi import lib, check, ptr
+        v = self.solver_vectors
+        if p < 1:
+            raise ValueError(f"second_order_correction_step: p counts from 1, got {p}")
+        if p == 1:
+            self._set_aug_rhs_perturbed(v.c, v.c_trial, alpha_max, mu, kappa_d)
+        else:
+            self._set_aug_rhs_perturbed(self._w1.dual(), None, 0.0, mu, kappa_d)
+        ok = self._solve_refine_wrapper(self._w1, self.p, self.w)
+        alpha = self._sites[2:3]
+        sp = self._sp()
+        check(lib.b2_get_alpha_max(self.kkt._bounds.h, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(self._w1.primal()), float(tau), ptr(alpha), sp))
+        check(lib.b2_soc_trial(v.n_tot, ptr(alpha), ptr(v.x), ptr(self._w1.primal()), ptr(v.x_trial), sp))
+        return ok, alpha
+
+    def restore_direction(self, mu, kappa_d=1e-5, primal_regularization=0.0, dual_regularization=0.0):
+        """The direction at the end of a restore! iteration (solver.jl:390-402), after the caller's eval_lag_hess_wrapper! (values in
+        kkt.hess): compress_*, set_aug_diagonal! from the solver vectors, the type's _set_aug_diagonal!, build_kkt!, factorize!,
+        set_aug_rhs!(c) with dual_inf_perturbation! (ind_llb / ind_uub of barrier.llb_uub), solve_refine_wrapper!.  No inertia
+        correction, as in the reference.  The regularisations are MadNLP's default_primal_regularization / default_dual_regularization.
+        Returns whether the solve succeeded; the direction is in d.  Exact Hessian only."""
+        from .capi import lib, check, ptr
+        self._refuse_quasi_newton("restore_direction")
+        k, v = self.kkt, self.solver_vectors
+        k.compress_jacobian()
+        k.compress_hessian()
+        check(lib.b2_set_aug_diagonal_iterate(k._bounds.h, v.m, float(primal_regularization), float(dual_regularization), ptr(v.x),
+                                              ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower),
+                                              ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self._sp()))
+        k.set_aug_diagonal_()
+        self._factorize_wrapper()
+        self._set_aug_rhs_perturbed(v.c, None, 0.0, mu, kappa_d)
+        return self._solve_refine_wrapper()
 
     def _load_ifr_from(self, rr):
         """the curvature test's inputs from the restorer's solver vectors (one launch)"""

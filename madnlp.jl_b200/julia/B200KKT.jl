@@ -801,6 +801,160 @@ get_varphi_d_R(kkt::B200IFRKKT, f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho)
     _reduce(kkt, :b2_get_varphi_d_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(f_R), _ptr(x), _ptr(xl), _ptr(xu),
             _ptr(dx), _ptr(pp), _ptr(nn), _ptr(dpp), _ptr(dnn), mu_R, rho)
 
+# ---- the other solve sites (src/IPM/solver.jl): initialize_dual with DualInitializeLeastSquares (:86-97), robust!'s return to the regular
+# phase (:518-530), second_order_correction (:547-608) and restore! (:300-411).  The factorisation and the refined solve stay MadNLP's
+# (factorize_wrapper!, solve_refine_wrapper!); the right-hand sides, the y rule, get_F, restore!'s step and the trial point are one launch
+# each (csrc/solve_sites.cu), with every step length read by the kernels from device memory.  The filter tests, the callbacks and the
+# counters stay MadNLP's.  robust! calls b200_reinitialize_dual! in place of its exit block (one line, INTEGRATION.md).  Like the rest of
+# this file, NOT RUN.
+function _set_initial_rhs!(solver::B200RRSolver{T}) where T
+    pl, m = ifr_plans(MadNLP.get_kkt(solver)), length(MadNLP.get_c(solver))
+    check(ccall((:b2_set_initial_rhs, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), pl.bounds, m,
+                _ptr(MadNLP.full(MadNLP.get_f(solver))), _ptr(MadNLP.full(MadNLP.get_zl(solver))), _ptr(MadNLP.full(MadNLP.get_zu(solver))),
+                _ptr(MadNLP.full(MadNLP.get_p(solver))), _sp()), SolveException)
+end
+
+function _dual_init_select!(solver::B200RRSolver{T}, solved::Bool) where T
+    pl, y = ifr_plans(MadNLP.get_kkt(solver)), MadNLP.get_y(solver)
+    check(ccall((:b2_dual_init_select, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, Int32, Cdouble, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                pl.bounds, length(y), _ptr(MadNLP.dual(MadNLP.get_d(solver))), Int32(solved), MadNLP.get_opt(solver).constr_mult_init_max,
+                _ptr(y), _ptr(pl.result), _sp()), SolveException)
+    return
+end
+
+# set_aug_rhs!(solver, kkt, w, mu) + dual_inf_perturbation!; w = c, or c_trial + alpha c when c_trial !== nothing
+function _set_aug_rhs_perturbed!(solver::B200RRSolver{T}, c, c_trial, alpha) where T
+    pl, o = ifr_plans(MadNLP.get_kkt(solver)), MadNLP.get_opt(solver)
+    v = map(MadNLP.full, (MadNLP.get_x(solver), MadNLP.get_xl(solver), MadNLP.get_xu(solver), MadNLP.get_f(solver), MadNLP.get_zl(solver),
+                          MadNLP.get_zu(solver)))
+    llb = CuVector{Int64}(MadNLP.get_ind_llb(solver) .- 1); uub = CuVector{Int64}(MadNLP.get_ind_uub(solver) .- 1)
+    check(ccall((:b2_set_aug_rhs_perturbed, libb200kkt), Cint,
+                (Ptr{Cvoid}, Int64, ntuple(_ -> CuPtr{T}, 9)..., Cdouble, Cdouble, Cdouble, Int64, CuPtr{Int64}, Int64, CuPtr{Int64}, CuPtr{T},
+                 Ptr{Cvoid}), pl.bounds, length(c), map(_ptr, v)..., _ptr(MadNLP.get_jacl(solver)), _ptr(c),
+                c_trial === nothing ? CU_NULL : _ptr(c_trial), Float64(alpha), MadNLP.get_mu(solver), o.kappa_d, length(llb), _ptr(llb),
+                length(uub), _ptr(uub), _ptr(MadNLP.full(MadNLP.get_p(solver))), _sp()), SolveException)
+end
+
+function MadNLP.initialize_dual(solver::B200RRSolver{T}, ::Type{MadNLP.DualInitializeLeastSquares}) where T
+    _set_initial_rhs!(solver)
+    MadNLP.factorize_wrapper!(solver)
+    is_solved = MadNLP.solve_refine_wrapper!(MadNLP.get_d(solver), solver, MadNLP.get_p(solver), MadNLP.get__w4(solver))
+    _dual_init_select!(solver, is_solved)
+end
+
+# robust!'s exit block (solver.jl:518-530), in its order: no compress_hessian!, so a dense augmented system keeps its stale diag_hess
+function b200_reinitialize_dual!(solver::B200RRSolver{T}) where T
+    _set_initial_rhs!(solver)
+    MadNLP.initialize!(MadNLP.get_kkt(solver))
+    MadNLP.factorize_wrapper!(solver)
+    MadNLP.solve_refine_wrapper!(MadNLP.get_d(solver), solver, MadNLP.get_p(solver), MadNLP.get__w4(solver))
+    _dual_init_select!(solver, true)
+end
+
+function MadNLP.second_order_correction(solver::B200RRSolver{T}, alpha_max, theta, varphi, theta_trial, varphi_d,
+                                        switching_condition::Bool) where T
+    o, kkt, pl = MadNLP.get_opt(solver), MadNLP.get_kkt(solver), ifr_plans(MadNLP.get_kkt(solver))
+    w1 = MadNLP.get__w1(solver)
+    x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
+    theta_soc_old = theta_trial
+    for p = 1:o.max_soc
+        # pass 1: wy = c_trial + alpha_max c on the fly; later passes: wy = dual(_w1), the previous correction's dual part (as the reference)
+        p == 1 ? _set_aug_rhs_perturbed!(solver, MadNLP.get_c(solver), MadNLP.get_c_trial(solver), alpha_max) :
+                 _set_aug_rhs_perturbed!(solver, MadNLP.dual(w1), nothing, zero(T))
+        MadNLP.solve_refine_wrapper!(w1, solver, MadNLP.get_p(solver), MadNLP.get__w4(solver))
+        check(ccall((:b2_get_alpha_max, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+                    pl.bounds, _ptr(x), _ptr(xl), _ptr(xu), _ptr(MadNLP.primal(w1)), MadNLP.get_tau(solver), _ptr(pl.result), _sp()), SolveException)
+        check(ccall((:b2_soc_trial, libb200kkt), Cint, (Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), length(x), _ptr(pl.result),
+                    _ptr(x), _ptr(MadNLP.primal(w1)), _ptr(MadNLP.full(MadNLP.get_x_trial(solver))), _sp()), SolveException)
+        alpha_soc = Array(view(pl.result, 1:1))[1]
+        MadNLP.eval_cons_wrapper!(solver, MadNLP.get_c_trial(solver), MadNLP.get_x_trial(solver))
+        MadNLP.set_obj_val_trial!(solver, MadNLP.eval_f_wrapper(solver, MadNLP.get_x_trial(solver)))
+        theta_soc = get_theta(kkt, MadNLP.get_c_trial(solver))
+        varphi_soc = MadNLP.get_varphi(MadNLP.get_obj_val_trial(solver), MadNLP.get_x_trial_lr(solver), MadNLP.get_xl_r(solver),
+                                       MadNLP.get_xu_r(solver), MadNLP.get_x_trial_ur(solver), MadNLP.get_mu(solver))
+        !MadNLP.is_filter_acceptable(MadNLP.get_filter(solver), theta_soc, varphi_soc) && break
+        if theta <= MadNLP.get_theta_min(solver) && switching_condition
+            if MadNLP.is_armijo(varphi_soc, varphi, o.eta_phi, MadNLP.get_alpha(solver), varphi_d)
+                MadNLP.set_ftype!(solver, "F"); MadNLP.set_alpha!(solver, alpha_soc)
+                return true
+            end
+        elseif MadNLP.is_sufficient_progress(theta_soc, theta, o.gamma_theta, varphi_soc, varphi, o.gamma_phi, MadNLP.has_constraints(solver))
+            MadNLP.set_ftype!(solver, "H"); MadNLP.set_alpha!(solver, alpha_soc)
+            return true
+        end
+        theta_soc > o.kappa_soc * theta_soc_old && break
+        theta_soc_old = theta_soc
+    end
+    return false
+end
+
+function MadNLP.restore!(solver::B200RRSolver{T}) where T
+    o, kkt, pl = MadNLP.get_opt(solver), MadNLP.get_kkt(solver), ifr_plans(MadNLP.get_kkt(solver))
+    MadNLP.set_del_w!(solver, zero(T))
+    w1, w2, d = MadNLP.get__w1(solver), MadNLP.get__w2(solver), MadNLP.get_d(solver)
+    x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
+    zl, zu, f = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver)), MadNLP.full(MadNLP.get_f(solver))
+    y, c, jacl = MadNLP.get_y(solver), MadNLP.get_c(solver), MadNLP.get_jacl(solver)
+    copyto!(MadNLP.primal(w1), MadNLP.primal(MadNLP.get_x(solver))); copyto!(MadNLP.dual(w1), y); copyto!(MadNLP.dual(w2), c)
+    get_F() = _reduce(kkt, :b2_get_pd_error, (Int64, ntuple(_ -> _V, 8)..., Cdouble), length(c), _ptr(c), _ptr(f), _ptr(zl), _ptr(zu),
+                      _ptr(jacl), _ptr(x), _ptr(xl), _ptr(xu), MadNLP.get_mu(solver))
+    F = get_F()
+    MadNLP.set_alpha_z!(solver, zero(T)); MadNLP.set_ftype!(solver, "R")
+    a = CUDA.zeros(T, 3)                                   # alpha_max, alpha_z, alpha
+    while true
+        check(ccall((:b2_get_alpha_max, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+                    pl.bounds, _ptr(x), _ptr(xl), _ptr(xu), _ptr(MadNLP.primal(d)), MadNLP.get_tau(solver), _ptr(a), _sp()), SolveException)
+        check(ccall((:b2_get_alpha_z, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+                    pl.bounds, _ptr(zl), _ptr(zu), _ptr(MadNLP.dual_lb(d)), _ptr(MadNLP.dual_ub(d)), MadNLP.get_tau(solver), _ptr(a) + sizeof(T),
+                    _sp()), SolveException)
+        check(ccall((:b2_restore_update, libb200kkt), Cint, (Ptr{Cvoid}, Int64, ntuple(_ -> CuPtr{T}, 11)..., Ptr{Cvoid}), pl.bounds,
+                    length(y), _ptr(a), _ptr(a) + sizeof(T), _ptr(a) + 2 * sizeof(T), _ptr(MadNLP.primal(d)), _ptr(MadNLP.dual(d)),
+                    _ptr(MadNLP.dual_lb(d)), _ptr(MadNLP.dual_ub(d)), _ptr(x), _ptr(y), _ptr(zl), _ptr(zu), _sp()), SolveException)
+        MadNLP.set_alpha!(solver, Array(view(a, 3:3))[1])
+        MadNLP.eval_cons_wrapper!(solver, c, MadNLP.get_x(solver))
+        MadNLP.eval_grad_f_wrapper!(solver, MadNLP.get_f(solver), MadNLP.get_x(solver))
+        MadNLP.set_obj_val!(solver, MadNLP.eval_f_wrapper(solver, MadNLP.get_x(solver)))
+        !o.jacobian_constant && MadNLP.eval_jac_wrapper!(solver, kkt, MadNLP.get_x(solver))
+        MadNLP.jtprod!(jacl, kkt, y)
+        F_trial = get_F()
+        if F_trial > o.soft_resto_pderror_reduction_factor * F
+            copyto!(MadNLP.primal(MadNLP.get_x(solver)), MadNLP.primal(w1)); copyto!(y, MadNLP.dual(w1)); copyto!(c, MadNLP.dual(w2))
+            return MadNLP.ROBUST
+        end
+        MadNLP.adjust_boundary!(MadNLP.get_x_lr(solver), MadNLP.get_xl_r(solver), MadNLP.get_x_ur(solver), MadNLP.get_xu_r(solver),
+                                MadNLP.get_mu(solver))
+        F = F_trial
+        theta = get_theta(kkt, c)
+        varphi = MadNLP.get_varphi(MadNLP.get_obj_val(solver), MadNLP.get_x_lr(solver), MadNLP.get_xl_r(solver), MadNLP.get_xu_r(solver),
+                                   MadNLP.get_x_ur(solver), MadNLP.get_mu(solver))
+        MadNLP.get_cnt(solver).k += 1
+        !(MadNLP.get_intermediate_callback(solver)(solver, MadNLP.UserCallbackRestore())::Bool) && return MadNLP.USER_REQUESTED_STOP
+        MadNLP.is_filter_acceptable(MadNLP.get_filter(solver), theta, varphi) ? (return MadNLP.REGULAR) : (MadNLP.get_cnt(solver).t += 1)
+        MadNLP.get_cnt(solver).k >= o.max_iter && return MadNLP.MAXIMUM_ITERATIONS_EXCEEDED
+        time() - MadNLP.get_cnt(solver).start_time >= o.max_wall_time && return MadNLP.MAXIMUM_WALLTIME_EXCEEDED
+        sd = MadNLP.get_sd(y, MadNLP.get_zl_r(solver), MadNLP.get_zu_r(solver), o.s_max)
+        sc = MadNLP.get_sc(MadNLP.get_zl_r(solver), MadNLP.get_zu_r(solver), o.s_max)
+        MadNLP.set_inf_pr!(solver, MadNLP.get_inf_pr(c))
+        MadNLP.set_inf_du!(solver, MadNLP.get_inf_du(MadNLP.primal(MadNLP.get_f(solver)), MadNLP.primal(MadNLP.get_zl(solver)),
+                                                     MadNLP.primal(MadNLP.get_zu(solver)), jacl, sd))
+        cl = (MadNLP.get_x_lr(solver), MadNLP.get_xl_r(solver), MadNLP.get_zl_r(solver), MadNLP.get_xu_r(solver), MadNLP.get_x_ur(solver),
+              MadNLP.get_zu_r(solver))
+        MadNLP.set_inf_compl!(solver, MadNLP.get_inf_compl(cl..., zero(T), sc))
+        MadNLP.set_inf_compl_mu!(solver, MadNLP.get_inf_compl(cl..., MadNLP.get_mu(solver), sc))
+        MadNLP.print_iter(solver)
+        !o.hessian_constant && MadNLP.eval_lag_hess_wrapper!(solver, kkt, MadNLP.get_x(solver), y)
+        check(ccall((:b2_set_aug_diagonal_iterate, libb200kkt), Cint, (Ptr{Cvoid}, Int64, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 11)..., Ptr{Cvoid}),
+                    pl.bounds, length(y), o.default_primal_regularization, o.default_dual_regularization, _ptr(x), _ptr(xl), _ptr(xu),
+                    _ptr(zl), _ptr(zu), _ptr(kkt.reg), _ptr(kkt.du_diag), _ptr(kkt.l_lower), _ptr(kkt.u_lower), _ptr(kkt.l_diag),
+                    _ptr(kkt.u_diag), _sp()), SolveException)
+        MadNLP._set_aug_diagonal!(kkt)
+        _set_aug_rhs_perturbed!(solver, c, nothing, zero(T))
+        MadNLP.factorize_wrapper!(solver)
+        MadNLP.solve_refine_wrapper!(d, solver, MadNLP.get_p(solver), MadNLP.get__w4(solver))
+        MadNLP.set_ftype!(solver, "f")
+    end
+end
+
 # ---- the adaptive barrier rules (get_adaptive_mu, src/IPM/barrier.jl:260-316) for the solvers this module owns.  The quality-function
 # rule keeps the reference's sequence (set_aug_rhs! with mu = 0, the two solves into _w3 / _w4 without refinement, on the factor the
 # solver holds) and moves the norms, the average complementarity, the centering right-hand side and the whole search to the device:

@@ -18,6 +18,10 @@ csrc/restoration.cu or of the restoration reductions in csrc/ipm_reductions.cu:
 A reduction returns a one-element device tensor (a slot of `results`, so several can be read with one copy) and never synchronises.
 The filter, _update_monotone_RR! and the step acceptance are host scalar logic and stay with the caller, as in the regular phase;
 IPMLinearAlgebra.restoration_step replays the linear algebra of one restoration iteration.
+
+SoftRestorer is restore! (src/IPM/solver.jl:300-411), the soft restoration the regular phase tries before robust!: the backup and
+rollback of the iterate, get_F and the step, over the SolverVectors of an IPMLinearAlgebra, whose restore_direction computes the
+next direction.  SolverVectors holds the solver vectors themselves, shared by the regular phase and, when passed in, a RobustRestorer.
 """
 from __future__ import annotations
 
@@ -32,11 +36,37 @@ from .capi import check, lib, ptr, stream_ptr
  R_VARPHI_D_R, R_LEN) = range(12)
 
 
-class RobustRestorer:
-    """The restorer of one KKT system (its index sets and reduction scratch are the KKT system's b2_bounds).  Scalars as in
-    types.jl: obj_val_R, theta_ref, mu_R, tau_R, zeta, and filter (a host list, as the reference's)."""
+class SolverVectors:
+    """The solver vectors of MadNLPSolver that the device kernels read and write, as device buffers: x, xl, xu, zl, zu, f, jacl and
+    x_trial of length n_tot (+-Inf for an absent bound; zl / zu full length), y, c and c_trial of length m.  One holder serves the
+    regular phase (IPMLinearAlgebra.solver_vectors) and, when passed to it, a RobustRestorer, so both phases see one iterate."""
+
+    NAMES = ("x", "xl", "xu", "zl", "zu", "f", "jacl", "x_trial", "y", "c", "c_trial")
 
     def __init__(self, kkt):
+        self.n_tot, self.m = len(kkt.pr_diag), len(kkt.du_diag)
+        dev = kkt.pr_diag.device
+        for name in self.NAMES:
+            setattr(self, name, torch.zeros(self.m if name in ("y", "c", "c_trial") else self.n_tot, dtype=torch.float64, device=dev))
+
+    def load(self, non_blocking=True, **vectors):
+        """Copy host or device vectors into the named buffers, e.g. load(x=..., y=...); a wrong length raises ValueError"""
+        for name, src in vectors.items():
+            if name not in self.NAMES:
+                raise ValueError(f"load: unknown solver vector {name!r}")
+            dst = getattr(self, name)
+            src = torch.as_tensor(src, dtype=torch.float64)
+            if src.numel() != dst.numel():
+                raise ValueError(f"load: {name} expects {dst.numel()} entries, got {src.numel()}")
+            dst.copy_(src, non_blocking=non_blocking)
+
+
+class RobustRestorer:
+    """The restorer of one KKT system (its index sets and reduction scratch are the KKT system's b2_bounds).  Scalars as in
+    types.jl: obj_val_R, theta_ref, mu_R, tau_R, zeta, and filter (a host list, as the reference's).  `vectors`: the SolverVectors to
+    work on (IPMLinearAlgebra.solver_vectors to share the regular phase's iterate); by default the restorer holds its own."""
+
+    def __init__(self, kkt, vectors=None):
         self.kkt = kkt
         self._b = kkt._bounds.h
         self.n_tot, self.m = len(kkt.pr_diag), len(kkt.du_diag)
@@ -46,8 +76,10 @@ class RobustRestorer:
         self.f_R, self.x_ref, self.D_R = z(self.n_tot), z(self.n_tot), z(self.n_tot)
         (self.pp, self.nn, self.zp, self.zn, self.dpp, self.dnn, self.dzp, self.dzn,
          self.pp_trial, self.nn_trial) = (z(self.m) for _ in range(10))
-        self.x, self.xl, self.xu, self.zl, self.zu, self.f, self.jacl = (z(self.n_tot) for _ in range(7))
-        self.y, self.c = z(self.m), z(self.m)
+        self.vectors = SolverVectors(kkt) if vectors is None else vectors
+        v = self.vectors
+        self.x, self.xl, self.xu, self.zl, self.zu, self.f, self.jacl, self.y, self.c = (v.x, v.xl, v.xu, v.zl, v.zu, v.f, v.jacl, v.y,
+                                                                                         v.c)
         self.results = z(R_LEN)
         self._norms_h = torch.zeros(2, dtype=torch.float64).pin_memory()
         self.obj_val_R = self.theta_ref = self.mu_R = self.tau_R = self.zeta = 0.0
@@ -62,12 +94,7 @@ class RobustRestorer:
 
     def load_inputs(self, x, xl, xu, zl, zu, y, f, jacl, c, non_blocking=True):
         """Copy the solver vectors the restoration kernels read into the restorer's buffers (n_tot: x, xl, xu, zl, zu, f, jacl; m: y, c)"""
-        for dst, src in ((self.x, x), (self.xl, xl), (self.xu, xu), (self.zl, zl), (self.zu, zu), (self.f, f), (self.jacl, jacl),
-                         (self.y, y), (self.c, c)):
-            src = torch.as_tensor(src, dtype=torch.float64)
-            if src.numel() != dst.numel():
-                raise ValueError(f"load_inputs: expected {dst.numel()} entries, got {src.numel()}")
-            dst.copy_(src, non_blocking=non_blocking)
+        self.vectors.load(non_blocking, x=x, xl=xl, xu=xu, zl=zl, zu=zu, f=f, jacl=jacl, y=y, c=c)
 
     # ---------------------------------------------------------------------------------------------------------- elementwise
     def initialize(self, mu, rho=1000.0, tau_min=0.99, theta_max=math.inf):
@@ -203,3 +230,87 @@ class RobustRestorer:
                                     ptr(self.nn), ptr(self.dpp), ptr(self.dnn), self.mu_R, float(rho), ptr(self._slot(R_VARPHI_D_R)),
                                     self._sp()))
         return self._slot(R_VARPHI_D_R)
+
+
+# slots of SoftRestorer.results
+S_F, S_F_TRIAL, S_ALPHA_MAX, S_ALPHA_Z, S_ALPHA, S_LEN = range(6)
+
+
+class SoftRestorer:
+    """restore! (src/IPM/solver.jl:300-411), MadNLP's soft restoration, on the device: the state of one call over the solver vectors,
+    work vectors and right-hand side of an IPMLinearAlgebra `la`.  Per iteration of the reference's loop:
+
+        update(tau)         alpha = min(get_alpha_max, get_alpha_z) and the step of x, y, zl_r, zu_r  (:324-339, one launch after the
+                            two reductions; the host never reads alpha)
+        (caller)            the callbacks (c, f, obj_val, jac) and jtprod! into la.solver_vectors
+        get_F(mu)           F_trial (:345-358)
+        read()              F, F_trial and alpha in one copy, for the caller's soft_resto_pderror_reduction_factor test
+        rollback()          on rejection: x, y and c back from _w1 / _w2 (:359-364), then robust!
+        accept()            F = F_trial, then adjust_boundary! (the caller, or RobustRestorer.adjust_boundary over the same vectors)
+                            and la.restore_direction(mu, kappa_d) for the next direction (:393-402)
+
+    begin(mu) opens the call: it backs x and y up into _w1 and c into _w2, and computes F.  The filter, the callbacks and the
+    iteration counters stay with the caller, as for robust!.  Reductions share the KKT system's scratch: one stream."""
+
+    def __init__(self, la):
+        self.la = la
+        self.kkt = la.kkt
+        self.vectors = la.solver_vectors
+        self._b = self.kkt._bounds.h
+        self.results = torch.zeros(S_LEN, dtype=torch.float64, device=la.d.values.device)
+        self._h = torch.zeros(S_LEN, dtype=torch.float64).pin_memory()
+
+    def _sp(self):
+        return stream_ptr(getattr(self.kkt, "stream", None))
+
+    def _slot(self, k):
+        return self.results[k:k + 1]
+
+    def _copy_many(self, pairs):
+        import ctypes as C
+        cnt = len(pairs)
+        src = (C.c_void_p * cnt)(*[s.data_ptr() for s, _ in pairs])
+        dst = (C.c_void_p * cnt)(*[d.data_ptr() for _, d in pairs])
+        ns = (C.c_int64 * cnt)(*[d.numel() for _, d in pairs])
+        check(lib.b2_copy_many(cnt, src, dst, ns, self._sp()))
+
+    def begin(self, mu):
+        """copyto!(primal(_w1), x); copyto!(dual(_w1), y); copyto!(dual(_w2), c) in one launch, then F = get_F(mu) (:301-323)"""
+        v, w1, w2 = self.vectors, self.la._w1, self.la._w2
+        self._copy_many(((v.x, w1.primal()), (v.y, w1.dual()), (v.c, w2.dual())))
+        self.get_F(mu, S_F)
+
+    def get_F(self, mu, slot=S_F_TRIAL):
+        """get_F(c, f, zl, zu, jacl, x_lr, xl_r, zl_r, xu_r, x_ur, zu_r, mu) (kernels.jl:572-610) into a result slot (F_trial by
+        default); returns the one-element device tensor"""
+        v = self.vectors
+        check(lib.b2_get_pd_error(self._b, v.m, ptr(v.c), ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(v.jacl), ptr(v.x), ptr(v.xl), ptr(v.xu),
+                                  float(mu), ptr(self._slot(slot)), self._sp()))
+        return self._slot(slot)
+
+    def update(self, tau):
+        """alpha_max = get_alpha_max(x, xl, xu, primal(d), tau); alpha = min(alpha_max, get_alpha_z(zl_r, zu_r, dual_lb(d), dual_ub(d),
+        tau)); x += alpha primal(d); y += alpha dual(d); zl_r += alpha dual_lb(d); zu_r += alpha dual_ub(d).  Returns alpha's slot."""
+        v, d, sp = self.vectors, self.la.d, self._sp()
+        check(lib.b2_get_alpha_max(self._b, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(d.primal()), float(tau), ptr(self._slot(S_ALPHA_MAX)), sp))
+        check(lib.b2_get_alpha_z(self._b, ptr(v.zl), ptr(v.zu), ptr(d.dual_lb()), ptr(d.dual_ub()), float(tau), ptr(self._slot(S_ALPHA_Z)),
+                                 sp))
+        check(lib.b2_restore_update(self._b, v.m, ptr(self._slot(S_ALPHA_MAX)), ptr(self._slot(S_ALPHA_Z)), ptr(self._slot(S_ALPHA)),
+                                    ptr(d.primal()), ptr(d.dual()), ptr(d.dual_lb()), ptr(d.dual_ub()), ptr(v.x), ptr(v.y), ptr(v.zl),
+                                    ptr(v.zu), sp))
+        return self._slot(S_ALPHA)
+
+    def read(self):
+        """F, F_trial and alpha as host floats (one copy, one synchronisation)"""
+        self._h.copy_(self.results, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return dict(F=float(self._h[S_F]), F_trial=float(self._h[S_F_TRIAL]), alpha=float(self._h[S_ALPHA]))
+
+    def accept(self):
+        """F = F_trial"""
+        check(lib.b2_copy(1, ptr(self._slot(S_F_TRIAL)), ptr(self._slot(S_F)), self._sp()))
+
+    def rollback(self):
+        """copyto!(primal(x), primal(_w1)); copyto!(y, dual(_w1)); copyto!(c, dual(_w2)) in one launch (:359-364)"""
+        v, w1, w2 = self.vectors, self.la._w1, self.la._w2
+        self._copy_many(((w1.primal(), v.x), (w1.dual(), v.y), (w2.dual(), v.c)))
