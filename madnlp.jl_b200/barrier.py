@@ -23,8 +23,9 @@ import numpy as np
 import torch
 
 from . import capi
-from .capi import check, lib, ptr, stream_ptr
-from .kkt import UnreducedKKTVector
+from .capi import check, lib, ptr
+from .capture import CapturedSequence
+from .kkt import SolverVectors, UnreducedKKTVector
 
 
 def _mu_min(tol, barrier_tol_factor):
@@ -115,17 +116,17 @@ def llb_uub(ind_lb, ind_ub, nvar):
 
 class AdaptiveBarrier:
     """The adaptive barrier rules of one KKT system.  Owns step_aff, step_cen, its own right-hand side p (the caller's d, p and w are not
-    touched), ind_llb / ind_uub on the device, the scalar array scal (capi.QF_* layout) and the search result, plus the solver vectors
-    the rules read (x, xl, xu, zl, zu, f, jacl: n_tot, +-Inf for an absent bound and zl / zu full length; c: m), which load_inputs
-    fills.  nvar: the number of model variables (default: n_tot minus the slacks of kkt.ind_ineq)."""
+    touched), ind_llb / ind_uub on the device, the scalar array scal (capi.QF_* layout) and the search result.  The rules read x, xl, xu,
+    zl, zu, f, jacl and c of `vectors`: the kkt.SolverVectors to work on (IPMLinearAlgebra.solver_vectors to share the solver's iterate);
+    by default the object holds its own, which load_inputs fills.  nvar: the number of model variables (default: n_tot minus the slacks
+    of kkt.ind_ineq)."""
 
-    def __init__(self, kkt, nvar=None, use_cuda_graph=True):
+    def __init__(self, kkt, nvar=None, use_cuda_graph=True, vectors=None):
         self.kkt = kkt
         self._b = kkt._bounds.h
         self.n_tot, self.m = len(kkt.pr_diag), len(kkt.du_diag)
         self.nlb, self.nub = len(kkt.l_diag), len(kkt.u_diag)
         self.nvar = self.n_tot - len(kkt.ind_ineq) if nvar is None else int(nvar)
-        self.use_cuda_graph = use_cuda_graph
         dev = kkt.pr_diag.device
         z = lambda k: torch.zeros(k, dtype=torch.float64, device=dev)
         self.step_aff = UnreducedKKTVector.for_kkt(kkt)
@@ -134,30 +135,22 @@ class AdaptiveBarrier:
         llb, uub = llb_uub(kkt.ind_lb, kkt.ind_ub, self.nvar)
         self.ind_llb = torch.from_numpy(llb).to(dev)
         self.ind_uub = torch.from_numpy(uub).to(dev)
-        self.x, self.xl, self.xu, self.zl, self.zu, self.f, self.jacl = (z(self.n_tot) for _ in range(7))
-        self.c = z(self.m)
+        self.vectors = SolverVectors(kkt) if vectors is None else vectors
         self.scal = z(capi.QF_SCAL_LEN)
         self.cc = z(2)                                              # LOQO: average and minimum complementarity
         self.result = z(capi.qf_result_len(capi.QF_MAX_GS_ITER))
         self._result_h = torch.zeros(capi.QF_TRACE, dtype=torch.float64).pin_memory()
-        self._graph = self._graph_key = None
+        self._graph = CapturedSequence(use_cuda_graph)
         self.last_result = None
 
-    def _sp(self):
-        return stream_ptr(getattr(self.kkt, "stream", None))
-
     def load_inputs(self, x, xl, xu, zl, zu, f, jacl, c, non_blocking=True):
-        """Copy the solver vectors the rules read into the object's buffers (n_tot: x, xl, xu, zl, zu, f, jacl; m: c)"""
-        for dst, src in ((self.x, x), (self.xl, xl), (self.xu, xu), (self.zl, zl), (self.zu, zu), (self.f, f), (self.jacl, jacl),
-                         (self.c, c)):
-            src = torch.as_tensor(src, dtype=torch.float64)
-            if src.numel() != dst.numel():
-                raise ValueError(f"load_inputs: expected {dst.numel()} entries, got {src.numel()}")
-            dst.copy_(src, non_blocking=non_blocking)
+        """Copy the solver vectors the rules read into `vectors` (n_tot: x, xl, xu, zl, zu, f, jacl; m: c)"""
+        self.vectors.load(non_blocking, x=x, xl=xl, xu=xu, zl=zl, zu=zu, f=f, jacl=jacl, c=c)
 
     def _average_complementarity(self, out):
-        check(lib.b2_get_average_complementarity(self._b, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu), ptr(out),
-                                                 self._sp()))
+        v = self.vectors
+        check(lib.b2_get_average_complementarity(self._b, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(out),
+                                                 self.kkt.stream_ptr()))
 
     def _read(self, src, k):
         self._result_h[:k].copy_(src[:k], non_blocking=True)
@@ -178,8 +171,9 @@ class AdaptiveBarrier:
             return barrier.mu_min
         if isinstance(barrier, LOQOUpdate):
             self._average_complementarity(self.cc[0:1])
-            check(lib.b2_get_min_complementarity(self._b, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu),
-                                                 ptr(self.cc[1:2]), self._sp()))
+            v = self.vectors
+            check(lib.b2_get_min_complementarity(self._b, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(self.cc[1:2]),
+                                                 self.kkt.stream_ptr()))
             avg, min_cc = self._read(self.cc, 2)
             return loqo_mu(avg, min_cc, barrier)
         if not isinstance(barrier, QualityFunctionUpdate):
@@ -189,37 +183,18 @@ class AdaptiveBarrier:
         self.scal[capi.QF_TAU:capi.QF_TAU + 1].fill_(float(tau))
         args = (float(barrier.sigma_min), float(barrier.sigma_max), float(barrier.mu_min), float(barrier.mu_max), float(barrier.sigma_tol),
                 int(barrier.max_gs_iter), float(kappa_d))
-        self._run(args)
+        # the device sequence: eager on the first call with these constants, captured on the second, replayed after
+        self._graph.run(lambda: self._sequence(*args), args)
         self.last_result = self._read(self.result, capi.QF_TRACE)
         barrier.n_update += 1
         return self.last_result[capi.QF_MU]
 
-    def _run(self, args):
-        """the device sequence; eager on the first call with these constants, captured on the second, replayed after"""
-        if not self.use_cuda_graph:
-            self._sequence(*args)
-            return
-        if self._graph_key != args:
-            self._graph, self._graph_key = None, args
-        if self._graph is None:
-            self._sequence(*args)
-            self._graph = False
-        elif self._graph is False:
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g):
-                self._sequence(*args)
-            self._graph = g
-            g.replay()
-        else:
-            self._graph.replay()
-
     def _sequence(self, sigma_min, sigma_max, mu_min, mu_max, sigma_tol, max_gs_iter, kappa_d):
-        k, sp, n = self.kkt, self._sp(), self.p.values.numel()
+        k, v, sp, n = self.kkt, self.vectors, self.kkt.stream_ptr(), self.p.values.numel()
         scal = ptr(self.scal)
         # affine step (barrier.jl:268-274)
-        check(lib.b2_set_aug_rhs(self._b, self.m, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.f), ptr(self.zl), ptr(self.zu),
-                                 ptr(self.jacl), ptr(self.c), 0.0, ptr(self.p.values), sp))
+        check(lib.b2_set_aug_rhs(self._b, self.m, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(v.jacl), ptr(v.c),
+                                 0.0, ptr(self.p.values), sp))
         check(lib.b2_primal_dual_norm2(self._b, self.m, ptr(self.p.values), scal + 8 * capi.QF_NRM_PRIMAL, sp))
         check(lib.b2_copy(n, ptr(self.p.values), ptr(self.step_aff.values), sp))
         k.solve_kkt(self.step_aff)
@@ -232,7 +207,7 @@ class AdaptiveBarrier:
         check(lib.b2_copy(n, ptr(self.p.values), ptr(self.step_cen.values), sp))
         k.solve_kkt(self.step_cen)
         # the search (:283-301)
-        check(lib.b2_qf_search(self._b, self.m, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu),
+        check(lib.b2_qf_search(self._b, self.m, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu),
                                ptr(self.step_aff.values), ptr(self.step_cen.values), scal, sigma_min, sigma_max, mu_min, mu_max, sigma_tol,
                                max_gs_iter, ptr(self.result), sp))
 

@@ -309,6 +309,16 @@ def ptr(t):
     return t.ctypes.data
 
 
+def copy_many(pairs, stream=None):
+    """b2_copy_many: copy every (src, dst) pair of float64 device tensors of one length each in ONE launch; at most 16 pairs (the
+    entry refuses more)."""
+    n = len(pairs)
+    src = (C.c_void_p * n)(*[s.data_ptr() for s, _ in pairs])
+    dst = (C.c_void_p * n)(*[d.data_ptr() for _, d in pairs])
+    ns = (C.c_int64 * n)(*[d.numel() for _, d in pairs])
+    check(lib.b2_copy_many(n, src, dst, ns, stream_ptr(stream)))
+
+
 def stream_ptr(stream=None):
     if stream is None:
         import torch

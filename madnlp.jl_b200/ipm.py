@@ -16,7 +16,7 @@ restoration_step replays a restoration iteration of robust! (src/IPM/solver.jl:4
     compress_* ; set_aug_RR! + _set_aug_diagonal! ; factorize_wrapper! ; set_aug_rhs_RR! ; inertia_correction! ; finish_aug_solve_RR!
 (the restorer's state and kernels: restoration.py).
 
-The other call sites of src/IPM that factorise or solve, over the solver vectors in `solver_vectors` (restoration.SolverVectors):
+The other call sites of src/IPM that factorise or solve, over the solver vectors in `solver_vectors` (kkt.SolverVectors):
     initialize_dual               initialize_dual(solver, DualInitializeLeastSquares)  (solver.jl:86-97)
     reinitialize_dual             robust!'s return to the regular phase               (solver.jl:518-530)
     second_order_correction_step  one pass of second_order_correction's loop          (solver.jl:547-608)
@@ -30,7 +30,11 @@ from dataclasses import dataclass
 
 import torch
 
-from .kkt import UnreducedKKTVector
+from .barrier import llb_uub
+from .capi import CURV_PASS, CURV_RESULT_LEN, check, copy_many, lib, ptr
+from .capture import CapturedSequence
+from .kkt import SolverVectors, UnreducedKKTVector
+from .quasi_newton import ExactHessian
 from .richardson import RichardsonIterator
 
 
@@ -60,35 +64,28 @@ def resolve_inertia_correction_method(method, linear_solver):
 
 
 class InertiaFreeCorrector:
-    """The InertiaFree corrector (src/IPM/inertiacorrector.jl:7-17): p0, d0, t, wx, g, plus the solver vectors set_g_ifr! and
-    set_aug_rhs_ifr! read (f, x, xl, xu, jacl: n_tot, +-Inf for an absent bound; c: m), which IPMLinearAlgebra.load_ifr_inputs
-    fills, and _w3, the work vector of the d0 solve."""
+    """The InertiaFree corrector (src/IPM/inertiacorrector.jl:7-17): p0, d0, t, wx, g, and _w3, the work vector of the d0 solve.
+    set_g_ifr! and set_aug_rhs_ifr! read the solver vectors (f, x, xl, xu, jacl, c) of the SolverVectors passed to set_rhs."""
 
     def __init__(self, kkt):
-        from . import capi
         self.p0 = UnreducedKKTVector.for_kkt(kkt)
         self.d0 = UnreducedKKTVector.for_kkt(kkt)
         self.w3 = UnreducedKKTVector.for_kkt(kkt)
-        n_tot, m = self.p0.n, self.p0.m
         z = lambda k: torch.zeros(k, dtype=torch.float64, device=self.p0.values.device)
-        self.t, self.wx, self.g = z(n_tot), z(n_tot), z(n_tot)
-        self.f, self.x, self.xl, self.xu, self.jacl = (z(n_tot) for _ in range(5))
-        self.c = z(m)
-        self.result_h = torch.zeros(capi.CURV_RESULT_LEN, dtype=torch.float64).pin_memory()
+        self.t, self.wx, self.g = z(self.p0.n), z(self.p0.n), z(self.p0.n)
+        self.result_h = torch.zeros(CURV_RESULT_LEN, dtype=torch.float64).pin_memory()
         self.last_result = None
 
-    def set_rhs(self, kkt, mu):
-        """set_g_ifr! (src/IPM/kernels.jl:242-248) and set_aug_rhs_ifr! (:233-240)"""
-        from .capi import lib, check, ptr, stream_ptr
-        sp = stream_ptr(getattr(kkt, "stream", None))
+    def set_rhs(self, kkt, mu, v):
+        """set_g_ifr! (src/IPM/kernels.jl:242-248) and set_aug_rhs_ifr! (:233-240) over the SolverVectors v"""
+        sp = kkt.stream_ptr()
         p0 = self.p0
-        check(lib.b2_set_g_ifr(p0.n, ptr(self.f), ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.jacl), float(mu), ptr(self.g), sp))
-        check(lib.b2_set_aug_rhs_ifr(p0.n, p0.m, p0.nlb, p0.nub, ptr(self.c), ptr(p0.values), sp))
+        check(lib.b2_set_g_ifr(p0.n, ptr(v.f), ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.jacl), float(mu), ptr(self.g), sp))
+        check(lib.b2_set_aug_rhs_ifr(p0.n, p0.m, p0.nlb, p0.nub, ptr(v.c), ptr(p0.values), sp))
 
     def direction_difference(self, kkt, d):
         """t = dx - n with n = primal(d0): copyto! then axpy!(-1, n, t), exact"""
-        from .capi import lib, check, ptr, stream_ptr
-        sp = stream_ptr(getattr(kkt, "stream", None))
+        sp = kkt.stream_ptr()
         check(lib.b2_copy(self.p0.n, ptr(d.primal()), ptr(self.t), sp))
         check(lib.b2_axpy(self.p0.n, -1.0, ptr(self.d0.primal()), ptr(self.t), sp))
 
@@ -98,7 +95,6 @@ class InertiaFreeCorrector:
         self.result_h.copy_(res, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         self.last_result = tuple(float(v) for v in self.result_h)
-        from .capi import CURV_PASS
         return self.last_result[CURV_PASS] == 1.0
 
 
@@ -106,7 +102,7 @@ class IPMLinearAlgebra:
     """Owns the work vectors of MadNLPSolver that the hot path touches (d, p, _w4) and drives one iteration.
 
     inertia_correction_method (MadNLP's option of the same name): "InertiaBased" (the default), "InertiaFree" (the curvature test
-    of Chiang & Zavala; its inputs come from load_ifr_inputs), "InertiaIgnore", or "InertiaAuto" (InertiaBased with every
+    of Chiang & Zavala; it reads solver_vectors, which load_ifr_inputs fills), "InertiaIgnore", or "InertiaAuto" (InertiaBased with every
     solver of this package, since each reports inertia).  inertia_free_tol is the curvature test's tolerance (default 0)."""
 
     def __init__(self, kkt, tol=1e-8, use_cuda_graph=True, speculate=True, inertia_correction_method="InertiaBased",
@@ -116,8 +112,8 @@ class IPMLinearAlgebra:
         self.kkt = kkt
         self.use_cuda_graph = use_cuda_graph
         self.speculate = speculate     # first refinement step queued before the inertia is known (see step())
-        self._prologue_graph = None
-        self._rr_graph = self._rr_graph_key = None      # restoration_step's prologue graph and what it was captured for
+        self._prologue_graph = CapturedSequence(use_cuda_graph)
+        self._rr_graph = CapturedSequence(use_cuda_graph)      # restoration_step's prologue
         self.iterator = RichardsonIterator(kkt, tol=tol, use_cuda_graph=use_cuda_graph)
         self.d = UnreducedKKTVector.for_kkt(kkt)
         self.p = UnreducedKKTVector.for_kkt(kkt)
@@ -125,38 +121,28 @@ class IPMLinearAlgebra:
         self.ifr = InertiaFreeCorrector(kkt) if self.inertia_correction_method == "InertiaFree" else None
         self.opt = InertiaOptions()
         self.del_w_last = 0.0
+        self.last_inertia = None
         self.cnt = dict(factorizations=0, backsolves=0, regularized=0, failed=0)
 
     def load_ifr_inputs(self, f, x, xl, xu, jacl, c, non_blocking=True):
-        """Copy the solver vectors the inertia-free test reads (f, x, xl, xu, jacl: n_tot; c: m) into the corrector's buffers"""
+        """Copy the solver vectors the inertia-free test reads (f, x, xl, xu, jacl: n_tot; c: m) into solver_vectors"""
         if self.ifr is None:
             raise ValueError("load_ifr_inputs needs inertia_correction_method = InertiaFree")
-        r = self.ifr
-        for dst, src in ((r.f, f), (r.x, x), (r.xl, xl), (r.xu, xu), (r.jacl, jacl), (r.c, c)):
-            src = torch.as_tensor(src, dtype=torch.float64)
-            if src.numel() != dst.numel():
-                raise ValueError(f"load_ifr_inputs: expected {dst.numel()} entries, got {src.numel()}")
-            dst.copy_(src, non_blocking=non_blocking)
+        self.solver_vectors.load(non_blocking, f=f, x=x, xl=xl, xu=xu, jacl=jacl, c=c)
 
     def load_iterate(self, it, non_blocking=True):
         """Copy one iterate's callback outputs / diagonal inputs into the KKT buffers (H2D when `it` holds pinned
         host tensors, D2D when it holds device tensors)."""
         k = self.kkt
-        pairs = ((k.get_jacobian(), it["jac"]), (k.get_hessian(), it["hess"]), (k.reg, it["reg"]), (k.du_diag, it["du_diag"]),
-                 (k.l_diag, it["l_diag"]), (k.u_diag, it["u_diag"]), (k.l_lower, it["l_lower"]), (k.u_lower, it["u_lower"]),
-                 (self.p.values, it["rhs"]))
-        if all(src.is_cuda for _, src in pairs):
+        pairs = ((it["jac"], k.get_jacobian()), (it["hess"], k.get_hessian()), (it["reg"], k.reg), (it["du_diag"], k.du_diag),
+                 (it["l_diag"], k.l_diag), (it["u_diag"], k.u_diag), (it["l_lower"], k.l_lower), (it["u_lower"], k.u_lower),
+                 (it["rhs"], self.p.values))
+        if all(src.is_cuda for src, _ in pairs):
             # device-resident producer: one launch for the nine vectors
-            import ctypes as C
-            from .capi import lib, check, stream_ptr
-            cnt = len(pairs)
-            src = (C.c_void_p * cnt)(*[s_.data_ptr() for _, s_ in pairs])
-            dst = (C.c_void_p * cnt)(*[d_.data_ptr() for d_, _ in pairs])
-            ns = (C.c_int64 * cnt)(*[d_.numel() for d_, _ in pairs])
-            assert all(d_.numel() == s_.numel() and s_.dtype == torch.float64 and s_.is_contiguous() for d_, s_ in pairs)
-            check(lib.b2_copy_many(cnt, src, dst, ns, stream_ptr(getattr(k, "stream", None))))
+            assert all(d_.numel() == s_.numel() and s_.dtype == torch.float64 and s_.is_contiguous() for s_, d_ in pairs)
+            copy_many(pairs, k.stream)
         else:
-            for d_, s_ in pairs:
+            for s_, d_ in pairs:
                 d_.copy_(s_, non_blocking=non_blocking)
 
     def load_iterate_host(self, host_iterates, idx):
@@ -209,10 +195,10 @@ class IPMLinearAlgebra:
             x, b, w = self.d, self.p, self.w
         ok = self.iterator.solve_refine(x, b, w)
         if not ok and self.kkt.linear_solver.improve():
-            # improve!() changed a factorisation parameter (pivot threshold) that the captured prologue has baked in:
-            # drop the captured graph so that every later step factorises with the new setting
-            self._prologue_graph = None
-            self._rr_graph = None
+            # improve!() changed a factorisation parameter (pivot threshold) that the captured prologues have baked in:
+            # drop the captured graphs so that every later step factorises with the new setting
+            self._prologue_graph.reset()
+            self._rr_graph.reset()
             self.kkt.factorize_kkt()
             ok = self.iterator.solve_refine(x, b, w)
         self.cnt["backsolves"] += self.iterator.ir
@@ -225,22 +211,10 @@ class IPMLinearAlgebra:
         behind ~0.2 ms of device work instead of sitting between two steps."""
         k = self.kkt
         if self.ifr is not None:
-            self.ifr.set_rhs(k, mu)
+            self.ifr.set_rhs(k, mu, self.solver_vectors)
         # compress_* + set_aug_diagonal! + the first factorize_wrapper! of inertia_correction!: fixed launch sequence,
         # replayed as one CUDA graph from the third step on (eager, capture, replay)
-        if not self.use_cuda_graph or self._prologue_graph is None:
-            self._prologue()
-            if self.use_cuda_graph:
-                self._prologue_graph = False
-        elif self._prologue_graph is False:
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g):
-                self._prologue()
-            self._prologue_graph = g
-            g.replay()
-        else:
-            self._prologue_graph.replay()
+        self._prologue_graph.run(self._prologue)
         self.cnt["factorizations"] += 1
         self._wait_rhs()
         if after_prologue is not None:
@@ -257,19 +231,13 @@ class IPMLinearAlgebra:
         rr: a RobustRestorer of this KKT system after rr.initialize; rho is MadNLP's option of that name, the regularisations its
         default_primal_regularization / default_dual_regularization.  Returns what inertia_correction! returns (False sends robust!
         to RESTORATION_FAILED); the direction is in d and rr.dpp, rr.dnn, rr.dzp, rr.dzn.  Under InertiaFree the curvature test reads
-        rr's f, x, xl, xu, jacl and c, as the reference's set_g_ifr! reads the solver's.  A quasi-Newton Hessian is refused."""
-        from .quasi_newton import ExactHessian
+        rr.vectors (its f, x, xl, xu, jacl and c), as the reference's set_g_ifr! reads the solver's.  A quasi-Newton Hessian is refused."""
         k = self.kkt
-        if not isinstance(getattr(k, "quasi_newton", ExactHessian()), ExactHessian):
-            raise ValueError("restoration_step: the restoration phase with a quasi-Newton Hessian is not supported")
+        self._refuse_quasi_newton("restoration_step")
         if rr.kkt is not k:
             raise ValueError("restoration_step: the RobustRestorer belongs to another KKT system")
         if self.ifr is not None:
-            self._load_ifr_from(rr)
-            self.ifr.set_rhs(k, mu)
-        # the graph bakes in the restorer's buffers and the scalars of set_aug_RR!: capture again when either changes (the key holds
-        # the restorer itself, so its buffers stay alive as long as a graph may replay them)
-        key = (rr, rr.zeta, float(primal_regularization), float(dual_regularization))
+            self.ifr.set_rhs(k, mu, rr.vectors)
 
         def prologue():
             k.compress_jacobian()
@@ -277,22 +245,9 @@ class IPMLinearAlgebra:
             rr.set_aug_RR(k, primal_regularization, dual_regularization)
             k.build_kkt()
             k.factorize_kkt()
-        old = self._rr_graph_key
-        if old is None or old[0] is not rr or old[1:] != key[1:]:
-            self._rr_graph, self._rr_graph_key = None, key
-        if not self.use_cuda_graph or self._rr_graph is None:
-            prologue()
-            if self.use_cuda_graph:
-                self._rr_graph = False
-        elif self._rr_graph is False:
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g):
-                prologue()
-            self._rr_graph = g
-            g.replay()
-        else:
-            self._rr_graph.replay()
+        # the graph bakes in the restorer's buffers and the scalars of set_aug_RR!: capture again when either changes (the key holds
+        # the restorer itself, so its buffers stay alive as long as a graph may replay them)
+        self._rr_graph.run(prologue, (rr, rr.zeta, float(primal_regularization), float(dual_regularization)))
         self.cnt["factorizations"] += 1
         rr.set_aug_rhs_RR(self.p, rho)
         ok = self._inertia_correction(mu)
@@ -303,10 +258,9 @@ class IPMLinearAlgebra:
     # ------------------------------------------------------------------------------------------- the other solve sites
     @property
     def solver_vectors(self):
-        """the solver vectors (restoration.SolverVectors) the solve sites below read and write, and the work vectors _w1, _w2 of
-        MadNLPSolver; allocated on first use"""
+        """the solver vectors (kkt.SolverVectors) the inertia-free test and the solve sites below read and write, and the work vectors
+        _w1, _w2 of MadNLPSolver; allocated on first use"""
         if getattr(self, "_sv", None) is None:
-            from .restoration import SolverVectors
             self._sv = SolverVectors(self.kkt)
             self._w1 = UnreducedKKTVector.for_kkt(self.kkt)
             self._w2 = UnreducedKKTVector.for_kkt(self.kkt)
@@ -315,44 +269,35 @@ class IPMLinearAlgebra:
             self._llb_uub_d = None
         return self._sv
 
-    def _sp(self):
-        from .capi import stream_ptr
-        return stream_ptr(getattr(self.kkt, "stream", None))
-
     def _refuse_quasi_newton(self, who):
-        from .quasi_newton import ExactHessian
         if not isinstance(getattr(self.kkt, "quasi_newton", ExactHessian()), ExactHessian):
-            raise ValueError(f"{who}: not supported with a quasi-Newton Hessian (as the restoration phase)")
+            raise ValueError(f"{who}: not supported with a quasi-Newton Hessian (the restoration phase and the sites it uses)")
 
     def _llb_uub(self):
         """ind_llb / ind_uub (src/Callbacks/nlpmodels.jl:391-392) on the device, the model variables being n_tot minus the slacks"""
         if self._llb_uub_d is None:
-            from .barrier import llb_uub
             k = self.kkt
             dev = self.d.values.device
             self._llb_uub_d = tuple(torch.from_numpy(a).to(dev) for a in llb_uub(k.ind_lb, k.ind_ub, len(k.pr_diag) - len(k.ind_ineq)))
         return self._llb_uub_d
 
     def _set_initial_rhs(self):
-        from .capi import lib, check, ptr
         v = self.solver_vectors
-        check(lib.b2_set_initial_rhs(self.kkt._bounds.h, v.m, ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(self.p.values), self._sp()))
+        check(lib.b2_set_initial_rhs(self.kkt._bounds.h, v.m, ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(self.p.values), self.kkt.stream_ptr()))
 
     def _set_aug_rhs_perturbed(self, c, c_trial, alpha, mu, kappa_d):
-        from .capi import lib, check, ptr
         v = self.solver_vectors
         llb, uub = self._llb_uub()
         check(lib.b2_set_aug_rhs_perturbed(self.kkt._bounds.h, v.m, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.f), ptr(v.zl), ptr(v.zu),
                                            ptr(v.jacl), ptr(c), None if c_trial is None else ptr(c_trial), float(alpha), float(mu),
                                            float(kappa_d), llb.numel(), ptr(llb) if llb.numel() else None, uub.numel(),
-                                           ptr(uub) if uub.numel() else None, ptr(self.p.values), self._sp()))
+                                           ptr(uub) if uub.numel() else None, ptr(self.p.values), self.kkt.stream_ptr()))
 
     def _dual_init_select(self, solved, constr_mult_init_max):
         """the y rule on the device, then one read of (norm, decision): returns (solved, ||dual(d)||_inf, y was copied)"""
-        from .capi import lib, check, ptr
         v = self.solver_vectors
         check(lib.b2_dual_init_select(self.kkt._bounds.h, v.m, ptr(self.d.dual()), int(bool(solved)), float(constr_mult_init_max),
-                                      ptr(v.y), ptr(self._sites), self._sp()))
+                                      ptr(v.y), ptr(self._sites), self.kkt.stream_ptr()))
         self._sites_h.copy_(self._sites[:2], non_blocking=True)
         torch.cuda.current_stream().synchronize()
         return bool(solved), float(self._sites_h[0]), float(self._sites_h[1]) == 1.0
@@ -388,7 +333,6 @@ class IPMLinearAlgebra:
         has it: the solve overwrote _w1, so wy is the dual part of the previous correction (Ipopt would use alpha_soc c_soc + c(x_soc)).
         The filter tests, the kappa_soc break and the callbacks stay with the caller, which evaluates c_trial at x_trial.  Returns
         (solved, the one-element device tensor holding alpha_soc)."""
-        from .capi import lib, check, ptr
         v = self.solver_vectors
         if p < 1:
             raise ValueError(f"second_order_correction_step: p counts from 1, got {p}")
@@ -398,7 +342,7 @@ class IPMLinearAlgebra:
             self._set_aug_rhs_perturbed(self._w1.dual(), None, 0.0, mu, kappa_d)
         ok = self._solve_refine_wrapper(self._w1, self.p, self.w)
         alpha = self._sites[2:3]
-        sp = self._sp()
+        sp = self.kkt.stream_ptr()
         check(lib.b2_get_alpha_max(self.kkt._bounds.h, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(self._w1.primal()), float(tau), ptr(alpha), sp))
         check(lib.b2_soc_trial(v.n_tot, ptr(alpha), ptr(v.x), ptr(self._w1.primal()), ptr(v.x_trial), sp))
         return ok, alpha
@@ -409,58 +353,28 @@ class IPMLinearAlgebra:
         set_aug_rhs!(c) with dual_inf_perturbation! (ind_llb / ind_uub of barrier.llb_uub), solve_refine_wrapper!.  No inertia
         correction, as in the reference.  The regularisations are MadNLP's default_primal_regularization / default_dual_regularization.
         Returns whether the solve succeeded; the direction is in d.  Exact Hessian only."""
-        from .capi import lib, check, ptr
         self._refuse_quasi_newton("restore_direction")
         k, v = self.kkt, self.solver_vectors
         k.compress_jacobian()
         k.compress_hessian()
         check(lib.b2_set_aug_diagonal_iterate(k._bounds.h, v.m, float(primal_regularization), float(dual_regularization), ptr(v.x),
                                               ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower),
-                                              ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self._sp()))
+                                              ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self.kkt.stream_ptr()))
         k.set_aug_diagonal_()
         self._factorize_wrapper()
         self._set_aug_rhs_perturbed(v.c, None, 0.0, mu, kappa_d)
         return self._solve_refine_wrapper()
 
-    def _load_ifr_from(self, rr):
-        """the curvature test's inputs from the restorer's solver vectors (one launch)"""
-        import ctypes as C
-        from .capi import lib, check, stream_ptr
-        r = self.ifr
-        pairs = ((r.f, rr.f), (r.x, rr.x), (r.xl, rr.xl), (r.xu, rr.xu), (r.jacl, rr.jacl), (r.c, rr.c))
-        cnt = len(pairs)
-        src = (C.c_void_p * cnt)(*[s_.data_ptr() for _, s_ in pairs])
-        dst = (C.c_void_p * cnt)(*[d_.data_ptr() for d_, _ in pairs])
-        ns = (C.c_int64 * cnt)(*[d_.numel() for d_, _ in pairs])
-        check(lib.b2_copy_many(cnt, src, dst, ns, stream_ptr(getattr(self.kkt, "stream", None))))
-
     def _inertia_correction(self, mu):
-        """inertia_correction! after its first factorize_wrapper! (src/IPM/solver.jl:611-783), for the method of this object"""
-        k = self.kkt
-        if self.inertia_correction_method != "InertiaBased":
-            return self._inertia_correction_without_inertia(mu)
-        # inertia_correction!(InertiaBased)
-        o = self.opt
-        n_trial = 0
+        """inertia_correction! after its first factorize_wrapper! (src/IPM/solver.jl:611-783), for the method of this object: one del_w
+        schedule; the methods differ in the trial (_trial) and in del_c, which InertiaBased sets only when the inertia asks for it and
+        InertiaFree / InertiaIgnore set on every trial.  `last_del_w` lists the del_w of each trial."""
+        k, o = self.kkt, self.opt
         del_w = del_c = del_w_prev = del_c_prev = 0.0
         self.last_del_w = []
-        ls = k.linear_solver
-        if self.speculate and hasattr(ls, "inertia_enqueue"):
-            # queue the inertia read AND the first refinement step behind the factorisation, block once for both
-            ls.inertia_enqueue()
-            self.iterator.start(self.d, self.p, self.w)
-            torch.cuda.current_stream().synchronize()
-            inertia = ls.inertia_fetch()
-            if k.is_inertia_correct(*inertia):
-                ok = self._solve_refine_wrapper()
-            else:
-                self.iterator.discard()
-                ok = False
-        else:
-            inertia = ls.inertia()
-            ok = self._solve_refine_wrapper() if k.is_inertia_correct(*inertia) else False
+        ok, inertia = self._trial(first=True)
         while not ok:
-            if n_trial == 0:
+            if not self.last_del_w:
                 del_w = o.first_hessian_perturbation if self.del_w_last == 0.0 else max(
                     o.min_hessian_perturbation, o.perturb_dec_fact * self.del_w_last)
             else:
@@ -469,67 +383,49 @@ class IPMLinearAlgebra:
                     self.cnt["failed"] += 1
                     return False
             del_c = (o.jacobian_regularization_value * mu ** o.jacobian_regularization_exponent
-                     if k.should_regularize_dual(*inertia) else 0.0)
+                     if inertia is None or k.should_regularize_dual(*inertia) else 0.0)
             k.regularize_diagonal(del_w - del_w_prev, del_c - del_c_prev)
             del_w_prev, del_c_prev = del_w, del_c
             self.last_del_w.append(del_w)
             self._factorize_wrapper()
-            inertia = k.linear_solver.inertia()
-            ok = self._solve_refine_wrapper() if k.is_inertia_correct(*inertia) else False
-            n_trial += 1
+            ok, inertia = self._trial()
             self.cnt["regularized"] += 1
         if del_w != 0.0:
             self.del_w_last = del_w
         self.last_inertia = inertia
         return True
 
-    def _trial_solves(self):
-        """InertiaFree: the d0 solve and, only if it succeeded, the d solve (the reference's `&&`), then t = dx - n.
-        InertiaIgnore: the d solve."""
-        r = self.ifr
-        if r is None:
-            return self._solve_refine_wrapper()
-        ok = self._solve_refine_wrapper(r.d0, r.p0, r.w3) and self._solve_refine_wrapper()
-        r.direction_difference(self.kkt, self.d)
-        return ok
+    def _trial(self, first=False):
+        """One trial on the factor just computed; returns (accepted, the inertia read, or None when the method reads none).
 
-    def _trial_accepted(self, ok):
+        InertiaBased (solver.jl:611-670): the d solve, only when the inertia is correct.  On the first trial with `speculate`, the
+        inertia read AND the first refinement step are queued behind the factorisation and the host blocks once for both.
+        InertiaFree (:672-737): the d0 solve and, only if it succeeded, the d solve (the reference's `&&`), t = dx - n, then the
+        curvature test.  InertiaIgnore (:739-783): the d solve."""
+        k, r = self.kkt, self.ifr
+        if self.inertia_correction_method == "InertiaBased":
+            ls = k.linear_solver
+            if first and self.speculate and hasattr(ls, "inertia_enqueue"):
+                ls.inertia_enqueue()
+                self.iterator.start(self.d, self.p, self.w)
+                torch.cuda.current_stream().synchronize()
+                inertia = ls.inertia_fetch()
+                if not k.is_inertia_correct(*inertia):
+                    self.iterator.discard()
+                    return False, inertia
+            else:
+                inertia = ls.inertia()
+                if not k.is_inertia_correct(*inertia):
+                    return False, inertia
+            return self._solve_refine_wrapper(), inertia
+        if r is None:
+            return self._solve_refine_wrapper(), None
+        ok = self._solve_refine_wrapper(r.d0, r.p0, r.w3) and self._solve_refine_wrapper()
+        r.direction_difference(k, self.d)
         # the reference evaluates curv_test first (`!curv_test(...) || !solve_status`); when a solve failed its value cannot change
         # the outcome, so the test only runs after successful solves
-        if not ok:
-            return False
-        return self.ifr is None or self.ifr.curvature_ok(self.kkt, self.inertia_free_tol)
+        return ok and r.curvature_ok(k, self.inertia_free_tol), None
 
-    def _inertia_correction_without_inertia(self, mu):
-        """inertia_correction!(::InertiaFree) (src/IPM/solver.jl:672-737) and (::InertiaIgnore) (:739-783), after the first
-        factorisation: the inertia is never read, and del_c is set on every trial.  `last_del_w` lists the del_w of each trial."""
-        k = self.kkt
-        o = self.opt
-        n_trial = 0
-        del_w = del_c = del_w_prev = del_c_prev = 0.0
-        self.last_del_w = []
-        self.last_inertia = None
-        ok = self._trial_solves()
-        while not self._trial_accepted(ok):
-            if n_trial == 0:
-                del_w = o.first_hessian_perturbation if self.del_w_last == 0.0 else max(
-                    o.min_hessian_perturbation, o.perturb_dec_fact * self.del_w_last)
-            else:
-                del_w *= o.perturb_inc_fact_first if self.del_w_last == 0.0 else o.perturb_inc_fact
-                if del_w > o.max_hessian_perturbation:
-                    self.cnt["failed"] += 1
-                    return False
-            del_c = o.jacobian_regularization_value * mu ** o.jacobian_regularization_exponent
-            k.regularize_diagonal(del_w - del_w_prev, del_c - del_c_prev)
-            del_w_prev, del_c_prev = del_w, del_c
-            self.last_del_w.append(del_w)
-            self._factorize_wrapper()
-            ok = self._trial_solves()
-            n_trial += 1
-            self.cnt["regularized"] += 1
-        if del_w != 0.0:
-            self.del_w_last = del_w
-        return True
 
 class HostIteratePipeline:
     """Double-buffered host<->device staging around `IPMLinearAlgebra.step` (the role of SparseWrapperModel's pinned buffers,
@@ -581,15 +477,11 @@ class HostIteratePipeline:
 
     def push_result(self):
         """queue the D2H of the step direction `d` behind the step just issued; returns the index of the pinned host buffer"""
-        import ctypes as C
-        from .capi import lib, check, stream_ptr
         slot = self._n_out & 1
         main = torch.cuda.current_stream()
         if self._n_out >= 2:
             main.wait_event(self.ev_d_out[slot])
-        d = self.la.d.values
-        src = (C.c_void_p * 1)(d.data_ptr()); dst = (C.c_void_p * 1)(self.d_stage[slot].data_ptr()); ns = (C.c_int64 * 1)(d.numel())
-        check(lib.b2_copy_many(1, src, dst, ns, stream_ptr(getattr(self.la.kkt, "stream", None))))
+        copy_many(((self.la.d.values, self.d_stage[slot]),), self.la.kkt.stream)
         self.ev_d_ready[slot].record(main)
         self.d2h.wait_event(self.ev_d_ready[slot])
         with torch.cuda.stream(self.d2h):

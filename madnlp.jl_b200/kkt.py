@@ -27,10 +27,6 @@ def _dz(n):
     return torch.zeros(int(n), dtype=torch.float64, device=_DEV)
 
 
-def _sp(stream=None):
-    return capi.stream_ptr(stream)
-
-
 def force_lower_triangular(I, J):
     """src/matrixtools.jl:129-137 (host, one-time, on the sparsity pattern)."""
     sw = J > I
@@ -64,7 +60,7 @@ def coo_to_csc_device(I, J, m, n):
     cmap = torch.zeros(max(nnz, 1), dtype=torch.int64, device=_DEV)
     ncsc = C.c_int64(0)
     check(lib.b2_coo_to_csc_device(m, n, nnz, ptr(Id) if nnz else None, ptr(Jd) if nnz else None, ptr(colptr), ptr(rowval), ptr(cmap),
-                                   C.byref(ncsc), _sp()))
+                                   C.byref(ncsc), capi.stream_ptr()))
     return colptr.cpu().numpy(), rowval.cpu().numpy()[:ncsc.value].copy(), cmap.cpu().numpy()[:nnz].copy()
 
 
@@ -147,8 +143,38 @@ class UnreducedKKTVector:
         return o
 
 
+class SolverVectors:
+    """The solver vectors of MadNLPSolver that the device kernels read and write, as device buffers: x, xl, xu, zl, zu, f, jacl and
+    x_trial of length n_tot (+-Inf for an absent bound; zl / zu full length), y, c and c_trial of length m.  The only holder of the
+    iterate: the regular phase (IPMLinearAlgebra.solver_vectors, which the inertia-free test and the solve sites read) and, when passed
+    to them, a RobustRestorer and an AdaptiveBarrier share one, so all of them see one iterate."""
+
+    NAMES = ("x", "xl", "xu", "zl", "zu", "f", "jacl", "x_trial", "y", "c", "c_trial")
+
+    def __init__(self, kkt):
+        self.n_tot, self.m = len(kkt.pr_diag), len(kkt.du_diag)
+        dev = kkt.pr_diag.device
+        for name in self.NAMES:
+            setattr(self, name, torch.zeros(self.m if name in ("y", "c", "c_trial") else self.n_tot, dtype=torch.float64, device=dev))
+
+    def load(self, non_blocking=True, **vectors):
+        """Copy host or device vectors into the named buffers, e.g. load(x=..., y=...); a wrong length raises ValueError"""
+        for name, src in vectors.items():
+            if name not in self.NAMES:
+                raise ValueError(f"load: unknown solver vector {name!r}")
+            dst = getattr(self, name)
+            src = torch.as_tensor(src, dtype=torch.float64)
+            if src.numel() != dst.numel():
+                raise ValueError(f"load: {name} expects {dst.numel()} entries, got {src.numel()}")
+            dst.copy_(src, non_blocking=non_blocking)
+
+
 class _KKTBase:
     stream = None
+
+    def stream_ptr(self):
+        """the stream every launch on this system (and on the host-layer objects built over it) goes to, as the ABI's argument"""
+        return capi.stream_ptr(self.stream)
 
     # ---- generic pieces (src/KKT/KKTsystem.jl:210-256, src/IPM/kernels.jl) ----
     def _init_common(self, cb, n_tot, m):
@@ -165,24 +191,24 @@ class _KKTBase:
     def set_aug_diagonal_(self):
         """_set_aug_diagonal!  (src/IPM/kernels.jl:22-27)."""
         check(lib.b2_set_aug_diagonal(self._bounds.h, ptr(self.reg), ptr(self.l_lower), ptr(self.l_diag),
-                                      ptr(self.u_lower), ptr(self.u_diag), ptr(self.pr_diag), _sp(self.stream)))
+                                      ptr(self.u_lower), ptr(self.u_diag), ptr(self.pr_diag), self.stream_ptr()))
 
     def regularize_diagonal(self, primal, dual):
         """src/KKT/KKTsystem.jl:222-226."""
         check(lib.b2_regularize_diagonal(self._n_tot, self._m, float(primal), float(dual), ptr(self.reg),
-                                         ptr(self.pr_diag), ptr(self.du_diag), _sp(self.stream)))
+                                         ptr(self.pr_diag), ptr(self.du_diag), self.stream_ptr()))
 
     def reduce_rhs(self, w):
-        check(lib.b2_reduce_rhs(self._bounds.h, self._m, ptr(self.l_diag), ptr(self.u_diag), ptr(w.values), _sp(self.stream)))
+        check(lib.b2_reduce_rhs(self._bounds.h, self._m, ptr(self.l_diag), ptr(self.u_diag), ptr(w.values), self.stream_ptr()))
 
     def finish_aug_solve(self, w):
         check(lib.b2_finish_aug_solve(self._bounds.h, self._m, ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag),
-                                      ptr(self.u_diag), ptr(w.values), _sp(self.stream)))
+                                      ptr(self.u_diag), ptr(w.values), self.stream_ptr()))
 
     def _kktmul(self, w, x, alpha, beta):
         check(lib.b2_kktmul(self._bounds.h, self._m, ptr(self.reg), ptr(self.du_diag), ptr(self.l_lower), ptr(self.u_lower),
                             ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta), ptr(x.values), ptr(w.values),
-                            _sp(self.stream)))
+                            self.stream_ptr()))
 
     def factorize_kkt(self):
         return self.linear_solver.factorize()
@@ -216,7 +242,7 @@ class _KKTBase:
         n_h = self._hess_mul(wx, t)
         check(lib.b2_mul_hess_blk_tail(self._bounds.h, n_h, self._unreduced, ptr(self.pr_diag), ptr(self.l_lower), ptr(self.l_diag),
                                        ptr(self.u_lower), ptr(self.u_diag), ptr(t), ptr(wx), ptr(n), ptr(g), float(tol), ptr(result),
-                                       _sp(self.stream)))
+                                       self.stream_ptr()))
 
     def mul_hess_blk(self, wx, t):
         """mul_hess_blk!(wx, kkt, t): wx = [Symmetric(H, :L) t[0:n_h) | 0] + t .* pr_diag (the unreduced system also subtracts
@@ -316,20 +342,20 @@ class _SparseKKTBase(_KKTBase):
     def compress_jacobian(self):
         """Sparse/utils.jl:36-40."""
         if self.ns:
-            check(lib.b2_fill(self.ns, -1.0, ptr(self.jac[-self.ns:]), _sp(self.stream)))
-        check(lib.b2_transfer(self._jac_plan.h, ptr(self.jac_com.nzval), ptr(self.jac), _sp(self.stream)))
+            check(lib.b2_fill(self.ns, -1.0, ptr(self.jac[-self.ns:]), self.stream_ptr()))
+        check(lib.b2_transfer(self._jac_plan.h, ptr(self.jac_com.nzval), ptr(self.jac), self.stream_ptr()))
 
     def compress_hessian(self):
         """Sparse/utils.jl:48-50."""
-        check(lib.b2_transfer(self._hess_plan.h, ptr(self.hess_com.nzval), ptr(self.hess), _sp(self.stream)))
+        check(lib.b2_transfer(self._hess_plan.h, ptr(self.hess_com.nzval), ptr(self.hess), self.stream_ptr()))
 
     def build_kkt(self):
         """augmented.jl:146-148 / unreduced.jl:178-180: transfer!(aug_com, aug_raw, aug_csc_map)."""
-        check(lib.b2_transfer(self._aug_plan.h, ptr(self.aug_com.nzval), ptr(self.V), _sp(self.stream)))
+        check(lib.b2_transfer(self._aug_plan.h, ptr(self.aug_com.nzval), ptr(self.V), self.stream_ptr()))
 
     def mul(self, w, x, alpha=1.0, beta=0.0):
         """src/IPM/factorization.jl:231-237 (one method for both sparse types)."""
-        sp = _sp(self.stream)
+        sp = self.stream_ptr()
         check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(x.values), ptr(w.values), alpha, beta, sp))
         check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x.dual()), ptr(w.values), alpha, 1.0, sp))
         check(lib.b2_spmv_n(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x.values), ptr(w.dual()), alpha, beta, sp))
@@ -341,12 +367,12 @@ class _SparseKKTBase(_KKTBase):
         pass
 
     def _hess_mul(self, wx, t):
-        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, self.stream_ptr()))
         return self.hess_com.n
 
     def jtprod(self, y, x):
         """Sparse/utils.jl:28-30."""
-        check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2_spmv_t(self._jac_spmv.h, ptr(self.jac_com.nzval), ptr(x), ptr(y), 1.0, 0.0, self.stream_ptr()))
 
 
 class SparseKKTSystem(_SparseKKTBase):
@@ -425,12 +451,12 @@ class SparseUnreducedKKTSystem(_SparseKKTBase):
         """_set_aug_diagonal!(::AbstractUnreducedKKTSystem) (src/IPM/kernels.jl:29-34): pr_diag = reg, sqrt of the multipliers."""
         check(lib.b2_set_aug_diagonal_unreduced(self._n_tot, len(self.l_lower), len(self.u_lower), ptr(self.reg), ptr(self.l_lower),
                                                 ptr(self.u_lower), ptr(self.pr_diag), ptr(self.l_lower_aug), ptr(self.u_lower_aug),
-                                                _sp(self.stream)))
+                                                self.stream_ptr()))
 
     def solve_kkt(self, w: UnreducedKKTVector):
         """src/IPM/factorization.jl:29-39: scale the bound-dual blocks, solve the full system, scale back."""
         args = (self._n_tot, self._m, len(self.l_lower), len(self.u_lower), ptr(self.l_lower_aug), ptr(self.u_lower_aug), ptr(w.values),
-                _sp(self.stream))
+                self.stream_ptr())
         check(lib.b2_unreduced_solve_pre(*args))
         self.linear_solver.solve_linear_system(w.full())
         check(lib.b2_unreduced_solve_post(*args))
@@ -468,7 +494,8 @@ class SparseCondensedKKTSystem(_KKTBase):
         if dev_sym:
             d32 = lambda a: torch.from_numpy(np.ascontiguousarray(a if len(a) else np.zeros(1), dtype=np.int32)).to(_DEV)
             pats = [d32(hcp), d32(hrv), d32(cp), d32(rv)]
-            check(lib.b2_condensed_symbolic_device(n, m, ptr(pats[0]), ptr(pats[1]), ptr(pats[2]), ptr(pats[3]), C.byref(h), C.byref(nnz_aug), _sp()))
+            check(lib.b2_condensed_symbolic_device(n, m, ptr(pats[0]), ptr(pats[1]), ptr(pats[2]), ptr(pats[3]), C.byref(h),
+                                                   C.byref(nnz_aug), capi.stream_ptr()))
         else:
             check(lib.b2_condensed_symbolic(n, m, hcp.ctypes.data, hrv.ctypes.data if len(hrv) else None, cp.ctypes.data,
                                             rv.ctypes.data if len(rv) else None, C.byref(h), C.byref(nnz_aug)))
@@ -500,16 +527,16 @@ class SparseCondensedKKTSystem(_KKTBase):
 
     def compress_jacobian(self):
         """condensed.jl:145-148."""
-        check(lib.b2_transfer(self._jt_plan.h, ptr(self.jt_csc.nzval), ptr(self.jac), _sp(self.stream)))
+        check(lib.b2_transfer(self._jt_plan.h, ptr(self.jt_csc.nzval), ptr(self.jac), self.stream_ptr()))
 
     def compress_hessian(self):
-        check(lib.b2_transfer(self._hess_plan.h, ptr(self.hess_com.nzval), ptr(self.hess), _sp(self.stream)))
+        check(lib.b2_transfer(self._hess_plan.h, ptr(self.hess_com.nzval), ptr(self.hess), self.stream_ptr()))
 
     def build_kkt(self):
         """condensed.jl:354-366 (+ :328-345)."""
         check(lib.b2_condensed_assemble(self._cond.h, ptr(self.aug_com.nzval), ptr(self.pr_diag), ptr(self.du_diag),
                                         ptr(self.hess_com.nzval), ptr(self.jt_csc.nzval), ptr(self.diag_buffer),
-                                        _sp(self.stream)))
+                                        self.stream_ptr()))
 
     def is_inertia_correct(self, num_pos, num_zero, num_neg):
         """condensed.jl:138-140."""
@@ -530,7 +557,7 @@ class SparseCondensedKKTSystem(_KKTBase):
 
     def solve_kkt(self, w: UnreducedKKTVector):
         """src/IPM/factorization.jl:143-167: pre (two launches), solve, post (one)."""
-        sp = _sp(self.stream)
+        sp = self.stream_ptr()
         check(lib.b2_condensed_solve_pre(*self._pre_args(), ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(w.values), sp))
         self.linear_solver.solve_linear_system(w.values[: self.n])
         check(lib.b2_condensed_solve_post(*self._post_args(), ptr(w.values), sp))
@@ -539,7 +566,7 @@ class SparseCondensedKKTSystem(_KKTBase):
     def refine_step(self, x, b, w, norms):
         """One Richardson step (src/LinearSolvers/backsolve.jl:45-52) in five launches: solve_kkt!(w); x += w; w = b - K x;
         norms[0] = ||w||_inf, norms[1] = ||x||_inf (device).  Same values as solve_kkt, b2_richardson_update and mul_norm."""
-        sp = _sp(self.stream)
+        sp = self.stream_ptr()
         check(lib.b2_condensed_refine_pre(*self._pre_args(), ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(w.values),
                                           ptr(norms), sp))
         self.linear_solver.solve_linear_system(w.values[: self.n])
@@ -548,22 +575,22 @@ class SparseCondensedKKTSystem(_KKTBase):
 
     def mul(self, w, x, alpha=1.0, beta=0.0):
         """src/IPM/factorization.jl:303-324."""
-        check(lib.b2_condensed_kkt_mul(*self._mul_args(), float(alpha), float(beta), ptr(x.values), ptr(w.values), _sp(self.stream)))
+        check(lib.b2_condensed_kkt_mul(*self._mul_args(), float(alpha), float(beta), ptr(x.values), ptr(w.values), self.stream_ptr()))
         return w
 
     def mul_norm(self, w, x, alpha, beta, norm_out):
         """mul! that also accumulates ||w||_inf of the result into the (zeroed) device scalar `norm_out`"""
         check(lib.b2_condensed_kkt_mul_norm(*self._mul_args(), float(alpha), float(beta), ptr(x.values), ptr(w.values), ptr(norm_out),
-                                            _sp(self.stream)))
+                                            self.stream_ptr()))
         return w
 
     def _hess_mul(self, wx, t):
-        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2_spmv_symlower(self._hess_spmv.h, ptr(self.hess_com.nzval), ptr(t), ptr(wx), 1.0, 0.0, self.stream_ptr()))
         return self.n
 
     def jtprod(self, y, x):
         """condensed.jl:150-156."""
-        check(lib.b2_spmv_n(self._jt_spmv.h, ptr(self.jt_csc.nzval), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2_spmv_n(self._jt_spmv.h, ptr(self.jt_csc.nzval), ptr(x), ptr(y), 1.0, 0.0, self.stream_ptr()))
         y[self.n:] = -x
 
 
@@ -606,17 +633,17 @@ class _DenseKKTBase(_KKTBase):
     def _gemv(self, trans, x, y, alpha, beta):
         """y = alpha*op(jac)*x + beta*y with jac the m x n column-major device matrix (own kernels, no cuBLAS)"""
         fn = lib.b2d_gemv_t if trans else lib.b2d_gemv_n
-        check(fn(self.m, self.n, self.m, ptr(self.jac), ptr(x), ptr(y), float(alpha), float(beta), _sp(self.stream)))
+        check(fn(self.m, self.n, self.m, ptr(self.jac), ptr(x), ptr(y), float(alpha), float(beta), self.stream_ptr()))
 
     def mul(self, w, x, alpha=1.0, beta=0.0):
         """src/IPM/factorization.jl:303-324 (AbstractDenseKKTSystem): symv + 2 gemv + one fused tail kernel (b2d_kkt_mul)."""
         check(lib.b2d_kkt_mul(self._dk.h, self._bounds.h, ptr(self.hess), ptr(self.jac), ptr(self.reg), ptr(self.du_diag),
                               ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta),
-                              ptr(x.values), ptr(w.values), _sp(self.stream)))
+                              ptr(x.values), ptr(w.values), self.stream_ptr()))
         return w
 
     def _hess_mul(self, wx, t):
-        check(lib.b2d_symv_lower(self.n, self.n, ptr(self.hess), ptr(t), ptr(wx), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2d_symv_lower(self.n, self.n, ptr(self.hess), ptr(t), ptr(wx), 1.0, 0.0, self.stream_ptr()))
         return self.n
 
     def jtprod(self, y, x):
@@ -681,18 +708,18 @@ class DenseCondensedKKTSystem(_DenseKKTBase):
         if self._ozaki is not None:
             check(lib.b2d_condensed_assemble_ozaki(self._ozaki.h, self.n, self.m, self.ns, self.n_eq, ptr(self._ind_ineq_d), ptr(self._ind_eq_d),
                                                    ptr(self.hess), ptr(self.jac), ptr(self.pr_diag), ptr(self.du_diag),
-                                                   ptr(self.diag_buffer), ptr(self.aug_com), _sp(self.stream)))
+                                                   ptr(self.diag_buffer), ptr(self.aug_com), self.stream_ptr()))
             return
         check(lib.b2d_condensed_assemble(self.n, self.m, self.ns, self.n_eq, ptr(self._ind_ineq_d), ptr(self._ind_eq_d),
                                          ptr(self.hess), ptr(self.jac), ptr(self.pr_diag), ptr(self.du_diag),
-                                         ptr(self.diag_buffer), ptr(self.aug_com), _sp(self.stream)))
+                                         ptr(self.diag_buffer), ptr(self.aug_com), self.stream_ptr()))
 
     def tensor_core_status(self):
         """True if the tensor-core (wgmma) assembly is active and none of its (bounded) pipeline waits ever timed out"""
         if self._ozaki is None:
             return None
         t = C.c_int32(0)
-        check(lib.b2d_ozaki_plan_status(self._ozaki.h, C.byref(t), _sp(self.stream)))
+        check(lib.b2d_ozaki_plan_status(self._ozaki.h, C.byref(t), self.stream_ptr()))
         return t.value == 0
 
     def is_inertia_correct(self, num_pos, num_zero, num_neg):
@@ -701,7 +728,7 @@ class DenseCondensedKKTSystem(_DenseKKTBase):
 
     def solve_kkt(self, w: UnreducedKKTVector):
         """src/IPM/factorization.jl:190-229: own kernels around the dense solve (b2d_kkt_solve_pre / _post)."""
-        sp = _sp(self.stream)
+        sp = self.stream_ptr()
         check(lib.b2d_kkt_solve_pre(self._dk.h, self._bounds.h, ptr(self.jac), ptr(self.pr_diag), ptr(self.diag_buffer),
                                     ptr(self.l_diag), ptr(self.u_diag), ptr(self.buffer), ptr(self.pd_buffer), ptr(w.values), sp))
         self.linear_solver.solve_linear_system(self.pd_buffer)
@@ -749,12 +776,12 @@ class DenseKKTSystem(_DenseKKTBase):
 
     def compress_hessian(self):
         """augmented.jl:158-161: diag!(diag_hess, hess)."""
-        check(lib.b2d_copy_diag(self.n, self.n, ptr(self.hess), ptr(self.diag_hess), _sp(self.stream)))
+        check(lib.b2d_copy_diag(self.n, self.n, ptr(self.hess), ptr(self.diag_hess), self.stream_ptr()))
 
     def build_kkt(self):
         """augmented.jl:116-156 as one kernel (k_dense_aug) that writes the whole lower triangle, zeros included."""
         check(lib.b2d_aug_assemble(self.n, self.m, self.ns, ptr(self._ind_ineq_d), ptr(self.hess), ptr(self.jac),
-                                   ptr(self.pr_diag), ptr(self.du_diag), ptr(self.diag_hess), ptr(self.aug_com), _sp(self.stream)))
+                                   ptr(self.pr_diag), ptr(self.du_diag), ptr(self.diag_hess), ptr(self.aug_com), self.stream_ptr()))
 
     def solve_kkt(self, w: UnreducedKKTVector):
         """src/IPM/factorization.jl:41-46 (AbstractReducedKKTSystem)."""
@@ -765,7 +792,7 @@ class DenseKKTSystem(_DenseKKTBase):
 
     def mul_aug(self, y, x):
         """augmented.jl:98-100: y = sym(aug_com) x from the lower triangle."""
-        check(lib.b2d_symv_lower(self.N, self.N, ptr(self.aug_com), ptr(x), ptr(y), 1.0, 0.0, _sp(self.stream)))
+        check(lib.b2d_symv_lower(self.N, self.N, ptr(self.aug_com), ptr(x), ptr(y), 1.0, 0.0, self.stream_ptr()))
         return y
 
 

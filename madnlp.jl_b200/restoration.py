@@ -21,7 +21,7 @@ IPMLinearAlgebra.restoration_step replays the linear algebra of one restoration 
 
 SoftRestorer is restore! (src/IPM/solver.jl:300-411), the soft restoration the regular phase tries before robust!: the backup and
 rollback of the iterate, get_F and the step, over the SolverVectors of an IPMLinearAlgebra, whose restore_direction computes the
-next direction.  SolverVectors holds the solver vectors themselves, shared by the regular phase and, when passed in, a RobustRestorer.
+next direction.  Both work over the solver vectors of kkt.SolverVectors.
 """
 from __future__ import annotations
 
@@ -29,36 +29,12 @@ import math
 
 import torch
 
-from .capi import check, lib, ptr, stream_ptr
+from .capi import check, copy_many, lib, ptr
+from .kkt import SolverVectors
 
 # slots of RobustRestorer.results
 (R_THETA, R_INF_PR, R_OBJ_VAL_R, R_THETA_R, R_INF_PR_R, R_INF_DU_R, R_INF_COMPL_R, R_ALPHA_MAX_R, R_ALPHA_Z_R, R_VARPHI_R,
  R_VARPHI_D_R, R_LEN) = range(12)
-
-
-class SolverVectors:
-    """The solver vectors of MadNLPSolver that the device kernels read and write, as device buffers: x, xl, xu, zl, zu, f, jacl and
-    x_trial of length n_tot (+-Inf for an absent bound; zl / zu full length), y, c and c_trial of length m.  One holder serves the
-    regular phase (IPMLinearAlgebra.solver_vectors) and, when passed to it, a RobustRestorer, so both phases see one iterate."""
-
-    NAMES = ("x", "xl", "xu", "zl", "zu", "f", "jacl", "x_trial", "y", "c", "c_trial")
-
-    def __init__(self, kkt):
-        self.n_tot, self.m = len(kkt.pr_diag), len(kkt.du_diag)
-        dev = kkt.pr_diag.device
-        for name in self.NAMES:
-            setattr(self, name, torch.zeros(self.m if name in ("y", "c", "c_trial") else self.n_tot, dtype=torch.float64, device=dev))
-
-    def load(self, non_blocking=True, **vectors):
-        """Copy host or device vectors into the named buffers, e.g. load(x=..., y=...); a wrong length raises ValueError"""
-        for name, src in vectors.items():
-            if name not in self.NAMES:
-                raise ValueError(f"load: unknown solver vector {name!r}")
-            dst = getattr(self, name)
-            src = torch.as_tensor(src, dtype=torch.float64)
-            if src.numel() != dst.numel():
-                raise ValueError(f"load: {name} expects {dst.numel()} entries, got {src.numel()}")
-            dst.copy_(src, non_blocking=non_blocking)
 
 
 class RobustRestorer:
@@ -86,9 +62,6 @@ class RobustRestorer:
         self.obj_val_R_trial = 0.0
         self.filter = []
 
-    def _sp(self):
-        return stream_ptr(getattr(self.kkt, "stream", None))
-
     def _slot(self, k):
         return self.results[k:k + 1]
 
@@ -102,7 +75,7 @@ class RobustRestorer:
         host needs mu_R = max(mu, ||c||_inf) as a kernel argument); then one launch writes x_ref, D_R, f_R, nn, pp, zp, zn, y and the
         clipped zl_r, zu_r, and one reduction queues obj_val_R (read with `fetch_obj_val_R`).  filter = [(theta_max, -Inf)].
         robust! then recomputes jacl = J'y (jtprod!, solver.jl:420) before its first step: zero here, since y = 0."""
-        sp = self._sp()
+        sp = self.kkt.stream_ptr()
         check(lib.b2_get_theta(self._b, self.m, ptr(self.c), ptr(self._slot(R_THETA)), sp))
         check(lib.b2_norm_inf(self.m, ptr(self.c), ptr(self._slot(R_INF_PR)), sp))
         self._norms_h.copy_(self.results[R_THETA:R_INF_PR + 1], non_blocking=True)
@@ -132,29 +105,30 @@ class RobustRestorer:
         check(lib.b2_set_aug_rr(self._b, self.m, float(primal_regularization), float(dual_regularization), self.zeta, ptr(self.D_R),
                                 ptr(self.pp), ptr(self.nn), ptr(self.zp), ptr(self.zn), ptr(self.x), ptr(self.xl), ptr(self.xu),
                                 ptr(self.zl), ptr(self.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower), ptr(k.u_lower), ptr(k.l_diag),
-                                ptr(k.u_diag), self._sp()))
+                                ptr(k.u_diag), self.kkt.stream_ptr()))
         k.set_aug_diagonal_()
 
     def set_aug_rhs_RR(self, p, rho=1000.0):
         """set_aug_rhs_RR! (kernels.jl:133-158) into the UnreducedKKTVector p"""
         check(lib.b2_set_aug_rhs_rr(self._b, self.m, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu), ptr(self.jacl),
                                     ptr(self.f_R), ptr(self.c), ptr(self.y), ptr(self.pp), ptr(self.nn), ptr(self.zp), ptr(self.zn),
-                                    self.mu_R, float(rho), ptr(p.values), self._sp()))
+                                    self.mu_R, float(rho), ptr(p.values), self.kkt.stream_ptr()))
 
     def finish_aug_solve_RR(self, d, rho=1000.0):
         """finish_aug_solve_RR!(dpp, dnn, dzp, dzn, y, dual(d), pp, nn, zp, zn, mu_R, rho) (kernels.jl:251-257)"""
         check(lib.b2_finish_aug_solve_rr(self.m, ptr(self.y), ptr(d.dual()), ptr(self.pp), ptr(self.nn), ptr(self.zp), ptr(self.zn),
-                                         self.mu_R, float(rho), ptr(self.dpp), ptr(self.dnn), ptr(self.dzp), ptr(self.dzn), self._sp()))
+                                         self.mu_R, float(rho), ptr(self.dpp), ptr(self.dnn), ptr(self.dzp), ptr(self.dzn),
+                                         self.kkt.stream_ptr()))
 
     def set_f_RR(self):
         """set_f_RR! (kernels.jl:106-110): f_R = zeta D_R^2 (x - x_ref)"""
-        check(lib.b2_set_f_rr(self.n_tot, self.zeta, ptr(self.D_R), ptr(self.x), ptr(self.x_ref), ptr(self.f_R), self._sp()))
+        check(lib.b2_set_f_rr(self.n_tot, self.zeta, ptr(self.D_R), ptr(self.x), ptr(self.x_ref), ptr(self.f_R), self.kkt.stream_ptr()))
 
     def reset_bound_dual(self, kappa_sigma=1e10, mu=None):
         """the four reset_bound_dual! calls of robust! (solver.jl:491-504) with mu_R: zl_r / zu_r (one launch), then zp with pp and
         zn with nn"""
         mu = self.mu_R if mu is None else float(mu)
-        sp = self._sp()
+        sp = self.kkt.stream_ptr()
         check(lib.b2_reset_bound_dual_lu(self._b, ptr(self.zl), ptr(self.zu), ptr(self.x), ptr(self.xl), ptr(self.xu), mu,
                                          float(kappa_sigma), sp))
         check(lib.b2_reset_bound_dual(self.m, ptr(self.zp), ptr(self.pp), mu, float(kappa_sigma), sp))
@@ -162,37 +136,37 @@ class RobustRestorer:
 
     def adjust_boundary(self, mu):
         """adjust_boundary!(x_lr, xl_r, x_ur, xu_r, mu) (kernels.jl:656-673), with the solver's mu"""
-        check(lib.b2_adjust_boundary(self._b, ptr(self.x), ptr(self.xl), ptr(self.xu), float(mu), self._sp()))
+        check(lib.b2_adjust_boundary(self._b, ptr(self.x), ptr(self.xl), ptr(self.xu), float(mu), self.kkt.stream_ptr()))
 
     # ---------------------------------------------------------------------------------------------------------- reductions
     def get_theta(self, c=None):
         """get_theta (kernels.jl:409): ||c||_1"""
-        check(lib.b2_get_theta(self._b, self.m, ptr(self.c if c is None else c), ptr(self._slot(R_THETA)), self._sp()))
+        check(lib.b2_get_theta(self._b, self.m, ptr(self.c if c is None else c), ptr(self._slot(R_THETA)), self.kkt.stream_ptr()))
         return self._slot(R_THETA)
 
     def get_obj_val_R(self, rho=1000.0, x=None, pp=None, nn=None):
         """get_obj_val_R(pp, nn, D_R, x, x_ref, rho, zeta) (:390-407)"""
         check(lib.b2_get_obj_val_r(self._b, self.m, ptr(self.pp if pp is None else pp), ptr(self.nn if nn is None else nn), ptr(self.D_R),
                                    ptr(self.x if x is None else x), ptr(self.x_ref), float(rho), self.zeta, ptr(self._slot(R_OBJ_VAL_R)),
-                                   self._sp()))
+                                   self.kkt.stream_ptr()))
         return self._slot(R_OBJ_VAL_R)
 
     def get_theta_R(self, c=None, pp=None, nn=None):
         """get_theta_R(c, pp, nn) (:411-421): sum |c - pp + nn|"""
         check(lib.b2_get_theta_r(self._b, self.m, ptr(self.c if c is None else c), ptr(self.pp if pp is None else pp),
-                                 ptr(self.nn if nn is None else nn), ptr(self._slot(R_THETA_R)), self._sp()))
+                                 ptr(self.nn if nn is None else nn), ptr(self._slot(R_THETA_R)), self.kkt.stream_ptr()))
         return self._slot(R_THETA_R)
 
     def get_inf_pr_R(self, c=None, pp=None, nn=None):
         """get_inf_pr_R(c, pp, nn) (:423-433): max |c - pp + nn|"""
         check(lib.b2_get_inf_pr_r(self._b, self.m, ptr(self.c if c is None else c), ptr(self.pp if pp is None else pp),
-                                  ptr(self.nn if nn is None else nn), ptr(self._slot(R_INF_PR_R)), self._sp()))
+                                  ptr(self.nn if nn is None else nn), ptr(self._slot(R_INF_PR_R)), self.kkt.stream_ptr()))
         return self._slot(R_INF_PR_R)
 
     def get_inf_du_R(self, rho, sd):
         """get_inf_du_R(f_R, y, zl, zu, jacl, zp, zn, rho, sd) (:435-454)"""
         check(lib.b2_get_inf_du_r(self._b, self.m, ptr(self.f_R), ptr(self.y), ptr(self.zl), ptr(self.zu), ptr(self.jacl), ptr(self.zp),
-                                  ptr(self.zn), float(rho), float(sd), ptr(self._slot(R_INF_DU_R)), self._sp()))
+                                  ptr(self.zn), float(rho), float(sd), ptr(self._slot(R_INF_DU_R)), self.kkt.stream_ptr()))
         return self._slot(R_INF_DU_R)
 
     def get_inf_compl_R(self, mu, sc):
@@ -200,35 +174,35 @@ class RobustRestorer:
         _update_monotone_RR! mu_R"""
         check(lib.b2_get_inf_compl_r(self._b, self.m, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu), ptr(self.pp),
                                      ptr(self.zp), ptr(self.nn), ptr(self.zn), float(mu), float(sc), ptr(self._slot(R_INF_COMPL_R)),
-                                     self._sp()))
+                                     self.kkt.stream_ptr()))
         return self._slot(R_INF_COMPL_R)
 
     def get_alpha_max_R(self, dx, tau_R=None):
         """get_alpha_max_R(x, xl, xu, dx, pp, dpp, nn, dnn, tau_R) (:486-515); dx: primal(d), n_tot"""
         tau = self.tau_R if tau_R is None else float(tau_R)
         check(lib.b2_get_alpha_max_r(self._b, self.m, ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(dx), ptr(self.pp), ptr(self.dpp),
-                                     ptr(self.nn), ptr(self.dnn), tau, ptr(self._slot(R_ALPHA_MAX_R)), self._sp()))
+                                     ptr(self.nn), ptr(self.dnn), tau, ptr(self._slot(R_ALPHA_MAX_R)), self.kkt.stream_ptr()))
         return self._slot(R_ALPHA_MAX_R)
 
     def get_alpha_z_R(self, dzl, dzu, tau_R=None):
         """get_alpha_z_R(zl_r, zu_r, dzl, dzu, zp, dzp, zn, dzn, tau_R) (:517-542); dzl / dzu: dual_lb(d) / dual_ub(d)"""
         tau = self.tau_R if tau_R is None else float(tau_R)
         check(lib.b2_get_alpha_z_r(self._b, self.m, ptr(self.zl), ptr(self.zu), ptr(dzl), ptr(dzu), ptr(self.zp), ptr(self.dzp),
-                                   ptr(self.zn), ptr(self.dzn), tau, ptr(self._slot(R_ALPHA_Z_R)), self._sp()))
+                                   ptr(self.zn), ptr(self.dzn), tau, ptr(self._slot(R_ALPHA_Z_R)), self.kkt.stream_ptr()))
         return self._slot(R_ALPHA_Z_R)
 
     def get_varphi_R(self, obj_val, x=None, pp=None, nn=None):
         """get_varphi_R(obj_val, x_lr, xl_r, xu_r, x_ur, pp, nn, mu_R) (:544-570); the line search passes the trial point"""
         check(lib.b2_get_varphi_r(self._b, self.m, float(obj_val), ptr(self.x if x is None else x), ptr(self.xl), ptr(self.xu),
                                   ptr(self.pp if pp is None else pp), ptr(self.nn if nn is None else nn), self.mu_R,
-                                  ptr(self._slot(R_VARPHI_R)), self._sp()))
+                                  ptr(self._slot(R_VARPHI_R)), self.kkt.stream_ptr()))
         return self._slot(R_VARPHI_R)
 
     def get_varphi_d_R(self, dx, rho=1000.0):
         """get_varphi_d_R(f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho) (:612-636)"""
         check(lib.b2_get_varphi_d_r(self._b, self.m, ptr(self.f_R), ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(dx), ptr(self.pp),
                                     ptr(self.nn), ptr(self.dpp), ptr(self.dnn), self.mu_R, float(rho), ptr(self._slot(R_VARPHI_D_R)),
-                                    self._sp()))
+                                    self.kkt.stream_ptr()))
         return self._slot(R_VARPHI_D_R)
 
 
@@ -260,24 +234,13 @@ class SoftRestorer:
         self.results = torch.zeros(S_LEN, dtype=torch.float64, device=la.d.values.device)
         self._h = torch.zeros(S_LEN, dtype=torch.float64).pin_memory()
 
-    def _sp(self):
-        return stream_ptr(getattr(self.kkt, "stream", None))
-
     def _slot(self, k):
         return self.results[k:k + 1]
-
-    def _copy_many(self, pairs):
-        import ctypes as C
-        cnt = len(pairs)
-        src = (C.c_void_p * cnt)(*[s.data_ptr() for s, _ in pairs])
-        dst = (C.c_void_p * cnt)(*[d.data_ptr() for _, d in pairs])
-        ns = (C.c_int64 * cnt)(*[d.numel() for _, d in pairs])
-        check(lib.b2_copy_many(cnt, src, dst, ns, self._sp()))
 
     def begin(self, mu):
         """copyto!(primal(_w1), x); copyto!(dual(_w1), y); copyto!(dual(_w2), c) in one launch, then F = get_F(mu) (:301-323)"""
         v, w1, w2 = self.vectors, self.la._w1, self.la._w2
-        self._copy_many(((v.x, w1.primal()), (v.y, w1.dual()), (v.c, w2.dual())))
+        copy_many(((v.x, w1.primal()), (v.y, w1.dual()), (v.c, w2.dual())), self.kkt.stream)
         self.get_F(mu, S_F)
 
     def get_F(self, mu, slot=S_F_TRIAL):
@@ -285,13 +248,13 @@ class SoftRestorer:
         default); returns the one-element device tensor"""
         v = self.vectors
         check(lib.b2_get_pd_error(self._b, v.m, ptr(v.c), ptr(v.f), ptr(v.zl), ptr(v.zu), ptr(v.jacl), ptr(v.x), ptr(v.xl), ptr(v.xu),
-                                  float(mu), ptr(self._slot(slot)), self._sp()))
+                                  float(mu), ptr(self._slot(slot)), self.kkt.stream_ptr()))
         return self._slot(slot)
 
     def update(self, tau):
         """alpha_max = get_alpha_max(x, xl, xu, primal(d), tau); alpha = min(alpha_max, get_alpha_z(zl_r, zu_r, dual_lb(d), dual_ub(d),
         tau)); x += alpha primal(d); y += alpha dual(d); zl_r += alpha dual_lb(d); zu_r += alpha dual_ub(d).  Returns alpha's slot."""
-        v, d, sp = self.vectors, self.la.d, self._sp()
+        v, d, sp = self.vectors, self.la.d, self.kkt.stream_ptr()
         check(lib.b2_get_alpha_max(self._b, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(d.primal()), float(tau), ptr(self._slot(S_ALPHA_MAX)), sp))
         check(lib.b2_get_alpha_z(self._b, ptr(v.zl), ptr(v.zu), ptr(d.dual_lb()), ptr(d.dual_ub()), float(tau), ptr(self._slot(S_ALPHA_Z)),
                                  sp))
@@ -308,9 +271,9 @@ class SoftRestorer:
 
     def accept(self):
         """F = F_trial"""
-        check(lib.b2_copy(1, ptr(self._slot(S_F_TRIAL)), ptr(self._slot(S_F)), self._sp()))
+        check(lib.b2_copy(1, ptr(self._slot(S_F_TRIAL)), ptr(self._slot(S_F)), self.kkt.stream_ptr()))
 
     def rollback(self):
         """copyto!(primal(x), primal(_w1)); copyto!(y, dual(_w1)); copyto!(c, dual(_w2)) in one launch (:359-364)"""
         v, w1, w2 = self.vectors, self.la._w1, self.la._w2
-        self._copy_many(((w1.primal(), v.x), (w1.dual(), v.y), (w2.dual(), v.c)))
+        copy_many(((w1.primal(), v.x), (w1.dual(), v.y), (w2.dual(), v.c)), self.kkt.stream)

@@ -9,8 +9,8 @@ from __future__ import annotations
 
 import torch
 
-from . import capi
 from .capi import lib, check, ptr
+from .capture import CapturedSequence
 
 
 class RichardsonIterator:
@@ -20,7 +20,7 @@ class RichardsonIterator:
     def __init__(self, kkt, tol=1e-8, richardson_max_iter=10, use_cuda_graph=True):
         self.kkt = kkt
         self.use_cuda_graph = use_cuda_graph
-        self._graphs = {}
+        self._graphs = {}           # one CapturedSequence per (x, b, w): the d / p / w and d0 / p0 / w3 solves alternate
         self.richardson_max_iter = richardson_max_iter
         self.richardson_tol = tol ** (5 / 4)
         self.richardson_acceptable_tol = tol ** (5 / 8)
@@ -36,7 +36,7 @@ class RichardsonIterator:
         if hasattr(kkt, "refine_step"):          # the same step fused into fewer launches (SparseCondensedKKTSystem)
             kkt.refine_step(x, b, w, self._norms)
             return
-        stream = capi.stream_ptr(getattr(kkt, "stream", None))
+        stream = kkt.stream_ptr()
         n = b.values.numel()
         kkt.solve_kkt(w)
         check(lib.b2_richardson_update(n, ptr(b.values), ptr(w.values), ptr(x.values), ptr(self._norms), stream))   # x += w; w = b; ||x||
@@ -48,25 +48,10 @@ class RichardsonIterator:
 
     def _launch_iteration(self, x, b, w):
         """queue one refinement step and the D2H copy of its norms; no host synchronisation"""
-        if not self.use_cuda_graph:
-            self._body(x, b, w)
-        else:
-            key = (x.values.data_ptr(), b.values.data_ptr(), w.values.data_ptr())
-            g = self._graphs.get(key)
-            if g is None:
-                # first use with these vectors: run eagerly (this also instantiates the solver's internal graphs) ...
-                self._body(x, b, w)
-                self._graphs[key] = False
-            elif g is False:
-                # ... second use: capture; the captured launch sequence is then replayed
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                with torch.cuda.graph(g):
-                    self._body(x, b, w)
-                self._graphs[key] = g
-                g.replay()
-            else:
-                g.replay()
+        key = (x.values.data_ptr(), b.values.data_ptr(), w.values.data_ptr())
+        if key not in self._graphs:
+            self._graphs[key] = CapturedSequence(self.use_cuda_graph)
+        self._graphs[key].run(lambda: self._body(x, b, w))
         self._norms_h.copy_(self._norms, non_blocking=True)
 
     def _fetch_norms(self):
@@ -77,7 +62,7 @@ class RichardsonIterator:
         """Queue ||b||, x = 0, w = b and the FIRST refinement step without blocking.  A caller may issue this right behind
         a factorisation, before it knows the inertia: the host then blocks once for both (IPMLinearAlgebra.step); if the
         factorisation is rejected the queued step is simply discarded (solve_refine! always restarts from x = 0)."""
-        stream = capi.stream_ptr(getattr(self.kkt, "stream", None))
+        stream = self.kkt.stream_ptr()
         n = b.values.numel()
         check(lib.b2_richardson_begin(n, ptr(b.values), ptr(w.values), ptr(x.values), ptr(self._norms[2:3]), stream))   # ||b||; x = 0; w = b
         self._launch_iteration(x, b, w)

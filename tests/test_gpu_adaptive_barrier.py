@@ -302,7 +302,7 @@ def test_graph_replay_bit_identical_to_eager():
             mu = ab.get_adaptive_mu(QualityFunctionUpdate(), 0.99 - 0.01 * k)
             out.append(np.concatenate([[mu], ab.result.cpu().numpy(), ab.step_aff.values.cpu().numpy(), ab.step_cen.values.cpu().numpy()]))
         if graph:
-            assert ab._graph not in (None, False)
+            assert ab._graph.graph not in (None, False)
         runs.append(out)
     for a, b in zip(*runs):
         assert np.array_equal(_bits(a), _bits(b))

@@ -107,7 +107,8 @@ def measure(kg, cb, steps, nxt, reps, flush):
     sp = torch.cuda.current_stream().cuda_stream
 
     def search():
-        check(lib.b2_qf_search(ab._b, m, ptr(ab.x), ptr(ab.xl), ptr(ab.xu), ptr(ab.zl), ptr(ab.zu), ptr(ab.step_aff.values),
+        v = ab.vectors
+        check(lib.b2_qf_search(ab._b, m, ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(ab.step_aff.values),
                                ptr(ab.step_cen.values), ptr(ab.scal), qf.sigma_min, qf.sigma_max, qf.mu_min, qf.mu_max, qf.sigma_tol,
                                qf.max_gs_iter, ptr(ab.result), sp))
     search_ms = timed(search, reps, flush)

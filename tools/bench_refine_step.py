@@ -69,7 +69,7 @@ def main():
         la.load_iterate(devit[i % len(devit)]); assert la.step(mu=its[i % len(its)].mu)
     torch.cuda.synchronize()
     itx = la.iterator
-    g = itx._graphs.get((la.d.values.data_ptr(), la.p.values.data_ptr(), la.w.values.data_ptr()))
+    g = getattr(itx._graphs.get((la.d.values.data_ptr(), la.p.values.data_ptr(), la.w.values.data_ptr())), "graph", None)
     assert isinstance(g, torch.cuda.CUDAGraph), "the refinement-step graph was not captured"
 
     ls = kkt.linear_solver

@@ -35,7 +35,7 @@ for i in range(24):
     h.append(time.perf_counter()); e[0].record()
     la.load_iterate(it)
     h.append(time.perf_counter()); e[1].record()
-    la._prologue_graph.replay()
+    la._prologue_graph.graph.replay()
     h.append(time.perf_counter()); e[2].record()
     kkt.linear_solver.inertia_enqueue(); itx.start(la.d, la.p, la.w)
     h.append(time.perf_counter()); e[3].record()
