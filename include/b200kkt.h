@@ -90,11 +90,28 @@ typedef struct b2_options {
                                 The sparse solver (b2_create*) rejects any value but STATIC.  BUNCH_KAUFMAN needs
                                 N <= 128 * (number of SMs of the device), 16,896 on an H100 SXM: its solve is one launch
                                 with one resident CTA per 128 rows; b2d_create rejects a larger N (B2_ERR_INVALID).      */
-    int32_t reserved[2];
+    int32_t sparse_pivoting; /* sparse solver (b2_*) only, B2_SPARSE_PIVOT_*: STATIC (default) pivots 1x1 with |d| < pivot_eps ->
+                                +-pivot_eps.  PAIRS: the analysis places every constraint dual it can match with a distinct primal
+                                neighbour immediately after that neighbour, in one supernode, and the factorisation takes the pair as
+                                one 2x2 pivot block when |a_kk| < alpha |a_k+1,k| (alpha = (1+sqrt(17))/8) and the block is indefinite,
+                                else as two 1x1 pivots (DESIGN.md section 3).  No rows move at run time.  b2_create accepts PAIRS only
+                                with kkt_n_primal > 0, n_parts == 1, dep_schedule bit 0 set and every front of order <= 64 after the
+                                analysis (B2_ERR_INVALID otherwise, before any device work; b2_create_symbolic_only skips the front-order
+                                condition so that tooling can inspect the tree).  The dense solver (b2d_create) rejects any value but
+                                STATIC.                                                                                    */
+    int32_t reserved[1];
 } b2_options;
 
 #define B2_DENSE_PIVOT_STATIC        0
 #define B2_DENSE_PIVOT_BUNCH_KAUFMAN 1
+#define B2_SPARSE_PIVOT_STATIC       0
+#define B2_SPARSE_PIVOT_PAIRS        1
+
+/* pivot kinds reported by b2_get_pivot_blocks */
+#define B2_PIVOT_1X1            0
+#define B2_PIVOT_1X1_PERTURBED  1
+#define B2_PIVOT_2X2_FIRST      2
+#define B2_PIVOT_2X2_SECOND     3
 
 int b2_options_default(b2_options* opt);
 
@@ -176,6 +193,13 @@ int b2_symbolic_exchange(b2_solver* s, int64_t* cbv_off, int64_t* exch_cb, int64
 /* test/debug: copy the numeric factor (lval_size doubles, panel layout of b2_symbolic_export) and D (n doubles, permuted
  * order) to the host; synchronises the device. */
 int b2_debug_get_factor(b2_solver* s, double* lval_h, double* dvec_h);
+/* analysis export of opt.sparse_pivoting = B2_SPARSE_PIVOT_PAIRS: pair_start_h[j] = 1 when permuted column j starts a candidate pair
+ * (j, j+1) -- a primal followed by its matched constraint dual, both in one supernode -- else 0; n entries.  All zero for STATIC. */
+int b2_symbolic_pairs(b2_solver* s, uint8_t* pair_start_h);
+/* test/debug: the pivots of the last factorisation of a PAIRS handle in elimination (permuted) order, n entries each on the host:
+ * kind_h B2_PIVOT_*; d_h D's diagonal (a perturbed pivot as +-pivot_eps); d_off_h D's subdiagonal (b at the first index of a 2x2
+ * block, else 0).  Synchronises the device; B2_ERR_INVALID on a STATIC handle. */
+int b2_get_pivot_blocks(b2_solver* s, int8_t* kind_h, double* d_h, double* d_off_h);
 /* test/debug: re-factor one warp-class front `reps` times with clock64() stamps at its 8 phase boundaries */
 int b2_debug_profile_front(b2_solver* s, int32_t sn, int32_t reps, int64_t* stamps_h);
 /* Debug: per-front device timeline of the team-class factor kernels.  With B2_SPARSE_TRACE=1 in the environment at b2_create every

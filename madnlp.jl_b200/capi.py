@@ -17,6 +17,8 @@ B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
 B2_DENSE_PIVOT_STATIC, B2_DENSE_PIVOT_BUNCH_KAUFMAN = 0, 1
+B2_SPARSE_PIVOT_STATIC, B2_SPARSE_PIVOT_PAIRS = 0, 1
+B2_PIVOT_1X1, B2_PIVOT_1X1_PERTURBED, B2_PIVOT_2X2_FIRST, B2_PIVOT_2X2_SECOND = 0, 1, 2, 3
 # layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
 CURV_WXT, CURV_WXN, CURV_GN, CURV_TT, CURV_LHS, CURV_PASS, CURV_RESULT_LEN = 0, 1, 2, 3, 4, 5, 6
 # layout of b2_dual_init_select's result (B2_DUAL_INIT_* in include/b200kkt.h)
@@ -53,11 +55,16 @@ class InertiaException(RuntimeError):
     pass
 
 
+class _Pivoting(C.Structure):
+    _fields_ = [("dense_pivoting", C.c_int32), ("sparse_pivoting", C.c_int32)]
+
+
 class _OptionsTail(C.Union):
-    """the three int32 after kkt_n_dual: `dense_pivoting` took the first (include/b200kkt.h).  `reserved` keeps the view of all
-    three at the offset it always had, so that code which reads `Options.reserved` still finds it there; the header's
-    `reserved[2]` (and the Julia shim's) is `reserved[1:]` here, and `reserved[0]` is `dense_pivoting`."""
-    _fields_ = [("dense_pivoting", C.c_int32), ("reserved", C.c_int32 * 3)]
+    """the three int32 after kkt_n_dual: `dense_pivoting` and `sparse_pivoting` took the first two (include/b200kkt.h).
+    `reserved` keeps the view of all three at the offset it always had, so that code which reads `Options.reserved` still finds
+    it there; the header's `reserved[1]` (and the Julia shim's) is `reserved[2:]` here."""
+    _anonymous_ = ("_pivoting",)
+    _fields_ = [("_pivoting", _Pivoting), ("reserved", C.c_int32 * 3)]
 
 
 class Options(C.Structure):
@@ -130,6 +137,8 @@ PROTOTYPES = {
     "b2_symbolic_owner": (C.c_int, [_p, _p]),
     "b2_symbolic_exchange": (C.c_int, [_p, _p, C.POINTER(_i64), C.POINTER(_i64)]),
     "b2_debug_get_factor": (C.c_int, [_p, _p, _p]),
+    "b2_symbolic_pairs": (C.c_int, [_p, _p]),
+    "b2_get_pivot_blocks": (C.c_int, [_p, _p, _p, _p]),
     "b2_debug_profile_front": (C.c_int, [_p, _i32, _i32, _p]),
     "b2d_debug_trace": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
     "b2_debug_trace": (C.c_int, [_p, _p, _p, _p, _p, _i64, C.POINTER(_i64)]),

@@ -302,6 +302,7 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     //          neighbour already precedes it, otherwise it is moved to just after its earliest unused neighbour (or, if every
     //          neighbour is taken, after its last neighbour).  Quasi-definite / condensed matrices do not need this (kkt_n_primal = 0).
     //          Only the constraint duals [kkt_n_primal, nc) take part; bound rows are placed at 1c.
+    std::vector<std::pair<int32_t, int32_t>> pairs;            // PAIRS: (primal, its matched dual), original numbering
     if (opt.kkt_n_primal > 0 && opt.kkt_n_primal < nc && opt.ordering != 3) {
         const int32_t np_ = opt.kkt_n_primal;
         const int32_t nd_ = nc - np_;
@@ -323,12 +324,31 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
         std::iota(duals.begin(), duals.end(), np_);
         std::sort(duals.begin(), duals.end(), [&](int32_t a, int32_t b) { return iperm[a] < iperm[b]; });
         std::vector<char> used(np_, 0);
+        std::vector<int32_t> jdeg(opt.pairs ? np_ : 0, 0);    // dual neighbours of each primal
+        for (int64_t q = 0; q < (opt.pairs ? dptr[nd_] : 0); ++q) jdeg[dnb[q]]++;
         std::vector<std::pair<int64_t, int32_t>> key(nc);
         for (int32_t v = 0; v < nc; ++v) key[v] = {2 * (int64_t)iperm[v], iperm[v]};
         for (int32_t v : duals) {
             const int64_t a = dptr[v - np_], b = dptr[v - np_ + 1];
             if (a == b) continue;                              // isolated dual row: nothing can help it
             int32_t partner = -1;
+            if (opt.pairs) {
+                // PAIRS: EVERY dual that can be matched goes immediately after its partner (key second -1: ahead of an unmatched dual
+                // placed after the same row), so that the two can form one 2 x 2 pivot.  Partner: the unused neighbour with the fewest
+                // dual neighbours (a column with one constraint, such as a free LP column, has no other dual to pair with), ties to
+                // the closest one that precedes the dual (it moves least), else to the earliest one after it.
+                auto better = [&](int32_t x, int32_t y) {      // x preferred over the current choice y
+                    if (y < 0) return true;
+                    if (jdeg[x] != jdeg[y]) return jdeg[x] < jdeg[y];
+                    const bool xb = iperm[x] < iperm[v], yb = iperm[y] < iperm[v];
+                    if (xb != yb) return xb;
+                    return xb ? iperm[x] > iperm[y] : iperm[x] < iperm[y];
+                };
+                for (int64_t q = a; q < b; ++q) if (!used[dnb[q]] && better(dnb[q], partner)) partner = dnb[q];
+                if (partner >= 0) { used[partner] = 1; key[v] = {2 * (int64_t)iperm[partner] + 1, -1}; pairs.push_back({partner, v}); }
+                else key[v] = {2 * (int64_t)std::max(iperm[dnb[b - 1]], iperm[v]) + 1, iperm[v]};
+                continue;
+            }
             for (int64_t q = a; q < b && iperm[dnb[q]] < iperm[v]; ++q) if (!used[dnb[q]]) { partner = dnb[q]; break; }
             if (partner >= 0) { used[partner] = 1; continue; } // an own preceding neighbour exists: the dual stays where it is
             for (int64_t q = a; q < b; ++q) if (!used[dnb[q]]) { partner = dnb[q]; break; }
@@ -389,6 +409,11 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     // (children's columns before the parent's) and the final DFS keep that
     for (size_t k = 0; k < bnb.size(); ++k)
         if (parent[iperm[nc + k]] != iperm[bnb[k]]) throw std::runtime_error("internal: a bound row's etree parent is not its variable");
+    // a matched pair (u, v) with v right after u and a_vu != 0 has parent(u) = v, and u, the last child of v, stays right before v in
+    // the postorder
+    for (const auto& pr : pairs)
+        if (iperm[pr.second] != iperm[pr.first] + 1 || parent[iperm[pr.first]] != iperm[pr.second])
+            throw std::runtime_error("internal: a matched dual does not follow its primal partner as its etree parent");
     std::vector<int64_t> cc;
     colcounts(n, rptr, rcol, parent, cc);
 
@@ -428,7 +453,35 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     for (int32_t s = 0; s < nfs; ++s) if (fpar[s] != -1) nd[fpar[s]].kids.push_back(s);
     const int64_t nemin = std::max(1, opt.nemin);
     const double zr = opt.relax_zeros;
+    // merge c into p (c's columns first)
+    auto merge = [&](int32_t p, int32_t c, int64_t w2, int64_t f2, int64_t z2) {
+        std::vector<std::pair<int32_t, int32_t>> r = nd[c].ranges;
+        r.insert(r.end(), nd[p].ranges.begin(), nd[p].ranges.end());
+        nd[p].ranges.swap(r);
+        nd[p].w = w2; nd[p].f = f2; nd[p].zeros = z2;
+        auto& pk = nd[p].kids;
+        pk.erase(std::find(pk.begin(), pk.end(), c));
+        pk.insert(pk.end(), nd[c].kids.begin(), nd[c].kids.end());
+        nd[c].kids.clear();
+        nd[c].merged = true;
+    };
+    // PAIRS: a pair split between a child supernode (ending with the primal) and its parent (starting with the dual) is merged
+    // whatever it costs, and FIRST, while the parent holds only its own columns: the child's last column then stays adjacent to the
+    // parent's first through every later merge and the final DFS.
+    std::vector<char> force(nfs, 0);
+    for (const auto& pr : pairs) {
+        const int32_t j = iperm[pr.first];
+        if (col2fs[j] != col2fs[j + 1]) force[col2fs[j]] = 1;
+    }
     for (int32_t p = 0; p < nfs; ++p) {  // ascending ids = children before parents
+        if (!pairs.empty()) {
+            const std::vector<int32_t> kids = nd[p].kids;
+            for (int32_t c : kids) {
+                if (!force[c]) continue;
+                const int64_t w2 = nd[p].w + nd[c].w, f2 = nd[c].w + nd[p].f, nnz2 = trap_nnz(w2, f2);
+                merge(p, c, w2, f2, nd[p].zeros + nd[c].zeros + nnz2 - trap_nnz(nd[p].w, nd[p].f) - trap_nnz(nd[c].w, nd[c].f));
+            }
+        }
         bool again = true;
         while (again) {
             again = false;
@@ -446,16 +499,7 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
                 // critical path (hand-off + staging per level on the device) for a few explicit zeros in a front of order <= 64
                 if (!ok && opt.chain_merge_f > 0 && nd[p].kids.size() == 1 && f2 <= std::min(opt.chain_merge_f, 64)) ok = true;
                 if (!ok) continue;
-                // merge c into p
-                std::vector<std::pair<int32_t, int32_t>> r = nd[c].ranges;
-                r.insert(r.end(), nd[p].ranges.begin(), nd[p].ranges.end());
-                nd[p].ranges.swap(r);
-                nd[p].w = w2; nd[p].f = f2; nd[p].zeros = z2;
-                auto& pk = nd[p].kids;
-                pk.erase(std::find(pk.begin(), pk.end(), c));
-                pk.insert(pk.end(), nd[c].kids.begin(), nd[c].kids.end());
-                nd[c].kids.clear();
-                nd[c].merged = true;
+                merge(p, c, w2, f2, z2);
                 again = true;
                 break;
             }
@@ -498,6 +542,13 @@ void analyse(int32_t n, const int32_t* colptr, const int32_t* rowval, const Anal
     S.sn_first = sn_first;
     std::vector<int32_t> col2sn(n);
     for (int32_t s = 0; s < ns; ++s) for (int32_t j = sn_first[s]; j < sn_first[s + 1]; ++j) col2sn[j] = s;
+    S.pair_start.assign(n, 0);
+    for (const auto& pr : pairs) {
+        const int32_t j = S.iperm[pr.first];
+        if (S.iperm[pr.second] != j + 1 || col2sn[j] != col2sn[j + 1])
+            throw std::runtime_error("internal: a matched pair is not adjacent inside one supernode");
+        S.pair_start[j] = 1;
+    }
 
     timer.lap("final permutation");
     // ---- 7. permuted lower CSC (by column) with source positions

@@ -17,6 +17,7 @@ struct AnalysisOptions {
     int kkt_n_primal = 0;      // augmented-KKT hint: dual rows are ordered after one primal neighbour
     int kkt_n_dual = 0;        // > 0: rows from kkt_n_primal + kkt_n_dual on are bound duals, ordered just before their neighbour
     int chain_merge_f = 0;     // > 0: single-child chains are merged while the front order stays <= this (latency, not flops)
+    bool pairs = false;        // B2_SPARSE_PIVOT_PAIRS: every matchable constraint dual right after a distinct primal neighbour, in one supernode
 };
 
 // One front per supernode.  Pivot columns [first, first+w) in the PERMUTED numbering; the front has
@@ -51,6 +52,7 @@ struct Symbolic {
     int32_t max_front = 0;
     int64_t top_rows = 0;             // sum of w over the shared top tree
     int64_t exch_cb = 0;              // doubles at the start of the update-block workspace that cross rank->top
+    std::vector<uint8_t> pair_start;  // [n] (AnalysisOptions::pairs) 1 where permuted column j starts a candidate 2x2 pivot (j, j+1)
 };
 
 // Checks the row classes of an unreduced KKT pattern: kkt_n_dual >= 0, kkt_n_primal + kkt_n_dual <= n, kkt_n_primal > 0 when

@@ -71,6 +71,12 @@ struct b2_solver {
     DevBuf<int32_t> d_flags;
     // hand-off slots of the single-launch solve (k_solve_dep), SLOT_EMPTY between launches: up [sum r] | down [sum r] | ypiv [n]
     DevBuf<double> d_slots;
+    // B2_SPARSE_PIVOT_PAIRS: per-supernode mask of the columns where a candidate 2 x 2 pivot starts; D's subdiagonal and the pivot
+    // kinds (B2_PIVOT_*) of the last factorisation, permuted order
+    bool pairs = false;
+    DevBuf<unsigned long long> d_pair_mask;
+    DevBuf<double> d_dsub;
+    DevBuf<int8_t> d_pkind;
     int32_t* h_counters = nullptr;   // pinned
     std::vector<int64_t> cbv_off;
     int64_t exch_cbv = 0;
@@ -173,6 +179,13 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
         // (the group ticket in slot nsuper re-arms itself: the CTA that takes the last group resets it)
         cudaMemsetAsync(s->d_flags.p, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
         const size_t sm = sizeof(double) * std::max<size_t>((size_t)FW_WARPS * TeamSmem<1>::doubles(P.dep_maxf1), (size_t)TeamSmem<2>::doubles(P.dep_maxf2));
+        if (s->pairs) {
+            PairArgs pa;
+            pa.mask = s->d_pair_mask.p; pa.dsub = s->d_dsub.p; pa.kind = s->d_pkind.p;
+            k_factor_dep_pairs<<<P.dep_ngroup, 128, sm, st>>>(a, s->d_childrec.p, ds, P.dep_maxf1, P.dep_maxf2, s->d_flags.p,
+                                                              s->d_counters.p + 4, s->d_flags.p + s->S.nsuper, pa);
+            return 2;
+        }
         k_factor_dep<<<P.dep_ngroup, 128, sm, st>>>(a, s->d_childrec.p, ds, P.dep_maxf1, P.dep_maxf2, s->d_flags.p, s->d_counters.p + 4,
                                                     s->d_flags.p + s->S.nsuper);
         return 2;
@@ -297,6 +310,11 @@ void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
     DepSched ds;
     ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
     ds.ngroup = P.dep_ngroup;
+    if (s->pairs) {
+        k_solve_dep_pairs<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
+                                                                   s->S.n, s->d_slots.p, (int64_t)s->d_slots.n, s->d_dsub.p);
+        return;
+    }
     k_solve_dep<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1, s->S.n,
                                                          s->d_slots.p, (int64_t)s->d_slots.n);
 }
@@ -306,6 +324,7 @@ int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_factor_warp<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_factor_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_factor_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_fwd_warp2<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute((k_fwd_warp2<1, SOLVE_FUSED_TEAMS>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -313,6 +332,7 @@ int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_fwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_solve_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_solve_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_big_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     return B2_OK;
 }
@@ -552,6 +572,18 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         const std::string bad = check_kkt_rows(n, colptr_h, rowval_h, opt->kkt_n_primal, opt->kkt_n_dual);
         if (!bad.empty()) { set_error("b2_create: " + bad); return B2_ERR_INVALID; }
     }
+    const bool pairs = opt && opt->sparse_pivoting == B2_SPARSE_PIVOT_PAIRS;
+    if (opt && opt->sparse_pivoting != B2_SPARSE_PIVOT_STATIC && !pairs) {
+        set_error("b2_create: sparse_pivoting must be B2_SPARSE_PIVOT_STATIC (0) or B2_SPARSE_PIVOT_PAIRS (1)");
+        return B2_ERR_INVALID;
+    }
+    if (pairs) {   // the 2 x 2 pivots exist in the single-launch team-class kernels only
+        const char* bad = opt->kkt_n_primal <= 0 ? "kkt_n_primal > 0 (an augmented KKT system)"
+                        : opt->n_parts > 1 ? "n_parts == 1"
+                        : !(opt->dep_schedule & 1) ? "dep_schedule bit 0 (the single-launch schedule)"
+                        : opt->small_front_max <= 32 ? "small_front_max > 32 (two-warp team fronts)" : nullptr;
+        if (bad) { set_error(std::string("b2_create: sparse_pivoting = B2_SPARSE_PIVOT_PAIRS needs ") + bad); return B2_ERR_INVALID; }
+    }
     b2_solver* s = new b2_solver();
     if (opt) s->opt = *opt; else b2_options_default(&s->opt);
     s->symbolic_only = symbolic_only;
@@ -565,6 +597,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         ao.n_parts = std::max(1, s->opt.n_parts);
         ao.kkt_n_primal = s->opt.kkt_n_primal;
         ao.kkt_n_dual = s->opt.kkt_n_dual;
+        ao.pairs = pairs;
         analyse(n, colptr_h, rowval_h, ao, user_perm_h, s->S);
     } catch (std::exception& e) {
         set_error(std::string("b2_create: analysis failed: ") + e.what());
@@ -573,6 +606,16 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
     }
     const Symbolic& S = s->S;
     const int ns = S.nsuper;
+    s->pairs = pairs;
+    if (pairs && !symbolic_only) {
+        const int fmax = std::min(W_MAX, s->opt.small_front_max);
+        if (S.max_front > fmax) {
+            set_error("b2_create: sparse_pivoting = B2_SPARSE_PIVOT_PAIRS needs every front of order <= " + std::to_string(fmax) +
+                      " after the analysis; the largest has order " + std::to_string(S.max_front));
+            delete s;
+            return B2_ERR_INVALID;
+        }
+    }
     // contribution-vector offsets: blocks crossing into the shared top tree first (exchange region)
     {
         s->cbv_off.assign(ns + 1, 0);
@@ -677,6 +720,16 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         }
         B2_CUDA_THROW(s->d_ws.alloc((size_t)std::max<int64_t>(1, S.cb_off[ns])));
         B2_CUDA_THROW(s->d_dvec.alloc(n));
+        if (pairs) {
+            std::vector<unsigned long long> pm(ns, 0);
+            for (int sn = 0; sn < ns; ++sn)
+                for (int j = S.sn_first[sn]; j < S.sn_first[sn + 1]; ++j) if (S.pair_start[j]) pm[sn] |= 1ull << (j - S.sn_first[sn]);
+            B2_CUDA_THROW(s->d_pair_mask.upload(pm.data(), pm.size()));
+            B2_CUDA_THROW(s->d_dsub.alloc(n));
+            B2_CUDA_THROW(s->d_pkind.alloc(n));
+            B2_CUDA_THROW(cudaMemset(s->d_dsub.p, 0, s->d_dsub.bytes()));
+            B2_CUDA_THROW(cudaMemset(s->d_pkind.p, 0, s->d_pkind.bytes()));
+        }
         B2_CUDA_THROW(s->d_xp.alloc(n));
         B2_CUDA_THROW(s->d_cbv.alloc((size_t)std::max<int64_t>(1, s->cbv_off[ns])));
         B2_CUDA_THROW(s->d_counters.alloc(8));
@@ -861,6 +914,7 @@ int b2_inertia_parts(b2_solver* s, int64_t* local_neg, int64_t* local_zero, int6
 
 int b2_solve_fwd_local(b2_solver* s, double* x_d, void* stream) {
     if (!s || s->symbolic_only || !x_d) return B2_ERR_INVALID;
+    if (s->pairs) { set_error("b2_solve_fwd_local: a PAIRS factor is solved by b2_solve only"); return B2_ERR_INVALID; }
     if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
     cudaStream_t st = as_stream(stream);
     const int n = s->S.n;
@@ -880,6 +934,7 @@ int b2_solve_top(b2_solver* s, double* x_d, void* stream) {
 
 int b2_solve_bwd_local(b2_solver* s, double* x_d, void* stream) {
     if (!s || s->symbolic_only || !x_d) return B2_ERR_INVALID;
+    if (s->pairs) { set_error("b2_solve_bwd_local: a PAIRS factor is solved by b2_solve only"); return B2_ERR_INVALID; }
     cudaStream_t st = as_stream(stream);
     int rc = run_solve_phase(s, 0, false, st);
     if (rc != B2_OK) return rc;
@@ -1050,6 +1105,23 @@ int b2_debug_get_factor(b2_solver* s, double* lval_h, double* dvec_h) {
     B2_CUDA(cudaDeviceSynchronize());
     if (lval_h) B2_CUDA(cudaMemcpy(lval_h, s->d_L.p, (size_t)s->S.lp_off[s->S.nsuper] * sizeof(double), cudaMemcpyDeviceToHost));
     if (dvec_h) B2_CUDA(cudaMemcpy(dvec_h, s->d_dvec.p, s->d_dvec.bytes(), cudaMemcpyDeviceToHost));
+    return B2_OK;
+}
+
+int b2_symbolic_pairs(b2_solver* s, uint8_t* pair_start_h) {
+    if (!s || !pair_start_h) return B2_ERR_INVALID;
+    std::memcpy(pair_start_h, s->S.pair_start.data(), (size_t)s->S.n);
+    return B2_OK;
+}
+
+int b2_get_pivot_blocks(b2_solver* s, int8_t* kind_h, double* d_h, double* d_off_h) {
+    if (!s || s->symbolic_only) { set_error("b2_get_pivot_blocks: solver has no device state"); return B2_ERR_INVALID; }
+    if (!s->pairs) { set_error("b2_get_pivot_blocks: the handle pivots statically (opt.sparse_pivoting = 0)"); return B2_ERR_INVALID; }
+    if (!s->factorized) { set_error("b2_get_pivot_blocks: not factorized"); return B2_ERR_FACTORIZATION; }
+    B2_CUDA(cudaDeviceSynchronize());
+    if (kind_h) B2_CUDA(cudaMemcpy(kind_h, s->d_pkind.p, s->d_pkind.bytes(), cudaMemcpyDeviceToHost));
+    if (d_h) B2_CUDA(cudaMemcpy(d_h, s->d_dvec.p, s->d_dvec.bytes(), cudaMemcpyDeviceToHost));
+    if (d_off_h) B2_CUDA(cudaMemcpy(d_off_h, s->d_dsub.p, s->d_dsub.bytes(), cudaMemcpyDeviceToHost));
     return B2_OK;
 }
 
@@ -1233,6 +1305,10 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
     if (!out || N <= 0 || lda < N || !A_d) { set_error("b2d_create: invalid argument"); return B2_ERR_INVALID; }
     if (opt && opt->dense_pivoting != B2_DENSE_PIVOT_STATIC && opt->dense_pivoting != B2_DENSE_PIVOT_BUNCH_KAUFMAN) {
         set_error("b2d_create: dense_pivoting must be B2_DENSE_PIVOT_STATIC (0) or B2_DENSE_PIVOT_BUNCH_KAUFMAN (1)");
+        return B2_ERR_INVALID;
+    }
+    if (opt && opt->sparse_pivoting != B2_SPARSE_PIVOT_STATIC) {
+        set_error("b2d_create: sparse_pivoting applies to the sparse solver (b2_create) only");
         return B2_ERR_INVALID;
     }
     int ndev = 0;

@@ -182,10 +182,19 @@ __device__ __forceinline__ void pivot_iter(double (&av)[32 * NW + 1], double& lp
     lp = l;
 }
 
-template <int NW, bool DEP = false>
+// B2_SPARSE_PIVOT_PAIRS (DESIGN.md section 3): bit j of mask[s] marks a candidate 2 x 2 pivot (j, j+1) of front s; the factorisation
+// writes each pivot's kind (B2_PIVOT_*) and D's subdiagonal (b at the first index of a 2 x 2 block, else 0), permuted order
+struct PairArgs {
+    const unsigned long long* mask = nullptr;
+    double* dsub = nullptr;
+    int8_t* kind = nullptr;
+};
+constexpr double PAIR_ALPHA = 0.6403882032022076;    // (1 + sqrt(17)) / 8, Bunch-Kaufman's growth bound
+
+template <int NW, bool DEP = false, bool PAIRS = false>
 __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const ChildRec* childrec, int s, double* sm_team,
                                                   int tid, int team, int maxf, int& nneg, int& npert, long long* prof = nullptr,
-                                                  int* done = nullptr, int* err = nullptr) {
+                                                  int* done = nullptr, int* err = nullptr, PairArgs pa = PairArgs()) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW, STAGE = TeamSmem<NW>::STAGE;
     double* F = sm_team;
     constexpr int CBS = FMAX + 4;                      // four pivot-column buffers
@@ -291,8 +300,72 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
     }
     B2_STAMP(4);
     if (a.ftrace && tid == 0) a.ftrace[3 * (size_t)s + 1] = global_ns();
-    // row `tid` of the front into registers: a[j] = F(tid, j)
     double av[FMAX + 1];
+    if constexpr (PAIRS) {
+        // Pivots with candidate 2 x 2 blocks, right-looking in shared memory (thread = row): pivot k's column (and k+1's for a block)
+        // is snapshotted in colbuf, then every row below updates itself.  Rule at a candidate pair with a = F(k,k), b = F(k+1,k),
+        // c = F(k+1,k+1): a 2 x 2 block when |a| < alpha |b| and d1 = (a / |b|) c - |b| < 0 (indefinite: one negative and one
+        // positive eigenvalue, the count of the reference's num_neg_ev, never perturbed); otherwise k is a 1 x 1 pivot (perturbed to
+        // +-eps when |a| < eps, as the static path does) and k+1 an ordinary one.  The multipliers of a block are dsytf2's.
+        const unsigned long long pm = pa.mask[s];
+        double* u1 = colbuf;
+        double* u2 = colbuf + CBS;
+        for (int k = 0; k < w;) {
+            team_sync<NW>(team);
+            const double av_ = F[k + k * f];
+            bool two = false;
+            double b_ = 0.0, c_ = 0.0;
+            if ((pm >> k) & 1ull) {
+                b_ = F[k + 1 + k * f];
+                c_ = F[(k + 1) * (f + 1)];
+                const double t = fabs(b_);
+                two = fabs(av_) < PAIR_ALPHA * t && (av_ / t) * c_ - t < 0.0;
+            }
+            if (!two) {
+                const bool tiny = !(fabs(av_) >= a.eps), neg = av_ < 0.0;
+                const double dk = tiny ? (neg ? -a.eps : a.eps) : av_;
+                npert += (tid == 0 && tiny) ? 1 : 0;
+                nneg += (tid == 0 && !tiny && neg) ? 1 : 0;
+                if (tid > k && tid < f) u1[tid] = F[tid + k * f];
+                team_sync<NW>(team);
+                if (tid > k && tid < f) {
+                    const double l = u1[tid] / dk;
+                    for (int j = k + 1; j <= tid; ++j) F[tid + j * f] = fma(-l, u1[j], F[tid + j * f]);
+                    F[tid + k * f] = l;
+                }
+                if (tid == 0) {
+                    F[k + k * f] = dk;
+                    pa.kind[d.col0 + k] = tiny ? 1 : 0;
+                    pa.dsub[d.col0 + k] = 0.0;
+                }
+                k += 1;
+            } else {
+                nneg += (tid == 0) ? 1 : 0;
+                if (tid > k + 1 && tid < f) { u1[tid] = F[tid + k * f]; u2[tid] = F[tid + (k + 1) * f]; }
+                team_sync<NW>(team);
+                if (tid > k + 1 && tid < f) {
+                    const double d11 = c_ / b_, d22 = av_ / b_, t = 1.0 / (d11 * d22 - 1.0), d21 = t / b_;
+                    const double x1 = u1[tid], x2 = u2[tid];
+                    const double l1 = d21 * (d11 * x1 - x2), l2 = d21 * (d22 * x2 - x1);
+                    for (int j = k + 2; j <= tid; ++j) F[tid + j * f] = fma(-l2, u2[j], fma(-l1, u1[j], F[tid + j * f]));
+                    F[tid + k * f] = l1;
+                    F[tid + (k + 1) * f] = l2;
+                }
+                if (tid == 0) {
+                    F[k + 1 + k * f] = 0.0;                // L11(k+1, k) of a block; D keeps a, b, c
+                    pa.kind[d.col0 + k] = 2;
+                    pa.kind[d.col0 + k + 1] = 3;
+                    pa.dsub[d.col0 + k] = b_;
+                    pa.dsub[d.col0 + k + 1] = 0.0;
+                }
+                k += 2;
+            }
+        }
+        team_sync<NW>(team);
+#pragma unroll
+        for (int j = 0; j < FMAX; ++j) av[j] = (w + j < f && tid < f) ? F[tid + (w + j) * f] : 0.0;
+    } else {
+    // row `tid` of the front into registers: a[j] = F(tid, j)
 #pragma unroll
     for (int j = 0; j < FMAX; ++j) av[j] = (j < f && tid < f) ? F[tid + j * f] : 0.0;
     av[FMAX] = 0.0;
@@ -348,6 +421,7 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
             }
         }
     }
+    }   // !PAIRS
     B2_STAMP(5);
     // update block first (it is all the parent waits for): av[j] holds column w+j of row tid -- registers only, no barrier needed
     if (tid >= w && tid < f) {
@@ -543,9 +617,10 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
     }
 }
 
-template <int NW, bool DEP = false>
+// PAIRS (DEP only): D^-1 over the 2 x 2 blocks that dsub marks (PairArgs), by dsytrs's formula
+template <int NW, bool DEP = false, bool PAIRS = false>
 __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double* sm_team, int tid, int team,
-                                               const ChildRec* childrec = nullptr, int* err = nullptr) {
+                                               const ChildRec* childrec = nullptr, int* err = nullptr, const double* dsub = nullptr) {
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* xs = sm_team;                              // [FMAX] gathered ancestor values at [xa, xa + r)
     double* xb = xs + FMAX;                            // [2][8]
@@ -581,6 +656,19 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
         slot_take(p, (tid < r ? 1u : 0u) | (tid < w ? 2u : 0u), v, err);
         if (tid < r) xs[xa + tid] = v[0];
         t = (tid < w) ? v[1] * dinv : 0.0;
+        if constexpr (PAIRS) {
+            // a block's partner row is in the same front: its forward value through xs[0, w), free until the back-substitution
+            if (tid < w) xs[tid] = v[1];
+            team_sync<NW>(team);
+            const int i = d.col0 + tid;
+            const bool first = tid < w && dsub[i] != 0.0, second = tid < w && tid > 0 && dsub[i - 1] != 0.0;
+            if (first || second) {
+                const int i0 = first ? i : i - 1, k0 = first ? tid : tid - 1;
+                const double akm1k = dsub[i0], akm1 = a.dvec[i0] / akm1k, ak = a.dvec[i0 + 1] / akm1k;
+                const double denom = akm1 * ak - 1.0, bkm1 = xs[k0] / akm1k, bk = xs[k0 + 1] / akm1k;
+                t = first ? (ak * bkm1 - bk) / denom : (akm1 * bk - bkm1) / denom;
+            }
+        }
     } else {
         pdl_wait();
         if (tid < r) xs[xa + tid] = a.xp[myrow];
@@ -748,6 +836,26 @@ __global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec
     }
 }
 
+// k_factor_dep with candidate 2 x 2 pivots (b2_options.sparse_pivoting = B2_SPARSE_PIVOT_PAIRS): the same schedule and hand-offs,
+// front_factor_team's PAIRS pivot loop.  A separate kernel, so that the static one is compiled exactly as before.
+__global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const ChildRec* childrec, DepSched ds, int maxf1, int maxf2,
+                                                          int* done, int* err, int* ticket, PairArgs pa) {
+    extern __shared__ __align__(16) double sm[];
+    const int g = claim_group(ticket, ds.ngroup);
+    const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
+    int nneg = 0, npert = 0;
+    if (type == 1) {
+        const int team = threadIdx.x >> 5, tid = threadIdx.x & 31;
+        if (team < n) front_factor_team<1, true, true>(a, childrec, ds.tasks[t0 + team], sm + (size_t)team * TeamSmem<1>::doubles(maxf1),
+                                                       tid, team, maxf1, nneg, npert, nullptr, done, err, pa);
+        if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
+    } else {
+        const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
+        if (team < n) front_factor_team<2, true, true>(a, childrec, ds.tasks[t0 + team], sm, tid, team, maxf2, nneg, npert, nullptr, done, err, pa);
+        if (tid == 0 && team < n) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ single-launch solve
 // Forward sweep, D^-1 and backward sweep of the whole (team-class, unsharded) tree in ONE launch.  The tasks are the groups of
 // k_factor_dep (DepSched: fronts in (level, id) order, four fronts of order <= 32 as one-warp teams or one front of order <= 64 as a
@@ -802,6 +910,53 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRe
             } else {
                 if (type == 1) front_bwd_team<1, true>(a, s, sm1[team], tid, team, childrec, err);
                 else front_bwd_team<2, true>(a, s, smd, tid, team, childrec, err);
+            }
+        }
+        __syncthreads();                                // (tk_sh is rewritten by the next claim)
+    }
+    if (threadIdx.x == 0) {
+        bad_sh = 0;
+        __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
+        if (atomicAdd(ctl + 1, 1) == (int)gridDim.x - 1) {
+            atomicExch(ctl, 0);
+            atomicExch(ctl + 1, 0);
+            __threadfence();
+            bad_sh = *(volatile int*)err;
+        }
+    }
+    __syncthreads();
+    if (bad_sh) {
+        for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
+        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
+    }
+}
+
+// k_solve_dep for a PAIRS factor (D with 2 x 2 blocks, front_bwd_team<.., PAIRS>); a separate kernel, so that the static one is
+// compiled exactly as before
+__global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl,
+                                                         int n, double* slots, int64_t nslot, const double* dsub) {
+    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
+    double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
+    __shared__ int tk_sh, bad_sh;
+    const int ntask = 2 * ds.ngroup;
+    for (;;) {
+        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
+        __syncthreads();
+        const int t = tk_sh;
+        if (t >= ntask) break;
+        const bool fwd = t < ds.ngroup;
+        const int g = fwd ? t : ntask - 1 - t;
+        const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
+        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
+        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        if (team < cnt) {
+            const int s = ds.tasks[t0 + team];
+            if (fwd) {
+                if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, err);
+                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
+            } else {
+                if (type == 1) front_bwd_team<1, true, true>(a, s, sm1[team], tid, team, childrec, err, dsub);
+                else front_bwd_team<2, true, true>(a, s, smd, tid, team, childrec, err, dsub);
             }
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)

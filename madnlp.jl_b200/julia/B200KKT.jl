@@ -37,17 +37,19 @@ Base.@kwdef mutable struct B200Options <: AbstractOptions
     b200_kkt_n_dual::Int32 = 0          # set by create_kkt_system(SparseUnreducedKKTSystem, ...) below
     b200_dense_pivoting::Int32 = 0      # B200DenseSolver only: 0 static (B2_DENSE_PIVOT_STATIC), 1 Bunch-Kaufman, as
                                         # lapack_algorithm = BUNCHKAUFMAN (B2_DENSE_PIVOT_BUNCH_KAUFMAN); B200Solver needs 0
+    b200_sparse_pivoting::Int32 = 0     # B200Solver only: 0 static (B2_SPARSE_PIVOT_STATIC), 1 2x2 pivots on matched
+                                        # primal-dual pairs (B2_SPARSE_PIVOT_PAIRS); B200DenseSolver needs 0
 end
 
 struct CB2Options
     ordering::Int32; nemin::Int32; relax_zeros::Float64; pivot_eps::Float64
     use_cuda_graph::Int32; small_front_max::Int32; n_parts::Int32; part_rank::Int32
     kkt_n_primal::Int32; fuse_max_fronts::Int32; dep_schedule::Int32; chain_merge_f::Int32; kkt_n_dual::Int32; dense_pivoting::Int32
-    reserved::NTuple{2,Int32}
+    sparse_pivoting::Int32; reserved::NTuple{1,Int32}
 end
 CB2Options(o::B200Options) = CB2Options(o.b200_ordering, o.b200_nemin, o.b200_relax_zeros, o.b200_pivot_eps,
     o.b200_use_cuda_graph, o.b200_small_front_max, 1, 0, o.b200_kkt_n_primal, o.b200_fuse_max_fronts, o.b200_dep_schedule, o.b200_chain_merge_f,
-    o.b200_kkt_n_dual, o.b200_dense_pivoting, ntuple(_ -> Int32(0), 2))
+    o.b200_kkt_n_dual, o.b200_dense_pivoting, o.b200_sparse_pivoting, ntuple(_ -> Int32(0), 1))
 
 last_error() = unsafe_string(ccall((:b2_last_error, libb200kkt), Cstring, ()))
 function check(rc::Cint, exc)

@@ -69,7 +69,8 @@ class B200SparseSolver:
         return np.dtype(dtype) == np.float64
 
     def introduce(self) -> str:
-        return f"b200kkt multifrontal LDL^T v{lib.b2_version()}"
+        pairs = " (2x2 pivots on primal-dual pairs)" if self.opt.sparse_pivoting == capi.B2_SPARSE_PIVOT_PAIRS else ""
+        return f"b200kkt multifrontal LDL^T v{lib.b2_version()}{pairs}"
 
     def is_async(self) -> bool:
         return True                          # returns before the GPU is done (linearsolvers.jl:67-69)
@@ -115,6 +116,13 @@ class B200SparseSolver:
         p = np.empty(self.n, dtype=np.int32)
         check(lib.b2_get_perm(self._h, p.ctypes.data))
         return p
+
+    def pivot_blocks(self):
+        """(kind, d, d_off) of the last factorisation in elimination order (b2_get_pivot_blocks; sparse_pivoting = PAIRS only)"""
+        kind = np.empty(self.n, dtype=np.int8)
+        d, e = np.empty(self.n), np.empty(self.n)
+        check(lib.b2_get_pivot_blocks(self._h, kind.ctypes.data, d.ctypes.data, e.ctypes.data))
+        return kind, d, e
 
 
 class B200DenseSolver:

@@ -574,3 +574,74 @@ def augmented_grid_kkt(nx: int, ny: int, nz: int, cons_per_node: float = 0.43, s
         I.append(n_tot + np.arange(m)); Jc.append(cols); V.append(rng.uniform(-1, 1, m))
     I.append(n_tot + np.arange(m)); Jc.append(n_tot + np.arange(m)); V.append(np.full(m, -delta))
     return n_tot + m, n_tot, m, np.concatenate(I).astype(np.int64), np.concatenate(Jc).astype(np.int64), np.concatenate(V)
+
+
+# --------------------------------------------------------------------------------------------
+# Sparse LP/QP with free, zero-curvature variables (sparse_pivoting = B2_SPARSE_PIVOT_PAIRS)
+# --------------------------------------------------------------------------------------------
+@dataclass
+class SparseLP:
+    n: int
+    m: int
+    jac_I: np.ndarray          # COO of the constraint Jacobian (m x n), 0-based
+    jac_J: np.ndarray
+    jac_V: np.ndarray
+    hess_I: np.ndarray         # COO of the lower Hessian (diagonal, bounded variables only)
+    hess_J: np.ndarray
+    hess_V: np.ndarray
+    ind_ineq: np.ndarray
+    ind_lb: np.ndarray
+    ind_ub: np.ndarray
+    n_free: int
+
+
+def sparse_free_lp(n: int = 400, m: int = 160, n_free: int = 60, n_eq: int = 100, per_col: int = 3, seed: int = 7):
+    """A sparse QP whose first `n_free` variables are free LP columns: no bounds, no curvature, and each in exactly one equality row.
+    The other variables are bounded in [0, 1] with a diagonal Hessian and `per_col` Jacobian entries each, in rows near j m / n
+    (a banded pattern: every front stays of order <= 64 with the pair ordering).  With the iterate (bound
+    terms log-uniform in [1e-3, 1e3], reg = 0, a zero (2,2) block) the augmented KKT matrix is nonsingular, but a free column's
+    diagonal is exactly 0: eliminated before its constraint row, as the static ordering does, it is a zero pivot that the static
+    rule perturbs.  Returns (SparseLP, iterate dict with the Jacobian / Hessian values and the IPM diagonals)."""
+    if not (0 <= n_free <= n_eq <= m < n):
+        raise ValueError("sparse_free_lp needs 0 <= n_free <= n_eq <= m < n")
+    rng = np.random.default_rng(seed)
+    rows, cols = [], []
+    for j in range(n_free):                                        # free column j: equality row j only
+        rows.append(j); cols.append(j)
+    for j in range(n_free, n):                                     # banded: rows near j m / n, so the fill stays local
+        c = j * m // n
+        for r in rng.choice(np.arange(c - per_col, c + per_col + 1) % m, size=per_col, replace=False):
+            rows.append(int(r)); cols.append(j)
+    I = np.array(rows, dtype=np.int64); J = np.array(cols, dtype=np.int64)
+    order = np.lexsort((I, J))
+    I, J = I[order], J[order]
+    V = rng.uniform(0.5, 1.5, len(I)) * rng.choice([-1.0, 1.0], len(I))
+    bounded = np.arange(n_free, n, dtype=np.int64)
+    ns = m - n_eq
+    ind = np.concatenate([bounded, np.arange(n, n + ns, dtype=np.int64)])
+    lp = SparseLP(n, m, I, J, V, bounded.copy(), bounded.copy(), np.exp(rng.uniform(np.log(1e-2), 0.0, len(bounded))),
+                  np.arange(n_eq, m, dtype=np.int64), ind, ind.copy(), n_free)
+    sigma = np.exp(rng.uniform(np.log(1e-3), np.log(1e3), len(ind)))
+    n_tot = n + ns
+    it = dict(jac=V.copy(), hess=lp.hess_V.copy(), l_diag=-np.ones(len(ind)), u_diag=-np.ones(len(ind)), l_lower=sigma / 2,
+              u_lower=sigma / 2, reg=np.zeros(n_tot), du_diag=np.zeros(m), rhs=rng.standard_normal(n_tot + m + 2 * len(ind)))
+    return lp, it
+
+
+def sparse_lp_augmented(lp: SparseLP, it: dict):
+    """The augmented KKT matrix [[H + Sigma + reg, J'], [J, -du_diag]] of `sparse_free_lp` (slacks after the variables, slack
+    column -1 in its inequality row) as a dense symmetric array, with n_tot = n + ns."""
+    ns = len(lp.ind_ineq)
+    n_tot = lp.n + ns
+    N = n_tot + lp.m
+    K = np.zeros((N, N))
+    d = it["reg"].copy()
+    d[lp.ind_lb] -= it["l_lower"] / it["l_diag"]
+    d[lp.ind_ub] -= it["u_lower"] / it["u_diag"]
+    K[np.arange(n_tot), np.arange(n_tot)] = d
+    K[lp.hess_I, lp.hess_J] += it["hess"]
+    K[n_tot + lp.jac_I, lp.jac_J] += it["jac"]
+    K[n_tot + lp.ind_ineq, lp.n + np.arange(ns)] = -1.0
+    K[np.arange(n_tot, N), np.arange(n_tot, N)] = -it["du_diag"]
+    K = np.tril(K)
+    return K + np.tril(K, -1).T, n_tot
