@@ -111,6 +111,13 @@ __device__ __forceinline__ unsigned long long ld_relaxed_b64(const double* p) {
     asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(v) : "l"(p));
     return v;
 }
+// two consecutive 8-byte words (16-byte aligned) in one access; each word is single-copy atomic on its own, not the pair
+__device__ __forceinline__ void ld_relaxed_v2_b64(const double* p, unsigned long long& v0, unsigned long long& v1) {
+    asm volatile("ld.relaxed.gpu.global.v2.b64 {%0, %1}, [%2];" : "=l"(v0), "=l"(v1) : "l"(p));
+}
+__device__ __forceinline__ void st_relaxed_v2_b64(double* p, unsigned long long v0, unsigned long long v1) {
+    asm volatile("st.relaxed.gpu.global.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"(v0), "l"(v1) : "memory");
+}
 __device__ __forceinline__ void st_release(int* p, int v) {
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }

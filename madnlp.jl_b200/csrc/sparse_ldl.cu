@@ -41,6 +41,8 @@ struct Phase {
     int dep_ngroup = 0, dep_type_off = 0, dep_ptr_off = 0, dep_tasks_off = 0, dep_maxf1 = 0, dep_maxf2 = 0;
     // single-launch solve (k_solve_dep: the same groups, condition and phase 0 only): persistent CTAs (0: the level-launch solve)
     int sol_grid = 0;
+    // its block form (k_solve_dep_block) for 2, 4 and 8 right-hand sides per walk: persistent CTAs of each width
+    int sol_grid_blk[3] = {0, 0, 0};
     cudaGraphExec_t g_factor = nullptr, g_fwd = nullptr, g_bwd = nullptr;
     int64_t n_factor_launches = 0, n_solve_launches = 0;
     int64_t n_fused_fronts = 0;
@@ -71,6 +73,9 @@ struct b2_solver {
     DevBuf<int32_t> d_flags;
     // hand-off slots of the single-launch solve (k_solve_dep), SLOT_EMPTY between launches: up [sum r] | down [sum r] | ypiv [n]
     DevBuf<double> d_slots;
+    // the same three slot arrays for the block solve (k_solve_dep_block), 8 words per index so that every width fits: up [8 sum r] |
+    // down [8 sum r] | ypiv [8 n].  Allocated with d_slots, since b2_solve may be captured into a caller's CUDA graph.
+    DevBuf<double> d_bslots;
     // B2_SPARSE_PIVOT_PAIRS: per-supernode mask of the columns where a candidate 2 x 2 pivot starts; D's subdiagonal and the pivot
     // kinds (B2_PIVOT_*) of the last factorisation, permuted order
     bool pairs = false;
@@ -319,6 +324,36 @@ void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
                                                          s->d_slots.p, (int64_t)s->d_slots.n);
 }
 
+// the block solve's dynamic shared memory per width: max(4 one-warp slices, 1 two-warp slice)
+template <int NR>
+constexpr size_t solve_block_smem() {
+    return sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1, NR>::doubles, (size_t)SolveSmem<2, NR>::doubles);
+}
+template <int NR>
+const void* solve_block_kernel(bool pairs) {
+    return pairs ? (const void*)k_solve_dep_block<NR, true> : (const void*)k_solve_dep_block<NR, false>;
+}
+
+// columns [0, ncol) of x (ld n) as ONE launch of k_solve_dep_block<NR>, 1 <= ncol <= NR
+template <int NR>
+void enqueue_solve_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
+    const Phase& P = s->phase[0];
+    SolveArgs a = solve_args(s);
+    a.perm = s->d_perm.p;
+    a.x = x;
+    const int64_t nr = s->cbv_off[s->S.nsuper];
+    a.up = s->d_bslots.p;
+    a.down = s->d_bslots.p + NR * nr;
+    a.ypiv = s->d_bslots.p + 2 * NR * nr;
+    DepSched ds;
+    ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
+    ds.ngroup = P.dep_ngroup;
+    const int w = NR == 2 ? 0 : NR == 4 ? 1 : 2;
+    auto kern = s->pairs ? k_solve_dep_block<NR, true> : k_solve_dep_block<NR, false>;
+    kern<<<P.sol_grid_blk[w], 128, solve_block_smem<NR>(), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
+                                                                 s->S.n, ncol, s->d_bslots.p, (int64_t)s->d_bslots.n, s->d_dsub.p);
+}
+
 int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_front_smem<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
@@ -333,6 +368,11 @@ int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_solve_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_solve_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    for (bool pairs : {false, true}) {
+        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<2>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<4>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<8>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    }
     B2_CUDA(cudaFuncSetAttribute(k_big_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     return B2_OK;
 }
@@ -751,6 +791,15 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             P.n_solve_launches = 1;
             B2_CUDA_THROW(s->d_slots.alloc((size_t)(2 * s->cbv_off[ns] + n)));
             B2_CUDA_THROW(cudaMemset(s->d_slots.p, SLOT_EMPTY_BYTE, s->d_slots.bytes()));     // every slot SLOT_EMPTY
+            // block solve: each width's grid from its own occupancy
+            const void* bk[3] = {solve_block_kernel<2>(pairs), solve_block_kernel<4>(pairs), solve_block_kernel<8>(pairs)};
+            const size_t bsm[3] = {solve_block_smem<2>(), solve_block_smem<4>(), solve_block_smem<8>()};
+            for (int w = 0; w < 3; ++w) {
+                B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bk[w], 128, bsm[w]));
+                P.sol_grid_blk[w] = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
+            }
+            B2_CUDA_THROW(s->d_bslots.alloc((size_t)8 * (2 * s->cbv_off[ns] + n)));
+            B2_CUDA_THROW(cudaMemset(s->d_bslots.p, SLOT_EMPTY_BYTE, s->d_bslots.bytes()));
         }
     } catch (std::exception&) {
         delete s;
@@ -949,10 +998,22 @@ int b2_solve_bwd_local(b2_solver* s, double* x_d, void* stream) {
 int b2_solve(b2_solver* s, double* x_d, int32_t nrhs, void* stream) {
     if (!s || s->symbolic_only || !x_d || nrhs < 1) { set_error("b2_solve: invalid argument"); return B2_ERR_INVALID; }
     if (s->opt.n_parts > 1) { set_error("b2_solve: multi-part solver needs the phased solve"); return B2_ERR_INVALID; }
-    if (s->phase[0].sol_grid) {          // every front team-class: one launch per right-hand side, in place on x
+    if (s->phase[0].sol_grid) {          // every front team-class: one launch per walk of the tree, in place on x
         if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
-        for (int c = 0; c < nrhs; ++c) enqueue_solve_dep(s, x_d + (size_t)c * s->S.n, as_stream(stream));
-        s->phase[0].n_solve_launches = 1;
+        cudaStream_t st = as_stream(stream);
+        if (nrhs == 1) {
+            enqueue_solve_dep(s, x_d, st);
+        } else {
+            // chunks of 8 columns, then the narrowest block width that holds the rest (12 columns: 8 + 4, 9: 8 + 1 of 2)
+            for (int c0 = 0; c0 < nrhs; c0 += 8) {
+                double* x = x_d + (size_t)c0 * s->S.n;
+                const int m = std::min(8, nrhs - c0);
+                if (m <= 2) enqueue_solve_block<2>(s, x, m, st);
+                else if (m <= 4) enqueue_solve_block<4>(s, x, m, st);
+                else enqueue_solve_block<8>(s, x, m, st);
+            }
+        }
+        s->phase[0].n_solve_launches = 1;  // per right-hand side
         B2_CUDA(cudaGetLastError());
         return B2_OK;
     }

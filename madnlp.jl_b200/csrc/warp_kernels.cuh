@@ -121,6 +121,78 @@ __device__ __forceinline__ void slot_take(double* const (&p)[K], unsigned need, 
     }
 }
 
+// Block hand-offs of the single-launch solve with NR right-hand sides (k_solve_dep_block): a slot index owns NR consecutive words,
+// word c for column c, and each word keeps the rule above -- the producer never stores SLOT_EMPTY, the consumer polls the words
+// themselves.  A consumer accepts a slot once none of its NR words is SLOT_EMPTY and then re-arms all of them.  NR = 1 is slot_put /
+// slot_take.
+template <int NR>
+__device__ __forceinline__ void slot_put_block(double* p, const double (&v)[NR]) {
+    if constexpr (NR == 1) {
+        slot_put(p, v[0]);
+    } else {
+        static_assert(NR % 2 == 0, "block slots are accessed in 16-byte pairs");
+        unsigned long long b[NR];
+#pragma unroll
+        for (int q = 0; q < NR; ++q) {
+            b[q] = (unsigned long long)__double_as_longlong(v[q]);
+            b[q] = b[q] == SLOT_EMPTY ? CANON_NAN : b[q];
+        }
+#pragma unroll
+        for (int q = 0; q < NR; q += 2) st_relaxed_v2_b64(p + q, b[q], b[q + 1]);
+    }
+}
+// slot_take over K block slots: a slot still incomplete at the time-out reads as NaN where it is empty and is not re-armed here (the
+// launch's time-out path re-arms every slot once all its CTAs are done)
+template <int K, int NR>
+__device__ __forceinline__ void slot_take_block(double* const (&p)[K], unsigned need, double (&v)[K][NR], int* err) {
+    if constexpr (NR == 1) {
+        double u[K];
+        slot_take(p, need, u, err);
+#pragma unroll
+        for (int c = 0; c < K; ++c) v[c][0] = u[c];
+    } else {
+        static_assert(NR % 2 == 0, "block slots are accessed in 16-byte pairs");
+        unsigned long long b[K][NR];
+#pragma unroll
+        for (int c = 0; c < K; ++c)
+#pragma unroll
+            for (int q = 0; q < NR; q += 2) {
+                if (need >> c & 1u) ld_relaxed_v2_b64(p[c] + q, b[c][q], b[c][q + 1]);
+                else b[c][q] = b[c][q + 1] = 0ull;
+            }
+        unsigned it = 0, pend;
+        for (;;) {
+            pend = 0;
+#pragma unroll
+            for (int c = 0; c < K; ++c) {
+                bool empty = false;
+#pragma unroll
+                for (int q = 0; q < NR; ++q) empty |= b[c][q] == SLOT_EMPTY;
+                pend |= ((need >> c & 1u) && empty) ? 1u << c : 0u;
+            }
+            if (!pend) break;
+            if (++it >= DEP_SPIN_MAX) {
+                atomicExch(err, 1);
+                break;
+            }
+            __nanosleep(DEP_SPIN_SLEEP_NS);
+#pragma unroll
+            for (int c = 0; c < K; ++c)
+                if (pend >> c & 1u)
+#pragma unroll
+                    for (int q = 0; q < NR; q += 2) ld_relaxed_v2_b64(p[c] + q, b[c][q], b[c][q + 1]);
+        }
+#pragma unroll
+        for (int c = 0; c < K; ++c) {
+#pragma unroll
+            for (int q = 0; q < NR; ++q) v[c][q] = __longlong_as_double((long long)b[c][q]);
+            if ((need >> c & 1u) && !(pend >> c & 1u))
+#pragma unroll
+                for (int q = 0; q < NR; q += 2) st_relaxed_v2_b64(p[c] + q, SLOT_EMPTY, SLOT_EMPTY);
+        }
+    }
+}
+
 // One pivot of front_factor_team's software-pipelined loop, for a window of NB live 8-column blocks: the latency chain of pivot k
 // (d_k -> reciprocal (approx + 2 Newton steps) -> l_k -> column k+1 -> publish -> arrive) and the pending row update of pivot k-1,
 // as one branch-free block.  The publish is a predicated st.shared + bar.arrive in ONE asm without a memory clobber, so that most
@@ -493,11 +565,13 @@ __global__ void __launch_bounds__(TeamsPerCta<NW>::value * NW * 32) k_factor_war
 // Forward:  thread = row i of the front; y_i in a register; the recurrence y_i -= L(i,k) y_k reads L from the staged
 //           column-major panel and y_k from a shuffle (one-warp teams) or a double-buffered shared slot (two-warp teams).
 // Backward: thread = pivot column j; t_j in a register; L(i,j) comes from the staged ROW-major copy `Lt`.
-template <int NW>
+// With NR right-hand sides (k_solve_dep_block) everything a front stages is fetched once and applied to all NR columns; a thread holds
+// NR values in registers, and ys/xs hold one FMAX plane per column.
+template <int NW, int NR = 1>
 struct SolveSmem {
     static constexpr int FMAX = 32 * NW;
-    // ys/xs [FMAX] | slots [16] | recs [MAXC] (4 doubles each) | panel [FMAX*FMAX]
-    static constexpr int doubles = FMAX + 16 + 4 * MAXC + FMAX * FMAX;
+    // ys/xs [NR][FMAX] | slots [16] | recs [MAXC] (4 doubles each) | panel [FMAX*FMAX]
+    static constexpr int doubles = NR * FMAX + 16 + 4 * MAXC + FMAX * FMAX;
 };
 
 // DEP: the front runs inside the single-launch solve (k_solve_dep).  It reads its right-hand side straight from the caller's
@@ -505,12 +579,15 @@ struct SolveSmem {
 // slots and its forward result into its `ypiv` slots (for its own backward task).  The backward sweep takes the ancestor values
 // from its `down` slots and its forward result from `ypiv`, writes its solution into x[perm[j]] and puts each child's ancestor
 // values into that child's `down` slots.  Without DEP (level-launch solve) the values go through xp and cbv instead.
-template <int NW, bool DEP = false>
+// NR > 1 (DEP only): NR right-hand sides in one walk, column q at x + q * ldx, the first ncol of them live (the others are computed
+// on zeros and never touch x); each column goes through exactly the operations of NR = 1, in the same order.
+template <int NW, bool DEP = false, int NR = 1>
 __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRec* childrec, int s, double* sm_team, int tid, int team,
-                                               int* err = nullptr) {
+                                               int* err = nullptr, int ncol = 1, int64_t ldx = 0) {
+    static_assert(NR == 1 || DEP, "block right-hand sides run in the single-launch solve only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
-    double* ys = sm_team;                              // [FMAX] assembly of the front's rhs
-    double* yb = ys + FMAX;                            // [2][8] broadcast slots
+    double* ys = sm_team;                              // [NR][FMAX] assembly of the front's rhs
+    double* yb = ys + NR * FMAX;                       // [2][8] broadcast slots
     ChildRec* recs = (ChildRec*)(yb + 16);             // [MAXC]
     double* P = (double*)(recs + MAXC);                // panel, column-major, ld f
     if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s] = global_ns();
@@ -526,31 +603,36 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
         const int nc = min(MAXC, d.nchild - c0);
         if (tid < nc) recs[tid] = childrec[d.child_off + c0 + tid];
         team_sync<NW>(team);
-        int tg[MAXC]; double vv[MAXC];
+        int tg[MAXC]; double vv[MAXC][NR];
 #pragma unroll
         for (int c = 0; c < MAXC; ++c) tg[c] = (c < nc && tid < recs[c].rc) ? a.rel[recs[c].rel_off + tid] : -1;
         if (c0 == 0) {                                  // (constant data is in flight; now the values of the levels below)
             if (!DEP) pdl_wait();
-            ys[tid] = (tid < w) ? (a.x ? a.x[pj] : a.xp[d.col0 + tid]) : 0.0;
+#pragma unroll
+            for (int q = 0; q < NR; ++q)
+                ys[q * FMAX + tid] = (tid < w) ? (a.x ? (q < ncol ? a.x[q * ldx + pj] : 0.0) : a.xp[d.col0 + tid]) : 0.0;
         }
         if (DEP) {                                      // every child's slots at once: one L2 round trip once the last one lands
             double* p[MAXC];
             unsigned need = 0;
 #pragma unroll
             for (int c = 0; c < MAXC; ++c) {
-                p[c] = a.up + (tg[c] >= 0 ? recs[c].cbv_off + tid : 0);
+                p[c] = a.up + (tg[c] >= 0 ? recs[c].cbv_off + tid : 0) * NR;
                 need |= (tg[c] >= 0) ? 1u << c : 0u;
             }
-            slot_take(p, need, vv, err);
+            slot_take_block(p, need, vv, err);
         } else {
 #pragma unroll
-            for (int c = 0; c < MAXC; ++c) vv[c] = (tg[c] >= 0) ? a.cbv[recs[c].cbv_off + tid] : 0.0;
+            for (int c = 0; c < MAXC; ++c) vv[c][0] = (tg[c] >= 0) ? a.cbv[recs[c].cbv_off + tid] : 0.0;
         }
         if (c0 == 0) team_sync<NW>(team);
 #pragma unroll
         for (int c = 0; c < MAXC; ++c) {               // ascending child order: deterministic sums
             if (c < nc) {
-                if (tg[c] >= 0) ys[tg[c]] += vv[c];
+                if (tg[c] >= 0) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) ys[q * FMAX + tg[c]] += vv[c][q];
+                }
                 team_sync<NW>(team);
             }
         }
@@ -558,7 +640,9 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
     if (DEP && a.strace && tid == 0) a.strace[6 * (size_t)s + 1] = global_ns();
     cp_async_wait_all();
     team_sync<NW>(team);
-    double y = ys[tid];
+    double y[NR];
+#pragma unroll
+    for (int q = 0; q < NR; ++q) y[q] = ys[q * FMAX + tid];
     if (NW == 1) {
         for (int k0 = 0; k0 < w; k0 += 8) {
             double l[8];
@@ -567,7 +651,10 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
                 const int k = k0 + u;
-                if (k < w) y = fma(-l[u], __shfl_sync(0xffffffffu, y, k), y);      // team-uniform
+                if (k < w) {                                                        // team-uniform
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) y[q] = fma(-l[u], __shfl_sync(0xffffffffu, y[q], k), y[q]);
+                }
             }
         }
     } else {
@@ -583,18 +670,30 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
 #pragma unroll
                 for (int u = 0; u < 8; ++u) {
                     const int k = k0 + u;
-                    if (k < w0) y = fma(-l[u], __shfl_sync(0xffffffffu, y, k), y);
+                    if (k < w0) {
+#pragma unroll
+                        for (int q = 0; q < NR; ++q) y[q] = fma(-l[u], __shfl_sync(0xffffffffu, y[q], k), y[q]);
+                    }
                 }
             }
-            if (tid < w0) ys[tid] = y;
+            if (tid < w0) {
+#pragma unroll
+                for (int q = 0; q < NR; ++q) ys[q * FMAX + tid] = y[q];
+            }
         }
         team_sync<NW>(team);
         if (tid >= 32) {
             if (tid < f) {
-                double acc = 0.0;
+                double acc[NR];
+#pragma unroll
+                for (int q = 0; q < NR; ++q) acc[q] = 0.0;
 #pragma unroll 8
-                for (int k = 0; k < w0; ++k) acc = fma(P[k * f + tid], ys[k], acc);
-                y -= acc;
+                for (int k = 0; k < w0; ++k) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) acc[q] = fma(P[k * f + tid], ys[q * FMAX + k], acc[q]);
+                }
+#pragma unroll
+                for (int q = 0; q < NR; ++q) y[q] -= acc[q];
             }
             for (int k0 = 32; k0 < w; k0 += 8) {
                 double l[8];
@@ -603,16 +702,23 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
 #pragma unroll
                 for (int u = 0; u < 8; ++u) {
                     const int k = k0 + u;
-                    if (k < w) y = fma(-l[u], __shfl_sync(0xffffffffu, y, k - 32), y);
+                    if (k < w) {
+#pragma unroll
+                        for (int q = 0; q < NR; ++q) y[q] = fma(-l[u], __shfl_sync(0xffffffffu, y[q], k - 32), y[q]);
+                    }
                 }
             }
         }
     }
     if (DEP) {
-        if (tid < f) slot_put(tid < w ? a.ypiv + d.col0 + tid : a.up + cvo + tid - w, y);
+        if constexpr (NR == 1) {
+            if (tid < f) slot_put(tid < w ? a.ypiv + d.col0 + tid : a.up + cvo + tid - w, y[0]);
+        } else {
+            if (tid < f) slot_put_block(tid < w ? a.ypiv + (d.col0 + tid) * NR : a.up + (cvo + tid - w) * NR, y);
+        }
         if (a.strace) { team_sync<NW>(team); if (tid == 0) a.strace[6 * (size_t)s + 2] = global_ns(); }
     } else {
-        if (tid < f) { if (tid < w) a.xp[d.col0 + tid] = y; else a.cbv[cvo + tid - w] = y; }
+        if (tid < f) { if (tid < w) a.xp[d.col0 + tid] = y[0]; else a.cbv[cvo + tid - w] = y[0]; }
         team_sync<NW>(team);
     }
 }
@@ -754,6 +860,181 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
     } else {
         if (tid < w) a.xp[d.col0 + tid] = t;
         team_sync<NW>(team);
+    }
+}
+
+// front_bwd_team<NW, true, PAIRS> for NR > 1 right-hand sides (k_solve_dep_block), as front_fwd_team<NW, true, NR>: every column goes
+// through the one-column operations in the same order.  (A separate function: an NR parameter on front_bwd_team changes the code
+// ptxas emits for the existing one-column kernels.)
+template <int NW, bool PAIRS, int NR>
+__device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, double* sm_team, int tid, int team, const ChildRec* childrec,
+                                                int* err, const double* dsub, int ncol, int64_t ldx) {
+    static_assert(NR % 2 == 0, "block slots are accessed in 16-byte pairs");
+    constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
+    double* xs = sm_team;                              // [NR][FMAX] gathered ancestor values at [xa, xa + r)
+    double* xb = xs + NR * FMAX;                       // [2][8]
+    ChildRec* recs = (ChildRec*)(xb + 16);             // [MAXC] the children, whose `down` slots this front fills
+    double* P = xb + 16 + 4 * MAXC;                    // row-major f x w panel (same slice layout as the forward sweep)
+    const FrontDesc d = a.desc[s];
+    const int f = d.f, w = d.w, r = f - w;
+    // xs is the whole front vector -- own pivots' x at [0, w), the ancestors' at [w, f) -- from which the children's hand-offs are
+    // gathered
+    const int xa = w;
+    {
+        const double* Lt = a.Lt + d.lp_off;
+        for (int e = tid; e < f * w; e += TEAM) cp_async8(P + e, Lt + e);
+    }
+    const int pj = (tid < w) ? a.perm[d.col0 + tid] : 0;
+    const double dinv = (tid < w) ? fast_rcp(a.dvec[d.col0 + tid]) : 0.0;
+    const int nc0 = min(MAXC, d.nchild);
+    int tg[MAXC];                                      // row of the front that child c's slot `tid` takes
+    double t[NR];
+    {
+        // the children's records and relative indices are constant: fetched before the wait, so that the hand-off to the
+        // children follows the back-substitution directly
+        if (tid < nc0) recs[tid] = childrec[d.child_off + tid];
+        team_sync<NW>(team);
+#pragma unroll
+        for (int c = 0; c < MAXC; ++c) tg[c] = (c < nc0 && tid < recs[c].rc) ? a.rel[recs[c].rel_off + tid] : -1;
+        // ancestor values (the parent's hand-off) and own forward result, at once
+        double* const p[2] = {a.down + (a.cbv_off[s] + tid) * NR, a.ypiv + (d.col0 + tid) * NR};
+        double v[2][NR];
+        slot_take_block(p, (tid < r ? 1u : 0u) | (tid < w ? 2u : 0u), v, err);
+#pragma unroll
+        for (int q = 0; q < NR; ++q) {
+            if (tid < r) xs[q * FMAX + xa + tid] = v[0][q];
+            t[q] = (tid < w) ? v[1][q] * dinv : 0.0;
+        }
+        if constexpr (PAIRS) {
+            // a block's partner row is in the same front: its forward value through xs[0, w), free until the back-substitution
+            if (tid < w) {
+#pragma unroll
+                for (int q = 0; q < NR; ++q) xs[q * FMAX + tid] = v[1][q];
+            }
+            team_sync<NW>(team);
+            const int i = d.col0 + tid;
+            const bool first = tid < w && dsub[i] != 0.0, second = tid < w && tid > 0 && dsub[i - 1] != 0.0;
+            if (first || second) {
+                const int i0 = first ? i : i - 1, k0 = first ? tid : tid - 1;
+                const double akm1k = dsub[i0], akm1 = a.dvec[i0] / akm1k, ak = a.dvec[i0 + 1] / akm1k;
+                const double denom = akm1 * ak - 1.0;
+#pragma unroll
+                for (int q = 0; q < NR; ++q) {
+                    const double bkm1 = xs[q * FMAX + k0] / akm1k, bk = xs[q * FMAX + k0 + 1] / akm1k;
+                    t[q] = first ? (ak * bkm1 - bk) / denom : (akm1 * bk - bkm1) / denom;
+                }
+            }
+        }
+    }
+    cp_async_wait_all();
+    team_sync<NW>(team);
+    {   // t_j -= sum_{i >= w} L(i,j) x_i : no recurrence
+        double acc[NR];
+#pragma unroll
+        for (int q = 0; q < NR; ++q) acc[q] = 0.0;
+        if (tid < w) {
+#pragma unroll 8
+            for (int i = 0; i < r; ++i) {
+#pragma unroll
+                for (int q = 0; q < NR; ++q) acc[q] = fma(P[(w + i) * w + tid], xs[q * FMAX + xa + i], acc[q]);
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < NR; ++q) t[q] -= acc[q];
+    }
+    // back-substitution with L11': x_k final -> t_j -= L(k,j) x_k for j < k
+    if (NW == 1) {
+        for (int k0 = w - 1; k0 >= 1; k0 -= 8) {
+            double l[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) { const int k = k0 - u; l[u] = (k >= 1 && tid < k) ? P[k * w + tid] : 0.0; }
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+                const int k = k0 - u;
+                if (k >= 1) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) t[q] = fma(-l[u], __shfl_sync(0xffffffffu, t[q], k), t[q]);
+                }
+            }
+        }
+    } else {
+        // blocked by warp (front_bwd_team): warp 1 finishes columns 32.. and publishes them in xs[32..w); warp 0 applies them
+        if (w > 32) {
+            if (tid >= 32) {
+                for (int k0 = w - 1; k0 >= 33; k0 -= 8) {
+                    double l[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { const int k = k0 - u; l[u] = (k >= 33 && tid < k) ? P[k * w + tid] : 0.0; }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        const int k = k0 - u;
+                        if (k >= 33) {
+#pragma unroll
+                            for (int q = 0; q < NR; ++q) t[q] = fma(-l[u], __shfl_sync(0xffffffffu, t[q], k - 32), t[q]);
+                        }
+                    }
+                }
+                if (tid < w) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) xs[q * FMAX + tid] = t[q];
+                }
+            }
+            team_sync<NW>(team);
+            if (tid < 32) {
+                double acc[NR];
+#pragma unroll
+                for (int q = 0; q < NR; ++q) acc[q] = 0.0;
+#pragma unroll 8
+                for (int k = 32; k < w; ++k) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) acc[q] = fma(P[k * w + tid], xs[q * FMAX + k], acc[q]);
+                }
+#pragma unroll
+                for (int q = 0; q < NR; ++q) t[q] -= acc[q];
+            }
+        }
+        if (tid < 32) {
+            for (int k0 = min(w, 32) - 1; k0 >= 1; k0 -= 8) {
+                double l[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) { const int k = k0 - u; l[u] = (k >= 1 && tid < k) ? P[k * w + tid] : 0.0; }
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                    const int k = k0 - u;
+                    if (k >= 1) {
+#pragma unroll
+                        for (int q = 0; q < NR; ++q) t[q] = fma(-l[u], __shfl_sync(0xffffffffu, t[q], k), t[q]);
+                    }
+                }
+            }
+        }
+    }
+    {
+        if (tid < w) {
+#pragma unroll
+            for (int q = 0; q < NR; ++q) {
+                xs[q * FMAX + tid] = t[q];
+                if (q < ncol) a.x[q * ldx + pj] = t[q];
+            }
+        }
+        team_sync<NW>(team);
+        // hand-off to the children: slot i of child c takes the front's value at row rel_c[i]
+        auto put_down = [&](int64_t cbv_off, int row) {
+            double v[NR];
+#pragma unroll
+            for (int q = 0; q < NR; ++q) v[q] = xs[q * FMAX + row];
+            slot_put_block(a.down + (cbv_off + tid) * NR, v);
+        };
+#pragma unroll
+        for (int c = 0; c < MAXC; ++c) if (tg[c] >= 0) put_down(recs[c].cbv_off, tg[c]);
+        for (int c0 = MAXC; c0 < d.nchild; c0 += MAXC) {          // (fronts with more than MAXC children)
+            const int nc = min(MAXC, d.nchild - c0);
+            team_sync<NW>(team);
+            if (tid < nc) recs[tid] = childrec[d.child_off + c0 + tid];
+            team_sync<NW>(team);
+            for (int c = 0; c < nc; ++c)
+                if (tid < recs[c].rc) put_down(recs[c].cbv_off, a.rel[recs[c].rel_off + tid]);
+        }
     }
 }
 
@@ -974,6 +1255,59 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const C
     __syncthreads();
     if (bad_sh) {
         for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
+        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
+    }
+}
+
+// k_solve_dep (PAIRS: k_solve_dep_pairs) for NR right-hand sides in one walk of the tree: the same tasks, tickets, count-out and
+// time-out path; every front stages its panel, descriptors, child records and relative indices once for all NR columns, and each
+// hand-off is a block slot of NR words (slot_take_block).  Column q is x + q * n; columns ncol .. NR-1 are padding, computed on zeros
+// and never read from or written to x.  Each column goes through the operations of the one-column kernel in the same order, so
+// column q of the result is bit-identical to a one-column solve of column q.  `slots` are the block slots (up | down | ypiv, NR words
+// per index); the {ticket, CTAs out} counters are k_solve_dep's.
+template <int NR, bool PAIRS>
+__global__ void __launch_bounds__(128) k_solve_dep_block(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
+                                                         int ncol, double* slots, int64_t nslot, const double* dsub) {
+    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
+    double (*sm1)[SolveSmem<1, NR>::doubles] = (double (*)[SolveSmem<1, NR>::doubles])smd;
+    __shared__ int tk_sh, bad_sh;
+    const int ntask = 2 * ds.ngroup;
+    for (;;) {
+        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
+        __syncthreads();
+        const int t = tk_sh;
+        if (t >= ntask) break;
+        const bool fwd = t < ds.ngroup;
+        const int g = fwd ? t : ntask - 1 - t;
+        const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
+        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
+        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        if (team < cnt) {
+            const int s = ds.tasks[t0 + team];
+            if (fwd) {
+                if (type == 1) front_fwd_team<1, true, NR>(a, childrec, s, sm1[team], tid, team, err, ncol, n);
+                else front_fwd_team<2, true, NR>(a, childrec, s, smd, tid, team, err, ncol, n);
+            } else {
+                if (type == 1) front_bwd_block<1, PAIRS, NR>(a, s, sm1[team], tid, team, childrec, err, dsub, ncol, n);
+                else front_bwd_block<2, PAIRS, NR>(a, s, smd, tid, team, childrec, err, dsub, ncol, n);
+            }
+        }
+        __syncthreads();                                // (tk_sh is rewritten by the next claim)
+    }
+    if (threadIdx.x == 0) {
+        bad_sh = 0;
+        __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
+        if (atomicAdd(ctl + 1, 1) == (int)gridDim.x - 1) {
+            atomicExch(ctl, 0);
+            atomicExch(ctl + 1, 0);
+            __threadfence();
+            bad_sh = *(volatile int*)err;
+        }
+    }
+    __syncthreads();
+    if (bad_sh) {
+        for (int q = 0; q < ncol; ++q)
+            for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[(int64_t)q * n + i] = __longlong_as_double((long long)CANON_NAN);
         for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
     }
 }

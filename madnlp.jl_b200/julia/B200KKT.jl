@@ -94,6 +94,16 @@ function solve_linear_system!(M::B200Solver{T}, x::CuVector{T}) where T
     return x
 end
 
+# the matrix method (src/LinearSolvers/linearsolvers.jl:102, CompactLBFGS's qn.H in src/IPM/factorization.jl:118): every column in
+# one b2_solve, which walks the elimination tree once per 8 columns instead of once per column
+function solve_linear_system!(M::B200Solver{T}, X::CuMatrix{T}) where T
+    stride(X, 2) == size(X, 1) || throw(ArgumentError("solve_linear_system!: X needs contiguous columns (stride(X, 2) == size(X, 1))"))
+    size(X, 2) == 0 && return X
+    check(ccall((:b2_solve, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, Int32, Ptr{Cvoid}), M.handle, pointer(X), Int32(size(X, 2)), stream_ptr()),
+          SolveException)
+    return X
+end
+
 is_inertia(::B200Solver) = true
 function inertia(M::B200Solver)
     p = Ref{Int64}(0); z = Ref{Int64}(0); n = Ref{Int64}(0)

@@ -80,6 +80,8 @@ class B200SparseSolver:
         return self
 
     def solve_linear_system(self, x):
+        """in place; a contiguous (nrhs, n) tensor is nrhs right-hand sides (column-major X with ld = n), solved in one b2_solve:
+        on the single-launch schedule one walk of the tree per 8 columns, each column bit-identical to its one-column solve"""
         assert x.is_cuda and x.dtype.is_floating_point and x.is_contiguous()
         nrhs = 1 if x.dim() == 1 else x.shape[0]
         check(lib.b2_solve(self._h, x.data_ptr(), nrhs, capi.stream_ptr(self.stream)))
