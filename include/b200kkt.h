@@ -742,6 +742,49 @@ int b2d_qn_state(b2d_qn* h, int32_t* instantiated, int32_t* accepted, double* sc
 /* Debug/test: host copies of bsk and r (n doubles each; r is written by DampedBFGS only); synchronises */
 int b2d_qn_debug_vectors(b2d_qn* h, double* bsk_h, double* rk_h, void* stream);
 
+/* ---- KrylovIterator: restarted GMRES preconditioned on the RIGHT by the KKT solve (x = M^-1 u, the preconditioned vectors kept).
+ * The caller runs solve_kkt! and mul! of its KKT type between these entries; one Arnoldi step k is
+ *     b2_krylov_scale(k, w)           v_k = w / s, z_k = v_k       (s = beta at k = 0, h_{k,k-1} after)
+ *     solve_kkt!(z_k) ; mul!(w, K, z_k, 1, 0)
+ *     b2_krylov_orthogonalize(k, w)   k + 2 modified Gram-Schmidt passes: h_{0..k,k}, h_{k+1,k}, the Givens update of g, the record
+ * and a cycle is b2_krylov_begin, steps k = 0, 1, ..., then b2_krylov_close followed by w -= K x and ||w||_inf into
+ * state[B2_KRYLOV_REC + B2_KRYLOV_REC_NORM_W] (b2_norm_inf, or a fused mul-norm).  The handle owns V ((restart + 1) x n) and Z
+ * (restart x n), contiguous with stride n, and the state below (device memory; doubles at these offsets).  No entry allocates or
+ * synchronises; reductions have a fixed order, so a captured sequence replays bit-identically.  One handle serves one stream at a
+ * time.  n >= 1, 1 <= restart <= 16. */
+#define B2_KRYLOV_MAX_RESTART 16
+#define B2_KRYLOV_H           0       /* 17 x 16 column-major: H, rotated into R in place */
+#define B2_KRYLOV_CS          272     /* 16: cosines of the rotations */
+#define B2_KRYLOV_SN          288     /* 16: sines */
+#define B2_KRYLOV_G           304     /* 17: the rotated beta e_1 */
+#define B2_KRYLOV_Y           321     /* 16: y of the last close */
+#define B2_KRYLOV_SCALE       337     /* the divisor of the next scale pass */
+#define B2_KRYLOV_REC         344     /* the record the host reads: */
+#define B2_KRYLOV_REC_EST     0       /*   |g_{k+1}| of the last step */
+#define B2_KRYLOV_REC_H       1       /*   h_{k+1,k} of the last step */
+#define B2_KRYLOV_REC_NORM_W  2       /*   ||b - K x||_inf after a close (accumulated by the caller's norm) */
+#define B2_KRYLOV_REC_NORM_X  3       /*   ||x||_inf after a close */
+#define B2_KRYLOV_REC_NORM_B  4       /*   ||b||_inf (first begin) */
+#define B2_KRYLOV_REC_NORM_B2 5       /*   ||b||_2 (first begin) */
+#define B2_KRYLOV_REC_LEN     8
+#define B2_KRYLOV_STATE_LEN   352
+typedef struct b2_krylov b2_krylov;
+int b2_krylov_create(int64_t n, int32_t restart, b2_krylov** out);
+int b2_krylov_destroy(b2_krylov* h);
+/* device pointers of V, Z and the state */
+int b2_krylov_buffers(b2_krylov* h, double** V_d, double** Z_d, double** state_d);
+/* start of a cycle.  first != 0: x = 0, w = b, the record zeroed, ||b||_inf and ||b||_2 into it.  Then beta = ||w||_2 and g = beta e_1
+ * (w holds r = b - K x; b and x are not read when first = 0).  2 launches (first) or 1 */
+int b2_krylov_begin(b2_krylov* h, int32_t first, const double* b_d, double* x_d, double* w_d, void* stream);
+/* v_k = z_k = w / s, 0 <= k < restart.  1 launch */
+int b2_krylov_scale(b2_krylov* h, int32_t k, const double* w_d, void* stream);
+/* w = K z_k on entry; MGS of w against v_0..v_k, h_{k+1,k} = ||w||_2, the Givens update and the record; w leaves as the unscaled
+ * v_{k+1}.  k + 2 launches */
+int b2_krylov_orthogonalize(b2_krylov* h, int32_t k, double* w_d, void* stream);
+/* close over m = k + 1 columns (1 <= m <= restart): y = R^-1 g (one warp), x += Z y, w = b, record NORM_W = 0 and
+ * NORM_X = ||x||_inf.  3 launches (a memset, the y solve and the pass) */
+int b2_krylov_close(b2_krylov* h, int32_t m, const double* b_d, double* x_d, double* w_d, void* stream);
+
 
 #ifdef __cplusplus
 }

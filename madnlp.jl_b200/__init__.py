@@ -11,6 +11,8 @@ Only what the hot path needs lives here (SURVEY.md section 8):
                   device dense quasi-Newton states of DenseKKTSystem and DenseCondensedKKTSystem)
   richardson, ipm the refinement loop and the `regular!` call-order replay used for the IPM-level metric, with the
                   InertiaBased (default), InertiaFree and InertiaIgnore regularisations
+  krylov          KrylovIterator: restarted GMRES refinement preconditioned on the right by the KKT solve (ipm's
+                  `iterator = "KrylovIterator"`)
   capture         the eager -> capture -> replay rule every CUDA graph of the host layer follows
   restoration     RobustRestorer: the feasibility restoration phase's state, kernels and reductions on the device
   barrier         the barrier update rules; AdaptiveBarrier: the quality-function and LOQO rules' new mu on the device
@@ -27,7 +29,7 @@ def __getattr__(name):
     # torch-dependent modules are imported lazily so that CPU-only tooling (ABI checks, symbolic analysis)
     # does not pay for `import torch`.
     import importlib
-    if name in ("kkt", "linear_solvers", "quasi_newton", "richardson", "ipm", "parallel", "restoration", "barrier",
+    if name in ("kkt", "linear_solvers", "quasi_newton", "richardson", "krylov", "ipm", "parallel", "restoration", "barrier",
                 "capture"):
         return importlib.import_module(f".{name}", __name__)
     raise AttributeError(name)

@@ -26,6 +26,9 @@ DUAL_INIT_NORM, DUAL_INIT_COPY, DUAL_INIT_RESULT_LEN = 0, 1, 2
 # the adaptive barrier's scalar array and b2_qf_search's result (B2_QF_* in include/b200kkt.h)
 QF_TAU, QF_NRM_PRIMAL, QF_NRM_DUAL, QF_MU_AVG, QF_SCAL_LEN = 0, 1, 2, 3, 4
 QF_SIGMA, QF_MU, QF_N_EVAL, QF_N_GS_ITER, QF_TOL_EXIT, QF_TRACE, QF_MAX_GS_ITER = 0, 1, 2, 3, 4, 8, 64
+# the Krylov iterator's state (B2_KRYLOV_* in include/b200kkt.h): offsets of y, of the record, and the record's entries
+KRYLOV_MAX_RESTART, KRYLOV_Y, KRYLOV_REC, KRYLOV_REC_LEN, KRYLOV_STATE_LEN = 16, 321, 344, 8, 352
+KREC_EST, KREC_H, KREC_NORM_W, KREC_NORM_X, KREC_NORM_B, KREC_NORM_B2 = 0, 1, 2, 3, 4, 5
 
 
 def qf_result_len(max_gs_iter):
@@ -268,6 +271,13 @@ PROTOTYPES = {
     "b2d_qn_rank2": (C.c_int, [_p, _p, _p, _p]),
     "b2d_qn_state": (C.c_int, [_p, C.POINTER(_i32), C.POINTER(_i32), _p, _p]),
     "b2d_qn_debug_vectors": (C.c_int, [_p, _p, _p, _p]),
+    "b2_krylov_create": (C.c_int, [_i64, _i32, _PP]),
+    "b2_krylov_destroy": (C.c_int, [_p]),
+    "b2_krylov_buffers": (C.c_int, [_p, _PP, _PP, _PP]),
+    "b2_krylov_begin": (C.c_int, [_p, _i32, _p, _p, _p, _p]),
+    "b2_krylov_scale": (C.c_int, [_p, _i32, _p, _p]),
+    "b2_krylov_orthogonalize": (C.c_int, [_p, _i32, _p, _p]),
+    "b2_krylov_close": (C.c_int, [_p, _i32, _p, _p, _p, _p]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

@@ -35,6 +35,7 @@ from .capi import CURV_PASS, CURV_RESULT_LEN, check, copy_many, lib, ptr
 from .capture import CapturedSequence
 from .kkt import SolverVectors, UnreducedKKTVector
 from .quasi_newton import ExactHessian
+from .krylov import KrylovIterator
 from .richardson import RichardsonIterator
 
 
@@ -103,10 +104,14 @@ class IPMLinearAlgebra:
 
     inertia_correction_method (MadNLP's option of the same name): "InertiaBased" (the default), "InertiaFree" (the curvature test
     of Chiang & Zavala; it reads solver_vectors, which load_ifr_inputs fills), "InertiaIgnore", or "InertiaAuto" (InertiaBased with every
-    solver of this package, since each reports inertia).  inertia_free_tol is the curvature test's tolerance (default 0)."""
+    solver of this package, since each reports inertia).  inertia_free_tol is the curvature test's tolerance (default 0).
+
+    iterator (MadNLP's option of the same name): "RichardsonIterator" (the default) or "KrylovIterator" (krylov.py: restarted GMRES
+    preconditioned on the right by the KKT solve, with krylov_options passed to it, e.g. krylov_restart, krylov_max_iter).  With
+    Krylov the first trial reads the inertia and then refines: the speculative first step is Richardson's."""
 
     def __init__(self, kkt, tol=1e-8, use_cuda_graph=True, speculate=True, inertia_correction_method="InertiaBased",
-                 inertia_free_tol=0.0):
+                 inertia_free_tol=0.0, iterator="RichardsonIterator", krylov_options=None):
         self.inertia_correction_method = resolve_inertia_correction_method(inertia_correction_method, kkt.linear_solver)
         self.inertia_free_tol = float(inertia_free_tol)
         self.kkt = kkt
@@ -114,7 +119,12 @@ class IPMLinearAlgebra:
         self.speculate = speculate     # first refinement step queued before the inertia is known (see step())
         self._prologue_graph = CapturedSequence(use_cuda_graph)
         self._rr_graph = CapturedSequence(use_cuda_graph)      # restoration_step's prologue
-        self.iterator = RichardsonIterator(kkt, tol=tol, use_cuda_graph=use_cuda_graph)
+        if iterator == "RichardsonIterator":
+            self.iterator = RichardsonIterator(kkt, tol=tol, use_cuda_graph=use_cuda_graph)
+        elif iterator == "KrylovIterator":
+            self.iterator = KrylovIterator(kkt, tol=tol, use_cuda_graph=use_cuda_graph, **(krylov_options or {}))
+        else:
+            raise ValueError(f"iterator must be RichardsonIterator or KrylovIterator; got {iterator!r}")
         self.d = UnreducedKKTVector.for_kkt(kkt)
         self.p = UnreducedKKTVector.for_kkt(kkt)
         self.w = UnreducedKKTVector.for_kkt(kkt)
@@ -405,7 +415,7 @@ class IPMLinearAlgebra:
         k, r = self.kkt, self.ifr
         if self.inertia_correction_method == "InertiaBased":
             ls = k.linear_solver
-            if first and self.speculate and hasattr(ls, "inertia_enqueue"):
+            if first and self.speculate and hasattr(ls, "inertia_enqueue") and isinstance(self.iterator, RichardsonIterator):
                 ls.inertia_enqueue()
                 self.iterator.start(self.d, self.p, self.w)
                 torch.cuda.current_stream().synchronize()

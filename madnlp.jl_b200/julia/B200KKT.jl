@@ -473,6 +473,112 @@ function b200_richardson_update!(b::CuVector{T}, w::CuVector{T}, x::CuVector{T},
         length(b), pointer(b), pointer(w), pointer(x), pointer(norms), stream_ptr()), SolveException)
 end
 
+# ---------------------------------------------------------------------------------------------------------------------
+# B200KrylovIterator: restarted GMRES preconditioned on the RIGHT by solve_kkt! (csrc/krylov.cu, madnlp.jl_b200/krylov.py), an
+# alternative to RichardsonIterator:  madnlp(nlp; iterator = B200KKT.B200KrylovIterator, ...).  It stops and accepts with
+# Richardson's residual ratio (tol^(5/4), tol^(5/8)), unlike MadNLPKrylov, which preconditions on the left and stops on the
+# absolute norm of the preconditioned residual.  solve_kkt! and mul! are MadNLP's own (they dispatch to this package's overloads);
+# everything else goes through the b2_krylov_* entries.  NOT RUN here, like the rest of this file.
+# ---------------------------------------------------------------------------------------------------------------------
+Base.@kwdef mutable struct B200KrylovOptions <: AbstractOptions
+    krylov_restart::Int = 5
+    krylov_max_iter::Int = 10
+    krylov_tol::Float64 = 1e-10
+    krylov_acceptable_tol::Float64 = 1e-5
+end
+
+mutable struct B200KrylovIterator{T, KKT} <: MadNLP.AbstractIterator{T}
+    kkt::KKT
+    opt::B200KrylovOptions
+    cnt::Any
+    logger::Any
+    handle::Ptr{Cvoid}
+    Z::Vector{Any}                     # UnreducedKKTVectors over the rows of Z
+    state::CuVector{T}                 # wraps the handle's state (B2_KRYLOV_STATE_LEN doubles)
+    rec::Vector{T}                     # page-locked host copy of the record (CUDA.pin)
+end
+
+const B2_KRYLOV_REC, B2_KRYLOV_STATE_LEN = 344, 352
+const KREC_EST, KREC_H, KREC_NORM_W, KREC_NORM_X, KREC_NORM_B, KREC_NORM_B2 = 1, 2, 3, 4, 5, 6    # 1-based
+
+default_options(::Type{B200KrylovIterator}, tol) = B200KrylovOptions(krylov_tol = tol^(5/4), krylov_acceptable_tol = tol^(5/8))
+
+function B200KrylovIterator(kkt; opt = B200KrylovOptions(), logger = MadNLP.MadNLPLogger(), cnt = nothing)
+    T = eltype(kkt.pr_diag)
+    N = length(kkt.pr_diag) + length(kkt.du_diag) + length(kkt.l_diag) + length(kkt.u_diag)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:b2_krylov_create, libb200kkt), Cint, (Int64, Int32, Ptr{Ptr{Cvoid}}), N, opt.krylov_restart, h), SolveException)
+    V = Ref{Ptr{Cvoid}}(C_NULL); Zp = Ref{Ptr{Cvoid}}(C_NULL); S = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:b2_krylov_buffers, libb200kkt), Cint, (Ptr{Cvoid}, Ptr{Ptr{Cvoid}}, Ptr{Ptr{Cvoid}}, Ptr{Ptr{Cvoid}}), h[], V, Zp, S),
+          SolveException)
+    wrap(p, n) = unsafe_wrap(CuArray, CuPtr{T}(UInt(p)), n)
+    n, m, nlb, nub = length(kkt.pr_diag), length(kkt.du_diag), length(kkt.l_diag), length(kkt.u_diag)
+    # the fields of MadNLP.UnreducedKKTVector (src/KKT/rhs.jl), built over row k of Z as its allocating constructor builds them
+    function zvec(k)
+        values = wrap(Zp[] + (k - 1) * N * sizeof(T), N)
+        x = MadNLP._madnlp_unsafe_wrap(values, n + m)
+        xp = MadNLP._madnlp_unsafe_wrap(values, n)
+        xl = MadNLP._madnlp_unsafe_wrap(values, m, n + 1)
+        xzl = MadNLP._madnlp_unsafe_wrap(values, nlb, n + m + 1)
+        xzu = MadNLP._madnlp_unsafe_wrap(values, nub, n + m + nlb + 1)
+        return MadNLP.UnreducedKKTVector(values, x, xp, view(xp, kkt.ind_lb), view(xp, kkt.ind_ub), xl, xzl, xzu)
+    end
+    Z = [zvec(k) for k in 1:opt.krylov_restart]
+    it = B200KrylovIterator{T, typeof(kkt)}(kkt, opt, cnt, logger, h[], Z, wrap(S[], B2_KRYLOV_STATE_LEN),
+                                            CUDA.pin(Vector{T}(undef, 8)))
+    finalizer(x -> ccall((:b2_krylov_destroy, libb200kkt), Cint, (Ptr{Cvoid},), x.handle), it)
+    return it
+end
+
+function _krylov_record!(it::B200KrylovIterator)
+    copyto!(it.rec, 1, it.state, B2_KRYLOV_REC + 1, 8)       # synchronises
+    return it.rec
+end
+
+function MadNLP.solve_refine!(x::MadNLP.AbstractKKTVector{T}, it::B200KrylovIterator{T}, b::MadNLP.AbstractKKTVector{T},
+                              w::MadNLP.AbstractKKTVector{T}) where T
+    kkt, o, h = it.kkt, it.opt, it.handle
+    xv, bv, wv = MadNLP.full(x), MadNLP.full(b), MadNLP.full(w)
+    ir = 0
+    check(ccall((:b2_krylov_begin, libb200kkt), Cint, (Ptr{Cvoid}, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                h, 1, pointer(bv), pointer(xv), pointer(wv), stream_ptr()), SolveException)
+    norm_b = norm_b2 = -one(T)
+    ratio = zero(T)
+    while true
+        k = 0
+        while true
+            check(ccall((:b2_krylov_scale, libb200kkt), Cint, (Ptr{Cvoid}, Int32, CuPtr{T}, Ptr{Cvoid}), h, k, pointer(wv), stream_ptr()),
+                  SolveException)
+            MadNLP.solve_kkt!(kkt, it.Z[k + 1])
+            MadNLP.mul!(w, kkt, it.Z[k + 1], one(T), zero(T))
+            check(ccall((:b2_krylov_orthogonalize, libb200kkt), Cint, (Ptr{Cvoid}, Int32, CuPtr{T}, Ptr{Cvoid}), h, k, pointer(wv),
+                        stream_ptr()), SolveException)
+            rec = _krylov_record!(it)
+            # ||b|| arrives with the first step's record (one read per Arnoldi iteration); for b = 0 that step ran on zeros
+            if norm_b < 0
+                norm_b, norm_b2 = rec[KREC_NORM_B], rec[KREC_NORM_B2]
+                norm_b == 0 && (it.cnt !== nothing && (it.cnt.ir = 0); return true)
+            end
+            ir += 1
+            (k + 1 == o.krylov_restart || ir >= o.krylov_max_iter || rec[KREC_H] == 0 ||
+             rec[KREC_EST] <= o.krylov_tol * norm_b2) && break
+            k += 1
+        end
+        check(ccall((:b2_krylov_close, libb200kkt), Cint, (Ptr{Cvoid}, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                    h, k + 1, pointer(bv), pointer(xv), pointer(wv), stream_ptr()), SolveException)
+        MadNLP.mul!(w, kkt, x, -one(T), one(T))
+        check(ccall((:b2_norm_inf, libb200kkt), Cint, (Int64, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}), length(wv), pointer(wv),
+                    pointer(it.state, B2_KRYLOV_REC + KREC_NORM_W), stream_ptr()), SolveException)
+        rec = _krylov_record!(it)
+        ratio = rec[KREC_NORM_W] / (min(rec[KREC_NORM_X], 1e6 * norm_b) + norm_b)
+        (ratio < o.krylov_tol || ir >= o.krylov_max_iter) && break
+        check(ccall((:b2_krylov_begin, libb200kkt), Cint, (Ptr{Cvoid}, Int32, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+                    h, 0, C_NULL, C_NULL, pointer(wv), stream_ptr()), SolveException)
+    end
+    it.cnt !== nothing && (it.cnt.ir = ir)
+    return ratio < o.krylov_acceptable_tol
+end
+
 # inertia read split in two (queue more work behind factorize!, block once): b2_inertia_enqueue / b2_inertia_fetch
 inertia_enqueue!(M::B200Solver) = check(ccall((:b2_inertia_enqueue, libb200kkt), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), M.handle, stream_ptr()), FactorizationException)
 function inertia_fetch(M::B200Solver)

@@ -111,13 +111,14 @@ def _bounds(n_tot, ind_lb, ind_ub):
 class UnreducedKKTVector:
     """src/KKT/rhs.jl:90-129: one contiguous device buffer [x (n_tot) | y (m) | zl (nlb) | zu (nub)] with views."""
 
-    def __init__(self, n, m, nlb, nub):
+    def __init__(self, n, m, nlb, nub, values=None):
+        """values: an existing float64 device tensor of n + m + nlb + nub entries to view (default: a new zero buffer)"""
         self.n, self.m, self.nlb, self.nub = int(n), int(m), int(nlb), int(nub)
-        self.values = _dz(n + m + nlb + nub)
+        self.values = _dz(n + m + nlb + nub) if values is None else values
 
     @classmethod
-    def for_kkt(cls, kkt):
-        return cls(len(kkt.pr_diag), len(kkt.du_diag), len(kkt.l_diag), len(kkt.u_diag))
+    def for_kkt(cls, kkt, values=None):
+        return cls(len(kkt.pr_diag), len(kkt.du_diag), len(kkt.l_diag), len(kkt.u_diag), values)
 
     def full(self):
         return self.values
