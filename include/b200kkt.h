@@ -43,6 +43,7 @@ extern "C" {
 #define B2_ERR_FACTORIZATION  4   /* numeric failure         (FactorizationException, linearsolvers.jl:134) */
 #define B2_ERR_SOLVE          5   /* solve before factorize  (SolveException,         linearsolvers.jl:135) */
 #define B2_ERR_NO_DEVICE      6   /* no CUDA device: the product path has no CPU fallback */
+#define B2_ERR_UNSUPPORTED    7   /* the driver refuses a feature the entry needs (e.g. CUDA graph conditional nodes) */
 
 #define B2_ORDER_METIS_ND 0   /* nested dissection (METIS_NodeND, statically linked)        */
 #define B2_ORDER_MINDEG   1   /* built-in minimum-degree                                    */
@@ -784,6 +785,51 @@ int b2_krylov_orthogonalize(b2_krylov* h, int32_t k, double* w_d, void* stream);
 /* close over m = k + 1 columns (1 <= m <= restart): y = R^-1 g (one warp), x += Z y, w = b, record NORM_W = 0 and
  * NORM_X = ||x||_inf.  3 launches (a memset, the y solve and the pass) */
 int b2_krylov_close(b2_krylov* h, int32_t m, const double* b_d, double* x_d, double* w_d, void* stream);
+
+/* ---- Richardson refinement as ONE CUDA graph (solve_refine!, src/LinearSolvers/backsolve.jl:27-76, for the first trial of
+ * inertia_correction!): the loop body runs under a conditional WHILE node and a one-thread test kernel decides on the device
+ * whether it runs again, so the host waits once per solve instead of once per refinement step.  The graph is
+ *     b2_richardson_begin (||b||, x = 0, w = b) ; WHILE { caller's step ; test }
+ * Building it:  b2_refine_loop_begin(h, ...)  -- captures the part before the WHILE node and starts capturing its body on `stream`
+ *               the caller issues one refinement step on `stream` (x += M^-1 w ; w = b - K x ; norms_d[0] = ||w||, norms_d[1] = ||x||)
+ *               b2_refine_loop_end(h, ...)    -- issues the test, ends the capture, instantiates
+ * then b2_refine_loop_launch(h, stream) replays it.  The last test writes the solve's record to pinned host memory, its sequence
+ * number last; b2_refine_loop_wait returns as soon as that record is there (before the graph's completion reaches the host, and
+ * also after any D2H copy queued on the stream before the launch), and b2_refine_loop_record reads it.  The test applies solve_refine!'s stopping rule in the same IEEE operations,
+ *     ratio = ||w|| / (min(||x||, 1e6 ||b||) + ||b||) ; ir += 1 ; stop when ir >= max_iter or ratio < tol
+ * (||b|| == 0: one step, ir = 0, ratio = 0), and also stops after the first step when the factorisation's inertia, read from the
+ * solver's device counters (b2_inertia_source), fails the KKT type's is_inertia_correct: num_zero == 0 and, where given (>= 0),
+ * num_pos == expect_pos and num_neg == expect_neg.  B2_ERR_UNSUPPORTED from begin / end: the driver refuses conditional graph
+ * nodes (the caller refines on the host); the stream is left out of capture. */
+typedef struct b2_inertia_source {
+    const int32_t* counters_d;    /* the solver's device pivot counters, written by its factorisation */
+    int64_t n;                    /* order of the factored matrix: num_pos = n - num_neg - num_zero */
+    int32_t neg[2], zero[2];      /* num_neg = the sum of counters_d[neg[k]] over the k with neg[k] >= 0; num_zero likewise */
+    int32_t fail;                 /* counters_d[fail] != 0: a device-wide wait timed out, the factorisation is not valid */
+    int32_t reserved;
+} b2_inertia_source;
+int b2_inertia_source_get(b2_solver* s, b2_inertia_source* out);       /* single-part solvers only */
+typedef struct b2_refine_record {
+    double ratio;                 /* residual ratio of the last step (0 when ||b|| == 0) */
+    double norm_w, norm_x, norm_b;
+    int64_t ir;                   /* steps counted by the stopping rule (solve_refine!'s cnt.ir) */
+    int64_t steps;                /* steps run */
+    int64_t num_pos, num_zero, num_neg;
+    int32_t inertia_ok;           /* the inertia test of the first step */
+    int32_t fail;                 /* counters_d[fail] of the first step */
+    int64_t seq;                  /* solves this handle has finished, written last */
+} b2_refine_record;
+typedef struct b2_refine_loop b2_refine_loop;
+int b2_refine_loop_create(b2_refine_loop** out);
+int b2_refine_loop_destroy(b2_refine_loop* h);
+/* any graph the handle held is dropped; b, w, x, norms_d (3 doubles: ||w||, ||x||, ||b||) are baked into the graph */
+int b2_refine_loop_begin(b2_refine_loop* h, int64_t n, const double* b_d, double* w_d, double* x_d, double* norms_d, void* stream);
+int b2_refine_loop_end(b2_refine_loop* h, const b2_inertia_source* src, int64_t expect_pos, int64_t expect_neg, int32_t max_iter,
+                       double tol, void* stream);
+int b2_refine_loop_launch(b2_refine_loop* h, void* stream);
+/* wait for the record of the last launch: polls it and the stream; an error of the stream is returned, not waited for */
+int b2_refine_loop_wait(b2_refine_loop* h);
+int b2_refine_loop_record(b2_refine_loop* h, b2_refine_record* out);
 
 
 #ifdef __cplusplus

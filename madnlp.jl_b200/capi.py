@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libb200kkt.so")
 
 B2_OK = 0
-B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE, B2_ERR_NO_DEVICE = 1, 2, 3, 4, 5, 6
+B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE, B2_ERR_NO_DEVICE, B2_ERR_UNSUPPORTED = 1, 2, 3, 4, 5, 6, 7
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
 B2_DENSE_PIVOT_STATIC, B2_DENSE_PIVOT_BUNCH_KAUFMAN = 0, 1
@@ -87,6 +87,19 @@ class Stats(C.Structure):
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class InertiaSource(C.Structure):
+    """b2_inertia_source: where a solver's factorisation leaves its pivot counts on the device"""
+    _fields_ = [("counters_d", C.c_void_p), ("n", C.c_int64), ("neg", C.c_int32 * 2), ("zero", C.c_int32 * 2), ("fail", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class RefineRecord(C.Structure):
+    """b2_refine_record: what one launch of a refinement-loop graph leaves in pinned host memory"""
+    _fields_ = [("ratio", C.c_double), ("norm_w", C.c_double), ("norm_x", C.c_double), ("norm_b", C.c_double), ("ir", C.c_int64),
+                ("steps", C.c_int64), ("num_pos", C.c_int64), ("num_zero", C.c_int64), ("num_neg", C.c_int64), ("inertia_ok", C.c_int32),
+                ("fail", C.c_int32), ("seq", C.c_int64)]
 
 
 class SymbolicSizes(C.Structure):
@@ -278,6 +291,14 @@ PROTOTYPES = {
     "b2_krylov_scale": (C.c_int, [_p, _i32, _p, _p]),
     "b2_krylov_orthogonalize": (C.c_int, [_p, _i32, _p, _p]),
     "b2_krylov_close": (C.c_int, [_p, _i32, _p, _p, _p, _p]),
+    "b2_inertia_source_get": (C.c_int, [_p, C.POINTER(InertiaSource)]),
+    "b2_refine_loop_create": (C.c_int, [_PP]),
+    "b2_refine_loop_destroy": (C.c_int, [_p]),
+    "b2_refine_loop_begin": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
+    "b2_refine_loop_end": (C.c_int, [_p, C.POINTER(InertiaSource), _i64, _i64, _i32, _f64, _p]),
+    "b2_refine_loop_launch": (C.c_int, [_p, _p]),
+    "b2_refine_loop_wait": (C.c_int, [_p]),
+    "b2_refine_loop_record": (C.c_int, [_p, C.POINTER(RefineRecord)]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

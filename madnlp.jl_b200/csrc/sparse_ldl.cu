@@ -941,6 +941,14 @@ int b2_inertia_fetch(b2_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t*
     return B2_OK;
 }
 
+// the counters b2_inertia_fetch reads, for a device-side inertia test (b2_refine_loop_end)
+int b2_inertia_source_get(b2_solver* s, b2_inertia_source* out) {
+    if (!s || s->symbolic_only || !out) { set_error("b2_inertia_source_get: invalid argument"); return B2_ERR_INVALID; }
+    if (s->opt.n_parts > 1) { set_error("b2_inertia_source_get: a multi-part solver's counters hold one rank's view only"); return B2_ERR_INVALID; }
+    *out = b2_inertia_source{s->d_counters.p, (int64_t)s->S.n, {0, 2}, {1, 3}, 4, 0};
+    return B2_OK;
+}
+
 int b2_inertia(b2_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg, void* stream) {
     int rc = b2_inertia_enqueue(s, stream);
     if (rc != B2_OK) return rc;

@@ -418,7 +418,7 @@ class IPMLinearAlgebra:
             if first and self.speculate and hasattr(ls, "inertia_enqueue") and isinstance(self.iterator, RichardsonIterator):
                 ls.inertia_enqueue()
                 self.iterator.start(self.d, self.p, self.w)
-                torch.cuda.current_stream().synchronize()
+                self.iterator.wait()
                 inertia = ls.inertia_fetch()
                 if not k.is_inertia_correct(*inertia):
                     self.iterator.discard()

@@ -543,6 +543,11 @@ class SparseCondensedKKTSystem(_KKTBase):
         """condensed.jl:138-140."""
         return num_zero == 0 and num_pos == self.n
 
+    def inertia_rule(self):
+        """is_inertia_correct as data, for the test on the device that ends a refinement-loop graph (richardson.py):
+        num_zero == 0 and (num_pos, num_neg) == this pair where not None"""
+        return self.n, None
+
     def should_regularize_dual(self, num_pos, num_zero, num_neg):
         return True                                                    # condensed.jl:141
 

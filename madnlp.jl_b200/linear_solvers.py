@@ -104,6 +104,12 @@ class B200SparseSolver:
         check(lib.b2_inertia_fetch(self._h, C.byref(p), C.byref(z), C.byref(n)))
         return (p.value, z.value, n.value)
 
+    def inertia_source(self):
+        """where the factorisation leaves the pivot counts on the device (capi.InertiaSource), for an inertia test on the device"""
+        src = capi.InertiaSource()
+        check(lib.b2_inertia_source_get(self._h, C.byref(src)))
+        return src
+
     def improve(self) -> bool:
         ch = C.c_int32(0)
         check(lib.b2_improve(self._h, C.byref(ch)))

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Where one IPM step of the headline workload spends its time: CUDA-event and host-clock durations of its segments
 (load_iterate | prologue graph = assembly + factorisation | first refinement step | further steps), medians over the
-24 iterates after warm-up, L2 flushed before each step like bench.py."""
+24 iterates after warm-up, L2 flushed before each step like bench.py.  Where the refinement loop runs as one graph
+(richardson.py), `first` is the whole loop and `more` the host's turn-around after it."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "oracle")):
