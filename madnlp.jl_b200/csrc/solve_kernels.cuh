@@ -45,6 +45,26 @@ __global__ void k_perm_out(int n, const int32_t* __restrict__ perm, const double
     pdl_sync();
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) x[perm[i]] = xp[i];
 }
+// NR right-hand sides (the level-launch block solve): column q of x at x + q * n, xp holding the NR columns interleaved at [i * NR + q].
+// Columns ncol .. NR-1 of xp are padding and start at zero; they are never written back.
+template <int NR>
+__global__ void k_perm_in_block(int n, int ncol, const int32_t* __restrict__ perm, const double* __restrict__ x, double* __restrict__ xp) {
+    pdl_sync();
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int p = perm[i];
+#pragma unroll
+        for (int q = 0; q < NR; ++q) xp[(size_t)i * NR + q] = q < ncol ? x[(size_t)q * n + p] : 0.0;
+    }
+}
+template <int NR>
+__global__ void k_perm_out_block(int n, int ncol, const int32_t* __restrict__ perm, const double* __restrict__ xp, double* __restrict__ x) {
+    pdl_sync();
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int p = perm[i];
+#pragma unroll
+        for (int q = 0; q < NR; ++q) if (q < ncol) x[(size_t)q * n + p] = xp[(size_t)i * NR + q];
+    }
+}
 // masked variant for the multi-GPU back-substitution: only rows this rank finalises are written, others zeroed
 __global__ void k_perm_out_masked(int n, const int32_t* __restrict__ perm, const uint8_t* __restrict__ mask_p,
                                   const double* __restrict__ xp, double* __restrict__ x) {

@@ -44,6 +44,8 @@ struct Phase {
     // its block form (k_solve_dep_block) for 2, 4 and 8 right-hand sides per walk: persistent CTAs of each width
     int sol_grid_blk[3] = {0, 0, 0};
     cudaGraphExec_t g_factor = nullptr, g_fwd = nullptr, g_bwd = nullptr;
+    // the level-launch block solve's two sweeps for 2, 4 and 8 right-hand sides, one graph per width (captured on first use)
+    cudaGraphExec_t g_blk[3] = {nullptr, nullptr, nullptr};
     int64_t n_factor_launches = 0, n_solve_launches = 0;
     int64_t n_fused_fronts = 0;
 };
@@ -76,6 +78,9 @@ struct b2_solver {
     // the same three slot arrays for the block solve (k_solve_dep_block), 8 words per index so that every width fits: up [8 sum r] |
     // down [8 sum r] | ypiv [8 n].  Allocated with d_slots, since b2_solve may be captured into a caller's CUDA graph.
     DevBuf<double> d_bslots;
+    // the level-launch block solve's (b2_solve, nrhs > 1, on a tree that is not single-launch) xp [8 n] | side [8 n] | cbv [8 sum r],
+    // a width-NR solve holding NR interleaved columns at the start of each.  Allocated at creation for the same reason as d_bslots.
+    DevBuf<double> d_xblk;
     // B2_SPARSE_PIVOT_PAIRS: per-supernode mask of the columns where a candidate 2 x 2 pivot starts; D's subdiagonal and the pivot
     // kinds (B2_PIVOT_*) of the last factorisation, permuted order
     bool pairs = false;
@@ -98,6 +103,7 @@ struct b2_solver {
             if (p.g_factor) cudaGraphExecDestroy(p.g_factor);
             if (p.g_fwd) cudaGraphExecDestroy(p.g_fwd);
             if (p.g_bwd) cudaGraphExecDestroy(p.g_bwd);
+            for (cudaGraphExec_t g : p.g_blk) if (g) cudaGraphExecDestroy(g);
         }
         if (cap_stream) cudaStreamDestroy(cap_stream);
         if (h_counters) cudaFreeHost(h_counters);
@@ -228,8 +234,18 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
     return nl;
 }
 
+// one sweep of phase `ph`, level by level.  NR = 1: the one-column solve on xp / cbv.  NR > 1: the block kernels on NR interleaved
+// columns of the block workspace (d_xblk), with the same launches as NR = 1.
+template <int NR>
 int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
     SolveArgs a = solve_args(s);
+    BigSolveArgs bs = big_solve_args(s);
+    if constexpr (NR > 1) {
+        const int64_t n = s->S.n;
+        a.xp = bs.s.xp = s->d_xblk.p;
+        bs.side = s->d_xblk.p + 8 * n;
+        a.cbv = bs.s.cbv = s->d_xblk.p + 16 * n;
+    }
     const int32_t* sched = s->d_sched.p;
     int64_t nl = 0;
     const Phase& P = s->phase[ph];
@@ -247,17 +263,32 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
         const ChildRec* cr = s->d_childrec.p;
         const WarpSched wsched = warp_sched(s, L);
         if (L.nw == 1 && fused) {     // bottom subtrees: more one-warp teams per CTA, fewer sequential rounds per stage
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, SOLVE_FUSED_TEAMS * 32, (size_t)SOLVE_FUSED_TEAMS * SolveSmem<1>::doubles * sizeof(double));
-            if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1, SOLVE_FUSED_TEAMS>, a, cr, wsched);
-            else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1, SOLVE_FUSED_TEAMS>, a, wsched);
+            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, SOLVE_FUSED_TEAMS * 32, (size_t)SOLVE_FUSED_TEAMS * SolveSmem<1, NR>::doubles * sizeof(double));
+            if constexpr (NR == 1) {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1, SOLVE_FUSED_TEAMS>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1, SOLVE_FUSED_TEAMS>, a, wsched);
+            } else {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, a, wsched);
+            }
         } else if (L.nw == 1) {
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, FW_WARPS * 32, (size_t)FW_WARPS * SolveSmem<1>::doubles * sizeof(double));
-            if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1>, a, cr, wsched);
-            else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1>, a, wsched);
+            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, FW_WARPS * 32, (size_t)FW_WARPS * SolveSmem<1, NR>::doubles * sizeof(double));
+            if constexpr (NR == 1) {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1>, a, wsched);
+            } else {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<1, FW_WARPS, NR>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<1, FW_WARPS, NR>, a, wsched);
+            }
         } else {
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, 64, (size_t)SolveSmem<2>::doubles * sizeof(double));
-            if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<2>, a, cr, wsched);
-            else cudaLaunchKernelEx(&cfg, k_bwd_warp2<2>, a, wsched);
+            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, 64, (size_t)SolveSmem<2, NR>::doubles * sizeof(double));
+            if constexpr (NR == 1) {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<2>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<2>, a, wsched);
+            } else {
+                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<2, 1, NR>, a, cr, wsched);
+                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<2, 1, NR>, a, wsched);
+            }
         }
         ++nl;
     };
@@ -269,27 +300,42 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
         if (lv.W.n_cta) warp_launch(lv.W);
         if (lv.W2.n_cta) warp_launch(lv.W2);
         if (lv.nC) {
-            const BigSolveArgs bs = big_solve_args(s);
             const int32_t* lc = sched + lv.offC;
             const int nblk = (lv.maxwC + BS - 1) / BS;
+            const size_t fsm = (size_t)bs_smem_doubles<NR>() * sizeof(double), bsm = (size_t)NR * BS * sizeof(double);
             if (forward) {
-                k_bs_fwd_init<<<lv.nC, 1024, 0, st>>>(bs, lc);
-                k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, 0, 0);
+                if constexpr (NR == 1) {
+                    k_bs_fwd_init<<<lv.nC, 1024, 0, st>>>(bs, lc);
+                    k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, 0, 0);
+                } else {
+                    k_bs_fwd_init_block<NR><<<lv.nC, 1024, 0, st>>>(bs, lc);
+                    k_bs_head_block<NR><<<lv.nC, BS_NT, fsm, st>>>(bs, lc, 0, 0);
+                }
                 nl += 2;
                 for (int b = 0; b < nblk; ++b) {
                     const int rows = std::max(1, lv.maxfC - b * BS - 1);
-                    k_bs_fwd<<<dim3((rows + BSF_ROWS - 1) / BSF_ROWS, lv.nC), BS_NT, 0, st>>>(bs, lc, b);
+                    const dim3 grid((rows + BSF_ROWS - 1) / BSF_ROWS, lv.nC);
+                    if constexpr (NR == 1) k_bs_fwd<<<grid, BS_NT, 0, st>>>(bs, lc, b);
+                    else k_bs_fwd_block<NR><<<grid, BS_NT, fsm, st>>>(bs, lc, b);
                     ++nl;
                 }
             } else {
-                k_bs_bwd_init<<<dim3((lv.maxwC + 7) / 8, lv.nC), 256, 0, st>>>(bs, lc);
-                k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, -1, 1);
+                const dim3 ginit((lv.maxwC + 7) / 8, lv.nC), gfin((lv.maxwC + 255) / 256, lv.nC);
+                if constexpr (NR == 1) {
+                    k_bs_bwd_init<<<ginit, 256, 0, st>>>(bs, lc);
+                    k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, -1, 1);
+                } else {
+                    k_bs_bwd_init_block<NR><<<ginit, 256, 0, st>>>(bs, lc);
+                    k_bs_head_block<NR><<<lv.nC, BS_NT, bsm, st>>>(bs, lc, -1, 1);
+                }
                 nl += 2;
                 for (int b = nblk - 1; b >= 1; --b) {
-                    k_bs_bwd<<<dim3(b, lv.nC), BS_NT, 0, st>>>(bs, lc, b);
+                    if constexpr (NR == 1) k_bs_bwd<<<dim3(b, lv.nC), BS_NT, 0, st>>>(bs, lc, b);
+                    else k_bs_bwd_block<NR><<<dim3(b, lv.nC), BS_NT, bsm, st>>>(bs, lc, b);
                     ++nl;
                 }
-                k_bs_bwd_finish<<<dim3((lv.maxwC + 255) / 256, lv.nC), 256, 0, st>>>(bs, lc);
+                if constexpr (NR == 1) k_bs_bwd_finish<<<gfin, 256, 0, st>>>(bs, lc);
+                else k_bs_bwd_finish_block<NR><<<gfin, 256, 0, st>>>(bs, lc);
                 ++nl;
             }
         }
@@ -354,6 +400,20 @@ void enqueue_solve_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
                                                                  s->S.n, ncol, s->d_bslots.p, (int64_t)s->d_bslots.n, s->d_dsub.p);
 }
 
+// the level-launch block kernels of one width: dynamic shared memory above the 48 KB default
+template <int NR>
+cudaError_t set_level_block_attrs() {
+    const void* k[] = {(const void*)k_fwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, (const void*)k_bwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>,
+                       (const void*)k_fwd_warp2_block<1, FW_WARPS, NR>, (const void*)k_bwd_warp2_block<1, FW_WARPS, NR>,
+                       (const void*)k_fwd_warp2_block<2, 1, NR>, (const void*)k_bwd_warp2_block<2, 1, NR>,
+                       (const void*)k_bs_head_block<NR>, (const void*)k_bs_fwd_block<NR>, (const void*)k_bs_bwd_block<NR>};
+    for (const void* f : k) {
+        cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
 int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_front_smem<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
@@ -368,6 +428,9 @@ int set_smem_attrs() {
     B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_solve_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     B2_CUDA(cudaFuncSetAttribute(k_solve_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    B2_CUDA(set_level_block_attrs<2>());
+    B2_CUDA(set_level_block_attrs<4>());
+    B2_CUDA(set_level_block_attrs<8>());
     for (bool pairs : {false, true}) {
         B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<2>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<4>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -800,6 +863,8 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             }
             B2_CUDA_THROW(s->d_bslots.alloc((size_t)8 * (2 * s->cbv_off[ns] + n)));
             B2_CUDA_THROW(cudaMemset(s->d_bslots.p, SLOT_EMPTY_BYTE, s->d_bslots.bytes()));
+        } else if (s->opt.n_parts == 1) {
+            B2_CUDA_THROW(s->d_xblk.alloc((size_t)8 * (2 * n + s->cbv_off[ns])));
         }
     } catch (std::exception&) {
         delete s;
@@ -838,16 +903,44 @@ int run_solve_phase(b2_solver* s, int ph, bool fwd, cudaStream_t st) {
     if (s->opt.use_cuda_graph && !stream_is_capturing(st)) {
         if (!*g) {
             int64_t nl = 0;
-            int rc = capture(s, g, [&](cudaStream_t cs) { nl = enqueue_solve(s, ph, fwd, cs); });
+            int rc = capture(s, g, [&](cudaStream_t cs) { nl = enqueue_solve<1>(s, ph, fwd, cs); });
             if (rc != B2_OK) return rc;
             if (fwd) P.n_solve_launches = 2 * nl;
         }
         B2_CUDA(cudaGraphLaunch(*g, st));
     } else {
-        int64_t nl = enqueue_solve(s, ph, fwd, st);
+        int64_t nl = enqueue_solve<1>(s, ph, fwd, st);
         if (fwd) P.n_solve_launches = 2 * nl;
         B2_CUDA(cudaGetLastError());
     }
+    return B2_OK;
+}
+
+// columns [0, ncol) of x (ld n), 1 <= ncol <= NR, as ONE walk of a level-launch tree: permute into the block workspace, both sweeps
+// (replayed as one graph per width under the one-column rule of run_solve_phase), permute back.  The same launches as a one-column
+// solve.
+template <int NR>
+int solve_level_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
+    Phase& P = s->phase[0];
+    const int n = s->S.n;
+    const int grid = std::min(4 * sm_count(), (n + 255) / 256);
+    B2_CUDA(launch_pdl(k_perm_in_block<NR>, dim3(grid), dim3(256), 0, st, n, ncol, s->d_perm.p, x, s->d_xblk.p));
+    int64_t nl = 0;
+    auto sweeps = [&](cudaStream_t cs) { nl = enqueue_solve<NR>(s, 0, true, cs); enqueue_solve<NR>(s, 0, false, cs); };
+    if (s->opt.use_cuda_graph && !stream_is_capturing(st)) {
+        cudaGraphExec_t* g = &P.g_blk[NR == 2 ? 0 : NR == 4 ? 1 : 2];
+        if (!*g) {
+            int rc = capture(s, g, sweeps);
+            if (rc != B2_OK) return rc;
+            P.n_solve_launches = 2 * nl;
+        }
+        B2_CUDA(cudaGraphLaunch(*g, st));
+    } else {
+        sweeps(st);
+        P.n_solve_launches = 2 * nl;
+        B2_CUDA(cudaGetLastError());
+    }
+    B2_CUDA(launch_pdl(k_perm_out_block<NR>, dim3(grid), dim3(256), 0, st, n, ncol, s->d_perm.p, s->d_xblk.p, x));
     return B2_OK;
 }
 
@@ -1025,11 +1118,18 @@ int b2_solve(b2_solver* s, double* x_d, int32_t nrhs, void* stream) {
         B2_CUDA(cudaGetLastError());
         return B2_OK;
     }
-    for (int c = 0; c < nrhs; ++c) {
-        double* x = x_d + (size_t)c * s->S.n;
-        int rc = b2_solve_fwd_local(s, x, stream);
+    if (nrhs == 1) {
+        int rc = b2_solve_fwd_local(s, x_d, stream);
         if (rc != B2_OK) return rc;
-        rc = b2_solve_bwd_local(s, x, stream);
+        return b2_solve_bwd_local(s, x_d, stream);
+    }
+    // level-launch tree: chunks of 8 columns as on the single-launch schedule, each one walk of the factor
+    if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
+    cudaStream_t st = as_stream(stream);
+    for (int c0 = 0; c0 < nrhs; c0 += 8) {
+        double* x = x_d + (size_t)c0 * s->S.n;
+        const int m = std::min(8, nrhs - c0);
+        int rc = m <= 2 ? solve_level_block<2>(s, x, m, st) : m <= 4 ? solve_level_block<4>(s, x, m, st) : solve_level_block<8>(s, x, m, st);
         if (rc != B2_OK) return rc;
     }
     return B2_OK;
@@ -1062,7 +1162,7 @@ int b2_get_stats(b2_solver* s, b2_stats* st) {
         if (f <= smax) st->n_small_fronts++; else st->n_big_fronts++;
     }
     st->factor_bytes = (int64_t)S.lp_off[S.nsuper] * 8;
-    st->workspace_bytes = (int64_t)(S.cb_off[S.nsuper] + s->cbv_off[S.nsuper]) * 8;
+    st->workspace_bytes = (int64_t)(S.cb_off[S.nsuper] + s->cbv_off[S.nsuper]) * 8 + (int64_t)s->d_xblk.bytes();
     st->sep_rows = S.top_rows;
     st->n_factor_launches = s->phase[0].n_factor_launches + s->phase[1].n_factor_launches;
     st->n_solve_launches = s->phase[0].n_solve_launches + s->phase[1].n_solve_launches;

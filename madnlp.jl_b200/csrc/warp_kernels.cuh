@@ -579,12 +579,12 @@ struct SolveSmem {
 // slots and its forward result into its `ypiv` slots (for its own backward task).  The backward sweep takes the ancestor values
 // from its `down` slots and its forward result from `ypiv`, writes its solution into x[perm[j]] and puts each child's ancestor
 // values into that child's `down` slots.  Without DEP (level-launch solve) the values go through xp and cbv instead.
-// NR > 1 (DEP only): NR right-hand sides in one walk, column q at x + q * ldx, the first ncol of them live (the others are computed
-// on zeros and never touch x); each column goes through exactly the operations of NR = 1, in the same order.
+// NR > 1 with DEP: NR right-hand sides in one walk, column q at x + q * ldx, the first ncol of them live (the others are computed
+// on zeros and never touch x).  NR > 1 without DEP (k_fwd_warp2_block): xp and cbv hold NR interleaved columns, entry i of column q
+// at [i * NR + q].  Either way each column goes through exactly the operations of NR = 1, in the same order.
 template <int NW, bool DEP = false, int NR = 1>
 __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRec* childrec, int s, double* sm_team, int tid, int team,
                                                int* err = nullptr, int ncol = 1, int64_t ldx = 0) {
-    static_assert(NR == 1 || DEP, "block right-hand sides run in the single-launch solve only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* ys = sm_team;                              // [NR][FMAX] assembly of the front's rhs
     double* yb = ys + NR * FMAX;                       // [2][8] broadcast slots
@@ -610,7 +610,7 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
             if (!DEP) pdl_wait();
 #pragma unroll
             for (int q = 0; q < NR; ++q)
-                ys[q * FMAX + tid] = (tid < w) ? (a.x ? (q < ncol ? a.x[q * ldx + pj] : 0.0) : a.xp[d.col0 + tid]) : 0.0;
+                ys[q * FMAX + tid] = (tid < w) ? (a.x ? (q < ncol ? a.x[q * ldx + pj] : 0.0) : a.xp[DEP ? d.col0 + tid : (d.col0 + tid) * NR + q]) : 0.0;
         }
         if (DEP) {                                      // every child's slots at once: one L2 round trip once the last one lands
             double* p[MAXC];
@@ -623,7 +623,10 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
             slot_take_block(p, need, vv, err);
         } else {
 #pragma unroll
-            for (int c = 0; c < MAXC; ++c) vv[c][0] = (tg[c] >= 0) ? a.cbv[recs[c].cbv_off + tid] : 0.0;
+            for (int c = 0; c < MAXC; ++c) {
+#pragma unroll
+                for (int q = 0; q < NR; ++q) vv[c][q] = (tg[c] >= 0) ? a.cbv[(recs[c].cbv_off + tid) * NR + q] : 0.0;
+            }
         }
         if (c0 == 0) team_sync<NW>(team);
 #pragma unroll
@@ -718,7 +721,10 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
         }
         if (a.strace) { team_sync<NW>(team); if (tid == 0) a.strace[6 * (size_t)s + 2] = global_ns(); }
     } else {
-        if (tid < f) { if (tid < w) a.xp[d.col0 + tid] = y[0]; else a.cbv[cvo + tid - w] = y[0]; }
+        if (tid < f) {
+#pragma unroll
+            for (int q = 0; q < NR; ++q) { if (tid < w) a.xp[(d.col0 + tid) * NR + q] = y[q]; else a.cbv[(cvo + tid - w) * NR + q] = y[q]; }
+        }
         team_sync<NW>(team);
     }
 }
@@ -863,13 +869,14 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
     }
 }
 
-// front_bwd_team<NW, true, PAIRS> for NR > 1 right-hand sides (k_solve_dep_block), as front_fwd_team<NW, true, NR>: every column goes
-// through the one-column operations in the same order.  (A separate function: an NR parameter on front_bwd_team changes the code
-// ptxas emits for the existing one-column kernels.)
-template <int NW, bool PAIRS, int NR>
+// front_bwd_team<NW, DEP, PAIRS> for NR > 1 right-hand sides, as front_fwd_team<NW, DEP, NR>: every column goes through the one-column
+// operations in the same order.  DEP: k_solve_dep_block; without DEP: k_bwd_warp2_block, on NR interleaved columns of xp.  (A separate
+// function: an NR parameter on front_bwd_team changes the code ptxas emits for the existing one-column kernels.)
+template <int NW, bool PAIRS, int NR, bool DEP = true>
 __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, double* sm_team, int tid, int team, const ChildRec* childrec,
                                                 int* err, const double* dsub, int ncol, int64_t ldx) {
     static_assert(NR % 2 == 0, "block slots are accessed in 16-byte pairs");
+    static_assert(DEP || !PAIRS, "pair factors are solved on the single-launch schedule only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* xs = sm_team;                              // [NR][FMAX] gathered ancestor values at [xa, xa + r)
     double* xb = xs + NR * FMAX;                       // [2][8]
@@ -877,19 +884,27 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
     double* P = xb + 16 + 4 * MAXC;                    // row-major f x w panel (same slice layout as the forward sweep)
     const FrontDesc d = a.desc[s];
     const int f = d.f, w = d.w, r = f - w;
-    // xs is the whole front vector -- own pivots' x at [0, w), the ancestors' at [w, f) -- from which the children's hand-offs are
+    // DEP: xs is the whole front vector -- own pivots' x at [0, w), the ancestors' at [w, f) -- from which the children's hand-offs are
     // gathered
-    const int xa = w;
+    const int xa = DEP ? w : 0;
     {
         const double* Lt = a.Lt + d.lp_off;
         for (int e = tid; e < f * w; e += TEAM) cp_async8(P + e, Lt + e);
     }
-    const int pj = (tid < w) ? a.perm[d.col0 + tid] : 0;
+    const int myrow = (!DEP && tid < r) ? a.rows[d.rows_off + w + tid] : 0;
+    const int pj = (DEP && tid < w) ? a.perm[d.col0 + tid] : 0;
     const double dinv = (tid < w) ? fast_rcp(a.dvec[d.col0 + tid]) : 0.0;
     const int nc0 = min(MAXC, d.nchild);
     int tg[MAXC];                                      // row of the front that child c's slot `tid` takes
     double t[NR];
-    {
+    if constexpr (!DEP) {
+        pdl_wait();
+#pragma unroll
+        for (int q = 0; q < NR; ++q) {
+            if (tid < r) xs[q * FMAX + tid] = a.xp[myrow * NR + q];
+            t[q] = (tid < w) ? a.xp[(d.col0 + tid) * NR + q] * dinv : 0.0;
+        }
+    } else {
         // the children's records and relative indices are constant: fetched before the wait, so that the hand-off to the
         // children follows the back-substitution directly
         if (tid < nc0) recs[tid] = childrec[d.child_off + tid];
@@ -1009,7 +1024,13 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
             }
         }
     }
-    {
+    if constexpr (!DEP) {
+        if (tid < w) {
+#pragma unroll
+            for (int q = 0; q < NR; ++q) a.xp[(d.col0 + tid) * NR + q] = t[q];
+        }
+        team_sync<NW>(team);
+    } else {
         if (tid < w) {
 #pragma unroll
             for (int q = 0; q < NR; ++q) {
@@ -1067,6 +1088,38 @@ __global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2(SolveArgs a, Warp
     for (int st = s1 - 1; st >= s0; --st) {
         const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
         for (int q = team; q < cnt; q += NTEAM) front_bwd_team<NW>(a, ws.list[off + q], sm[team], tid, team);
+        if (s1 - s0 > 1) __syncthreads();
+    }
+    pdl_wait();
+}
+
+// k_fwd_warp2 / k_bwd_warp2 for NR right-hand sides (b2_solve's level-launch block solve): xp and cbv hold NR interleaved columns
+template <int NW, int NTEAM, int NR>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2_block(SolveArgs a, const ChildRec* childrec, WarpSched ws) {
+    extern __shared__ __align__(16) double smd[];
+    double (*sm)[SolveSmem<NW, NR>::doubles] = (double (*)[SolveSmem<NW, NR>::doubles])smd;
+    const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
+    pdl_trigger();
+    const int s0 = ws.cta_ptr[blockIdx.x], s1 = ws.cta_ptr[blockIdx.x + 1];
+    for (int st = s0; st < s1; ++st) {
+        const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
+        for (int q = team; q < cnt; q += NTEAM) front_fwd_team<NW, false, NR>(a, childrec, ws.list[off + q], sm[team], tid, team);
+        if (s1 - s0 > 1) __syncthreads();
+    }
+    pdl_wait();
+}
+
+template <int NW, int NTEAM, int NR>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a, WarpSched ws) {
+    extern __shared__ __align__(16) double smd[];
+    double (*sm)[SolveSmem<NW, NR>::doubles] = (double (*)[SolveSmem<NW, NR>::doubles])smd;
+    const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
+    pdl_trigger();
+    const int s0 = ws.cta_ptr[blockIdx.x], s1 = ws.cta_ptr[blockIdx.x + 1];
+    for (int st = s1 - 1; st >= s0; --st) {
+        const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
+        for (int q = team; q < cnt; q += NTEAM)
+            front_bwd_block<NW, false, NR, false>(a, ws.list[off + q], sm[team], tid, team, nullptr, nullptr, nullptr, 0, 0);
         if (s1 - s0 > 1) __syncthreads();
     }
     pdl_wait();
