@@ -831,6 +831,69 @@ int b2_refine_loop_launch(b2_refine_loop* h, void* stream);
 int b2_refine_loop_wait(b2_refine_loop* h);
 int b2_refine_loop_record(b2_refine_loop* h, b2_refine_record* out);
 
+/* ---- The trials of inertia_correction! after a wrong first inertia (src/IPM/solver.jl:611-670) as ONE CUDA graph:
+ *     WHILE { schedule ; regularise ; caller's build_kkt + factorize ; trial test ;
+ *             IF { b2_richardson_begin ; WHILE { caller's refinement step ; the test of b2_refine_loop } } ; close }
+ * so the host waits once for all the regularised trials of a step instead of once per trial and per refinement step.  The
+ * schedule kernel reproduces the host's del_w sequence operation for operation:
+ *     first trial:  del_w = first_hessian_perturbation if del_w_last == 0, else max(min_hessian_perturbation, perturb_dec_fact * del_w_last)
+ *     later trials: del_w *= (del_w_last == 0 ? perturb_inc_fact_first : perturb_inc_fact); stop as failed when del_w > max_hessian_perturbation
+ *     del_c = the launch's del_c when dual_always or the previous inertia has num_zero != 0, else 0
+ * (max is Python's: the first argument unless the second is greater) and regularises by (del_w - del_w_prev, del_c - del_c_prev)
+ * with the arithmetic of b2_regularize_diagonal.  The trial test applies the KKT type's inertia rule (as b2_refine_loop_end) to the
+ * solver's device counters; only a right inertia runs the refinement.  The close accepts when ratio < acceptable_tol (0 when
+ * ||b|| == 0), goes round again after a wrong inertia, and hands over to the host when the inertia is right but the refinement is
+ * not acceptable (the improve! retry changes the factorisation's pivot threshold, which this graph bakes in) or when the
+ * factorisation reports a timed-out wait (the host's inertia read reports it).
+ * Building it:  b2_inertia_loop_begin   -- starts capturing the WHILE body on `stream` (schedule and regularise are issued)
+ *               the caller issues its build_kkt and factorisation on `stream`
+ *               b2_inertia_loop_refine  -- the trial test, the IF node, b2_richardson_begin; starts capturing the refinement body
+ *               the caller issues one refinement step (as for b2_refine_loop_begin)
+ *               b2_inertia_loop_end     -- the refinement test, the close; instantiates (and ends any capture left open)
+ * B2_ERR_UNSUPPORTED from these: the driver refuses (nested) conditional graph nodes, and the caller keeps the host loop.  The
+ * record is written to pinned host memory by the close, its sequence number last, as b2_refine_loop's. */
+typedef struct b2_inertia_options {
+    double first_hessian_perturbation, min_hessian_perturbation, max_hessian_perturbation;
+    double perturb_inc_fact_first, perturb_inc_fact, perturb_dec_fact;
+} b2_inertia_options;
+#define B2_TRIALS_ACCEPTED 1      /* a trial with the right inertia whose refinement is acceptable */
+#define B2_TRIALS_FAILED   2      /* del_w went past max_hessian_perturbation */
+#define B2_TRIALS_HANDOVER 3      /* the last trial's inertia is right and its refinement not acceptable: improve! is the host's */
+#define B2_TRIALS_FAULT    4      /* the last factorisation's counters report a timed-out wait (not a valid inertia) */
+typedef struct b2_inertia_record {
+    int32_t status;               /* B2_TRIALS_* */
+    int32_t inertia_ok;           /* the inertia test of the last trial */
+    int64_t trials;               /* regularised trials run (factorisations); the del_w of each: b2_inertia_loop_record */
+    double del_w, del_w_prev, del_c_prev;   /* the schedule's state after the last trial */
+    int64_t num_pos, num_zero, num_neg;     /* inertia of the last factorisation */
+    int64_t ir;                   /* of the last solve (status ACCEPTED or HANDOVER) */
+    double ratio;
+    int64_t ir_total;             /* ir summed over the solves that ended a trial: the host's cnt.backsolves adds it */
+    int64_t seq;                  /* launches this handle has finished, written last */
+} b2_inertia_record;
+/* trials a step can take before del_w > max_hessian_perturbation: from min(min_, first_hessian_perturbation), by the smaller of
+ * the two increase factors.  B2_ERR_UNSUPPORTED when the schedule is unbounded (a factor <= 1, a start <= 0, an infinite or NaN
+ * bound) or bounded above 2^20 trials.  Host only. */
+int b2_inertia_trial_bound(const b2_inertia_options* opt, int64_t* out);
+typedef struct b2_inertia_loop b2_inertia_loop;
+/* the del_w list is sized by b2_inertia_trial_bound (its errors are returned) */
+int b2_inertia_loop_create(const b2_inertia_options* opt, b2_inertia_loop** out);
+int b2_inertia_loop_destroy(b2_inertia_loop* h);
+/* any graph the handle held is dropped; reg, pr_diag (n_tot), du_diag (m) are baked in */
+int b2_inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
+                          int32_t dual_always, void* stream);
+/* expect_pos / expect_neg as for b2_refine_loop_end; b, w, x (n) and norms_d (3 doubles) as for b2_refine_loop_begin */
+int b2_inertia_loop_refine(b2_inertia_loop* h, const b2_inertia_source* src, int64_t expect_pos, int64_t expect_neg, int64_t n,
+                           const double* b_d, double* w_d, double* x_d, double* norms_d, void* stream);
+int b2_inertia_loop_end(b2_inertia_loop* h, int32_t max_iter, double tol, double acceptable_tol, void* stream);
+/* one step's trials: del_w_last as the host holds it, del_c = jacobian_regularization_value * mu^jacobian_regularization_exponent,
+ * num_zero of the first trial's inertia (the dual rule of the first regularised trial).  The previous launch must have been waited for */
+int b2_inertia_loop_launch(b2_inertia_loop* h, double del_w_last, double del_c, int64_t num_zero, void* stream);
+/* wait for the record of the last launch: polls it and the stream; an error of the stream is returned, not waited for */
+int b2_inertia_loop_wait(b2_inertia_loop* h);
+/* the record and the first min(trials, cap) entries of the del_w list */
+int b2_inertia_loop_record(b2_inertia_loop* h, b2_inertia_record* out, double* del_w_out, int64_t cap);
+
 
 #ifdef __cplusplus
 }

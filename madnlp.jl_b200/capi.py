@@ -102,6 +102,22 @@ class RefineRecord(C.Structure):
                 ("fail", C.c_int32), ("seq", C.c_int64)]
 
 
+class InertiaSchedule(C.Structure):
+    """b2_inertia_options: the del_w schedule of inertia_correction! (MadNLP's options of these names)"""
+    _fields_ = [(k, C.c_double) for k in ("first_hessian_perturbation", "min_hessian_perturbation", "max_hessian_perturbation",
+                                          "perturb_inc_fact_first", "perturb_inc_fact", "perturb_dec_fact")]
+
+
+TRIALS_ACCEPTED, TRIALS_FAILED, TRIALS_HANDOVER, TRIALS_FAULT = 1, 2, 3, 4
+
+
+class InertiaRecord(C.Structure):
+    """b2_inertia_record: what one launch of an inertia-correction graph leaves in pinned host memory"""
+    _fields_ = [("status", C.c_int32), ("inertia_ok", C.c_int32), ("trials", C.c_int64), ("del_w", C.c_double),
+                ("del_w_prev", C.c_double), ("del_c_prev", C.c_double), ("num_pos", C.c_int64), ("num_zero", C.c_int64),
+                ("num_neg", C.c_int64), ("ir", C.c_int64), ("ratio", C.c_double), ("ir_total", C.c_int64), ("seq", C.c_int64)]
+
+
 class SymbolicSizes(C.Structure):
     _fields_ = [(k, C.c_int64) for k in (
         "n", "n_supernodes", "n_rows", "n_children", "n_rel", "n_amap", "n_levels", "lval_size", "cb_size")]
@@ -299,6 +315,15 @@ PROTOTYPES = {
     "b2_refine_loop_launch": (C.c_int, [_p, _p]),
     "b2_refine_loop_wait": (C.c_int, [_p]),
     "b2_refine_loop_record": (C.c_int, [_p, C.POINTER(RefineRecord)]),
+    "b2_inertia_trial_bound": (C.c_int, [C.POINTER(InertiaSchedule), C.POINTER(_i64)]),
+    "b2_inertia_loop_create": (C.c_int, [C.POINTER(InertiaSchedule), _PP]),
+    "b2_inertia_loop_destroy": (C.c_int, [_p]),
+    "b2_inertia_loop_begin": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _i32, _p]),
+    "b2_inertia_loop_refine": (C.c_int, [_p, C.POINTER(InertiaSource), _i64, _i64, _i64, _p, _p, _p, _p, _p]),
+    "b2_inertia_loop_end": (C.c_int, [_p, _i32, _f64, _f64, _p]),
+    "b2_inertia_loop_launch": (C.c_int, [_p, _f64, _f64, _i64, _p]),
+    "b2_inertia_loop_wait": (C.c_int, [_p]),
+    "b2_inertia_loop_record": (C.c_int, [_p, C.POINTER(InertiaRecord), _p, _i64]),
 }
 
 for _name, (_res, _args) in PROTOTYPES.items():

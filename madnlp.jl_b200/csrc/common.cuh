@@ -122,4 +122,14 @@ inline cudaError_t launch_pdl(void (*kern)(P...), dim3 grid, dim3 block, size_t 
 }
 #endif
 
+// ---- conditional graph nodes (refine_loop.cu), shared by the refinement-loop and the inertia-correction graphs
+// the CUDA errors by which a driver refuses conditional nodes (anything else is a fault and is reported as one)
+bool conditional_unsupported(cudaError_t e);
+// leave no capture open on the stream (a capture-to-graph's graph belongs to its owner) and clear the sticky error
+void abort_capture(cudaStream_t st);
+// solve_refine!'s stopping rule and the KKT type's inertia test after one refinement step, one thread; sets `cond` (a WHILE node)
+cudaError_t launch_refine_test(cudaStream_t st, cudaGraphConditionalHandle cond, const double* norms, const b2_inertia_source& src,
+                               int64_t expect_pos, int64_t expect_neg, int32_t max_iter, double tol, b2_refine_record* rec,
+                               b2_refine_record* out);
+
 }  // namespace b2

@@ -79,23 +79,41 @@ __global__ void k_refine_test(cudaGraphConditionalHandle cond, const double* __r
     cudaGraphSetConditional(cond, more ? 1u : 0u);
 }
 
-// the CUDA errors by which a driver refuses conditional nodes (anything else is a fault and is reported as one)
-bool unsupported(cudaError_t e) { return e == cudaErrorNotSupported || e == cudaErrorCallRequiresNewerDriver; }
+}  // namespace
 
-// leave no capture open on the stream and drop the half-built graph
-void abort_build(b2_refine_loop* h, cudaStream_t st) {
+namespace b2 {
+
+bool conditional_unsupported(cudaError_t e) { return e == cudaErrorNotSupported || e == cudaErrorCallRequiresNewerDriver; }
+
+void abort_capture(cudaStream_t st) {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     if (cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone) {
         cudaGraph_t g = nullptr;
-        cudaStreamEndCapture(st, &g);       // (capture-to-graph: g is the handle's own graph, dropped below)
+        cudaStreamEndCapture(st, &g);       // (capture-to-graph: g is the owner's own graph, dropped by the owner)
     }
     cudaGetLastError();
+}
+
+cudaError_t launch_refine_test(cudaStream_t st, cudaGraphConditionalHandle cond, const double* norms, const b2_inertia_source& src,
+                               int64_t expect_pos, int64_t expect_neg, int32_t max_iter, double tol, b2_refine_record* rec,
+                               b2_refine_record* out) {
+    k_refine_test<<<1, 1, 0, st>>>(cond, norms, src, expect_pos, expect_neg, max_iter, tol, rec, out);
+    return cudaGetLastError();
+}
+
+}  // namespace b2
+
+namespace {
+
+// leave no capture open on the stream and drop the half-built graph
+void abort_build(b2_refine_loop* h, cudaStream_t st) {
+    abort_capture(st);
     h->drop();
 }
 
 int fail_build(b2_refine_loop* h, cudaStream_t st, cudaError_t e, const char* what) {
     abort_build(h, st);
-    if (unsupported(e)) {
+    if (conditional_unsupported(e)) {
         set_error(std::string(what) + ": conditional CUDA graph nodes are not available (" + cudaGetErrorString(e) + ")");
         return B2_ERR_UNSUPPORTED;
     }
@@ -159,8 +177,7 @@ int b2_refine_loop_end(b2_refine_loop* h, const b2_inertia_source* src, int64_t 
         set_error("b2_refine_loop_end: invalid argument (or no b2_refine_loop_begin before it)");
         return B2_ERR_INVALID;
     }
-    k_refine_test<<<1, 1, 0, st>>>(h->cond, h->norms, *src, expect_pos, expect_neg, max_iter, tol, h->rec.p, h->rec_h);
-    RL_TRY(cudaGetLastError(), "k_refine_test");
+    RL_TRY(launch_refine_test(st, h->cond, h->norms, *src, expect_pos, expect_neg, max_iter, tol, h->rec.p, h->rec_h), "k_refine_test");
     cudaGraph_t g = nullptr;
     RL_TRY(cudaStreamEndCapture(st, &g), "cudaStreamEndCapture(body)");
     RL_TRY(cudaGraphInstantiate(&h->exec, h->graph, 0), "cudaGraphInstantiate");

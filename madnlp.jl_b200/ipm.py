@@ -26,12 +26,15 @@ The model callbacks themselves are out of scope (SURVEY.md 8a A0): an iterate su
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 
+from . import capi
 from .barrier import llb_uub
-from .capi import CURV_PASS, CURV_RESULT_LEN, check, copy_many, lib, ptr
+from .capi import B2_ERR_UNSUPPORTED, B2_OK, CURV_PASS, CURV_RESULT_LEN, check, copy_many, lib, ptr
 from .capture import CapturedSequence
 from .kkt import SolverVectors, UnreducedKKTVector
 from .quasi_newton import ExactHessian
@@ -53,6 +56,36 @@ class InertiaOptions:
 
 
 INERTIA_CORRECTION_METHODS = ("InertiaAuto", "InertiaBased", "InertiaIgnore", "InertiaFree")
+
+
+def inertia_trial_bound(opt):
+    """the most regularised trials one inertia_correction! can take with these InertiaOptions (b2_inertia_trial_bound), or None when
+    the del_w schedule is unbounded"""
+    cap = C.c_int64(0)
+    rc = lib.b2_inertia_trial_bound(C.byref(_schedule(opt)), C.byref(cap))
+    if rc == B2_ERR_UNSUPPORTED:
+        return None
+    check(rc)
+    return cap.value
+
+
+def _schedule(opt):
+    return capi.InertiaSchedule(*(float(getattr(opt, name)) for name, _ in capi.InertiaSchedule._fields_))
+
+
+class _TrialsLoop:
+    """one b2_inertia_loop handle: the graph of the trials after a wrong first inertia, its record and its del_w list"""
+
+    def __init__(self, opt, cap):
+        self.h = C.c_void_p()
+        check(lib.b2_inertia_loop_create(C.byref(_schedule(opt)), C.byref(self.h)))
+        self.rec = capi.InertiaRecord()
+        self.del_w = np.zeros(cap, dtype=np.float64)
+
+    def __del__(self):
+        if getattr(self, "h", None) and lib is not None:
+            lib.b2_inertia_loop_destroy(self.h)
+            self.h = None
 
 
 def resolve_inertia_correction_method(method, linear_solver):
@@ -133,6 +166,7 @@ class IPMLinearAlgebra:
         self.del_w_last = 0.0
         self.last_inertia = None
         self.cnt = dict(factorizations=0, backsolves=0, regularized=0, failed=0)
+        self._trials = None         # (the setting the trials graph bakes in, _TrialsLoop, None before it is built, False if refused)
 
     def load_ifr_inputs(self, f, x, xl, xu, jacl, c, non_blocking=True):
         """Copy the solver vectors the inertia-free test reads (f, x, xl, xu, jacl: n_tot; c: m) into solver_vectors"""
@@ -203,16 +237,22 @@ class IPMLinearAlgebra:
         """solve_refine_wrapper!(x, solver, b, w); (d, p, _w4) by default"""
         if x is None:
             x, b, w = self.d, self.p, self.w
-        ok = self.iterator.solve_refine(x, b, w)
-        if not ok and self.kkt.linear_solver.improve():
-            # improve!() changed a factorisation parameter (pivot threshold) that the captured prologues have baked in:
-            # drop the captured graphs so that every later step factorises with the new setting
-            self._prologue_graph.reset()
-            self._rr_graph.reset()
-            self.kkt.factorize_kkt()
-            ok = self.iterator.solve_refine(x, b, w)
+        ok = self.iterator.solve_refine(x, b, w) or self._improve_and_solve(x, b, w)
         self.cnt["backsolves"] += self.iterator.ir
         return ok
+
+    def _improve_and_solve(self, x, b, w):
+        """the retry of solve_refine_wrapper! after a refinement that is not acceptable: improve!() and, when it changed the
+        factorisation, factorise and solve again"""
+        if not self.kkt.linear_solver.improve():
+            return False
+        # improve!() changed a factorisation parameter (pivot threshold) that the captured prologues and the trials graph have baked
+        # in: drop the captured graphs so that every later step factorises with the new setting
+        self._prologue_graph.reset()
+        self._rr_graph.reset()
+        self._trials = None
+        self.kkt.factorize_kkt()
+        return self.iterator.solve_refine(x, b, w)
 
     def step(self, mu=1e-2, after_prologue=None):
         """One `regular!` linear-algebra pass; returns True when a step direction was obtained.  `after_prologue` (optional
@@ -378,11 +418,48 @@ class IPMLinearAlgebra:
     def _inertia_correction(self, mu):
         """inertia_correction! after its first factorize_wrapper! (src/IPM/solver.jl:611-783), for the method of this object: one del_w
         schedule; the methods differ in the trial (_trial) and in del_c, which InertiaBased sets only when the inertia asks for it and
-        InertiaFree / InertiaIgnore set on every trial.  `last_del_w` lists the del_w of each trial."""
-        k, o = self.kkt, self.opt
-        del_w = del_c = del_w_prev = del_c_prev = 0.0
+        InertiaFree / InertiaIgnore set on every trial.  `last_del_w` lists the del_w of each trial.
+
+        After a first trial that fails, InertiaBased runs the remaining trials as one CUDA graph where _trials_loop has one
+        (csrc/inertia_loop.cu): the host launches it, waits once and takes the counters and the schedule's state from its record.
+        The graph is built on the second step of a setting, whatever its first trial gives, so that it is ready when a step first
+        meets a wrong inertia; a step whose first trial succeeds never launches it.
+        When the graph hands over (a right inertia whose refinement is not acceptable: the improve! retry is the host's), the host
+        finishes that trial and goes on with its own loop from that state."""
         self.last_del_w = []
+        self._trials_loop()             # here, so that the host's check runs while the factorisation does
         ok, inertia = self._trial(first=True)
+        del_w = del_w_prev = del_c_prev = 0.0
+        loop = self._trials[1] if self._trials else None            # (an improve!() in the first trial dropped the graph)
+        if not ok and loop:
+            rec = self._run_trials_loop(loop, mu, inertia)
+            self.last_del_w += loop.del_w[: rec.trials].tolist()
+            del_w, del_w_prev, del_c_prev = rec.del_w, rec.del_w_prev, rec.del_c_prev
+            inertia = (rec.num_pos, rec.num_zero, rec.num_neg)
+            self.cnt["factorizations"] += rec.trials
+            self.cnt["regularized"] += rec.trials - 1            # the last trial counts once the host has its outcome
+            if rec.status == capi.TRIALS_FAILED:
+                self.cnt["regularized"] += 1
+                self.cnt["failed"] += 1
+                return False
+            if rec.status == capi.TRIALS_FAULT:
+                ok, inertia = self._trial()                       # the host's inertia read reports the failed factorisation
+            else:
+                it = self.iterator
+                it.ir, it.residual_ratio = rec.ir, rec.ratio
+                if rec.status == capi.TRIALS_ACCEPTED:
+                    ok = True
+                    self.cnt["backsolves"] += rec.ir_total
+                else:
+                    ok = self._improve_and_solve(self.d, self.p, self.w)
+                    self.cnt["backsolves"] += it.ir
+            self.cnt["regularized"] += 1
+        return self._trials_from(mu, ok, inertia, del_w, del_w_prev, del_c_prev)
+
+    def _trials_from(self, mu, ok, inertia, del_w, del_w_prev, del_c_prev):
+        """inertia_correction!'s loop of regularised trials on the host, from a state: the outcome and inertia of the last trial, its
+        del_w, the del_w and del_c the diagonal holds (0 before the first regularisation) and last_del_w"""
+        k, o = self.kkt, self.opt
         while not ok:
             if not self.last_del_w:
                 del_w = o.first_hessian_perturbation if self.del_w_last == 0.0 else max(
@@ -404,6 +481,69 @@ class IPMLinearAlgebra:
             self.del_w_last = del_w
         self.last_inertia = inertia
         return True
+
+    def _trials_loop(self):
+        """the graph of the trials after a wrong first inertia, or None: the host loop.  It covers InertiaBased with the Richardson
+        loop on the device, the exact Hessian, a single-part sparse solver that exposes its pivot counters and a KKT type that states
+        its inertia and dual rules as data (SparseKKTSystem, SparseUnreducedKKTSystem, SparseCondensedKKTSystem).  As for the
+        refinement-loop graph, the first step of a setting runs every launch eagerly and the second builds the graph."""
+        k, it = self.kkt, self.iterator
+        ls = k.linear_solver
+        if not (self.inertia_correction_method == "InertiaBased" and isinstance(it, RichardsonIterator) and it._device_loop
+                and isinstance(getattr(k, "quasi_newton", ExactHessian()), ExactHessian) and hasattr(k, "inertia_rule")
+                and hasattr(k, "dual_rule") and hasattr(ls, "inertia_source") and ls.opt.n_parts == 1):
+            self._trials = None
+            return None
+        setting = (tuple(vars(self.opt).values()), k.inertia_rule(), k.dual_rule(), it.richardson_max_iter, it.richardson_tol,
+                   it.richardson_acceptable_tol, self.d.values.data_ptr(), self.p.values.data_ptr(), self.w.values.data_ptr())
+        if self._trials is None or self._trials[0] != setting:
+            self._trials = (setting, None)
+            return None
+        if self._trials[1] is None:
+            self._trials = (setting, self._build_trials_loop() or False)
+        return self._trials[1] or None
+
+    def _build_trials_loop(self):
+        """capture the trials graph over (d, p, w): the type's build_kkt and factorisation, then its refinement step (C-ABI launches
+        only, so a raw stream capture of them holds no PyTorch allocation).  None: the schedule is unbounded or the driver refuses
+        nested conditional nodes"""
+        k, it = self.kkt, self.iterator
+        x, b, w = self.d, self.p, self.w
+        cap = inertia_trial_bound(self.opt)
+        if cap is None:
+            return None
+        loop = _TrialsLoop(self.opt, cap)
+        src = k.linear_solver.inertia_source()
+        pos, neg = k.inertia_rule()
+        torch.cuda.synchronize()
+        # captured on a side stream, as torch.cuda.graph does: the legacy default stream cannot be captured
+        with torch.cuda.stream(torch.cuda.Stream()):
+            sp = k.stream_ptr()
+            rc = lib.b2_inertia_loop_begin(loop.h, k._n_tot, k._m, ptr(k.reg), ptr(k.pr_diag), ptr(k.du_diag), int(k.dual_rule()), sp)
+            if rc == B2_OK:
+                try:
+                    k.build_kkt()
+                    k.factorize_kkt()
+                    rc = lib.b2_inertia_loop_refine(loop.h, C.byref(src), -1 if pos is None else pos, -1 if neg is None else neg,
+                                                    b.values.numel(), ptr(b.values), ptr(w.values), ptr(x.values), ptr(it._norms), sp)
+                    if rc == B2_OK:
+                        it._body(x, b, w)
+                finally:
+                    end = lib.b2_inertia_loop_end(loop.h, it.richardson_max_iter, it.richardson_tol, it.richardson_acceptable_tol, sp)
+                    rc = end if rc == B2_OK else rc
+        if rc == B2_ERR_UNSUPPORTED:
+            return None
+        check(rc)
+        return loop
+
+    def _run_trials_loop(self, loop, mu, inertia):
+        """launch the trials graph for this step, wait for its record; del_c is computed as the host loop computes it"""
+        o = self.opt
+        del_c = o.jacobian_regularization_value * mu ** o.jacobian_regularization_exponent
+        check(lib.b2_inertia_loop_launch(loop.h, float(self.del_w_last), float(del_c), int(inertia[1]), self.kkt.stream_ptr()))
+        check(lib.b2_inertia_loop_wait(loop.h))
+        check(lib.b2_inertia_loop_record(loop.h, C.byref(loop.rec), loop.del_w.ctypes.data, loop.del_w.size))
+        return loop.rec
 
     def _trial(self, first=False):
         """One trial on the factor just computed; returns (accepted, the inertia read, or None when the method reads none).

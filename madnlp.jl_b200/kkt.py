@@ -334,6 +334,15 @@ class _SparseKKTBase(_KKTBase):
     def num_variables(self):
         return len(self.pr_diag)
 
+    def inertia_rule(self):
+        """is_inertia_correct (src/KKT/KKTsystem.jl:242-244) as data, for the inertia-correction graph (ipm.py): num_zero == 0 and
+        num_pos == n_tot"""
+        return self.num_variables(), None
+
+    def dual_rule(self):
+        """should_regularize_dual as data: False = only when num_zero != 0 (src/KKT/KKTsystem.jl:252-254)"""
+        return False
+
     def get_jacobian(self):
         return self.jac_callback
 
@@ -550,6 +559,10 @@ class SparseCondensedKKTSystem(_KKTBase):
 
     def should_regularize_dual(self, num_pos, num_zero, num_neg):
         return True                                                    # condensed.jl:141
+
+    def dual_rule(self):
+        """should_regularize_dual as data: True = always"""
+        return True
 
     def _pre_args(self):
         return (self._bounds.h, self._jt_spmv.h, self.n, self.m, ptr(self.jt_csc.nzval), ptr(self.pr_diag), ptr(self.diag_buffer))
