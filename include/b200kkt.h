@@ -214,6 +214,10 @@ int b2_debug_trace(b2_solver* s, uint64_t* stamps_h, int32_t* parent_h, int32_t*
  * forward, {3,4,5} backward, as left by the last solve.  *count = number of uint64 values (0 when tracing is off); stamps are
  * copied when capacity >= *count. */
 int b2_debug_trace_solve(b2_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count);
+/* Debug (also on a symbolic-only handle): the ticket order of the single-launch factorisation and solve (dep_schedule bit 0, used
+ * when every front has order <= 64) over this rank's supernodes: depth from the root descending, then level, then id.  *count =
+ * number of supernodes in it; order_h is filled when capacity >= *count (may be NULL). */
+int b2_debug_dep_order(b2_solver* s, int32_t* order_h, int64_t capacity, int64_t* count);
 
 /* ------------------------------------------------------------------ dense LDL^T */
 typedef struct b2d_solver b2d_solver;

@@ -175,6 +175,7 @@ PROTOTYPES = {
     "b2d_debug_trace": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
     "b2_debug_trace": (C.c_int, [_p, _p, _p, _p, _p, _i64, C.POINTER(_i64)]),
     "b2_debug_trace_solve": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
+    "b2_debug_dep_order": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
     "b2d_create": (C.c_int, [_i32, _i32, _p, C.POINTER(Options), _PP]),
     "b2d_destroy": (C.c_int, [_p]),
     "b2d_factorize": (C.c_int, [_p, _p]),

@@ -455,6 +455,25 @@ int capture(b2_solver* s, cudaGraphExec_t* out, Fn fn) {
     return B2_OK;
 }
 
+// The fronts (mine[sn] set) of the single-launch schedule in ticket order: depth from the root descending, then level, then id.  A
+// child is deeper than its parent, so the order is topological (what the schedule's forward progress rests on: claim_group), and the
+// fronts at the bottom of the longest root paths -- the critical path -- hold the first tickets.  In (level, id) order they shared
+// level 0 with every leaf of the tree, and their parents waited for a CTA slot until the 3,314 leaves of OPF-10k had been claimed
+// (tools/trace_sparse.py).
+std::vector<int32_t> dep_ticket_order(const Symbolic& S, const std::vector<char>& mine) {
+    const int ns = S.nsuper;
+    std::vector<int32_t> depth(ns, 0), order;
+    for (int sn = ns - 1; sn >= 0; --sn) {         // parents have larger ids
+        const int p = S.sn_parent[sn];
+        depth[sn] = (p >= 0 && mine[p]) ? depth[p] + 1 : 0;
+    }
+    for (int sn = 0; sn < ns; ++sn) if (mine[sn]) order.push_back(sn);
+    std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) {
+        return depth[x] != depth[y] ? depth[x] > depth[y] : S.sn_level[x] < S.sn_level[y];
+    });
+    return order;
+}
+
 void build_schedule(b2_solver* s) {
     const Symbolic& S = s->S;
     const int ns = S.nsuper;
@@ -502,9 +521,7 @@ void build_schedule(b2_solver* s) {
             int cntm = 0;
             for (int sn = 0; sn < ns && all_team; ++sn) if (mine[sn]) { int w, f; fdim(sn, w, f); all_team = f <= wmax; ++cntm; }
             if (all_team && cntm > 0) {
-                std::vector<int32_t> order;
-                for (int l = 0; l < S.nlevels; ++l)
-                    for (int q = S.level_ptr[l]; q < S.level_ptr[l + 1]; ++q) if (mine[S.level_sn[q]]) order.push_back(S.level_sn[q]);
+                const std::vector<int32_t> order = dep_ticket_order(S, mine);
                 std::vector<int32_t> gtype, gptr(1, 0), tasks;
                 size_t k = 0;
                 while (k < order.size()) {
@@ -1256,6 +1273,17 @@ int b2_debug_trace(b2_solver* s, uint64_t* stamps_h, int32_t* parent_h, int32_t*
     } else if (stamps_h) {
         std::memset(stamps_h, 0, (size_t)3 * ns * sizeof(uint64_t));
     }
+    return B2_OK;
+}
+
+int b2_debug_dep_order(b2_solver* s, int32_t* order_h, int64_t capacity, int64_t* count) {
+    if (!s || !count) { set_error("b2_debug_dep_order: invalid argument"); return B2_ERR_INVALID; }
+    const int rank = std::max(0, s->opt.part_rank);
+    std::vector<char> mine(s->S.nsuper);
+    for (int sn = 0; sn < s->S.nsuper; ++sn) mine[sn] = s->S.owner[sn] == rank;
+    const std::vector<int32_t> order = dep_ticket_order(s->S, mine);
+    *count = (int64_t)order.size();
+    if (order_h && capacity >= *count) std::copy(order.begin(), order.end(), order_h);
     return B2_OK;
 }
 

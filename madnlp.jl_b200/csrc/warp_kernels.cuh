@@ -79,12 +79,9 @@ struct TeamSmem {
     }
 };
 
-// dependency flags of the single-launch factorisation (k_factor_dep): zeroed before the launch, a flag is ready when it holds `want`
-// (stored with st_release by the front that finishes)
+// dependency flags of the single-launch factorisation (k_factor_dep): zeroed before the launch, a flag is ready when it holds 1
+// (stored with st_release by the front that finishes); a wait polls at most DEP_SPIN_MAX times, DEP_SPIN_SLEEP_NS apart
 constexpr unsigned DEP_SPIN_MAX = 1u << 24, DEP_SPIN_SLEEP_NS = 32;
-__device__ __forceinline__ void flag_wait(const int* flag, int* err, int want = 1) {
-    if (!bounded_spin<DEP_SPIN_MAX, DEP_SPIN_SLEEP_NS>(err, [&](unsigned) { return ld_acquire(flag) == want; })) __threadfence();
-}
 
 // Hand-off slots of the single-launch solve: the value is its own flag.  A slot holds SLOT_EMPTY (ptx.cuh) until its one producer
 // stores the value; its one consumer polls the value itself (no flag, no release fence, one L2 round trip per hand-off) and stores
@@ -93,7 +90,7 @@ __device__ __forceinline__ void slot_put(double* p, double v) {
     const unsigned long long b = (unsigned long long)__double_as_longlong(v);
     st_relaxed_b64(p, b == SLOT_EMPTY ? CANON_NAN : b);
 }
-// take the slots p[c] with bit c of `need` set: poll them all at once until none is empty, then re-arm each.  Bounded like flag_wait:
+// take the slots p[c] with bit c of `need` set: poll them all at once until none is empty, then re-arm each.  Bounded like the flag polls:
 // a slot still empty at the time-out sets *err (the solve then writes NaN into x) and reads as NaN.
 template <int K>
 __device__ __forceinline__ void slot_take(double* const (&p)[K], unsigned need, double (&v)[K], int* err) {
@@ -319,11 +316,23 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
         int nrec = min(MAXC, d.nchild - cb0) - ro;
         if (DEP) {
             if (tid < 32) {
-                if (tid == 0) flag_wait(done + recs[ro].sn, err);          // child front finished (its update block is in L2)
-                __syncwarp();
-                int v = (tid == 0) ? 1 : 0;
-                if (tid > 0 && tid < nrec) v = ld_acquire(done + recs[ro + tid].sn);
-                const unsigned m = __ballot_sync(0xffffffffu, v != 0);
+                // lane c polls child ro + c's flag: the round starts once child ro has finished (its update block is in L2) and
+                // takes along the finished prefix behind it, read in the same poll -- no second, dependent round trip for the
+                // children behind the one it waited for
+                const int* fl = done + recs[ro + (tid < nrec ? tid : 0)].sn;
+                unsigned m, it = 0;
+                for (;;) {
+                    const int v = (tid < nrec) ? ld_acquire(fl) : 0;
+                    m = __ballot_sync(0xffffffffu, v != 0);
+                    if (m & 1u) break;
+                    if (++it >= DEP_SPIN_MAX) {                              // never hang the device, report instead
+                        if (tid == 0) atomicExch(err, 1);
+                        __threadfence();
+                        m = 1u;
+                        break;
+                    }
+                    __nanosleep(DEP_SPIN_SLEEP_NS);
+                }
                 if (tid == 0) *nready_sh = __ffs(~m) - 1;                  // length of the finished prefix (>= 1)
             }
             team_sync<NW>(team);
@@ -1133,14 +1142,14 @@ __global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a
 struct DepSched {
     const int32_t* grp_type;   // 1 or 2 (warps per team)
     const int32_t* grp_ptr;    // [ngroup+1] into tasks
-    const int32_t* tasks;      // supernode ids in topological (level, id) order
+    const int32_t* tasks;      // supernode ids in topological ticket order (dep_ticket_order in sparse_ldl.cu)
     int ngroup;
 };
 
 // Forward progress: a CTA only ever waits for groups that come EARLIER in the topological order.  Groups are therefore claimed
 // through an atomic ticket instead of blockIdx.x: whichever CTA the hardware starts first takes the earliest unclaimed group, so a
 // running CTA never waits for work that no running (or finished) CTA owns -- independent of the block dispatch order, which the
-// programming model does not specify (the bounded spin in flag_wait stays as a second line of defence).
+// programming model does not specify (the bounded spin of the flag polls stays as a second line of defence).
 __device__ __forceinline__ int claim_group(int* ticket, int ngroup) {
     __shared__ int g_sh;
     if (threadIdx.x == 0) {
@@ -1192,7 +1201,7 @@ __global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const Ch
 
 // ------------------------------------------------------------------------------------------------ single-launch solve
 // Forward sweep, D^-1 and backward sweep of the whole (team-class, unsharded) tree in ONE launch.  The tasks are the groups of
-// k_factor_dep (DepSched: fronts in (level, id) order, four fronts of order <= 32 as one-warp teams or one front of order <= 64 as a
+// k_factor_dep (DepSched: fronts in ticket order, four fronts of order <= 32 as one-warp teams or one front of order <= 64 as a
 // two-warp team per group):
 //   ticket [0, ngroup)          forward sweep of group t: a front takes its children's contribution vectors from their `up` slots
 //   ticket [ngroup, 2 ngroup)   backward sweep of the groups in reverse order: a front takes its ancestors' values from its `down`

@@ -2,7 +2,8 @@
 """Per-front device timeline of the single-launch multifrontal factorisation (k_factor_dep) on the headline workload.
 Run with B2_SPARSE_TRACE=1 (set below): every front stamps %globaltimer when its team starts, when its children have been
 assembled and when it has finished (b2_debug_trace).  Prints the span, the number of fronts in flight over time and the
-critical path from the root down (the child that finishes last at every level).
+critical path from the root down (the child that finishes last at every level), with the median hand-off gap and compute per hop
+and the time the path's fronts spent waiting for their CTA to become resident.
 
     python tools/trace_sparse.py [case]            # the factorisation (k_factor_dep)
     python tools/trace_sparse.py [case] --solve    # one solve (k_solve_dep, b2_debug_trace_solve)
@@ -129,6 +130,7 @@ for s_, p_ in enumerate(parent):
 root = int(np.argmax(np.where(ok, t[:, 2], -1)))
 print("critical path (root first): sn  w  f  nchild | start  assembled  end | wait-for-children  compute | gap to last child")
 s_ = root
+hops = []
 while True:
     ch = [c for c in children[s_] if ok[c]]
     last = max(ch, key=lambda c: t[c, 2]) if ch else None
@@ -137,4 +139,11 @@ while True:
                                                                      t[s_, 1] - t[s_, 0], t[s_, 2] - t[s_, 1], gap))
     if last is None:
         break
+    # (gap, compute, how long the front's team started after its last child had finished: time spent waiting for a CTA)
+    hops.append((gap, t[s_, 2] - t[s_, 1], max(0.0, t[s_, 0] - t[last, 2])))
     s_ = last
+if hops:
+    g = np.array(hops)
+    print("%d tree hops on the path: gap last child done -> assembled median %.2f us (mean %.2f), compute median %.2f us; "
+          "%.1f us in all of parents' teams starting after their last child had finished (waiting for a CTA)"
+          % (len(g), np.median(g[:, 0]), g[:, 0].mean(), np.median(g[:, 1]), g[:, 2].sum()))
