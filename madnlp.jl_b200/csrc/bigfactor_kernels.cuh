@@ -5,8 +5,9 @@
 //                   (4 sub-blocks of 32: register LDL^T by one warp, sub-panel substitution, in-block trailing update),
 //                   written back (unit-lower L11, D), and its unit-lower INVERSE is formed in place and stored to the
 //                   Linv buffer -- the same blocks the multi-CTA triangular solves use (bigsolve_kernels.cuh).
-//   k_big_trsm      rows below the block:  L21 = A21 * L11^{-T} * D^{-1}  as a DMMA GEMM against Linv (64 rows per CTA,
-//                   operands streamed by cp.async), in place.
+//   k_big_trsm_subst  rows below the block (sparse fronts):  L21 = A21 * L11^{-T} * D^{-1}  by forward substitution against L11
+//                   (64 rows per CTA), in place -- componentwise backward stable whatever cond(L11) is.
+//   k_big_trsm      the same rows for the dense solver, as a DMMA GEMM against Linv (operands streamed by cp.async), in place.
 //   k_big_update_pipe_bulk (front_kernels.cuh)  trailing update with all 128 pivots at once.
 //
 // so a front of order N costs 3*N/128 dependent launches instead of 13*N/128, and the diagonal-block inversion is no
@@ -344,6 +345,63 @@ __global__ void __launch_bounds__(256, 2) k_big_trsm(FactorArgs a, const int32_t
     const int i = tid & (TR_ROWS - 1);
     if (r0 + i < f) {
         for (int cc = tid >> 6; cc < nb; cc += 4) Lp[(size_t)(kb + cc) * f + r0 + i] = Cs[i * GU_LDC + cc] * dinv[cc];
+    }
+    trace_exit(a, 8 * (kb / DB) + TR_TRSM);
+}
+
+// The same L21 for the sparse solver's big fronts, by forward substitution against L11 instead of a product with its inverse:
+//   X(i, c) = A21(i, c) - sum_{k < c} X(i, k) l(c, k),   L21(i, c) = X(i, c) / d_c.
+// A product with the inverse is not componentwise backward stable: its error grows with cond(L11), and the augmented KKT systems
+// with a small dual regularisation (delta ~ 1e-8, late IPM iterates) make the diagonal blocks ill-conditioned enough that the factor
+// misses |A - L D L^T| <= c u (|A| + |L||D||L^T|) by up to ~40x.  Substitution meets it whatever cond(L11) is.  L11 lands in shared
+// memory once (l(c, k) at Ls[k * DB + c]); 4 lanes share a row, lane t owns the columns c = t + 4 j in registers, and column k's
+// final value goes to the row's other lanes by one shuffle per pivot: no block-wide barrier inside the 128-step recurrence.
+constexpr size_t TS_SMEM = (size_t)(DB * DB + DB) * sizeof(double);
+__global__ void __launch_bounds__(256, 1) k_big_trsm_subst(FactorArgs a, const int32_t* __restrict__ list, int kb) {
+    const int s = list[blockIdx.y];
+    const FrontDesc d = a.desc[s];
+    if (kb >= d.w) return;
+    const int f = d.f, nb = min(DB, d.w - kb);
+    const int r0 = kb + nb + blockIdx.x * TR_ROWS;
+    if (r0 >= f) return;
+    trace_enter(a, 8 * (kb / DB) + TR_TRSM);
+    extern __shared__ __align__(16) double ts_sm[];
+    double* Ls = ts_sm;                                               // [k][c]: l(c, k) for k < c < nb, else 0
+    double* dd = Ls + DB * DB;                                        // [c]: d_c (1 past nb)
+    double* Lp = a.L + d.lp_off;
+    const int tid = threadIdx.x, lane = tid & 31, t = lane & 3;
+    const int i = (tid >> 5) * 8 + (lane >> 2);                       // this thread's row of the 64-row tile
+    for (int e = tid; e < DB * DB; e += 256) {
+        const int c = e & (DB - 1), k = e >> 7;
+        Ls[e] = (c < nb && c > k) ? Lp[(size_t)(kb + k) * f + kb + c] : 0.0;
+    }
+    if (tid < DB) dd[tid] = (tid < nb) ? Lp[(size_t)(kb + tid) * f + kb + tid] : 1.0;
+    const bool row_ok = r0 + i < f;
+    double x[DB / 4];
+#pragma unroll
+    for (int j = 0; j < DB / 4; ++j) {
+        const int c = t + 4 * j;
+        x[j] = (row_ok && c < nb) ? Lp[(size_t)(kb + c) * f + r0 + i] : 0.0;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j0 = 0; j0 < DB / 4; ++j0)
+#pragma unroll
+        for (int t0 = 0; t0 < 4; ++t0) {
+            const int k = 4 * j0 + t0;                                // x(i, k) is final: it sits in x[j0] of lane t0 of the row
+            const double xk = __shfl_sync(0xffffffffu, x[j0], (lane & ~3) | t0);
+            const double* lk = Ls + k * DB;
+#pragma unroll
+            for (int j = j0; j < DB / 4; ++j)
+                if (t + 4 * j > k) x[j] = fma(-xk, lk[t + 4 * j], x[j]);
+        }
+    if (row_ok) {
+        // every read of this tile's A21 rows was into this thread's registers, so the in-place store is safe
+#pragma unroll
+        for (int j = 0; j < DB / 4; ++j) {
+            const int c = t + 4 * j;
+            if (c < nb) Lp[(size_t)(kb + c) * f + r0 + i] = x[j] / dd[c];
+        }
     }
     trace_exit(a, 8 * (kb / DB) + TR_TRSM);
 }

@@ -118,7 +118,7 @@ void launch_big_step(const FactorArgs& a, const int32_t* lb, int nfronts, int ob
     static bool attr = false;
     if (!attr) {
         cudaFuncSetAttribute(k_big_diag128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Diag128Smem));
-        cudaFuncSetAttribute(k_big_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM);
+        cudaFuncSetAttribute(k_big_trsm_subst, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TS_SMEM);
         cudaFuncSetAttribute(k_big_update_pipe_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GU_SMEM_BULK);
         attr = true;
     }
@@ -126,7 +126,8 @@ void launch_big_step(const FactorArgs& a, const int32_t* lb, int nfronts, int ob
     if (nl) ++*nl;
     const int rem = maxf - ob - 1;                  // rows below the first pivot of the block (upper bound over the fronts)
     if (rem <= 0) return;
-    k_big_trsm<<<dim3((rem + TR_ROWS - 1) / TR_ROWS, nfronts), 256, GU_SMEM, st>>>(a, lb, ob, Linv, linv_off, 0);
+    // rows below the block by substitution (componentwise backward stable; the inverse stays for the solve's diagonal blocks)
+    k_big_trsm_subst<<<dim3((rem + TR_ROWS - 1) / TR_ROWS, nfronts), 256, TS_SMEM, st>>>(a, lb, ob);
     k_big_update_pipe_bulk<<<dim3((rem + GU_M - 1) / GU_M, (rem + GU_N - 1) / GU_N, nfronts), GU_NT_BULK, GU_SMEM_BULK, st>>>(a, lb, ob, DB, DB, 1 << 30, 1);
     if (nl) *nl += 2;
 }

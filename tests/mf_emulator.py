@@ -60,7 +60,8 @@ class Symbolic:
         return ch
 
     # ---- numeric replay -------------------------------------------------------------------------------
-    def factorize(self, nzval, eps=1e-13):
+    def factorize(self, nzval, eps=1e-13, extend_add=None):
+        """`extend_add(F, s, c, rl, cb)`, when given, replaces F[ix_(rl, rl)] += cb for child c of front s (lets a test break it)"""
         ns = self.ns
         L = np.zeros(self.lval_size)
         d = np.zeros(self.n)
@@ -77,7 +78,10 @@ class Symbolic:
             F[dst % f, dst // f] = nzval[self.amap_src[a0:a1]]
             for c in ch[s]:                                     # ascending child id
                 rl = self.rel[self.rel_ptr[c]:self.rel_ptr[c + 1]]
-                F[np.ix_(rl, rl)] += cbs[c]
+                if extend_add is None:
+                    F[np.ix_(rl, rl)] += cbs[c]
+                else:
+                    extend_add(F, s, c, rl, cbs[c])
                 cbs[c] = None
             F = np.tril(F)
             for k in range(w):
