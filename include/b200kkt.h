@@ -96,8 +96,8 @@ typedef struct b2_options {
                                 neighbour immediately after that neighbour, in one supernode, and the factorisation takes the pair as
                                 one 2x2 pivot block when |a_kk| < alpha |a_k+1,k| (alpha = (1+sqrt(17))/8) and the block is indefinite,
                                 else as two 1x1 pivots (DESIGN.md section 3).  No rows move at run time.  b2_create accepts PAIRS only
-                                with kkt_n_primal > 0, n_parts == 1, dep_schedule bit 0 set and every front of order <= 64 after the
-                                analysis (B2_ERR_INVALID otherwise, before any device work; b2_create_symbolic_only skips the front-order
+                                with kkt_n_primal > 0, n_parts == 1, dep_schedule bit 0 set and every front of order <= 96 after the
+                                analysis (fronts of order 65..96 run as four-warp teams) (B2_ERR_INVALID otherwise, before any device work; b2_create_symbolic_only skips the front-order
                                 condition so that tooling can inspect the tree).  The dense solver (b2d_create) rejects any value but
                                 STATIC.                                                                                    */
     int32_t reserved[1];
@@ -215,7 +215,7 @@ int b2_debug_trace(b2_solver* s, uint64_t* stamps_h, int32_t* parent_h, int32_t*
  * copied when capacity >= *count. */
 int b2_debug_trace_solve(b2_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count);
 /* Debug (also on a symbolic-only handle): the ticket order of the single-launch factorisation and solve (dep_schedule bit 0, used
- * when every front has order <= 64) over this rank's supernodes: depth from the root descending, then level, then id.  *count =
+ * when every front has order <= 64, or <= 96 with sparse_pivoting = PAIRS) over this rank's supernodes: depth from the root descending, then level, then id.  *count =
  * number of supernodes in it; order_h is filled when capacity >= *count (may be NULL). */
 int b2_debug_dep_order(b2_solver* s, int32_t* order_h, int64_t capacity, int64_t* count);
 

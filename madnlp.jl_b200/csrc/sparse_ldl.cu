@@ -39,6 +39,7 @@ struct Phase {
     // single-launch dependency-driven schedule (used instead of fused + levels when every front is team-class)
     int offAllC = 0, nAllC = 0, maxwAllC = 0;       // every M/B front of the phase (diagonal-block inversion)
     int dep_ngroup = 0, dep_type_off = 0, dep_ptr_off = 0, dep_tasks_off = 0, dep_maxf1 = 0, dep_maxf2 = 0;
+    int dep_maxf4 = 0;                              // PAIRS: the largest front of order 65..96 (0: no four-warp group)
     // single-launch solve (k_solve_dep: the same groups, condition and phase 0 only): persistent CTAs (0: the level-launch solve)
     int sol_grid = 0;
     // its block form (k_solve_dep_block) for 2, 4 and 8 right-hand sides per walk: persistent CTAs of each width
@@ -51,6 +52,7 @@ struct Phase {
 };
 
 constexpr int W_MAX = 64;        // team-per-front classes: f <= 32 (one warp), f <= 64 (two warps)
+constexpr int W_MAX_PAIRS = 96;  // PAIRS adds a four-warp class, 64 < f <= 96 (single-launch schedule only)
 
 }  // namespace
 
@@ -190,11 +192,12 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
         ds.grp_type = sched + P.dep_type_off; ds.grp_ptr = sched + P.dep_ptr_off; ds.tasks = sched + P.dep_tasks_off; ds.ngroup = P.dep_ngroup;
         // (the group ticket in slot nsuper re-arms itself: the CTA that takes the last group resets it)
         cudaMemsetAsync(s->d_flags.p, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
-        const size_t sm = sizeof(double) * std::max<size_t>((size_t)FW_WARPS * TeamSmem<1>::doubles(P.dep_maxf1), (size_t)TeamSmem<2>::doubles(P.dep_maxf2));
+        size_t sm = sizeof(double) * std::max<size_t>((size_t)FW_WARPS * TeamSmem<1>::doubles(P.dep_maxf1), (size_t)TeamSmem<2>::doubles(P.dep_maxf2));
         if (s->pairs) {
             PairArgs pa;
             pa.mask = s->d_pair_mask.p; pa.dsub = s->d_dsub.p; pa.kind = s->d_pkind.p;
-            k_factor_dep_pairs<<<P.dep_ngroup, 128, sm, st>>>(a, s->d_childrec.p, ds, P.dep_maxf1, P.dep_maxf2, s->d_flags.p,
+            if (P.dep_maxf4) sm = std::max(sm, sizeof(double) * TeamSmem<4>::doubles(P.dep_maxf4));
+            k_factor_dep_pairs<<<P.dep_ngroup, 128, sm, st>>>(a, s->d_childrec.p, ds, P.dep_maxf1, P.dep_maxf2, P.dep_maxf4, s->d_flags.p,
                                                               s->d_counters.p + 4, s->d_flags.p + s->S.nsuper, pa);
             return 2;
         }
@@ -346,7 +349,13 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
     return nl;
 }
 
-constexpr size_t SOLVE_DEP_SMEM = sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1>::doubles, (size_t)SolveSmem<2>::doubles);
+// dynamic shared memory of the single-launch solve with NR columns per walk: max(4 one-warp slices, 1 two-warp slice), and on a PAIRS
+// tree with fronts of order 65..96 (maxf4 > 0) one four-warp slice whose panel holds the largest of them
+template <int NR>
+size_t solve_dep_smem(int maxf4) {
+    const size_t d = std::max<size_t>((size_t)4 * SolveSmem<1, NR>::doubles, (size_t)SolveSmem<2, NR>::doubles);
+    return sizeof(double) * (maxf4 ? std::max<size_t>(d, (size_t)SolveSmem<4, NR>::doubles_panel(maxf4)) : d);
+}
 
 // the whole solve of one right-hand side x (original order, in place) as ONE launch of k_solve_dep
 void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
@@ -363,19 +372,14 @@ void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
     ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
     ds.ngroup = P.dep_ngroup;
     if (s->pairs) {
-        k_solve_dep_pairs<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
+        k_solve_dep_pairs<<<P.sol_grid, 128, solve_dep_smem<1>(P.dep_maxf4), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
                                                                    s->S.n, s->d_slots.p, (int64_t)s->d_slots.n, s->d_dsub.p);
         return;
     }
-    k_solve_dep<<<P.sol_grid, 128, SOLVE_DEP_SMEM, st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1, s->S.n,
+    k_solve_dep<<<P.sol_grid, 128, solve_dep_smem<1>(0), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1, s->S.n,
                                                          s->d_slots.p, (int64_t)s->d_slots.n);
 }
 
-// the block solve's dynamic shared memory per width: max(4 one-warp slices, 1 two-warp slice)
-template <int NR>
-constexpr size_t solve_block_smem() {
-    return sizeof(double) * std::max<size_t>((size_t)4 * SolveSmem<1, NR>::doubles, (size_t)SolveSmem<2, NR>::doubles);
-}
 template <int NR>
 const void* solve_block_kernel(bool pairs) {
     return pairs ? (const void*)k_solve_dep_block<NR, true> : (const void*)k_solve_dep_block<NR, false>;
@@ -397,7 +401,7 @@ void enqueue_solve_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
     ds.ngroup = P.dep_ngroup;
     const int w = NR == 2 ? 0 : NR == 4 ? 1 : 2;
     auto kern = s->pairs ? k_solve_dep_block<NR, true> : k_solve_dep_block<NR, false>;
-    kern<<<P.sol_grid_blk[w], 128, solve_block_smem<NR>(), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
+    kern<<<P.sol_grid_blk[w], 128, solve_dep_smem<NR>(P.dep_maxf4), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
                                                                  s->S.n, ncol, s->d_bslots.p, (int64_t)s->d_bslots.n, s->d_dsub.p);
 }
 
@@ -481,6 +485,7 @@ void build_schedule(b2_solver* s) {
     const int rank = std::max(0, s->opt.part_rank);
     const int smax = s->opt.small_front_max;
     const int wmax = std::min(W_MAX, smax);
+    const int tmax = s->pairs ? W_MAX_PAIRS : wmax;   // largest front of the single-launch schedule's team classes
     const int w1max = std::min(32, smax);     // one-warp teams; fused subtrees are built from these only
     const int fuse_max = s->opt.fuse_max_fronts;
     std::vector<int32_t> sched;
@@ -520,14 +525,17 @@ void build_schedule(b2_solver* s) {
         if ((s->opt.dep_schedule & 1) && s->opt.n_parts <= 1 && wmax > 32) {
             bool all_team = true;
             int cntm = 0;
-            for (int sn = 0; sn < ns && all_team; ++sn) if (mine[sn]) { int w, f; fdim(sn, w, f); all_team = f <= wmax; ++cntm; }
+            for (int sn = 0; sn < ns && all_team; ++sn) if (mine[sn]) { int w, f; fdim(sn, w, f); all_team = f <= tmax; ++cntm; }
             if (all_team && cntm > 0) {
                 const std::vector<int32_t> order = dep_ticket_order(S, mine);
                 std::vector<int32_t> gtype, gptr(1, 0), tasks;
                 size_t k = 0;
                 while (k < order.size()) {
                     int w, f; fdim(order[k], w, f);
-                    if (f > 32) {
+                    if (f > W_MAX) {                           // (only a PAIRS tree gets here with such a front: tmax)
+                        gtype.push_back(4); tasks.push_back(order[k]); ++k;
+                        P.dep_maxf4 = std::max(P.dep_maxf4, f);
+                    } else if (f > 32) {
                         gtype.push_back(2); tasks.push_back(order[k]); ++k;
                         P.dep_maxf2 = std::max(P.dep_maxf2, f);
                     } else {
@@ -729,10 +737,10 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
     const int ns = S.nsuper;
     s->pairs = pairs;
     if (pairs && !symbolic_only) {
-        const int fmax = std::min(W_MAX, s->opt.small_front_max);
-        if (S.max_front > fmax) {
-            set_error("b2_create: sparse_pivoting = B2_SPARSE_PIVOT_PAIRS needs every front of order <= " + std::to_string(fmax) +
-                      " after the analysis; the largest has order " + std::to_string(S.max_front));
+        if (S.max_front > W_MAX_PAIRS) {
+            set_error("b2_create: sparse_pivoting = B2_SPARSE_PIVOT_PAIRS needs every front of order <= " + std::to_string(W_MAX_PAIRS) +
+                      " (fronts of order <= 64 run as one- or two-warp teams, 65..96 as a four-warp team) after the analysis; the largest"
+                      " has order " + std::to_string(S.max_front));
             delete s;
             return B2_ERR_INVALID;
         }
@@ -827,7 +835,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(s->d_L.alloc((size_t)S.lp_off[ns] + 2));          // (+2: the bulk-copy staging may read one aligned pair past a panel)
         B2_CUDA_THROW(s->d_Lt.alloc((size_t)S.lp_off[ns]));
         {
-            const int wmax_ = std::min(W_MAX, s->opt.small_front_max);
+            const int wmax_ = pairs ? W_MAX_PAIRS : std::min(W_MAX, s->opt.small_front_max);   // (PAIRS: no front inverts its L11)
             std::vector<int64_t> lo(ns, -1);
             int64_t tot = 0;
             for (int sn = 0; sn < ns; ++sn) {
@@ -842,9 +850,12 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         B2_CUDA_THROW(s->d_ws.alloc((size_t)std::max<int64_t>(1, S.cb_off[ns])));
         B2_CUDA_THROW(s->d_dvec.alloc(n));
         if (pairs) {
-            std::vector<unsigned long long> pm(ns, 0);
+            std::vector<unsigned long long> pm(2 * (size_t)ns, 0);     // two words per supernode: w <= f <= 96
             for (int sn = 0; sn < ns; ++sn)
-                for (int j = S.sn_first[sn]; j < S.sn_first[sn + 1]; ++j) if (S.pair_start[j]) pm[sn] |= 1ull << (j - S.sn_first[sn]);
+                for (int j = S.sn_first[sn]; j < S.sn_first[sn + 1]; ++j) {
+                    const int k = j - S.sn_first[sn];
+                    if (S.pair_start[j]) pm[2 * (size_t)sn + (k >> 6)] |= 1ull << (k & 63);
+                }
             B2_CUDA_THROW(s->d_pair_mask.upload(pm.data(), pm.size()));
             B2_CUDA_THROW(s->d_dsub.alloc(n));
             B2_CUDA_THROW(s->d_pkind.alloc(n));
@@ -866,7 +877,8 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         if (Phase& P = s->phase[0]; P.dep_ngroup) {
             // persistent grid: as many CTAs as fit on the device at once (a size, not a correctness condition), at most one per task
             int per_sm = 0;
-            B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_dep, 128, SOLVE_DEP_SMEM));
+            B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pairs ? (const void*)k_solve_dep_pairs : (const void*)k_solve_dep,
+                                                                        128, solve_dep_smem<1>(P.dep_maxf4)));
             const int ntask = 2 * P.dep_ngroup;
             P.sol_grid = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
             P.n_solve_launches = 1;
@@ -874,7 +886,7 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
             B2_CUDA_THROW(cudaMemset(s->d_slots.p, SLOT_EMPTY_BYTE, s->d_slots.bytes()));     // every slot SLOT_EMPTY
             // block solve: each width's grid from its own occupancy
             const void* bk[3] = {solve_block_kernel<2>(pairs), solve_block_kernel<4>(pairs), solve_block_kernel<8>(pairs)};
-            const size_t bsm[3] = {solve_block_smem<2>(), solve_block_smem<4>(), solve_block_smem<8>()};
+            const size_t bsm[3] = {solve_dep_smem<2>(P.dep_maxf4), solve_dep_smem<4>(P.dep_maxf4), solve_dep_smem<8>(P.dep_maxf4)};
             for (int w = 0; w < 3; ++w) {
                 B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bk[w], 128, bsm[w]));
                 P.sol_grid_blk[w] = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));

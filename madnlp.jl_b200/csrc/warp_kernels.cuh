@@ -38,7 +38,8 @@ struct WarpSched {
 };
 
 // ------------------------------------------------------------------------------------------------ factor
-// A front is owned by a TEAM of NW warps (NW = 1: order <= 32, NW = 2: order <= 64); thread `tid` of the team owns
+// A front is owned by a TEAM of NW warps (NW = 1: order <= 32, NW = 2: order <= 64; NW = 4: order <= 96, PAIRS only, whose pivot
+// loop runs in shared memory); thread `tid` of the team owns
 // ROW tid of the front and keeps it in registers as a sliding window: after pivot k, a[j] holds column k+1+j.
 // Per pivot the only shared-memory traffic is the broadcast of the pivot column (double-buffered, one team barrier).
 // Global loads are issued in independent batches (memory-level parallelism instead of one L2 round trip per element).
@@ -74,8 +75,11 @@ struct TeamSmem {
     static constexpr int FMAX = 32 * NW;
     static constexpr int STAGE = (NW == 1) ? 1024 : 4096;   // doubles; one child always fits (rc^2 <= (FMAX-1)^2)
     static __host__ __device__ int fsize(int maxf) { return (maxf * maxf + 1) & ~1; }   // keeps `stage` 16-byte aligned
+    // the four-warp class (PAIRS fronts of order 65..96) sizes its stage by its largest front: a child's block has rc <= f - 1 of its
+    // parent, so one child still always fits, and a launch whose fronts stop at order 66 needs 78 KB instead of 156 KB
+    static __host__ __device__ int stage(int maxf) { return NW <= 2 ? STAGE : fsize(maxf); }
     static __host__ __device__ int doubles(int maxf) {
-        return fsize(maxf) + 4 * (FMAX + 4) + (MAXC * FMAX) / 2 + MAXC * 4 + STAGE;
+        return fsize(maxf) + 4 * (FMAX + 4) + (MAXC * FMAX) / 2 + MAXC * 4 + stage(maxf);
     }
 };
 
@@ -251,8 +255,9 @@ __device__ __forceinline__ void pivot_iter(double (&av)[32 * NW + 1], double& lp
     lp = l;
 }
 
-// B2_SPARSE_PIVOT_PAIRS (DESIGN.md section 3): bit j of mask[s] marks a candidate 2 x 2 pivot (j, j+1) of front s; the factorisation
-// writes each pivot's kind (B2_PIVOT_*) and D's subdiagonal (b at the first index of a 2 x 2 block, else 0), permuted order
+// B2_SPARSE_PIVOT_PAIRS (DESIGN.md section 3): bit j of the 128-bit mask[2s] | mask[2s+1] << 64 marks a candidate 2 x 2 pivot (j, j+1)
+// of front s; the factorisation writes each pivot's kind (B2_PIVOT_*) and D's subdiagonal (b at the first index of a 2 x 2 block,
+// else 0), permuted order
 struct PairArgs {
     const unsigned long long* mask = nullptr;
     double* dsub = nullptr;
@@ -264,7 +269,9 @@ template <int NW, bool DEP = false, bool PAIRS = false>
 __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const ChildRec* childrec, int s, double* sm_team,
                                                   int tid, int team, int maxf, int& nneg, int& npert, long long* prof = nullptr,
                                                   int* done = nullptr, int* err = nullptr, PairArgs pa = PairArgs()) {
-    constexpr int FMAX = 32 * NW, TEAM = 32 * NW, STAGE = TeamSmem<NW>::STAGE;
+    static_assert(NW <= 2 || (DEP && PAIRS), "the four-warp class runs the single-launch PAIRS factorisation only");
+    constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
+    const int STAGE = TeamSmem<NW>::stage(maxf);
     double* F = sm_team;
     constexpr int CBS = FMAX + 4;                      // four pivot-column buffers
     double* colbuf = F + TeamSmem<NW>::fsize(maxf);    // [4][CBS]
@@ -381,14 +388,14 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
     }
     B2_STAMP(4);
     if (a.ftrace && tid == 0) a.ftrace[3 * (size_t)s + 1] = global_ns();
-    double av[FMAX + 1];
+    double av[NW <= 2 ? FMAX + 1 : 1];                 // (four warps: a row of up to 96 doubles would spill; it stays in F)
     if constexpr (PAIRS) {
         // Pivots with candidate 2 x 2 blocks, right-looking in shared memory (thread = row): pivot k's column (and k+1's for a block)
         // is snapshotted in colbuf, then every row below updates itself.  Rule at a candidate pair with a = F(k,k), b = F(k+1,k),
         // c = F(k+1,k+1): a 2 x 2 block when |a| < alpha |b| and d1 = (a / |b|) c - |b| < 0 (indefinite: one negative and one
         // positive eigenvalue, the count of the reference's num_neg_ev, never perturbed); otherwise k is a 1 x 1 pivot (perturbed to
         // +-eps when |a| < eps, as the static path does) and k+1 an ordinary one.  The multipliers of a block are dsytf2's.
-        const unsigned long long pm = pa.mask[s];
+        const unsigned long long pm = pa.mask[2 * s], pm_hi = (NW > 2) ? pa.mask[2 * s + 1] : 0ull;
         double* u1 = colbuf;
         double* u2 = colbuf + CBS;
         for (int k = 0; k < w;) {
@@ -396,7 +403,7 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
             const double av_ = F[k + k * f];
             bool two = false;
             double b_ = 0.0, c_ = 0.0;
-            if ((pm >> k) & 1ull) {
+            if (((NW <= 2 || k < 64) ? pm >> k : pm_hi >> (k - 64)) & 1ull) {
                 b_ = F[k + 1 + k * f];
                 c_ = F[(k + 1) * (f + 1)];
                 const double t = fabs(b_);
@@ -443,8 +450,10 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
             }
         }
         team_sync<NW>(team);
+        if constexpr (NW <= 2) {
 #pragma unroll
-        for (int j = 0; j < FMAX; ++j) av[j] = (w + j < f && tid < f) ? F[tid + (w + j) * f] : 0.0;
+            for (int j = 0; j < FMAX; ++j) av[j] = (w + j < f && tid < f) ? F[tid + (w + j) * f] : 0.0;
+        }
     } else {
     // row `tid` of the front into registers: a[j] = F(tid, j)
 #pragma unroll
@@ -505,11 +514,16 @@ __device__ __forceinline__ void front_factor_team(const FactorArgs& a, const Chi
     }   // !PAIRS
     B2_STAMP(5);
     // update block first (it is all the parent waits for): av[j] holds column w+j of row tid -- registers only, no barrier needed
+    // (four warps: straight from row tid of F, which only thread tid has written since the pivot loop's last barrier)
     if (tid >= w && tid < f) {
         double* CBo = a.ws + d.cb_off;
         const int ir = tid - w;
+        if constexpr (NW <= 2) {
 #pragma unroll
-        for (int j = 0; j < FMAX; ++j) if (j <= ir) CBo[(size_t)j * r + ir] = av[j];
+            for (int j = 0; j < FMAX; ++j) if (j <= ir) CBo[(size_t)j * r + ir] = av[j];
+        } else {
+            for (int j = 0; j <= ir; ++j) CBo[(size_t)j * r + ir] = F[tid + (w + j) * f];
+        }
     }
     // hand-off: the team barrier orders every thread's stores before thread 0's st.release.gpu (release is cumulative over the
     // barrier's synchronises-with edge -- the CUTLASS semaphore pattern), so no team-wide __threadfence() is needed.  The same
@@ -581,6 +595,8 @@ struct SolveSmem {
     static constexpr int FMAX = 32 * NW;
     // ys/xs [NR][FMAX] | slots [16] | recs [MAXC] (4 doubles each) | panel [FMAX*FMAX]
     static constexpr int doubles = NR * FMAX + 16 + 4 * MAXC + FMAX * FMAX;
+    // the same slice with the panel sized by the largest front it holds (the four-warp class: FMAX^2 would be 128 KB)
+    static __host__ __device__ constexpr int doubles_panel(int maxf) { return NR * FMAX + 16 + 4 * MAXC + maxf * maxf; }
 };
 
 // DEP: the front runs inside the single-launch solve (k_solve_dep).  It reads its right-hand side straight from the caller's
@@ -594,6 +610,7 @@ struct SolveSmem {
 template <int NW, bool DEP = false, int NR = 1>
 __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRec* childrec, int s, double* sm_team, int tid, int team,
                                                int* err = nullptr, int ncol = 1, int64_t ldx = 0) {
+    static_assert(NW <= 2 || DEP, "the four-warp class runs in the single-launch solve only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* ys = sm_team;                              // [NR][FMAX] assembly of the front's rhs
     double* yb = ys + NR * FMAX;                       // [2][8] broadcast slots
@@ -669,7 +686,7 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
                 }
             }
         }
-    } else {
+    } else if (NW == 2) {
         // two-warp team, blocked by warp: warp 0 eliminates pivots 0..31 among its own rows with shuffles and publishes
         // them; warp 1 applies them in one parallel pass, then eliminates pivots 32.. among its rows -- two barriers per
         // front instead of one per pivot
@@ -721,6 +738,45 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
                 }
             }
         }
+    } else {
+        // four-warp team, blocked by warp as above: in round b, warp b (which has applied blocks < b) eliminates pivots
+        // [32b, 32b+32) among its own rows with shuffles and publishes them; every warp below applies them in one pass
+        const int wp = tid >> 5;
+        for (int kb = 0; kb < w; kb += 32) {
+            const int ke = min(w, kb + 32);
+            if (wp == kb >> 5) {
+                for (int k0 = kb; k0 < ke; k0 += 8) {
+                    double l[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { const int k = k0 + u; l[u] = (k < ke && tid > k && tid < f) ? P[k * f + tid] : 0.0; }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        const int k = k0 + u;
+                        if (k < ke) {
+#pragma unroll
+                            for (int q = 0; q < NR; ++q) y[q] = fma(-l[u], __shfl_sync(0xffffffffu, y[q], k - kb), y[q]);
+                        }
+                    }
+                }
+                if (tid < ke) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) ys[q * FMAX + tid] = y[q];
+                }
+            }
+            team_sync<NW>(team);
+            if (wp > (kb >> 5) && tid < f) {
+                double acc[NR];
+#pragma unroll
+                for (int q = 0; q < NR; ++q) acc[q] = 0.0;
+#pragma unroll 8
+                for (int k = kb; k < ke; ++k) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) acc[q] = fma(P[k * f + tid], ys[q * FMAX + k], acc[q]);
+                }
+#pragma unroll
+                for (int q = 0; q < NR; ++q) y[q] -= acc[q];
+            }
+        }
     }
     if (DEP) {
         if constexpr (NR == 1) {
@@ -742,6 +798,7 @@ __device__ __forceinline__ void front_fwd_team(const SolveArgs& a, const ChildRe
 template <int NW, bool DEP = false, bool PAIRS = false>
 __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double* sm_team, int tid, int team,
                                                const ChildRec* childrec = nullptr, int* err = nullptr, const double* dsub = nullptr) {
+    static_assert(NW <= 2 || DEP, "the four-warp class runs in the single-launch solve only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* xs = sm_team;                              // [FMAX] gathered ancestor values at [xa, xa + r)
     double* xb = xs + FMAX;                            // [2][8]
@@ -818,7 +875,7 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
                 if (k >= 1) t = fma(-l[u], __shfl_sync(0xffffffffu, t, k), t);
             }
         }
-    } else {
+    } else if (NW == 2) {
         // blocked by warp (see the forward sweep): warp 1 finishes columns 32.. with shuffles and publishes them in
         // xs[32..w) (the gathered ancestors occupy xs[0 .. f-w) with f - w < 32 here, or xs[w .. f) with DEP); warp 0 applies
         // them in one pass
@@ -856,6 +913,36 @@ __device__ __forceinline__ void front_bwd_team(const SolveArgs& a, int s, double
                 }
             }
         }
+    } else {
+        // four-warp team, last block first: in round b, warp b (which has applied blocks > b) finishes columns [32b, 32b+32) with
+        // shuffles and publishes them in xs[32b..) (own pivots' region: the ancestors are at xs[w .. f)); every warp above applies
+        // them in one pass
+        const int wp = tid >> 5;
+        for (int kb = ((w - 1) >> 5) * 32; kb >= 0; kb -= 32) {
+            const int ke = min(w, kb + 32);
+            if (wp == kb >> 5) {
+                for (int k0 = ke - 1; k0 >= kb + 1; k0 -= 8) {
+                    double l[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { const int k = k0 - u; l[u] = (k >= kb + 1 && tid < k) ? P[k * w + tid] : 0.0; }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        const int k = k0 - u;
+                        if (k >= kb + 1) t = fma(-l[u], __shfl_sync(0xffffffffu, t, k - kb), t);
+                    }
+                }
+                if (kb > 0 && tid < w) xs[tid] = t;
+            }
+            if (kb > 0) {
+                team_sync<NW>(team);
+                if (wp < (kb >> 5)) {
+                    double acc = 0.0;
+#pragma unroll 8
+                    for (int k = kb; k < ke; ++k) acc = fma(P[k * w + tid], xs[k], acc);
+                    t -= acc;
+                }
+            }
+        }
     }
     if (DEP) {
         if (tid < w) { xs[tid] = t; a.x[pj] = t; }
@@ -886,6 +973,7 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
                                                 int* err, const double* dsub, int ncol, int64_t ldx) {
     static_assert(NR % 2 == 0, "block slots are accessed in 16-byte pairs");
     static_assert(DEP || !PAIRS, "pair factors are solved on the single-launch schedule only");
+    static_assert(NW <= 2 || (DEP && PAIRS), "the four-warp class holds PAIRS fronts on the single-launch schedule only");
     constexpr int FMAX = 32 * NW, TEAM = 32 * NW;
     double* xs = sm_team;                              // [NR][FMAX] gathered ancestor values at [xa, xa + r)
     double* xb = xs + NR * FMAX;                       // [2][8]
@@ -981,7 +1069,7 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
                 }
             }
         }
-    } else {
+    } else if (NW == 2) {
         // blocked by warp (front_bwd_team): warp 1 finishes columns 32.. and publishes them in xs[32..w); warp 0 applies them
         if (w > 32) {
             if (tid >= 32) {
@@ -1029,6 +1117,46 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
 #pragma unroll
                         for (int q = 0; q < NR; ++q) t[q] = fma(-l[u], __shfl_sync(0xffffffffu, t[q], k), t[q]);
                     }
+                }
+            }
+        }
+    } else {
+        // four-warp team, last block first (front_bwd_team)
+        const int wp = tid >> 5;
+        for (int kb = ((w - 1) >> 5) * 32; kb >= 0; kb -= 32) {
+            const int ke = min(w, kb + 32);
+            if (wp == kb >> 5) {
+                for (int k0 = ke - 1; k0 >= kb + 1; k0 -= 8) {
+                    double l[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { const int k = k0 - u; l[u] = (k >= kb + 1 && tid < k) ? P[k * w + tid] : 0.0; }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        const int k = k0 - u;
+                        if (k >= kb + 1) {
+#pragma unroll
+                            for (int q = 0; q < NR; ++q) t[q] = fma(-l[u], __shfl_sync(0xffffffffu, t[q], k - kb), t[q]);
+                        }
+                    }
+                }
+                if (kb > 0 && tid < w) {
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) xs[q * FMAX + tid] = t[q];
+                }
+            }
+            if (kb > 0) {
+                team_sync<NW>(team);
+                if (wp < (kb >> 5)) {
+                    double acc[NR];
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) acc[q] = 0.0;
+#pragma unroll 8
+                    for (int k = kb; k < ke; ++k) {
+#pragma unroll
+                        for (int q = 0; q < NR; ++q) acc[q] = fma(P[k * w + tid], xs[q * FMAX + k], acc[q]);
+                    }
+#pragma unroll
+                    for (int q = 0; q < NR; ++q) t[q] -= acc[q];
                 }
             }
         }
@@ -1138,9 +1266,10 @@ __global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a
 // ------------------------------------------------------------------------------------------------ single-launch schedule
 // The whole (team-class) elimination tree in ONE launch per sweep: CTAs are issued in topological order, a front waits on
 // its children's completion flags (acquire loads on global memory, bounded spin) instead of on a kernel boundary.  A CTA
-// of 128 threads runs a GROUP of tasks: four one-warp teams (fronts of order <= 32) or one two-warp team (order <= 64).
+// of 128 threads runs a GROUP of tasks: four one-warp teams (fronts of order <= 32) or one two-warp team (order <= 64); with PAIRS
+// also one four-warp team (order 65..96).
 struct DepSched {
-    const int32_t* grp_type;   // 1 or 2 (warps per team)
+    const int32_t* grp_type;   // 1 or 2 (warps per team); PAIRS also 4 (one front of order 65..96)
     const int32_t* grp_ptr;    // [ngroup+1] into tasks
     const int32_t* tasks;      // supernode ids in topological ticket order (dep_ticket_order in sparse_ldl.cu)
     int ngroup;
@@ -1180,9 +1309,10 @@ __global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec
 }
 
 // k_factor_dep with candidate 2 x 2 pivots (b2_options.sparse_pivoting = B2_SPARSE_PIVOT_PAIRS): the same schedule and hand-offs,
-// front_factor_team's PAIRS pivot loop.  A separate kernel, so that the static one is compiled exactly as before.
+// front_factor_team's PAIRS pivot loop.  A separate kernel, so that the static one is compiled exactly as before.  Its groups also
+// come as type 4: one front of order 65..96 as a four-warp team (the pair ordering makes fronts larger: DESIGN.md section 3).
 __global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const ChildRec* childrec, DepSched ds, int maxf1, int maxf2,
-                                                          int* done, int* err, int* ticket, PairArgs pa) {
+                                                          int maxf4, int* done, int* err, int* ticket, PairArgs pa) {
     extern __shared__ __align__(16) double sm[];
     const int g = claim_group(ticket, ds.ngroup);
     const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
@@ -1192,10 +1322,14 @@ __global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const Ch
         if (team < n) front_factor_team<1, true, true>(a, childrec, ds.tasks[t0 + team], sm + (size_t)team * TeamSmem<1>::doubles(maxf1),
                                                        tid, team, maxf1, nneg, npert, nullptr, done, err, pa);
         if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
-    } else {
+    } else if (type == 2) {
         const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
         if (team < n) front_factor_team<2, true, true>(a, childrec, ds.tasks[t0 + team], sm, tid, team, maxf2, nneg, npert, nullptr, done, err, pa);
         if (tid == 0 && team < n) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
+    } else {
+        const int tid = threadIdx.x;
+        front_factor_team<4, true, true>(a, childrec, ds.tasks[t0], sm, tid, 0, maxf4, nneg, npert, nullptr, done, err, pa);
+        if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
     }
 }
 
@@ -1275,10 +1409,10 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRe
 }
 
 // k_solve_dep for a PAIRS factor (D with 2 x 2 blocks, front_bwd_team<.., PAIRS>); a separate kernel, so that the static one is
-// compiled exactly as before
+// compiled exactly as before.  A type-4 group is one front of order 65..96 on a four-warp slice (SolveSmem<4>::doubles_panel).
 __global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl,
                                                          int n, double* slots, int64_t nslot, const double* dsub) {
-    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
+    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice, 1 four-warp slice)
     double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
     __shared__ int tk_sh, bad_sh;
     const int ntask = 2 * ds.ngroup;
@@ -1290,16 +1424,18 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const C
         const bool fwd = t < ds.ngroup;
         const int g = fwd ? t : ntask - 1 - t;
         const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
-        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
-        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        const int team = (type == 1) ? (threadIdx.x >> 5) : (type == 2) ? (threadIdx.x >> 6) : 0;
+        const int tid = (type == 1) ? (threadIdx.x & 31) : (type == 2) ? (threadIdx.x & 63) : threadIdx.x;
         if (team < cnt) {
             const int s = ds.tasks[t0 + team];
             if (fwd) {
                 if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, err);
-                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
+                else if (type == 2) front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
+                else front_fwd_team<4, true>(a, childrec, s, smd, tid, 0, err);
             } else {
                 if (type == 1) front_bwd_team<1, true, true>(a, s, sm1[team], tid, team, childrec, err, dsub);
-                else front_bwd_team<2, true, true>(a, s, smd, tid, team, childrec, err, dsub);
+                else if (type == 2) front_bwd_team<2, true, true>(a, s, smd, tid, team, childrec, err, dsub);
+                else front_bwd_team<4, true, true>(a, s, smd, tid, 0, childrec, err, dsub);
             }
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)
@@ -1327,8 +1463,10 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const C
 // and never read from or written to x.  Each column goes through the operations of the one-column kernel in the same order, so
 // column q of the result is bit-identical to a one-column solve of column q.  `slots` are the block slots (up | down | ypiv, NR words
 // per index); the {ticket, CTAs out} counters are k_solve_dep's.
+// (PAIRS: a minimum of one CTA per SM lifts ptxas's 128-register target, under which the four-warp class spilled 48 bytes at NR = 4;
+// the static instantiations compile exactly as without the minimum)
 template <int NR, bool PAIRS>
-__global__ void __launch_bounds__(128) k_solve_dep_block(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
+__global__ void __launch_bounds__(128, PAIRS ? 1 : 0) k_solve_dep_block(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
                                                          int ncol, double* slots, int64_t nslot, const double* dsub) {
     extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
     double (*sm1)[SolveSmem<1, NR>::doubles] = (double (*)[SolveSmem<1, NR>::doubles])smd;
@@ -1342,16 +1480,25 @@ __global__ void __launch_bounds__(128) k_solve_dep_block(SolveArgs a, const Chil
         const bool fwd = t < ds.ngroup;
         const int g = fwd ? t : ntask - 1 - t;
         const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
-        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
-        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
+        int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
+        if constexpr (PAIRS) {                          // (type 4: one front of order 65..96 as a four-warp team)
+            if (type == 4) { team = 0; tid = threadIdx.x; }
+        }
         if (team < cnt) {
             const int s = ds.tasks[t0 + team];
             if (fwd) {
                 if (type == 1) front_fwd_team<1, true, NR>(a, childrec, s, sm1[team], tid, team, err, ncol, n);
-                else front_fwd_team<2, true, NR>(a, childrec, s, smd, tid, team, err, ncol, n);
+                else if constexpr (PAIRS) {
+                    if (type == 4) front_fwd_team<4, true, NR>(a, childrec, s, smd, tid, 0, err, ncol, n);
+                    else front_fwd_team<2, true, NR>(a, childrec, s, smd, tid, team, err, ncol, n);
+                } else front_fwd_team<2, true, NR>(a, childrec, s, smd, tid, team, err, ncol, n);
             } else {
                 if (type == 1) front_bwd_block<1, PAIRS, NR>(a, s, sm1[team], tid, team, childrec, err, dsub, ncol, n);
-                else front_bwd_block<2, PAIRS, NR>(a, s, smd, tid, team, childrec, err, dsub, ncol, n);
+                else if constexpr (PAIRS) {
+                    if (type == 4) front_bwd_block<4, PAIRS, NR>(a, s, smd, tid, 0, childrec, err, dsub, ncol, n);
+                    else front_bwd_block<2, PAIRS, NR>(a, s, smd, tid, team, childrec, err, dsub, ncol, n);
+                } else front_bwd_block<2, PAIRS, NR>(a, s, smd, tid, team, childrec, err, dsub, ncol, n);
             }
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Factorise, solve and one IPMLinearAlgebra.step with sparse_pivoting = PAIRS against STATIC (CUDA events, medians over --reps),
-on sparse_free_lp and on case10000_goc's SparseKKTSystem.  A configuration that b2_create refuses is reported as refused.
+on sparse_free_lp and on case1354_pegase's and case10000_goc's SparseKKTSystem.  A configuration that b2_create refuses is reported as refused.
 
     python tools/bench_sparse_pairs.py [--reps 50]
 """
@@ -42,10 +42,11 @@ def _time(fn, reps):
 def _cases():
     lp, it = W.sparse_free_lp(n=20000, m=8000, n_free=3000, n_eq=5000)
     yield "sparse_free_lp", o.Callback(lp.n, lp.m, lp.jac_I, lp.jac_J, lp.hess_I, lp.hess_J, lp.ind_ineq, lp.ind_lb, lp.ind_ub), it
-    model, st = W.acopf_case("case10000_goc")
-    i0 = W.ipm_iterates(model, st, 1, seed=3)[0]
-    it = dict(jac=i0.jac, hess=i0.hess, rhs=i0.rhs, **{f: getattr(i0, f) for f in FIELDS})
-    yield "case10000_goc", o.Callback(st.nvar, st.ncon, st.jac_I, st.jac_J, st.hess_I, st.hess_J, st.ind_ineq, st.ind_lb, st.ind_ub), it
+    for case in ("case1354_pegase", "case10000_goc"):
+        model, st = W.acopf_case(case)
+        i0 = W.ipm_iterates(model, st, 1, seed=3)[0]
+        it = dict(jac=i0.jac, hess=i0.hess, rhs=i0.rhs, **{f: getattr(i0, f) for f in FIELDS})
+        yield case, o.Callback(st.nvar, st.ncon, st.jac_I, st.jac_J, st.hess_I, st.hess_J, st.ind_ineq, st.ind_lb, st.ind_ub), it
 
 
 def main():

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Symbolic cost of sparse_pivoting = PAIRS against STATIC (host analysis only, no GPU): nnz(L), levels, the largest front and
-whether every front is still team-class (order <= 64, what b2_create needs to accept PAIRS), for the augmented and unreduced KKT
+whether b2_create accepts PAIRS on the tree (every front of order <= 96: one- and two-warp teams up to 64, a four-warp team above),
+for the augmented and unreduced KKT
 patterns of the given AC-OPF cases.
 
     python tools/pair_pivot_report.py case1354_pegase case10000_goc
@@ -21,7 +22,7 @@ W = pkg.workloads
 
 
 def main(cases):
-    print(f"{'case':18s} {'pattern':10s} {'pivoting':8s} {'nnz(L)':>12s} {'levels':>7s} {'max front':>9s} {'team-class':>10s} {'pairs':>7s}")
+    print(f"{'case':18s} {'pattern':10s} {'pivoting':8s} {'nnz(L)':>12s} {'levels':>7s} {'max front':>9s} {'accepted':>10s} {'pairs':>7s}")
     for case in cases:
         st = W.acopf_case(case)[1]
         cb = o.Callback(st.nvar, st.ncon, st.jac_I, st.jac_J, st.hess_I, st.hess_J, st.ind_ineq, st.ind_lb, st.ind_ub)
@@ -38,7 +39,7 @@ def main(cases):
                 S = PairSymbolic(k.N, cp, rv, sparse_pivoting=piv, **kw)
                 st_ = S.stats
                 print(f"{case:18s} {pattern:10s} {('PAIRS' if piv else 'STATIC'):8s} {st_['nnz_l']:12d} {st_['n_levels']:7d} "
-                      f"{st_['max_front']:9d} {str(st_['max_front'] <= 64):>10s} {int(S.pair_start.sum()):7d}", flush=True)
+                      f"{st_['max_front']:9d} {str(st_['max_front'] <= 96):>10s} {int(S.pair_start.sum()):7d}", flush=True)
 
 
 if __name__ == "__main__":
