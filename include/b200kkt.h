@@ -307,8 +307,11 @@ int b2d_copy_diag(int32_t n, int32_t lda, const double* A_d, double* d_d, void* 
 
 /* The same assembly with the J' D J contraction on the Hopper tensor cores: fp64 is cut into 8 signed 7-bit digits per entry
  * (Ozaki scheme) and the 36 digit-pair products run as exact int8 GEMMs on wgmma.mma_async (s8) with TMA-staged operands
- * (csrc/ozaki_kernels.cuh); the result agrees with the fp64 contraction to ~1e-14 of max|W| (parity bar 1e-13,
- * tests/test_gpu_parity_large.py).  The plan owns the digit planes (8 * n_pad * ns_pad bytes), exponents, tile list and tensor maps.
+ * (csrc/ozaki_kernels.cuh).  Entry by entry, with a = sqrt(D) J_I and e_m the frexp exponent of max_i |a_im|:
+ *   |W^ - W|_mn <= 2^-51 ns 2^(e_m + e_n) + 2^-52 (|W| + |H_mn| + |pr_m|)
+ * from the truncation of each entry below 2^-56 of its column's maximum, the digit pairs s + t >= 8 that are never multiplied
+ * (2^-53.2 per term) and the fp64 Horner sum; results under- and overflow as the fp64 contraction's do, and a column holding
+ * a NaN or an Inf gives NaN in its row and column (tests/test_gpu_dense_assembly_entrywise.py).  The plan owns the digit planes (8 * n_pad * ns_pad bytes), exponents, tile list and tensor maps.
  * ns <= 16384.  b2d_ozaki_plan_status reports whether a (bounded) pipeline wait ever timed out. */
 typedef struct b2d_ozaki_plan b2d_ozaki_plan;
 int b2d_ozaki_plan_create(int32_t n, int32_t ns, b2d_ozaki_plan** out);

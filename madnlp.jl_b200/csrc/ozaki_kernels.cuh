@@ -9,6 +9,10 @@
 //   2. G_d = sum_{s+t=d} Q_s' Q_t  for d = 0..S-1 : 36 exact int8 x int8 -> int32 GEMMs (|G_d| <= 8 * K * 127^2 < 2^31 for
 //      K <= 16384), the d-sums accumulate inside the wgmma accumulators
 //   3. W(m,n) = 2^(e_m + e_n - 14) * sum_d 2^(-7d) G_d(m,n)   evaluated in fp64 (Horner) by the epilogue
+//   A column holding a NaN or an Inf makes its row and column of W NaN (the fp64 contraction is non-finite there).
+//   Error (DESIGN.md section 3, checked entry by entry in tests/test_dense_assembly_entrywise_oracle.py):
+//   |W^ - W| <= 2^-51 ns 2^(e_m + e_n) before the final rounding -- truncation below 2^-56 of the column max (2^-55), the
+//   dropped digit pairs s + t >= 8 (127^2 sum_{d>=8} (15 - d) 2^(-7(d+2)) = 2^-53.2) and the Horner sum (~2^-53), per term
 //
 // Kernel (one 64 x 64 output tile per CTA, 288 threads):
 //   warp 8 lane 0 : TMA producer  -- the 8 A-digit tiles and 8 B-digit tiles of a 64-deep K block into a 3-stage ring
@@ -19,6 +23,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <cfloat>
 #include <cstdint>
 
 #include "ptx.cuh"
@@ -39,6 +44,10 @@ static_assert(S * BN * GLD * 4 <= STAGES * STAGE_BYTES, "the parked accumulators
 constexpr uint32_t SPIN_MAX = 1u << 22;                             // tries of a bounded mbarrier wait
 
 // ------------------------------------------------------------------------------------------------ digit split
+// expo[m] of a column that holds a NaN or an Inf: the epilogue writes NaN wherever row m or column m of W is read, as the fp64
+// contraction would give a non-finite value there (frexp exponents of finite doubles lie in [-1073, 1024])
+constexpr int EXPO_NONFINITE = 1 << 20;
+
 // one CTA per column m of the operand A (K x M): a(i, m) = (scale ? sqrt(scale[i]) : 1) * src[m*lds + (rows ? rows[i] : i)];
 // exponent of the column, then S int8 digits per element into Q[s][m][i] (row length Kpad, rows beyond K stay zero)
 __global__ void __launch_bounds__(256) k_ozaki_split(int K, int Kpad, int Mpad, const double* __restrict__ src, int64_t lds,
@@ -48,20 +57,22 @@ __global__ void __launch_bounds__(256) k_ozaki_split(int K, int Kpad, int Mpad, 
     const double* col = src + (size_t)m * lds;
     __shared__ double red[256];
     double mx = 0.0;
+    int bad = 0;
     for (int i = threadIdx.x; i < K; i += 256) {
-        const double a = col[rows ? rows[i] : i] * (scale ? sqrt(scale[i]) : 1.0);
-        mx = fmax(mx, fabs(a));
+        const double a = fabs(col[rows ? rows[i] : i] * (scale ? sqrt(scale[i]) : 1.0));
+        mx = fmax(mx, a);                           // (fmax drops a NaN: the flag catches it)
+        bad |= !(a <= DBL_MAX);
     }
     red[threadIdx.x] = mx;
-    __syncthreads();
+    bad = __syncthreads_or(bad);
     for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + o]); __syncthreads(); }
     mx = red[0];
     int e = 0;
-    if (mx > 0.0 && mx < 1e300) frexp(mx, &e);      // mx = f * 2^e, f in [0.5, 1)  ->  |a| * 2^-e < 1   (inf/nan columns: digits 0)
+    if (bad) e = EXPO_NONFINITE;
+    else if (mx > 0.0) frexp(mx, &e);               // mx = f * 2^e, f in [0.5, 1)  ->  |a| * 2^-e < 1 (subnormal mx included)
     if (threadIdx.x == 0) expo[m] = e;
     for (int i = threadIdx.x; i < K; i += 256) {
-        double x = ldexp(col[rows ? rows[i] : i] * (scale ? sqrt(scale[i]) : 1.0), -e);    // exact scaling
-        if (!(fabs(x) < 1.0)) x = 0.0;
+        double x = bad ? 0.0 : ldexp(col[rows ? rows[i] : i] * (scale ? sqrt(scale[i]) : 1.0), -e);    // exact scaling
 #pragma unroll
         for (int s = 0; s < S; ++s) {
             x *= (double)(1 << WB);                 // exact
@@ -106,8 +117,8 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// 2^e for |e| <= 1022 (exponent field only)
-__device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(min(max(e, -1022), 1023) + 1023) << 52); }
+// 2^e for -1022 <= e <= 1023 (exponent field only)
+__device__ __forceinline__ double pow2i(int e) { return __longlong_as_double((long long)(e + 1023) << 52); }
 
 // accumulators of consumer warpgroup G: {0, 1, 6, 7} and {2, 3, 4, 5} -- d has d + 1 digit pairs, 18 pairs each
 __host__ __device__ constexpr int acc_digit(int G, int j) { return G == 0 ? (j < 2 ? j : j + 4) : j + 2; }
@@ -207,8 +218,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
     const int ml = threadIdx.x & (BM - 1);
     const int m = bm * BM + ml;
     const int em = expo[m];
-    const double pm = pow2i(em - 2 * WB);                 // 2^(e_m - 14): exact scaling factors, applied as two
-                                                          // multiplications (cheaper than one ldexp per entry)
 #pragma unroll 4
     for (int nl = threadIdx.x >> 6; nl < BN; nl += 256 / BM) {
         const int n = bn * BN + nl;
@@ -216,7 +225,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_ozaki_syrk(const __grid_constan
 #pragma unroll
         for (int d = S - 1; d >= 0; --d) h = fma(h, 1.0 / (1 << WB), (double)Gs[((size_t)d * BN + nl) * GLD + ml]);
         if (n < nvalid && m < nvalid && (!lower_only || m >= n)) {
-            double v = (h * pm) * pow2i(expo[n]);
+            const int en = expo[n], E = em + en - 2 * WB;
+            // h * 2^E rounded once (the bits of ldexp, without its branches), so W underflows and overflows where the fp64
+            // contraction does: h = 0 or 2^-49 <= |h| < 2^29, so h * 2^A is exact, and the second product rounds
+            const int A = min(max(E, -970), 990);
+            double v = (h * pow2i(A)) * pow2i(min(max(E - A, -1022), 1023));
+            if (em == EXPO_NONFINITE || en == EXPO_NONFINITE) v = __longlong_as_double(0x7ff8000000000000LL);
             if (hess) v += hess[(size_t)n * ldh + m];
             if (pr && m == n) v += pr[m];
             C[(size_t)n * ldc + m] = v;
