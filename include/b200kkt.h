@@ -375,6 +375,35 @@ int b2_unreduced_solve_pre(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, c
                            const double* u_lower_aug_d, double* w_d, void* stream);
 int b2_unreduced_solve_post(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const double* l_lower_aug_d,
                             const double* u_lower_aug_d, double* w_d, void* stream);
+/* ScaledSparseKKTSystem (K2.5, src/KKT/Sparse/scaled_augmented.jl): the augmented system under the congruence by the scaling factor
+ * s = sqrt((x - xl)(xu - x)) over the bounds a variable has.  Here l_diag = x - xl and u_diag = xu - x, both positive (the opposite
+ * sign of the reduced systems').  One launch each, one thread per variable (b2_bounds' inverse maps), no atomics; every formula is
+ * evaluated with rounding intrinsics in the reference's order, so the results are bit-identical to its broadcasts.
+ *   b2_scaled_set_aug_diagonal   _set_aug_diagonal! (IPM/kernels.jl:47-68): s = (1 * sqrt(l_diag)) * sqrt(u_diag) (factors of the
+ *                                bounds present), pr_diag = (xlzu + xuzl) + reg * (s * s) with xlzu = u_lower * l_diag, xuzl = l_lower *
+ *                                u_diag (0 for a missing multiplier, times the other bound's distance when there is one); scaling = s
+ *   b2_scaled_transfer           build_kkt! (scaled_augmented.jl:209-236) on aug_com: transfer! through the plan of the K2 COO layout
+ *                                with each source scaled before the slot's sum (pr_diag and du_diag sources by 1, Hessian sources
+ *                                (v s_i) s_j, Jacobian and slack sources v s_j).  colptr / rowval: aug_com's pattern on the device, n columns
+ *   b2_scaled_solve_pre / _post  solve_kkt! (IPM/factorization.jl:48-74) around b2_solve on primal_dual(w):
+ *                                pre xp = xp s + (r3 + r4); post xp = xp s, wzl = (wzl - l_lower xp) / l_diag,
+ *                                wzu = (-wzu + u_lower xp) / u_diag
+ *   b2_scaled_kktmul             mul!'s diagonal and bound part (IPM/factorization.jl:239-251), after the three SpMVs of b2_kktmul's
+ *                                callers: the bound rows take + xzl l_diag and - xzu u_diag
+ *   b2_scaled_regularize_diagonal regularize_diagonal! (scaled_augmented.jl:238-242): reg += dw; pr_diag += dw (s s); du_diag -= dc */
+int b2_scaled_set_aug_diagonal(b2_bounds* b, const double* reg_d, const double* l_lower_d, const double* l_diag_d,
+                               const double* u_lower_d, const double* u_diag_d, double* pr_diag_d, double* scaling_d, void* stream);
+int b2_scaled_transfer(b2_transfer_plan* p, int64_t n, int64_t n_tot, const int32_t* colptr_d, const int32_t* rowval_d,
+                       const double* scaling_d, double* dst_nz_d, const double* V_d, void* stream);
+int b2_scaled_solve_pre(b2_bounds* b, int64_t m, const double* l_diag_d, const double* u_diag_d, const double* scaling_d, double* w_d,
+                        void* stream);
+int b2_scaled_solve_post(b2_bounds* b, int64_t m, const double* l_lower_d, const double* u_lower_d, const double* l_diag_d,
+                         const double* u_diag_d, const double* scaling_d, double* w_d, void* stream);
+int b2_scaled_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const double* du_diag_d, const double* l_lower_d,
+                     const double* u_lower_d, const double* l_diag_d, const double* u_diag_d, double alpha, double beta,
+                     const double* x_d, double* w_d, void* stream);
+int b2_scaled_regularize_diagonal(int64_t n_tot, int64_t m, double dw, double dc, const double* scaling_d, double* reg_d,
+                                  double* pr_diag_d, double* du_diag_d, void* stream);
 /* reg += dw; pr_diag += dw; du_diag -= dc   (KKTsystem.jl:222-226) */
 int b2_regularize_diagonal(int64_t n_tot, int64_t m, double dw, double dc, double* reg_d, double* pr_diag_d,
                            double* du_diag_d, void* stream);
@@ -534,6 +563,11 @@ int b2_set_aug_rr(b2_bounds* b, int64_t m, double del_w, double del_c, double ze
                   const double* nn_d, const double* zp_d, const double* zn_d, const double* x_d, const double* xl_d, const double* xu_d,
                   const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d, double* u_lower_d,
                   double* l_diag_d, double* u_diag_d, void* stream);
+/* set_aug_RR!(::ScaledSparseKKTSystem) (:89-104): b2_set_aug_rr with l_diag = x_lr - xl_r and u_diag = xu_r - x_ur (K2.5's signs) */
+int b2_set_aug_rr_scaled(b2_bounds* b, int64_t m, double del_w, double del_c, double zeta, const double* D_R_d, const double* pp_d,
+                         const double* nn_d, const double* zp_d, const double* zn_d, const double* x_d, const double* xl_d, const double* xu_d,
+                         const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d, double* u_lower_d,
+                         double* l_diag_d, double* u_diag_d, void* stream);
 /* set_aug_rhs_RR! (:133-158): p = [ -f_R + zl - zu - jacl | -c + pp - nn + (mu_R - (rho - y) pp) ./ zp - (mu_R - (rho + y) nn) ./ zn |
  *                                  (xl_r - x_lr) zl_r + mu_R | (xu_r - x_ur) zu_r - mu_R ] */
 int b2_set_aug_rhs_rr(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d,
@@ -594,6 +628,11 @@ int b2_get_varphi_d_r(b2_bounds* b, int64_t m, const double* f_R_d, const double
 int b2_set_aug_diagonal_iterate(b2_bounds* b, int64_t m, double del_w, double del_c, const double* x_d, const double* xl_d, const double* xu_d,
                                 const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d,
                                 double* u_lower_d, double* l_diag_d, double* u_diag_d, void* stream);
+/* set_aug_diagonal!(::ScaledSparseKKTSystem, solver) (:36-45) before b2_scaled_set_aug_diagonal: b2_set_aug_diagonal_iterate with
+ * l_diag = x_lr - xl_r and u_diag = xu_r - x_ur (K2.5's signs) */
+int b2_set_aug_diagonal_iterate_scaled(b2_bounds* b, int64_t m, double del_w, double del_c, const double* x_d, const double* xl_d,
+                                       const double* xu_d, const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d,
+                                       double* l_lower_d, double* u_lower_d, double* l_diag_d, double* u_diag_d, void* stream);
 /* set_aug_rhs!(solver, kkt, w, mu) (:113-130) then dual_inf_perturbation!(px, ind_llb, ind_uub, mu, kappa_d) (:818-823) in one launch,
  * bit-identical to b2_set_aug_rhs followed by the perturbation: p = [-f + zl - zu - jacl | -w | (xl_r - x_lr) zl_r + mu | (xu_r - x_ur) zu_r
  * - mu], then px[ind_llb] -= mu kappa_d, px[ind_uub] += mu kappa_d (mu kappa_d formed once).  w = c when c_trial_d is NULL, else
@@ -889,6 +928,10 @@ int b2_inertia_loop_destroy(b2_inertia_loop* h);
 /* any graph the handle held is dropped; reg, pr_diag (n_tot), du_diag (m) are baked in */
 int b2_inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
                           int32_t dual_always, void* stream);
+/* b2_inertia_loop_begin for ScaledSparseKKTSystem: the regularisation is b2_scaled_regularize_diagonal's, pr_diag += dw (s s) with
+ * scaling_d the system's scaling factor (n_tot) */
+int b2_inertia_loop_begin_scaled(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
+                                 const double* scaling_d, int32_t dual_always, void* stream);
 /* expect_pos / expect_neg as for b2_refine_loop_end; b, w, x (n) and norms_d (3 doubles) as for b2_refine_loop_begin */
 int b2_inertia_loop_refine(b2_inertia_loop* h, const b2_inertia_source* src, int64_t expect_pos, int64_t expect_neg, int64_t n,
                            const double* b_d, double* w_d, double* x_d, double* norms_d, void* stream);

@@ -217,6 +217,12 @@ PROTOTYPES = {
     "b2_unreduced_solve_pre": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p, _p]),
     "b2_unreduced_solve_post": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p, _p]),
     "b2_regularize_diagonal": (C.c_int, [_i64, _i64, _f64, _f64, _p, _p, _p, _p]),
+    "b2_scaled_set_aug_diagonal": (C.c_int, [_p] + [_p] * 7 + [_p]),
+    "b2_scaled_transfer": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _p, _p, _p]),
+    "b2_scaled_solve_pre": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
+    "b2_scaled_solve_post": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p, _p]),
+    "b2_scaled_kktmul": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p, _f64, _f64, _p, _p, _p]),
+    "b2_scaled_regularize_diagonal": (C.c_int, [_i64, _i64, _f64, _f64, _p, _p, _p, _p, _p]),
     "b2_reduce_rhs": (C.c_int, [_p, _i64, _p, _p, _p, _p]),
     "b2_finish_aug_solve": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p, _p]),
     "b2_spmv_plan_create": (C.c_int, [_i32, _i32, _p, _p, _PP]),
@@ -249,6 +255,7 @@ PROTOTYPES = {
     "b2_mul_hess_blk_tail": (C.c_int, [_p, _i64, _i32] + [_p] * 9 + [_f64, _p, _p]),
     "b2_rr_init": (C.c_int, [_p, _i64, _p, _p, _f64, _f64] + [_p] * 10 + [_p]),
     "b2_set_aug_rr": (C.c_int, [_p, _i64, _f64, _f64, _f64] + [_p] * 16 + [_p]),
+    "b2_set_aug_rr_scaled": (C.c_int, [_p, _i64, _f64, _f64, _f64] + [_p] * 16 + [_p]),
     "b2_set_aug_rhs_rr": (C.c_int, [_p, _i64] + [_p] * 13 + [_f64, _f64, _p, _p]),
     "b2_finish_aug_solve_rr": (C.c_int, [_i64] + [_p] * 6 + [_f64, _f64] + [_p] * 4 + [_p]),
     "b2_set_f_rr": (C.c_int, [_i64, _f64, _p, _p, _p, _p, _p]),
@@ -266,6 +273,7 @@ PROTOTYPES = {
     "b2_get_varphi_r": (C.c_int, [_p, _i64, _f64] + [_p] * 5 + [_f64, _p, _p]),
     "b2_get_varphi_d_r": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _p, _p]),
     "b2_set_aug_diagonal_iterate": (C.c_int, [_p, _i64, _f64, _f64] + [_p] * 11 + [_p]),
+    "b2_set_aug_diagonal_iterate_scaled": (C.c_int, [_p, _i64, _f64, _f64] + [_p] * 11 + [_p]),
     "b2_set_aug_rhs_perturbed": (C.c_int, [_p, _i64] + [_p] * 9 + [_f64, _f64, _f64, _i64, _p, _i64, _p, _p, _p]),
     "b2_set_initial_rhs": (C.c_int, [_p, _i64, _p, _p, _p, _p, _p]),
     "b2_dual_init_select": (C.c_int, [_p, _i64, _p, _i32, _f64, _p, _p, _p]),
@@ -320,6 +328,7 @@ PROTOTYPES = {
     "b2_inertia_loop_create": (C.c_int, [C.POINTER(InertiaSchedule), _PP]),
     "b2_inertia_loop_destroy": (C.c_int, [_p]),
     "b2_inertia_loop_begin": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _i32, _p]),
+    "b2_inertia_loop_begin_scaled": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _p, _i32, _p]),
     "b2_inertia_loop_refine": (C.c_int, [_p, C.POINTER(InertiaSource), _i64, _i64, _i64, _p, _p, _p, _p, _p]),
     "b2_inertia_loop_end": (C.c_int, [_p, _i32, _f64, _f64, _p]),
     "b2_inertia_loop_launch": (C.c_int, [_p, _f64, _f64, _i64, _p]),

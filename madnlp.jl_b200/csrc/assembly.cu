@@ -107,6 +107,63 @@ extern "C" int b2_transfer(b2_transfer_plan* p, double* dst_nz_d, const double* 
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// build_kkt!(::ScaledSparseKKTSystem) (scaled_augmented.jl:209-236): transfer! of V with every COO source scaled first, in one pass
+// over the CSC slots of aug_com and in b2_transfer's summation order.  A slot at (row r, column c) of the lower triangle takes
+//   c >= n_tot (du_diag)  : v            r >= n_tot (Jacobian, slack) : v * s[c]
+//   r, c < n_tot          : v for a pr_diag source (COO index k < n_tot), (v * s[r]) * s[c] for a Hessian source
+// so a diagonal slot that sums pr_diag and Hessian sources scales each on its own.  The column of a slot comes from colptr: the
+// CTA finds the columns of its first and last slot, each thread bisects between them (a few steps: a CTA spans few columns).
+// ---------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int64_t slot_column(const int32_t* __restrict__ colptr, int64_t lo, int64_t hi, int64_t slot) {
+    while (lo < hi) {                                  // the last column c in [lo, hi] with colptr[c] <= slot
+        const int64_t mid = (lo + hi + 1) >> 1;
+        if (colptr[mid] <= slot) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+__global__ void k_scaled_transfer(int64_t nslot, int64_t ncol, int64_t n_tot, const int32_t* __restrict__ ptr, const int32_t* __restrict__ src,
+                                  const int32_t* __restrict__ colptr, const int32_t* __restrict__ rowval, const double* __restrict__ sf,
+                                  const double* __restrict__ V, double* __restrict__ dst) {
+    __shared__ int64_t cspan[2];
+    pdl_sync();
+    const int64_t s0 = (int64_t)blockIdx.x * blockDim.x;
+    if (threadIdx.x < 2) cspan[threadIdx.x] = slot_column(colptr, 0, ncol - 1, threadIdx.x ? std::min<int64_t>(s0 + blockDim.x, nslot) - 1 : s0);
+    __syncthreads();
+    const int64_t i = s0 + threadIdx.x;
+    if (i >= nslot) return;
+    const int64_t c = slot_column(colptr, cspan[0], cspan[1], i);
+    const int64_t r = rowval[i];
+    const int a = ptr[i], b = ptr[i + 1];
+    double acc = 0.0;
+    if (c >= n_tot) {
+        for (int q = a; q < b; ++q) acc = __dadd_rn(acc, V[src[q]]);
+    } else if (r >= n_tot) {
+        const double sc = sf[c];
+        for (int q = a; q < b; ++q) acc = __dadd_rn(acc, __dmul_rn(V[src[q]], sc));
+    } else {
+        const double sr = sf[r], sc = sf[c];
+        for (int q = a; q < b; ++q) {
+            const int k = src[q];
+            const double v = V[k];
+            acc = __dadd_rn(acc, k < n_tot ? v : __dmul_rn(__dmul_rn(v, sr), sc));
+        }
+    }
+    dst[i] = acc;
+}
+
+extern "C" int b2_scaled_transfer(b2_transfer_plan* p, int64_t n, int64_t n_tot, const int32_t* colptr_d, const int32_t* rowval_d,
+                                  const double* scaling_d, double* dst_nz_d, const double* V_d, void* stream) {
+    B2_NEED(p && n >= 0 && n_tot >= 0 && n_tot <= n && (p->nnz_csc == 0 || (n > 0 && colptr_d && rowval_d && dst_nz_d && V_d)),
+            "b2_scaled_transfer");
+    B2_NEED(n_tot == 0 || p->nnz_csc == 0 || scaling_d, "b2_scaled_transfer");
+    if (p->nnz_csc == 0) return B2_OK;
+    launch_pdl(k_scaled_transfer, dim3((unsigned)((p->nnz_csc + 255) / 256)), dim3(256), 0, as_stream(stream), p->nnz_csc, n, n_tot,
+               p->ptr.p, p->src.p, colptr_d, rowval_d, scaling_d, V_d, dst_nz_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // sparse condensed KKT:  aug = tril(H) + diag(pr_diag[1:n]) + tril(Jt * D * Jt')
 // ---------------------------------------------------------------------------------------------------------
 __global__ void k_diag_buffer(int64_t m, const double* __restrict__ Ss, const double* __restrict__ Sd, double* __restrict__ D) {

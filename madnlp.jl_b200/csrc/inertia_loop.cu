@@ -88,13 +88,25 @@ __global__ void k_trial_schedule(TrialState* __restrict__ s, b2_inertia_options 
     *s = t;
 }
 
-// b2_regularize_diagonal's pass (k_regularize) with dw, dc read from the device: reg += dw ; pr_diag += dw ; du_diag -= dc
+// b2_regularize_diagonal's pass (k_regularize) with dw, dc read from the device: reg += dw ; pr_diag += dw ; du_diag -= dc.
+// SCALED: b2_scaled_regularize_diagonal's (k_scaled_regularize): pr_diag += dw (s s) with the scaling factor s of K2.5
+template <bool SCALED>
 __global__ void k_trial_regularize(const TrialState* __restrict__ s, int64_t n_tot, int64_t m, double* __restrict__ reg,
-                                   double* __restrict__ pr, double* __restrict__ du) {
+                                   double* __restrict__ pr, double* __restrict__ du, const double* __restrict__ sf) {
     const double dw = s->dw, dc = s->dc;
     GRID_STRIDE(i, n_tot + m) {
-        if (i < n_tot) { reg[i] += dw; pr[i] += dw; }
-        else du[i - n_tot] -= dc;
+        if (SCALED) {
+            if (i < n_tot) {
+                const double f = sf[i];
+                reg[i] = __dadd_rn(reg[i], dw);
+                pr[i] = __dadd_rn(pr[i], __dmul_rn(dw, __dmul_rn(f, f)));
+            } else {
+                du[i - n_tot] = __dsub_rn(du[i - n_tot], dc);
+            }
+        } else {
+            if (i < n_tot) { reg[i] += dw; pr[i] += dw; }
+            else du[i - n_tot] -= dc;
+        }
     }
 }
 
@@ -242,12 +254,9 @@ int b2_inertia_loop_destroy(b2_inertia_loop* h) {
     return B2_OK;
 }
 
-int b2_inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
-                          int32_t dual_always, void* stream) {
-    if (!h || n_tot < 0 || m < 0 || (n_tot && (!reg_d || !pr_diag_d)) || (m && !du_diag_d)) {
-        set_error("b2_inertia_loop_begin: invalid argument");
-        return B2_ERR_INVALID;
-    }
+namespace {
+int inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
+                       const double* scaling_d, int32_t dual_always, void* stream) {
     cudaStream_t st = as_stream(stream);
     h->drop();
     IL_TRY(cudaGraphCreate(&h->graph, 0), "cudaGraphCreate");
@@ -261,10 +270,30 @@ int b2_inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* 
     k_trial_schedule<<<1, 1, 0, st>>>(h->state.p, h->opt, dual_always ? 1 : 0, h->del_w.p);
     IL_TRY(cudaGetLastError(), "k_trial_schedule");
     if (n_tot + m) {
-        k_trial_regularize<<<grid_elem(n_tot + m), 256, 0, st>>>(h->state.p, n_tot, m, reg_d, pr_diag_d, du_diag_d);
+        if (scaling_d) k_trial_regularize<true><<<grid_elem(n_tot + m), 256, 0, st>>>(h->state.p, n_tot, m, reg_d, pr_diag_d, du_diag_d, scaling_d);
+        else k_trial_regularize<false><<<grid_elem(n_tot + m), 256, 0, st>>>(h->state.p, n_tot, m, reg_d, pr_diag_d, du_diag_d, nullptr);
         IL_TRY(cudaGetLastError(), "k_trial_regularize");
     }
     return B2_OK;
+}
+}  // namespace
+
+int b2_inertia_loop_begin(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
+                          int32_t dual_always, void* stream) {
+    if (!h || n_tot < 0 || m < 0 || (n_tot && (!reg_d || !pr_diag_d)) || (m && !du_diag_d)) {
+        set_error("b2_inertia_loop_begin: invalid argument");
+        return B2_ERR_INVALID;
+    }
+    return inertia_loop_begin(h, n_tot, m, reg_d, pr_diag_d, du_diag_d, nullptr, dual_always, stream);
+}
+
+int b2_inertia_loop_begin_scaled(b2_inertia_loop* h, int64_t n_tot, int64_t m, double* reg_d, double* pr_diag_d, double* du_diag_d,
+                                 const double* scaling_d, int32_t dual_always, void* stream) {
+    if (!h || n_tot < 0 || m < 0 || (n_tot && (!reg_d || !pr_diag_d || !scaling_d)) || (m && !du_diag_d)) {
+        set_error("b2_inertia_loop_begin_scaled: invalid argument");
+        return B2_ERR_INVALID;
+    }
+    return inertia_loop_begin(h, n_tot, m, reg_d, pr_diag_d, du_diag_d, scaling_d, dual_always, stream);
 }
 
 int b2_inertia_loop_refine(b2_inertia_loop* h, const b2_inertia_source* src, int64_t expect_pos, int64_t expect_neg, int64_t n,

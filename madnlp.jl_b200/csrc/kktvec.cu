@@ -376,6 +376,157 @@ extern "C" int b2_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const dou
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// ScaledSparseKKTSystem (K2.5, src/KKT/Sparse/scaled_augmented.jl).  l_diag = x - xl and u_diag = xu - x are positive here.
+// One thread per variable i reads its bound positions p = lbpos[i], q = ubpos[i] (-1: no such bound), so every output entry has
+// one writer and there are no atomics.  Every product and sum is a rounding intrinsic in the reference's broadcast order: no FMA
+// contraction, the results are bit-identical to the broadcasts.
+// ---------------------------------------------------------------------------------------------------------
+// _set_aug_diagonal!(::ScaledSparseKKTSystem) (IPM/kernels.jl:47-68):
+//   xlzu = (q ? zu : 0) * (p ? l_diag : -)  ;  xuzl = (p ? zl : 0) * (q ? u_diag : -)  ;  s = (1 * sqrt(l_diag)) * sqrt(u_diag)
+//   pr_diag = (xlzu + xuzl) + reg * (s * s)  ;  scaling_factor = s
+__global__ void k_scaled_set_aug_diagonal(int64_t n_tot, const int32_t* __restrict__ lbpos, const int32_t* __restrict__ ubpos,
+                                          const double* __restrict__ reg, const double* __restrict__ ll, const double* __restrict__ ld,
+                                          const double* __restrict__ ul, const double* __restrict__ ud, double* __restrict__ pr,
+                                          double* __restrict__ sf) {
+    pdl_sync();
+    GRID_STRIDE(i, n_tot) {
+        const int p = lbpos[i], q = ubpos[i];
+        double xlzu = q >= 0 ? ul[q] : 0.0;
+        double xuzl = p >= 0 ? ll[p] : 0.0;
+        double s = 1.0;
+        if (p >= 0) { xlzu = __dmul_rn(xlzu, ld[p]); s = __dmul_rn(s, __dsqrt_rn(ld[p])); }
+        if (q >= 0) { xuzl = __dmul_rn(xuzl, ud[q]); s = __dmul_rn(s, __dsqrt_rn(ud[q])); }
+        pr[i] = __dadd_rn(__dadd_rn(xlzu, xuzl), __dmul_rn(reg[i], __dmul_rn(s, s)));
+        sf[i] = s;
+    }
+}
+extern "C" int b2_scaled_set_aug_diagonal(b2_bounds* b, const double* reg_d, const double* l_lower_d, const double* l_diag_d,
+                                          const double* u_lower_d, const double* u_diag_d, double* pr_diag_d, double* scaling_d,
+                                          void* stream) {
+    B2_NEED(b && (b->n_tot == 0 || (reg_d && pr_diag_d && scaling_d)), "b2_scaled_set_aug_diagonal");
+    B2_NEED((b->nlb == 0 || (l_lower_d && l_diag_d)) && (b->nub == 0 || (u_lower_d && u_diag_d)), "b2_scaled_set_aug_diagonal");
+    if (b->n_tot == 0) return B2_OK;
+    launch_pdl(k_scaled_set_aug_diagonal, dim3(grid_elem(b->n_tot)), dim3(256), 0, as_stream(stream), b->n_tot, b->lbpos.p, b->ubpos.p,
+               reg_d, l_lower_d, l_diag_d, u_lower_d, u_diag_d, pr_diag_d, scaling_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+// solve_kkt!(::ScaledSparseKKTSystem) (IPM/factorization.jl:48-74) around b2_solve on primal_dual(w), one launch on each side.
+// pre:  r3 = ((p ? wzl : 0) * (q ? sqrt(u_diag) : -)) / (p ? sqrt(l_diag) : -)
+//       r4 = ((q ? wzu : 0) * (p ? sqrt(l_diag) : -)) / (q ? sqrt(u_diag) : -)      xp = xp * s + (r3 + r4)
+// post: xp = xp * s ; wzl = (wzl - l_lower * xp) / l_diag ; wzu = (-wzu + u_lower * xp) / u_diag
+// In post the thread of variable i owns xp[i] and its two bound duals, so the scaled xp it reads is its own write.
+template <bool POST>
+__global__ void k_scaled_solve(int64_t n_tot, int64_t m, int64_t nlb, const int32_t* __restrict__ lbpos, const int32_t* __restrict__ ubpos,
+                               const double* __restrict__ ll, const double* __restrict__ ul, const double* __restrict__ ld,
+                               const double* __restrict__ ud, const double* __restrict__ sf, double* __restrict__ w) {
+    pdl_sync();
+    double* wzl = w + n_tot + m;
+    double* wzu = wzl + nlb;
+    GRID_STRIDE(i, n_tot) {
+        const int p = lbpos[i], q = ubpos[i];
+        if (!POST) {
+            double r3 = p >= 0 ? wzl[p] : 0.0;
+            double r4 = q >= 0 ? wzu[q] : 0.0;
+            if (q >= 0) r3 = __dmul_rn(r3, __dsqrt_rn(ud[q]));
+            if (p >= 0) { r3 = __ddiv_rn(r3, __dsqrt_rn(ld[p])); r4 = __dmul_rn(r4, __dsqrt_rn(ld[p])); }
+            if (q >= 0) r4 = __ddiv_rn(r4, __dsqrt_rn(ud[q]));
+            w[i] = __dadd_rn(__dmul_rn(w[i], sf[i]), __dadd_rn(r3, r4));
+        } else {
+            const double x = __dmul_rn(w[i], sf[i]);
+            w[i] = x;
+            if (p >= 0) wzl[p] = __ddiv_rn(__dsub_rn(wzl[p], __dmul_rn(ll[p], x)), ld[p]);
+            if (q >= 0) wzu[q] = __ddiv_rn(__dadd_rn(neg(wzu[q]), __dmul_rn(ul[q], x)), ud[q]);
+        }
+    }
+}
+template <bool POST>
+static int scaled_solve(const char* name, b2_bounds* b, int64_t m, const double* ll, const double* ul, const double* ld, const double* ud,
+                        const double* sf, double* w, void* stream) {
+    if (!b || m < 0 || !w || (b->n_tot && !sf) || (b->nlb && (!ld || (POST && !ll))) || (b->nub && (!ud || (POST && !ul)))) {
+        set_error(std::string(name) + ": invalid argument");
+        return B2_ERR_INVALID;
+    }
+    if (b->n_tot == 0) return B2_OK;
+    launch_pdl(k_scaled_solve<POST>, dim3(grid_elem(b->n_tot)), dim3(256), 0, as_stream(stream), b->n_tot, m, b->nlb, b->lbpos.p,
+               b->ubpos.p, ll, ul, ld, ud, sf, w);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+extern "C" int b2_scaled_solve_pre(b2_bounds* b, int64_t m, const double* l_diag_d, const double* u_diag_d, const double* scaling_d,
+                                   double* w_d, void* stream) {
+    return scaled_solve<false>("b2_scaled_solve_pre", b, m, nullptr, nullptr, l_diag_d, u_diag_d, scaling_d, w_d, stream);
+}
+extern "C" int b2_scaled_solve_post(b2_bounds* b, int64_t m, const double* l_lower_d, const double* u_lower_d, const double* l_diag_d,
+                                    const double* u_diag_d, const double* scaling_d, double* w_d, void* stream) {
+    return scaled_solve<true>("b2_scaled_solve_post", b, m, l_lower_d, u_lower_d, l_diag_d, u_diag_d, scaling_d, w_d, stream);
+}
+
+// mul!(w, ::ScaledSparseKKTSystem, x, alpha, beta)'s diagonal and bound part (IPM/factorization.jl:239-251), after the SpMVs:
+//   xp_w += (alpha reg) xp ; xp_w[ind_lb] -= alpha xzl ; xp_w[ind_ub] += alpha xzu ; y_w += (alpha du_diag) y
+//   wzl = beta wzl + alpha (xp[ind_lb] l_lower + xzl l_diag) ; wzu = beta wzu + alpha (xp[ind_ub] u_lower - xzu u_diag)
+// beta wzl is taken as 0 when beta == 0, as b2_kktmul does.
+__global__ void k_scaled_kktmul(KktMulArgs a, const double* __restrict__ x, double* __restrict__ w) {
+    const double* xzl = x + a.n_tot + a.m;
+    const double* xzu = xzl + a.nlb;
+    GRID_STRIDE(t, a.n_tot + a.m + a.nlb + a.nub) {
+        const double wt = w[t];
+        double v;
+        if (t < a.n_tot) {
+            v = __dadd_rn(wt, __dmul_rn(__dmul_rn(a.alpha, a.reg[t]), x[t]));
+            const int p = a.lbpos[t], q = a.ubpos[t];
+            if (p >= 0) v = __dsub_rn(v, __dmul_rn(a.alpha, xzl[p]));
+            if (q >= 0) v = __dadd_rn(v, __dmul_rn(a.alpha, xzu[q]));
+        } else if (t < a.n_tot + a.m) {
+            v = __dadd_rn(wt, __dmul_rn(__dmul_rn(a.alpha, a.du[t - a.n_tot]), x[t]));
+        } else if (t < a.n_tot + a.m + a.nlb) {
+            const int64_t k = t - a.n_tot - a.m;
+            v = __dadd_rn(scl(a.beta, wt), __dmul_rn(a.alpha, __dadd_rn(__dmul_rn(x[a.ind_lb[k]], a.ll[k]), __dmul_rn(xzl[k], a.ld[k]))));
+        } else {
+            const int64_t k = t - a.n_tot - a.m - a.nlb;
+            v = __dadd_rn(scl(a.beta, wt), __dmul_rn(a.alpha, __dsub_rn(__dmul_rn(x[a.ind_ub[k]], a.ul[k]), __dmul_rn(xzu[k], a.ud[k]))));
+        }
+        w[t] = v;
+    }
+}
+extern "C" int b2_scaled_kktmul(b2_bounds* b, int64_t m, const double* reg_d, const double* du_diag_d, const double* l_lower_d,
+                                const double* u_lower_d, const double* l_diag_d, const double* u_diag_d, double alpha, double beta,
+                                const double* x_d, double* w_d, void* stream) {
+    B2_NEED(b && m >= 0 && x_d && w_d && (b->n_tot == 0 || reg_d) && (m == 0 || du_diag_d), "b2_scaled_kktmul");
+    B2_NEED((b->nlb == 0 || (l_lower_d && l_diag_d)) && (b->nub == 0 || (u_lower_d && u_diag_d)), "b2_scaled_kktmul");
+    KktMulArgs a = make_kktmul(b, m, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d, alpha, beta);
+    const int64_t tot = a.n_tot + a.m + a.nlb + a.nub;
+    if (tot == 0) return B2_OK;
+    k_scaled_kktmul<<<grid_elem(tot), 256, 0, as_stream(stream)>>>(a, x_d, w_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+// regularize_diagonal!(::ScaledSparseKKTSystem) (scaled_augmented.jl:238-242): reg += dw ; pr_diag += dw (s s) ; du_diag -= dc
+__global__ void k_scaled_regularize(int64_t n_tot, int64_t m, double dw, double dc, const double* __restrict__ sf, double* __restrict__ reg,
+                                    double* __restrict__ pr, double* __restrict__ du) {
+    GRID_STRIDE(i, n_tot + m) {
+        if (i < n_tot) {
+            const double s = sf[i];
+            reg[i] = __dadd_rn(reg[i], dw);
+            pr[i] = __dadd_rn(pr[i], __dmul_rn(dw, __dmul_rn(s, s)));
+        } else {
+            du[i - n_tot] = __dsub_rn(du[i - n_tot], dc);
+        }
+    }
+}
+extern "C" int b2_scaled_regularize_diagonal(int64_t n_tot, int64_t m, double dw, double dc, const double* scaling_d, double* reg_d,
+                                             double* pr_diag_d, double* du_diag_d, void* stream) {
+    B2_NEED(n_tot >= 0 && m >= 0 && (n_tot == 0 || (scaling_d && reg_d && pr_diag_d)) && (m == 0 || du_diag_d),
+            "b2_scaled_regularize_diagonal");
+    if (n_tot + m == 0) return B2_OK;
+    k_scaled_regularize<<<grid_elem(n_tot + m), 256, 0, as_stream(stream)>>>(n_tot, m, dw, dc, scaling_d, reg_d, pr_diag_d, du_diag_d);
+    B2_CUDA(cudaGetLastError());
+    return B2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // solve_kkt!(::SparseCondensedKKTSystem) pre / post  (IPM/factorization.jl:143-167)
 // ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void norm_inf_commit(double mx, unsigned long long* out) {   // NaN-propagating max of non-negative doubles

@@ -56,6 +56,8 @@ __global__ void k_rr_init(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, co
 
 // ---- set_aug_RR! (kernels.jl:72-84), segments [n_tot | m | nlb | nub]:
 //   reg = del_w + zeta D_R^2 ; du_diag = -del_c - pp ./ zp - nn ./ zn ; l_lower = zl_r ; l_diag = xl_r - x_lr ; u_lower = zu_r ; u_diag = x_ur - xu_r
+// SCALED: set_aug_RR!(::ScaledSparseKKTSystem) (kernels.jl:89-104), the same but l_diag = x_lr - xl_r, u_diag = xu_r - x_ur
+template <bool SCALED>
 __global__ void k_set_aug_RR(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const int64_t* __restrict__ ind_lb,
                              const int64_t* __restrict__ ind_ub, double del_w, double del_c, double zeta, const double* __restrict__ D_R,
                              const double* __restrict__ pp, const double* __restrict__ nn, const double* __restrict__ zp,
@@ -75,11 +77,11 @@ __global__ void k_set_aug_RR(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub,
         } else if (t < n_tot + m + nlb) {
             const int64_t i = t - n_tot - m, k = ind_lb[i];
             l_lower[i] = zl[k];
-            l_diag[i] = __dsub_rn(xl[k], x[k]);
+            l_diag[i] = SCALED ? __dsub_rn(x[k], xl[k]) : __dsub_rn(xl[k], x[k]);
         } else {
             const int64_t i = t - n_tot - m - nlb, k = ind_ub[i];
             u_lower[i] = zu[k];
-            u_diag[i] = __dsub_rn(x[k], xu[k]);
+            u_diag[i] = SCALED ? __dsub_rn(xu[k], x[k]) : __dsub_rn(x[k], xu[k]);
         }
     }
 }
@@ -204,19 +206,32 @@ int b2_rr_init(b2_bounds* b, int64_t m, const double* x_d, const double* c_d, do
               f_R_d, pp_d, nn_d, zp_d, zn_d, y_d, zl_d, zu_d);
 }
 
+#define B2_SET_AUG_RR_CHECKS(who)                                                     \
+    B2_NEED(b && m >= 0, who);                                                        \
+    B2_NEED(b->n_tot == 0 || (D_R_d && reg_d), who);                                  \
+    B2_NEED(m == 0 || (pp_d && nn_d && zp_d && zn_d && du_diag_d), who);              \
+    B2_NEED(b->nlb + b->nub == 0 || (x_d && xl_d && xu_d), who);                      \
+    B2_NEED(b->nlb == 0 || (zl_d && l_lower_d && l_diag_d), who);                     \
+    B2_NEED(b->nub == 0 || (zu_d && u_lower_d && u_diag_d), who)
+
 int b2_set_aug_rr(b2_bounds* b, int64_t m, double del_w, double del_c, double zeta, const double* D_R_d, const double* pp_d,
                   const double* nn_d, const double* zp_d, const double* zn_d, const double* x_d, const double* xl_d, const double* xu_d,
                   const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d, double* u_lower_d,
                   double* l_diag_d, double* u_diag_d, void* stream) {
-    B2_NEED(b && m >= 0, "b2_set_aug_rr");
-    B2_NEED(b->n_tot == 0 || (D_R_d && reg_d), "b2_set_aug_rr");
-    B2_NEED(m == 0 || (pp_d && nn_d && zp_d && zn_d && du_diag_d), "b2_set_aug_rr");
-    B2_NEED(b->nlb + b->nub == 0 || (x_d && xl_d && xu_d), "b2_set_aug_rr");
-    B2_NEED(b->nlb == 0 || (zl_d && l_lower_d && l_diag_d), "b2_set_aug_rr");
-    B2_NEED(b->nub == 0 || (zu_d && u_lower_d && u_diag_d), "b2_set_aug_rr");
+    B2_SET_AUG_RR_CHECKS("b2_set_aug_rr");
     const int64_t tot = b->n_tot + m + b->nlb + b->nub;
-    B2_LAUNCH("b2_set_aug_rr", k_set_aug_RR, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, del_w, del_c, zeta, D_R_d, pp_d,
+    B2_LAUNCH("b2_set_aug_rr", k_set_aug_RR<false>, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, del_w, del_c, zeta, D_R_d, pp_d,
               nn_d, zp_d, zn_d, x_d, xl_d, xu_d, zl_d, zu_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d);
+}
+
+int b2_set_aug_rr_scaled(b2_bounds* b, int64_t m, double del_w, double del_c, double zeta, const double* D_R_d, const double* pp_d,
+                         const double* nn_d, const double* zp_d, const double* zn_d, const double* x_d, const double* xl_d, const double* xu_d,
+                         const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d, double* l_lower_d, double* u_lower_d,
+                         double* l_diag_d, double* u_diag_d, void* stream) {
+    B2_SET_AUG_RR_CHECKS("b2_set_aug_rr_scaled");
+    const int64_t tot = b->n_tot + m + b->nlb + b->nub;
+    B2_LAUNCH("b2_set_aug_rr_scaled", k_set_aug_RR<true>, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, del_w, del_c, zeta,
+              D_R_d, pp_d, nn_d, zp_d, zn_d, x_d, xl_d, xu_d, zl_d, zu_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d);
 }
 
 int b2_set_aug_rhs_rr(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* zl_d,

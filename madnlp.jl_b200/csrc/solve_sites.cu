@@ -28,6 +28,8 @@ __device__ __forceinline__ double axpy1(double y, double a, double x) { return _
 
 // ---- set_aug_diagonal! (kernels.jl:4-20) before _set_aug_diagonal!, segments [n_tot | m | nlb | nub]:
 //   reg = del_w ; du_diag = -del_c ; l_lower = zl_r, l_diag = xl_r - x_lr ; u_lower = zu_r, u_diag = x_ur - xu_r
+// SCALED: set_aug_diagonal!(::ScaledSparseKKTSystem) (kernels.jl:36-45), the same but l_diag = x_lr - xl_r, u_diag = xu_r - x_ur
+template <bool SCALED>
 __global__ void k_set_aug_diagonal_iterate(int64_t n_tot, int64_t m, int64_t nlb, int64_t nub, const int64_t* __restrict__ ind_lb,
                                            const int64_t* __restrict__ ind_ub, double del_w, double del_c, const double* __restrict__ x,
                                            const double* __restrict__ xl, const double* __restrict__ xu, const double* __restrict__ zl,
@@ -45,11 +47,11 @@ __global__ void k_set_aug_diagonal_iterate(int64_t n_tot, int64_t m, int64_t nlb
         } else if (t < n_tot + m + nlb) {
             const int64_t i = t - n_tot - m, k = ind_lb[i];
             l_lower[i] = zl[k];
-            l_diag[i] = __dsub_rn(xl[k], x[k]);
+            l_diag[i] = SCALED ? __dsub_rn(x[k], xl[k]) : __dsub_rn(xl[k], x[k]);
         } else {
             const int64_t i = t - n_tot - m - nlb, k = ind_ub[i];
             u_lower[i] = zu[k];
-            u_diag[i] = __dsub_rn(x[k], xu[k]);
+            u_diag[i] = SCALED ? __dsub_rn(xu[k], x[k]) : __dsub_rn(x[k], xu[k]);
         }
     }
 }
@@ -193,8 +195,21 @@ int b2_set_aug_diagonal_iterate(b2_bounds* b, int64_t m, double del_w, double de
     B2_NEED(b->nlb == 0 || (xl_d && zl_d && l_lower_d && l_diag_d), "b2_set_aug_diagonal_iterate");
     B2_NEED(b->nub == 0 || (xu_d && zu_d && u_lower_d && u_diag_d), "b2_set_aug_diagonal_iterate");
     const int64_t tot = b->n_tot + m + b->nlb + b->nub;
-    B2_LAUNCH("b2_set_aug_diagonal_iterate", k_set_aug_diagonal_iterate, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, del_w,
+    B2_LAUNCH("b2_set_aug_diagonal_iterate", k_set_aug_diagonal_iterate<false>, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p, b->ind_ub.p, del_w,
               del_c, x_d, xl_d, xu_d, zl_d, zu_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d);
+}
+
+int b2_set_aug_diagonal_iterate_scaled(b2_bounds* b, int64_t m, double del_w, double del_c, const double* x_d, const double* xl_d,
+                                       const double* xu_d, const double* zl_d, const double* zu_d, double* reg_d, double* du_diag_d,
+                                       double* l_lower_d, double* u_lower_d, double* l_diag_d, double* u_diag_d, void* stream) {
+    B2_NEED(b && m >= 0, "b2_set_aug_diagonal_iterate_scaled");
+    B2_NEED((b->n_tot == 0 || reg_d) && (m == 0 || du_diag_d), "b2_set_aug_diagonal_iterate_scaled");
+    B2_NEED(b->nlb + b->nub == 0 || x_d, "b2_set_aug_diagonal_iterate_scaled");
+    B2_NEED(b->nlb == 0 || (xl_d && zl_d && l_lower_d && l_diag_d), "b2_set_aug_diagonal_iterate_scaled");
+    B2_NEED(b->nub == 0 || (xu_d && zu_d && u_lower_d && u_diag_d), "b2_set_aug_diagonal_iterate_scaled");
+    const int64_t tot = b->n_tot + m + b->nlb + b->nub;
+    B2_LAUNCH("b2_set_aug_diagonal_iterate_scaled", k_set_aug_diagonal_iterate<true>, tot, b->n_tot, m, b->nlb, b->nub, b->ind_lb.p,
+              b->ind_ub.p, del_w, del_c, x_d, xl_d, xu_d, zl_d, zu_d, reg_d, du_diag_d, l_lower_d, u_lower_d, l_diag_d, u_diag_d);
 }
 
 int b2_set_aug_rhs_perturbed(b2_bounds* b, int64_t m, const double* x_d, const double* xl_d, const double* xu_d, const double* f_d,

@@ -146,6 +146,9 @@ class IPMLinearAlgebra:
     def __init__(self, kkt, tol=1e-8, use_cuda_graph=True, speculate=True, inertia_correction_method="InertiaBased",
                  inertia_free_tol=0.0, iterator="RichardsonIterator", krylov_options=None):
         self.inertia_correction_method = resolve_inertia_correction_method(inertia_correction_method, kkt.linear_solver)
+        if kkt._scaled and self.inertia_correction_method == "InertiaFree":
+            # the reference has no mul_hess_blk! for this type (src/IPM/factorization.jl:326-350)
+            raise ValueError("inertia_correction_method = InertiaFree is not supported by the KKT formulation ScaledSparseKKTSystem")
         self.inertia_free_tol = float(inertia_free_tol)
         self.kkt = kkt
         self.use_cuda_graph = use_cuda_graph
@@ -407,9 +410,10 @@ class IPMLinearAlgebra:
         k, v = self.kkt, self.solver_vectors
         k.compress_jacobian()
         k.compress_hessian()
-        check(lib.b2_set_aug_diagonal_iterate(k._bounds.h, v.m, float(primal_regularization), float(dual_regularization), ptr(v.x),
-                                              ptr(v.xl), ptr(v.xu), ptr(v.zl), ptr(v.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower),
-                                              ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self.kkt.stream_ptr()))
+        # ScaledSparseKKTSystem's set_aug_diagonal! (src/IPM/kernels.jl:36-45) writes l_diag = x - xl and u_diag = xu - x
+        fn = lib.b2_set_aug_diagonal_iterate_scaled if k._scaled else lib.b2_set_aug_diagonal_iterate
+        check(fn(k._bounds.h, v.m, float(primal_regularization), float(dual_regularization), ptr(v.x), ptr(v.xl), ptr(v.xu), ptr(v.zl),
+                 ptr(v.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower), ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self.kkt.stream_ptr()))
         k.set_aug_diagonal_()
         self._factorize_wrapper()
         self._set_aug_rhs_perturbed(v.c, None, 0.0, mu, kappa_d)
@@ -485,8 +489,8 @@ class IPMLinearAlgebra:
     def _trials_loop(self):
         """the graph of the trials after a wrong first inertia, or None: the host loop.  It covers InertiaBased with the Richardson
         loop on the device, the exact Hessian, a single-part sparse solver that exposes its pivot counters and a KKT type that states
-        its inertia and dual rules as data (SparseKKTSystem, SparseUnreducedKKTSystem, SparseCondensedKKTSystem).  As for the
-        refinement-loop graph, the first step of a setting runs every launch eagerly and the second builds the graph."""
+        its inertia and dual rules as data (SparseKKTSystem, SparseUnreducedKKTSystem, ScaledSparseKKTSystem, SparseCondensedKKTSystem).
+        As for the refinement-loop graph, the first step of a setting runs every launch eagerly and the second builds the graph."""
         k, it = self.kkt, self.iterator
         ls = k.linear_solver
         if not (self.inertia_correction_method == "InertiaBased" and isinstance(it, RichardsonIterator) and it._device_loop
@@ -519,7 +523,11 @@ class IPMLinearAlgebra:
         # captured on a side stream, as torch.cuda.graph does: the legacy default stream cannot be captured
         with torch.cuda.stream(torch.cuda.Stream()):
             sp = k.stream_ptr()
-            rc = lib.b2_inertia_loop_begin(loop.h, k._n_tot, k._m, ptr(k.reg), ptr(k.pr_diag), ptr(k.du_diag), int(k.dual_rule()), sp)
+            if k._scaled:                   # regularize_diagonal! of K2.5: pr_diag += dw s^2
+                rc = lib.b2_inertia_loop_begin_scaled(loop.h, k._n_tot, k._m, ptr(k.reg), ptr(k.pr_diag), ptr(k.du_diag),
+                                                      ptr(k.scaling_factor), int(k.dual_rule()), sp)
+            else:
+                rc = lib.b2_inertia_loop_begin(loop.h, k._n_tot, k._m, ptr(k.reg), ptr(k.pr_diag), ptr(k.du_diag), int(k.dual_rule()), sp)
             if rc == B2_OK:
                 try:
                     k.build_kkt()

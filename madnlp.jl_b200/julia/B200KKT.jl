@@ -360,6 +360,7 @@ end
 # runs the stock constructor.  Plans (transfer maps, SpMV plans, bounds) live beside the solver, as for the condensed type.
 # ---------------------------------------------------------------------------------------------------------------------
 const B200UnreducedKKT{T} = MadNLP.SparseUnreducedKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200Solver}
+const B200ScaledKKT{T} = MadNLP.ScaledSparseKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200Solver}
 
 function MadNLP.create_kkt_system(::Type{MadNLP.SparseUnreducedKKTSystem}, cb::MadNLP.SparseCallback, linear_solver::Type{<:B200Solver};
                                   opt_linear_solver = default_options(linear_solver), kwargs...)
@@ -377,7 +378,7 @@ mutable struct UnreducedPlans
 end
 const _uplans = IdDict{Any,UnreducedPlans}()
 
-function uplans(kkt::B200UnreducedKKT{T}) where T
+function uplans(kkt::Union{B200UnreducedKKT{T},B200ScaledKKT{T}}) where T   # (K2.5: the same plans)
     get!(_uplans, kkt.linear_solver) do
         h0(v) = Array(v) .- one(eltype(v))
         tplan(map_d, nnz_csc) = begin
@@ -452,6 +453,100 @@ end
 
 # jtprod! (Sparse/utils.jl:28-30): y = jac_com' x
 function MadNLP.jtprod!(y::CuVector{T}, kkt::B200UnreducedKKT{T}, x::CuVector{T}) where T
+    check(ccall((:b2_spmv_t, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
+        uplans(kkt).jac_spmv, pointer(MadNLP.nzval(kkt.jac_com)), pointer(x), pointer(y), one(T), zero(T), stream_ptr()), SolveException)
+    return y
+end
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ScaledSparseKKTSystem (K2.5, src/KKT/Sparse/scaled_augmented.jl) with B200Solver.  The layout is SparseKKTSystem's, so
+# create_kkt_system fills kkt_n_primal = n_tot as for K2 and runs the stock constructor; the plans are the unreduced type's (uplans)
+# plus aug_com's pattern on the device, which b2_scaled_transfer reads.  build_kkt! scales V's sources on their way into aug_com: the
+# constructor's scaled_aug_raw is never written.  l_diag = x - xl and u_diag = xu - x (positive), as the reference has them.
+# ---------------------------------------------------------------------------------------------------------------------
+function MadNLP.create_kkt_system(::Type{MadNLP.ScaledSparseKKTSystem}, cb::MadNLP.SparseCallback, linear_solver::Type{<:B200Solver};
+                                  opt_linear_solver = default_options(linear_solver), kwargs...)
+    opt_linear_solver.b200_kkt_n_primal == 0 && (opt_linear_solver.b200_kkt_n_primal = cb.nvar + length(cb.ind_ineq))
+    return invoke(MadNLP.create_kkt_system, Tuple{Type{MadNLP.ScaledSparseKKTSystem},MadNLP.SparseCallback,Type},
+                  MadNLP.ScaledSparseKKTSystem, cb, linear_solver; opt_linear_solver = opt_linear_solver, kwargs...)
+end
+
+const _scaled_pattern = IdDict{Any,Tuple{CuVector{Int32},CuVector{Int32}}}()
+scaled_pattern(kkt::B200ScaledKKT) = get!(_scaled_pattern, kkt.linear_solver) do
+    (CuVector{Int32}(Array(kkt.aug_com.colPtr) .- 1), CuVector{Int32}(Array(kkt.aug_com.rowVal) .- 1))
+end
+
+# build_kkt! (scaled_augmented.jl:209-236): one pass over aug_com's slots, each COO source scaled before the slot's sum
+function MadNLP.build_kkt!(kkt::B200ScaledKKT{T}) where T
+    cp, rv = scaled_pattern(kkt)
+    check(ccall((:b2_scaled_transfer, libb200kkt), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Int32}, CuPtr{Int32}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        uplans(kkt).aug_plan, size(kkt.aug_com, 1), length(kkt.pr_diag), pointer(cp), pointer(rv), pointer(kkt.scaling_factor),
+        pointer(MadNLP.nzval(kkt.aug_com)), pointer(kkt.aug_raw.V), stream_ptr()), FactorizationException)
+end
+MadNLP.compress_hessian!(kkt::B200ScaledKKT) = _transfer(uplans(kkt).hess_plan, MadNLP.nzval(kkt.hess_com), kkt.hess_raw.V)
+function MadNLP.compress_jacobian!(kkt::B200ScaledKKT{T}) where T
+    ns = length(kkt.ind_ineq)
+    ns > 0 && check(ccall((:b2_fill, libb200kkt), Cint, (Int64, Cdouble, CuPtr{T}, Ptr{Cvoid}),
+        ns, -one(T), pointer(kkt.jac, length(kkt.jac) - ns + 1), stream_ptr()), FactorizationException)
+    _transfer(uplans(kkt).jac_plan, MadNLP.nzval(kkt.jac_com), kkt.jac_raw.V)
+end
+
+# _set_aug_diagonal! (src/IPM/kernels.jl:47-68): pr_diag and scaling_factor in one launch
+function MadNLP._set_aug_diagonal!(kkt::B200ScaledKKT{T}) where T
+    check(ccall((:b2_scaled_set_aug_diagonal, libb200kkt), Cint, (Ptr{Cvoid}, ntuple(_ -> CuPtr{T}, 7)..., Ptr{Cvoid}),
+        uplans(kkt).bounds, pointer(kkt.reg), pointer(kkt.l_lower), pointer(kkt.l_diag), pointer(kkt.u_lower), pointer(kkt.u_diag),
+        pointer(kkt.pr_diag), pointer(kkt.scaling_factor), stream_ptr()), FactorizationException)
+    return
+end
+
+# set_aug_diagonal! (src/IPM/kernels.jl:36-45): reg, du_diag, l_lower = zl_r, u_lower = zu_r, l_diag = x_lr - xl_r, u_diag = xu_r - x_ur
+# in one launch, then _set_aug_diagonal!
+function MadNLP.set_aug_diagonal!(kkt::B200ScaledKKT{T}, solver::MadNLP.AbstractMadNLPSolver{T}) where T
+    o = MadNLP.get_opt(solver)
+    v(f) = pointer(MadNLP.full(f(solver)))
+    check(ccall((:b2_set_aug_diagonal_iterate_scaled, libb200kkt), Cint, (Ptr{Cvoid}, Int64, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 11)..., Ptr{Cvoid}),
+        uplans(kkt).bounds, length(kkt.du_diag), o.default_primal_regularization, o.default_dual_regularization, v(MadNLP.get_x),
+        v(MadNLP.get_xl), v(MadNLP.get_xu), v(MadNLP.get_zl), v(MadNLP.get_zu), pointer(kkt.reg), pointer(kkt.du_diag),
+        pointer(kkt.l_lower), pointer(kkt.u_lower), pointer(kkt.l_diag), pointer(kkt.u_diag), stream_ptr()), FactorizationException)
+    MadNLP._set_aug_diagonal!(kkt)
+end
+
+# regularize_diagonal! (scaled_augmented.jl:238-242): reg += primal; pr_diag += primal s^2; du_diag -= dual
+function MadNLP.regularize_diagonal!(kkt::B200ScaledKKT{T}, primal, dual) where T
+    check(ccall((:b2_scaled_regularize_diagonal, libb200kkt), Cint, (Int64, Int64, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 4)..., Ptr{Cvoid}),
+        length(kkt.pr_diag), length(kkt.du_diag), primal, dual, pointer(kkt.scaling_factor), pointer(kkt.reg), pointer(kkt.pr_diag),
+        pointer(kkt.du_diag), stream_ptr()), FactorizationException)
+end
+
+# solve_kkt! (src/IPM/factorization.jl:48-74): one launch on each side of b2_solve on primal_dual(w)
+function MadNLP.solve_kkt!(kkt::B200ScaledKKT{T}, w::MadNLP.AbstractKKTVector) where T
+    wv = MadNLP.full(w); b = uplans(kkt).bounds; m = length(kkt.du_diag)
+    check(ccall((:b2_scaled_solve_pre, libb200kkt), Cint, (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        b, m, pointer(kkt.l_diag), pointer(kkt.u_diag), pointer(kkt.scaling_factor), pointer(wv), stream_ptr()), SolveException)
+    solve_linear_system!(kkt.linear_solver, MadNLP.primal_dual(w))
+    check(ccall((:b2_scaled_solve_post, libb200kkt), Cint, (Ptr{Cvoid}, Int64, ntuple(_ -> CuPtr{T}, 6)..., Ptr{Cvoid}),
+        b, m, pointer(kkt.l_lower), pointer(kkt.u_lower), pointer(kkt.l_diag), pointer(kkt.u_diag), pointer(kkt.scaling_factor),
+        pointer(wv), stream_ptr()), SolveException)
+    return w
+end
+
+# mul! (src/IPM/factorization.jl:239-251): the three SpMVs, then the diagonal and bound part with K2.5's signs
+function MadNLP.mul!(w::MadNLP.AbstractKKTVector{T}, kkt::B200ScaledKKT{T}, x::MadNLP.AbstractKKTVector, alpha = one(T), beta = zero(T)) where T
+    p = uplans(kkt); st = stream_ptr(); xv = MadNLP.full(x); wv = MadNLP.full(w)
+    spmv(name, plan, nz, xp, yp, b) = check(ccall((name, libb200kkt), Cint,
+        (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}), plan, pointer(nz), xp, yp, alpha, b, st), SolveException)
+    spmv(:b2_spmv_symlower, p.hess_spmv, MadNLP.nzval(kkt.hess_com), pointer(xv), pointer(wv), beta)
+    spmv(:b2_spmv_t, p.jac_spmv, MadNLP.nzval(kkt.jac_com), pointer(MadNLP.dual(x)), pointer(wv), one(T))
+    spmv(:b2_spmv_n, p.jac_spmv, MadNLP.nzval(kkt.jac_com), pointer(xv), pointer(MadNLP.dual(w)), beta)
+    check(ccall((:b2_scaled_kktmul, libb200kkt), Cint,
+        (Ptr{Cvoid}, Int64, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, CuPtr{T}, CuPtr{T}, Ptr{Cvoid}),
+        p.bounds, length(kkt.du_diag), pointer(kkt.reg), pointer(kkt.du_diag), pointer(kkt.l_lower), pointer(kkt.u_lower),
+        pointer(kkt.l_diag), pointer(kkt.u_diag), alpha, beta, pointer(xv), pointer(wv), st), SolveException)
+    return w
+end
+
+function MadNLP.jtprod!(y::CuVector{T}, kkt::B200ScaledKKT{T}, x::CuVector{T}) where T
     check(ccall((:b2_spmv_t, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, CuPtr{T}, CuPtr{T}, Cdouble, Cdouble, Ptr{Cvoid}),
         uplans(kkt).jac_spmv, pointer(MadNLP.nzval(kkt.jac_com)), pointer(x), pointer(y), one(T), zero(T), stream_ptr()), SolveException)
     return y
@@ -748,6 +843,8 @@ end
 # solver's own vectors; b2_set_g_ifr / b2_set_aug_rhs_ifr are their one-launch equivalents.  Like the rest of this file, NOT RUN.
 const B200SparseAugKKT{T} = MadNLP.SparseKKTSystem{T,VT,MT,QN,LS} where {VT<:CuVector{T},MT,QN,LS<:B200Solver}
 const B200IFRKKT{T} = Union{B200SparseAugKKT{T},B200UnreducedKKT{T},B200CondensedKKT{T},B200AnyDenseKKT{T}}
+# the types whose restoration phase and solve sites run here: the inertia-free ones and ScaledSparseKKTSystem, which has no mul_hess_blk!
+const B200RRKKT{T} = Union{B200IFRKKT{T},B200ScaledKKT{T}}
 
 mutable struct IFRPlans
     hess_spmv::Ptr{Cvoid}        # b2_spmv_plan of hess_com (C_NULL for the dense types)
@@ -757,7 +854,7 @@ mutable struct IFRPlans
 end
 const _ifr_plans = IdDict{Any,IFRPlans}()      # linear solver -> plans
 
-function ifr_plans(kkt::B200IFRKKT)
+function ifr_plans(kkt::B200RRKKT)
     get!(_ifr_plans, kkt.linear_solver) do
         sp = C_NULL
         if !(kkt isa B200AnyDenseKKT)
@@ -813,15 +910,17 @@ end
 # filter_line_search_RR! call them instead (one line per call site, INTEGRATION.md).  The b2_bounds object and a result slot come from
 # ifr_plans.  Every vector is the solver's own full vector (zl / zu via full(...), +-Inf bounds); indices 0-based on the device side.
 # Like the rest of this file, NOT RUN.
-const B200RRSolver{T} = MadNLP.MadNLPSolver{T,VT,VI,KKT} where {VT,VI,KKT<:B200IFRKKT{T}}
+const B200RRSolver{T} = MadNLP.MadNLPSolver{T,VT,VI,KKT} where {VT,VI,KKT<:B200RRKKT{T}}
 _ptr(v) = pointer(v)
 _sp() = stream_ptr()
 
-function MadNLP.set_aug_RR!(kkt::B200IFRKKT{T}, solver::MadNLP.AbstractMadNLPSolver, RR::MadNLP.RobustRestorer) where T
+function MadNLP.set_aug_RR!(kkt::B200RRKKT{T}, solver::MadNLP.AbstractMadNLPSolver, RR::MadNLP.RobustRestorer) where T
     p, o = ifr_plans(kkt), MadNLP.get_opt(solver)
     x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
     zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
-    check(ccall((:b2_set_aug_rr, libb200kkt), Cint,
+    # ScaledSparseKKTSystem's set_aug_RR! (kernels.jl:89-104) writes l_diag = x - xl and u_diag = xu - x
+    entry = kkt isa B200ScaledKKT ? :b2_set_aug_rr_scaled : :b2_set_aug_rr
+    check(ccall((entry, libb200kkt), Cint,
                 (Ptr{Cvoid}, Int64, Cdouble, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 16)..., Ptr{Cvoid}),
                 p.bounds, length(RR.pp), o.default_primal_regularization, o.default_dual_regularization, RR.zeta, _ptr(RR.D_R),
                 _ptr(RR.pp), _ptr(RR.nn), _ptr(RR.zp), _ptr(RR.zn), _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl), _ptr(zu), _ptr(kkt.reg),
@@ -830,7 +929,7 @@ function MadNLP.set_aug_RR!(kkt::B200IFRKKT{T}, solver::MadNLP.AbstractMadNLPSol
     return
 end
 
-function MadNLP.set_aug_rhs_RR!(solver::MadNLP.AbstractMadNLPSolver, kkt::B200IFRKKT{T}, RR::MadNLP.RobustRestorer, rho) where T
+function MadNLP.set_aug_rhs_RR!(solver::MadNLP.AbstractMadNLPSolver, kkt::B200RRKKT{T}, RR::MadNLP.RobustRestorer, rho) where T
     pl = ifr_plans(kkt)
     x, xl, xu = MadNLP.full(MadNLP.get_x(solver)), MadNLP.full(MadNLP.get_xl(solver)), MadNLP.full(MadNLP.get_xu(solver))
     zl, zu = MadNLP.full(MadNLP.get_zl(solver)), MadNLP.full(MadNLP.get_zu(solver))
@@ -878,7 +977,7 @@ function MadNLP.initialize_robust_restorer!(solver::B200RRSolver{T}) where T
 end
 
 # finish_aug_solve_RR!(dpp, dnn, dzp, dzn, l, dl, pp, nn, zp, zn, mu_R, rho) (src/IPM/kernels.jl:251-257)
-function finish_aug_solve_RR!(kkt::B200IFRKKT{T}, dpp, dnn, dzp, dzn, l, dl, pp, nn, zp, zn, mu_R, rho) where T
+function finish_aug_solve_RR!(kkt::B200RRKKT{T}, dpp, dnn, dzp, dzn, l, dl, pp, nn, zp, zn, mu_R, rho) where T
     check(ccall((:b2_finish_aug_solve_rr, libb200kkt), Cint, (Int64, ntuple(_ -> CuPtr{T}, 6)..., Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 4)...,
                 Ptr{Cvoid}), length(l), _ptr(l), _ptr(dl), _ptr(pp), _ptr(nn), _ptr(zp), _ptr(zn), mu_R, rho, _ptr(dpp), _ptr(dnn),
                 _ptr(dzp), _ptr(dzn), _sp()), SolveException)
@@ -887,35 +986,35 @@ end
 
 # the reductions (kernels.jl:390-636): one launch each into the plans' result slot, then one read.  Arguments as in the reference
 # (vectors full length: x, xl, xu, zl, zu, f_R, jacl, dx n_tot; c, l, pp, nn, zp, zn and steps m; dzl / dzu compressed).
-function _reduce(kkt::B200IFRKKT{T}, sym::Symbol, argt::Tuple, args...) where T
+function _reduce(kkt::B200RRKKT{T}, sym::Symbol, argt::Tuple, args...) where T
     pl = ifr_plans(kkt)
     check(ccall(Libdl.dlsym(Libdl.dlopen(libb200kkt), sym), Cint, (Ptr{Cvoid}, argt..., CuPtr{T}, Ptr{Cvoid}), pl.bounds, args...,
                 _ptr(pl.result), _sp()), SolveException)
     return Array(view(pl.result, 1:1))[1]
 end
 const _V = CuPtr{Float64}
-get_theta(kkt::B200IFRKKT, c) = _reduce(kkt, :b2_get_theta, (Int64, _V), length(c), _ptr(c))
-get_theta_R(kkt::B200IFRKKT, c, p, n) = _reduce(kkt, :b2_get_theta_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
-get_inf_pr_R(kkt::B200IFRKKT, c, p, n) = _reduce(kkt, :b2_get_inf_pr_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
-get_obj_val_R(kkt::B200IFRKKT, p, n, D_R, x, x_ref, rho, zeta) =
+get_theta(kkt::B200RRKKT, c) = _reduce(kkt, :b2_get_theta, (Int64, _V), length(c), _ptr(c))
+get_theta_R(kkt::B200RRKKT, c, p, n) = _reduce(kkt, :b2_get_theta_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
+get_inf_pr_R(kkt::B200RRKKT, c, p, n) = _reduce(kkt, :b2_get_inf_pr_r, (Int64, _V, _V, _V), length(c), _ptr(c), _ptr(p), _ptr(n))
+get_obj_val_R(kkt::B200RRKKT, p, n, D_R, x, x_ref, rho, zeta) =
     _reduce(kkt, :b2_get_obj_val_r, (Int64, _V, _V, _V, _V, _V, Cdouble, Cdouble), length(p), _ptr(p), _ptr(n), _ptr(D_R), _ptr(x),
             _ptr(x_ref), rho, zeta)
-get_inf_du_R(kkt::B200IFRKKT, f_R, l, zl, zu, jacl, zp, zn, rho, sd) =
+get_inf_du_R(kkt::B200RRKKT, f_R, l, zl, zu, jacl, zp, zn, rho, sd) =
     _reduce(kkt, :b2_get_inf_du_r, (Int64, ntuple(_ -> _V, 7)..., Cdouble, Cdouble), length(l), _ptr(f_R), _ptr(l), _ptr(zl), _ptr(zu),
             _ptr(jacl), _ptr(zp), _ptr(zn), rho, sd)
-get_inf_compl_R(kkt::B200IFRKKT, x, xl, xu, zl, zu, pp, zp, nn, zn, mu_R, sc) =
+get_inf_compl_R(kkt::B200RRKKT, x, xl, xu, zl, zu, pp, zp, nn, zn, mu_R, sc) =
     _reduce(kkt, :b2_get_inf_compl_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(x), _ptr(xl), _ptr(xu), _ptr(zl),
             _ptr(zu), _ptr(pp), _ptr(zp), _ptr(nn), _ptr(zn), mu_R, sc)
-get_alpha_max_R(kkt::B200IFRKKT, x, xl, xu, dx, pp, dpp, nn, dnn, tau_R) =
+get_alpha_max_R(kkt::B200RRKKT, x, xl, xu, dx, pp, dpp, nn, dnn, tau_R) =
     _reduce(kkt, :b2_get_alpha_max_r, (Int64, ntuple(_ -> _V, 8)..., Cdouble), length(pp), _ptr(x), _ptr(xl), _ptr(xu), _ptr(dx), _ptr(pp),
             _ptr(dpp), _ptr(nn), _ptr(dnn), tau_R)
-get_alpha_z_R(kkt::B200IFRKKT, zl, zu, dzl, dzu, zp, dzp, zn, dzn, tau_R) =
+get_alpha_z_R(kkt::B200RRKKT, zl, zu, dzl, dzu, zp, dzp, zn, dzn, tau_R) =
     _reduce(kkt, :b2_get_alpha_z_r, (Int64, ntuple(_ -> _V, 8)..., Cdouble), length(zp), _ptr(zl), _ptr(zu), _ptr(dzl), _ptr(dzu), _ptr(zp),
             _ptr(dzp), _ptr(zn), _ptr(dzn), tau_R)
-get_varphi_R(kkt::B200IFRKKT, obj_val, x, xl, xu, pp, nn, mu_R) =
+get_varphi_R(kkt::B200RRKKT, obj_val, x, xl, xu, pp, nn, mu_R) =
     _reduce(kkt, :b2_get_varphi_r, (Int64, Cdouble, ntuple(_ -> _V, 5)..., Cdouble), length(pp), obj_val, _ptr(x), _ptr(xl), _ptr(xu),
             _ptr(pp), _ptr(nn), mu_R)
-get_varphi_d_R(kkt::B200IFRKKT, f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho) =
+get_varphi_d_R(kkt::B200RRKKT, f_R, x, xl, xu, dx, pp, nn, dpp, dnn, mu_R, rho) =
     _reduce(kkt, :b2_get_varphi_d_r, (Int64, ntuple(_ -> _V, 9)..., Cdouble, Cdouble), length(pp), _ptr(f_R), _ptr(x), _ptr(xl), _ptr(xu),
             _ptr(dx), _ptr(pp), _ptr(nn), _ptr(dpp), _ptr(dnn), mu_R, rho)
 
@@ -1061,7 +1160,8 @@ function MadNLP.restore!(solver::B200RRSolver{T}) where T
         MadNLP.set_inf_compl_mu!(solver, MadNLP.get_inf_compl(cl..., MadNLP.get_mu(solver), sc))
         MadNLP.print_iter(solver)
         !o.hessian_constant && MadNLP.eval_lag_hess_wrapper!(solver, kkt, MadNLP.get_x(solver), y)
-        check(ccall((:b2_set_aug_diagonal_iterate, libb200kkt), Cint, (Ptr{Cvoid}, Int64, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 11)..., Ptr{Cvoid}),
+        entry = kkt isa B200ScaledKKT ? :b2_set_aug_diagonal_iterate_scaled : :b2_set_aug_diagonal_iterate   # K2.5's bound signs
+        check(ccall((entry, libb200kkt), Cint, (Ptr{Cvoid}, Int64, Cdouble, Cdouble, ntuple(_ -> CuPtr{T}, 11)..., Ptr{Cvoid}),
                     pl.bounds, length(y), o.default_primal_regularization, o.default_dual_regularization, _ptr(x), _ptr(xl), _ptr(xu),
                     _ptr(zl), _ptr(zu), _ptr(kkt.reg), _ptr(kkt.du_diag), _ptr(kkt.l_lower), _ptr(kkt.u_lower), _ptr(kkt.l_diag),
                     _ptr(kkt.u_diag), _sp()), SolveException)

@@ -172,6 +172,7 @@ class SolverVectors:
 
 class _KKTBase:
     stream = None
+    _scaled = False         # True: K2.5's bound signs (l_diag = x - xl, u_diag = xu - x) and its scaled diagonal regularisation
 
     def stream_ptr(self):
         """the stream every launch on this system (and on the host-layer objects built over it) goes to, as the ABI's argument"""
@@ -471,6 +472,76 @@ class SparseUnreducedKKTSystem(_SparseKKTBase):
         self.linear_solver.solve_linear_system(w.full())
         check(lib.b2_unreduced_solve_post(*args))
         return w
+
+
+class ScaledSparseKKTSystem(_SparseKKTBase):
+    """src/KKT/Sparse/scaled_augmented.jl (K2.5): the augmented system of SparseKKTSystem under the congruence by the scaling factor
+    s = sqrt(X - Xl) sqrt(Xu - X) (each factor over the bounds the variable has, 1 for a free one):
+
+        [ s (W + reg) s + (X - Xl) Zu + (Xu - X) Zl    s J' ]
+        [ J s                                        du_diag ]
+
+    Its barrier block stays bounded as mu -> 0 where K2's Sigma = Zl / (X - Xl) grows without bound.  The COO layout of V, the
+    pattern, the COO->CSC maps, jac_com, hess_com and the linear solver are SparseKKTSystem's (scaled_augmented.jl:104-124 is
+    augmented.jl's); build_kkt scales V's sources on their way into aug_com (b2_scaled_transfer), so no scaled copy of V is kept.
+
+    Sign convention: l_diag = x - xl and u_diag = xu - x, both positive (IPM/kernels.jl:36-45), the OPPOSITE of the reduced systems'
+    xl - x and x - xu.  Whoever loads an iterate into l_diag / u_diag supplies these signs; the set_aug_diagonal! and set_aug_RR! sites
+    of the IPM layer write them (b2_set_aug_diagonal_iterate_scaled, b2_set_aug_rr_scaled).
+
+    get_jacobian, compress_*, jtprod and the Hessian product are SparseKKTSystem's; is_inertia_correct, inertia_rule and dual_rule
+    the reduced system's: while scaling_factor > 0 the inertia is K2's by congruence, (n_tot, 0, m) at a correct iterate.  Neither a
+    quasi-Newton Hessian (factorization.jl:183-188) nor the inertia-free test (no mul_hess_blk! in the reference) is supported."""
+    _scaled = True
+
+    def __init__(self, cb, linear_solver=B200SparseSolver, opt_linear_solver=None):
+        self._build(cb, linear_solver, opt_linear_solver, unreduced=False)
+        self.quasi_newton = ExactHessian()
+        self.scaling_factor = _dz(self.n_tot)
+        # aug_com's pattern on the device: b2_scaled_transfer reads the row and column of each slot from it
+        self._aug_colptr_d = torch.from_numpy(np.ascontiguousarray(self.aug_com.colptr, dtype=np.int32)).to(_DEV)
+        self._aug_rowval_d = torch.from_numpy(np.ascontiguousarray(self.aug_com.rowval, dtype=np.int32)).to(_DEV)
+
+    def initialize(self):
+        """scaled_augmented.jl:181-192."""
+        self._initialize_common()
+        self.l_lower.zero_(); self.u_lower.zero_(); self.l_diag.fill_(1.0); self.u_diag.fill_(1.0)
+        self.scaling_factor.fill_(1.0)
+        self.hess_com.nzval.zero_()
+
+    def set_aug_diagonal_(self):
+        """_set_aug_diagonal!(::ScaledSparseKKTSystem) (IPM/kernels.jl:47-68): pr_diag and scaling_factor in one launch."""
+        check(lib.b2_scaled_set_aug_diagonal(self._bounds.h, ptr(self.reg), ptr(self.l_lower), ptr(self.l_diag), ptr(self.u_lower),
+                                             ptr(self.u_diag), ptr(self.pr_diag), ptr(self.scaling_factor), self.stream_ptr()))
+
+    def build_kkt(self):
+        """scaled_augmented.jl:209-236 in one pass over aug_com's slots (b2_scaled_transfer)."""
+        check(lib.b2_scaled_transfer(self._aug_plan.h, self.N, self._n_tot, ptr(self._aug_colptr_d), ptr(self._aug_rowval_d),
+                                     ptr(self.scaling_factor), ptr(self.aug_com.nzval), ptr(self.V), self.stream_ptr()))
+
+    def regularize_diagonal(self, primal, dual):
+        """scaled_augmented.jl:238-242: reg += primal; pr_diag += primal s^2; du_diag -= dual."""
+        check(lib.b2_scaled_regularize_diagonal(self._n_tot, self._m, float(primal), float(dual), ptr(self.scaling_factor),
+                                                ptr(self.reg), ptr(self.pr_diag), ptr(self.du_diag), self.stream_ptr()))
+
+    def solve_kkt(self, w: UnreducedKKTVector):
+        """src/IPM/factorization.jl:48-74: one launch before the sparse solve, one after."""
+        sp = self.stream_ptr()
+        check(lib.b2_scaled_solve_pre(self._bounds.h, self._m, ptr(self.l_diag), ptr(self.u_diag), ptr(self.scaling_factor),
+                                      ptr(w.values), sp))
+        self.linear_solver.solve_linear_system(w.primal_dual())
+        check(lib.b2_scaled_solve_post(self._bounds.h, self._m, ptr(self.l_lower), ptr(self.u_lower), ptr(self.l_diag),
+                                       ptr(self.u_diag), ptr(self.scaling_factor), ptr(w.values), sp))
+        return w
+
+    def _kktmul(self, w, x, alpha, beta):
+        """mul!'s diagonal and bound part with K2.5's bound-row signs (src/IPM/factorization.jl:239-251)"""
+        check(lib.b2_scaled_kktmul(self._bounds.h, self._m, ptr(self.reg), ptr(self.du_diag), ptr(self.l_lower), ptr(self.u_lower),
+                                   ptr(self.l_diag), ptr(self.u_diag), float(alpha), float(beta), ptr(x.values), ptr(w.values),
+                                   self.stream_ptr()))
+
+    def _hess_blk(self, *args, **kwargs):
+        raise ValueError("mul_hess_blk!: not supported by the KKT formulation ScaledSparseKKTSystem (the inertia-free test needs it)")
 
 
 # ======================================================================================================
@@ -815,7 +886,8 @@ class DenseKKTSystem(_DenseKKTBase):
         return y
 
 
-_QN_UNSUPPORTED = {SparseUnreducedKKTSystem: "SparseUnreducedKKTSystem", SparseCondensedKKTSystem: "SparseCondensedKKTSystem"}
+_QN_UNSUPPORTED = {SparseUnreducedKKTSystem: "SparseUnreducedKKTSystem", SparseCondensedKKTSystem: "SparseCondensedKKTSystem",
+                   ScaledSparseKKTSystem: "ScaledSparseKKTSystem"}
 
 
 def create_kkt_system(kkt_type, cb, linear_solver=None, opt_linear_solver=None, hessian_approximation=ExactHessian,

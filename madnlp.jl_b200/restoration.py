@@ -102,10 +102,11 @@ class RobustRestorer:
         set_aug_diagonal_ (so SparseUnreducedKKTSystem keeps its _set_aug_diagonal!).  The regularisations are MadNLP's
         default_primal_regularization / default_dual_regularization."""
         k = self.kkt if kkt is None else kkt
-        check(lib.b2_set_aug_rr(self._b, self.m, float(primal_regularization), float(dual_regularization), self.zeta, ptr(self.D_R),
-                                ptr(self.pp), ptr(self.nn), ptr(self.zp), ptr(self.zn), ptr(self.x), ptr(self.xl), ptr(self.xu),
-                                ptr(self.zl), ptr(self.zu), ptr(k.reg), ptr(k.du_diag), ptr(k.l_lower), ptr(k.u_lower), ptr(k.l_diag),
-                                ptr(k.u_diag), self.kkt.stream_ptr()))
+        # ScaledSparseKKTSystem's set_aug_RR! (kernels.jl:89-104) writes l_diag = x - xl and u_diag = xu - x
+        fn = lib.b2_set_aug_rr_scaled if k._scaled else lib.b2_set_aug_rr
+        check(fn(self._b, self.m, float(primal_regularization), float(dual_regularization), self.zeta, ptr(self.D_R), ptr(self.pp),
+                 ptr(self.nn), ptr(self.zp), ptr(self.zn), ptr(self.x), ptr(self.xl), ptr(self.xu), ptr(self.zl), ptr(self.zu), ptr(k.reg),
+                 ptr(k.du_diag), ptr(k.l_lower), ptr(k.u_lower), ptr(k.l_diag), ptr(k.u_diag), self.kkt.stream_ptr()))
         k.set_aug_diagonal_()
 
     def set_aug_rhs_RR(self, p, rho=1000.0):
