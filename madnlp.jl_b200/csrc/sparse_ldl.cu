@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <stdexcept>
+#include <type_traits>
 #include <vector>
 
 #include "analysis.hpp"
@@ -40,12 +41,12 @@ struct Phase {
     int offAllC = 0, nAllC = 0, maxwAllC = 0;       // every M/B front of the phase (diagonal-block inversion)
     int dep_ngroup = 0, dep_type_off = 0, dep_ptr_off = 0, dep_tasks_off = 0, dep_maxf1 = 0, dep_maxf2 = 0;
     int dep_maxf4 = 0;                              // PAIRS: the largest front of order 65..96 (0: no four-warp group)
-    // single-launch solve (k_solve_dep: the same groups, condition and phase 0 only): persistent CTAs (0: the level-launch solve)
-    int sol_grid = 0;
-    // its block form (k_solve_dep_block) for 2, 4 and 8 right-hand sides per walk: persistent CTAs of each width
-    int sol_grid_blk[3] = {0, 0, 0};
+    // single-launch solve (k_solve_dep, and k_solve_dep_block for several right-hand sides: the same groups, condition and phase 0
+    // only): persistent CTAs per width, [width_index(NR)] (sol_grid[0] == 0: the level-launch solve)
+    int sol_grid[4] = {0, 0, 0, 0};
     cudaGraphExec_t g_factor = nullptr, g_fwd = nullptr, g_bwd = nullptr;
-    // the level-launch block solve's two sweeps for 2, 4 and 8 right-hand sides, one graph per width (captured on first use)
+    // the level-launch block solve's two sweeps for 2, 4 and 8 right-hand sides, one graph per width (captured on first use),
+    // [width_index(NR) - 1]
     cudaGraphExec_t g_blk[3] = {nullptr, nullptr, nullptr};
     int64_t n_factor_launches = 0, n_solve_launches = 0;
     int64_t n_fused_fronts = 0;
@@ -53,6 +54,12 @@ struct Phase {
 
 constexpr int W_MAX = 64;        // team-per-front classes: f <= 32 (one warp), f <= 64 (two warps)
 constexpr int W_MAX_PAIRS = 96;  // PAIRS adds a four-warp class, 64 < f <= 96 (single-launch schedule only)
+
+// b2_solve walks the tree with 1, 2, 4 or 8 right-hand sides at a time; each width has its own solve kernels
+template <int NR> using Width = std::integral_constant<int, NR>;
+constexpr int width_index(int NR) { return NR == 1 ? 0 : NR == 2 ? 1 : NR == 4 ? 2 : 3; }
+template <typename Fn>
+void for_each_width(Fn&& fn) { fn(Width<1>()); fn(Width<2>()); fn(Width<4>()); fn(Width<8>()); }
 
 }  // namespace
 
@@ -170,6 +177,14 @@ WarpSched warp_sched(b2_solver* s, const WarpLaunch& L) {
     return w;
 }
 
+// the groups of phase P's single-launch schedule (factorisation and solve)
+DepSched dep_sched(b2_solver* s, const Phase& P) {
+    DepSched ds;
+    ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
+    ds.ngroup = P.dep_ngroup;
+    return ds;
+}
+
 // issue the numeric factorisation of one phase on `st`; returns number of launches
 int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
     FactorArgs a = factor_args(s);
@@ -188,8 +203,7 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
         ++nl;
     };
     if (P.dep_ngroup && (s->opt.dep_schedule & 1)) {
-        DepSched ds;
-        ds.grp_type = sched + P.dep_type_off; ds.grp_ptr = sched + P.dep_ptr_off; ds.tasks = sched + P.dep_tasks_off; ds.ngroup = P.dep_ngroup;
+        const DepSched ds = dep_sched(s, P);
         // (the group ticket in slot nsuper re-arms itself: the CTA that takes the last group resets it)
         cudaMemsetAsync(s->d_flags.p, 0, (size_t)s->S.nsuper * sizeof(int32_t), st);
         size_t sm = sizeof(double) * std::max<size_t>((size_t)FW_WARPS * TeamSmem<1>::doubles(P.dep_maxf1), (size_t)TeamSmem<2>::doubles(P.dep_maxf2));
@@ -238,10 +252,47 @@ int64_t enqueue_factor(b2_solver* s, int ph, cudaStream_t st) {
     return nl;
 }
 
+// The kernels of a level-launch sweep over NR columns, by role: the one-column kernels for NR = 1, their _block forms otherwise, which
+// also take the big fronts' columns through dynamic shared memory (fsm bytes in the forward kernels, bsm in the backward ones).
+template <int NR>
+struct SolveKernels {
+    template <int NW, int NTEAM> static constexpr auto fwd_warp = k_fwd_warp2_block<NW, NTEAM, NR>;
+    template <int NW, int NTEAM> static constexpr auto bwd_warp = k_bwd_warp2_block<NW, NTEAM, NR>;
+    static constexpr auto fwd_init = k_bs_fwd_init_block<NR>;
+    static constexpr auto bwd_init = k_bs_bwd_init_block<NR>;
+    static constexpr auto head = k_bs_head_block<NR>;
+    static constexpr auto fwd = k_bs_fwd_block<NR>;
+    static constexpr auto bwd = k_bs_bwd_block<NR>;
+    static constexpr auto finish = k_bs_bwd_finish_block<NR>;
+    static constexpr size_t fsm = (size_t)bs_smem_doubles<NR>() * sizeof(double), bsm = (size_t)NR * BS * sizeof(double);
+};
+template <>
+struct SolveKernels<1> {
+    template <int NW, int NTEAM> static constexpr auto fwd_warp = k_fwd_warp2<NW, NTEAM>;
+    template <int NW, int NTEAM> static constexpr auto bwd_warp = k_bwd_warp2<NW, NTEAM>;
+    static constexpr auto fwd_init = k_bs_fwd_init;
+    static constexpr auto bwd_init = k_bs_bwd_init;
+    static constexpr auto head = k_bs_head;
+    static constexpr auto fwd = k_bs_fwd;
+    static constexpr auto bwd = k_bs_bwd;
+    static constexpr auto finish = k_bs_bwd_finish;
+    static constexpr size_t fsm = 0, bsm = 0;
+};
+
+// one launch of the team-per-front sweep kernel with NTEAM teams of NW warps per CTA (cfg: grid, stream and launch attributes)
+template <int NR, int NW, int NTEAM>
+void launch_warp_sweep(cudaLaunchConfig_t cfg, bool forward, const SolveArgs& a, const ChildRec* cr, const WarpSched& ws) {
+    cfg.blockDim = dim3(NTEAM * NW * 32);
+    cfg.dynamicSmemBytes = (size_t)NTEAM * SolveSmem<NW, NR>::doubles * sizeof(double);
+    if (forward) cudaLaunchKernelEx(&cfg, SolveKernels<NR>::template fwd_warp<NW, NTEAM>, a, cr, ws);
+    else cudaLaunchKernelEx(&cfg, SolveKernels<NR>::template bwd_warp<NW, NTEAM>, a, ws);
+}
+
 // one sweep of phase `ph`, level by level.  NR = 1: the one-column solve on xp / cbv.  NR > 1: the block kernels on NR interleaved
 // columns of the block workspace (d_xblk), with the same launches as NR = 1.
 template <int NR>
 int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
+    using K = SolveKernels<NR>;
     SolveArgs a = solve_args(s);
     BigSolveArgs bs = big_solve_args(s);
     if constexpr (NR > 1) {
@@ -257,43 +308,15 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
     cudaLaunchAttribute pattr[1];
     pattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     pattr[0].val.programmaticStreamSerializationAllowed = 1;
-    auto cfg_of = [&](int grid, int block, size_t sm) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = sm; cfg.stream = st;
-        cfg.attrs = pattr; cfg.numAttrs = 1;
-        return cfg;
-    };
     auto warp_launch = [&](const WarpLaunch& L, bool fused = false) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(L.n_cta); cfg.stream = st; cfg.attrs = pattr; cfg.numAttrs = 1;
         const ChildRec* cr = s->d_childrec.p;
         const WarpSched wsched = warp_sched(s, L);
-        if (L.nw == 1 && fused) {     // bottom subtrees: more one-warp teams per CTA, fewer sequential rounds per stage
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, SOLVE_FUSED_TEAMS * 32, (size_t)SOLVE_FUSED_TEAMS * SolveSmem<1, NR>::doubles * sizeof(double));
-            if constexpr (NR == 1) {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1, SOLVE_FUSED_TEAMS>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1, SOLVE_FUSED_TEAMS>, a, wsched);
-            } else {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, a, wsched);
-            }
-        } else if (L.nw == 1) {
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, FW_WARPS * 32, (size_t)FW_WARPS * SolveSmem<1, NR>::doubles * sizeof(double));
-            if constexpr (NR == 1) {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<1>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<1>, a, wsched);
-            } else {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<1, FW_WARPS, NR>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<1, FW_WARPS, NR>, a, wsched);
-            }
-        } else {
-            cudaLaunchConfig_t cfg = cfg_of(L.n_cta, 64, (size_t)SolveSmem<2, NR>::doubles * sizeof(double));
-            if constexpr (NR == 1) {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2<2>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2<2>, a, wsched);
-            } else {
-                if (forward) cudaLaunchKernelEx(&cfg, k_fwd_warp2_block<2, 1, NR>, a, cr, wsched);
-                else cudaLaunchKernelEx(&cfg, k_bwd_warp2_block<2, 1, NR>, a, wsched);
-            }
-        }
+        // (bottom subtrees: more one-warp teams per CTA, fewer sequential rounds per stage)
+        if (L.nw == 1 && fused) launch_warp_sweep<NR, 1, SOLVE_FUSED_TEAMS>(cfg, forward, a, cr, wsched);
+        else if (L.nw == 1) launch_warp_sweep<NR, 1, FW_WARPS>(cfg, forward, a, cr, wsched);
+        else launch_warp_sweep<NR, 2, 1>(cfg, forward, a, cr, wsched);
         ++nl;
     };
     if (forward && P.fused.n_cta) warp_launch(P.fused, true);
@@ -306,40 +329,24 @@ int64_t enqueue_solve(b2_solver* s, int ph, bool forward, cudaStream_t st) {
         if (lv.nC) {
             const int32_t* lc = sched + lv.offC;
             const int nblk = (lv.maxwC + BS - 1) / BS;
-            const size_t fsm = (size_t)bs_smem_doubles<NR>() * sizeof(double), bsm = (size_t)NR * BS * sizeof(double);
             if (forward) {
-                if constexpr (NR == 1) {
-                    k_bs_fwd_init<<<lv.nC, 1024, 0, st>>>(bs, lc);
-                    k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, 0, 0);
-                } else {
-                    k_bs_fwd_init_block<NR><<<lv.nC, 1024, 0, st>>>(bs, lc);
-                    k_bs_head_block<NR><<<lv.nC, BS_NT, fsm, st>>>(bs, lc, 0, 0);
-                }
+                K::fwd_init<<<lv.nC, 1024, 0, st>>>(bs, lc);
+                K::head<<<lv.nC, BS_NT, K::fsm, st>>>(bs, lc, 0, 0);
                 nl += 2;
                 for (int b = 0; b < nblk; ++b) {
                     const int rows = std::max(1, lv.maxfC - b * BS - 1);
-                    const dim3 grid((rows + BSF_ROWS - 1) / BSF_ROWS, lv.nC);
-                    if constexpr (NR == 1) k_bs_fwd<<<grid, BS_NT, 0, st>>>(bs, lc, b);
-                    else k_bs_fwd_block<NR><<<grid, BS_NT, fsm, st>>>(bs, lc, b);
+                    K::fwd<<<dim3((rows + BSF_ROWS - 1) / BSF_ROWS, lv.nC), BS_NT, K::fsm, st>>>(bs, lc, b);
                     ++nl;
                 }
             } else {
-                const dim3 ginit((lv.maxwC + 7) / 8, lv.nC), gfin((lv.maxwC + 255) / 256, lv.nC);
-                if constexpr (NR == 1) {
-                    k_bs_bwd_init<<<ginit, 256, 0, st>>>(bs, lc);
-                    k_bs_head<<<lv.nC, BS_NT, 0, st>>>(bs, lc, -1, 1);
-                } else {
-                    k_bs_bwd_init_block<NR><<<ginit, 256, 0, st>>>(bs, lc);
-                    k_bs_head_block<NR><<<lv.nC, BS_NT, bsm, st>>>(bs, lc, -1, 1);
-                }
+                K::bwd_init<<<dim3((lv.maxwC + 7) / 8, lv.nC), 256, 0, st>>>(bs, lc);
+                K::head<<<lv.nC, BS_NT, K::bsm, st>>>(bs, lc, -1, 1);
                 nl += 2;
                 for (int b = nblk - 1; b >= 1; --b) {
-                    if constexpr (NR == 1) k_bs_bwd<<<dim3(b, lv.nC), BS_NT, 0, st>>>(bs, lc, b);
-                    else k_bs_bwd_block<NR><<<dim3(b, lv.nC), BS_NT, bsm, st>>>(bs, lc, b);
+                    K::bwd<<<dim3(b, lv.nC), BS_NT, K::bsm, st>>>(bs, lc, b);
                     ++nl;
                 }
-                if constexpr (NR == 1) k_bs_bwd_finish<<<gfin, 256, 0, st>>>(bs, lc);
-                else k_bs_bwd_finish_block<NR><<<gfin, 256, 0, st>>>(bs, lc);
+                K::finish<<<dim3((lv.maxwC + 255) / 256, lv.nC), 256, 0, st>>>(bs, lc);
                 ++nl;
             }
         }
@@ -357,91 +364,63 @@ size_t solve_dep_smem(int maxf4) {
     return sizeof(double) * (maxf4 ? std::max<size_t>(d, (size_t)SolveSmem<4, NR>::doubles_panel(maxf4)) : d);
 }
 
-// the whole solve of one right-hand side x (original order, in place) as ONE launch of k_solve_dep
-void enqueue_solve_dep(b2_solver* s, double* x, cudaStream_t st) {
-    const Phase& P = s->phase[0];
-    SolveArgs a = solve_args(s);
-    a.perm = s->d_perm.p;
-    a.x = x;
-    a.strace = s->d_strace.p;
-    const int64_t nr = s->cbv_off[s->S.nsuper];
-    a.up = s->d_slots.p;
-    a.down = s->d_slots.p + nr;
-    a.ypiv = s->d_slots.p + 2 * nr;
-    DepSched ds;
-    ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
-    ds.ngroup = P.dep_ngroup;
-    if (s->pairs) {
-        k_solve_dep_pairs<<<P.sol_grid, 128, solve_dep_smem<1>(P.dep_maxf4), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
-                                                                   s->S.n, s->d_slots.p, (int64_t)s->d_slots.n, s->d_dsub.p);
-        return;
-    }
-    k_solve_dep<<<P.sol_grid, 128, solve_dep_smem<1>(0), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1, s->S.n,
-                                                         s->d_slots.p, (int64_t)s->d_slots.n);
+// the single-launch solve kernel for NR right-hand sides per walk, static or PAIRS
+template <int NR>
+const void* solve_dep_kernel(bool pairs) {
+    if constexpr (NR == 1) return pairs ? (const void*)k_solve_dep_pairs : (const void*)k_solve_dep;
+    else return pairs ? (const void*)k_solve_dep_block<NR, true> : (const void*)k_solve_dep_block<NR, false>;
 }
 
+// columns [0, ncol) of x (original order, ld n, in place), 1 <= ncol <= NR, as ONE launch of the single-launch solve: k_solve_dep
+// (k_solve_dep_pairs) on d_slots for NR = 1, k_solve_dep_block<NR> on d_bslots otherwise.  The hand-off slots are up [NR sum r] |
+// down [NR sum r] | ypiv [NR n].
 template <int NR>
-const void* solve_block_kernel(bool pairs) {
-    return pairs ? (const void*)k_solve_dep_block<NR, true> : (const void*)k_solve_dep_block<NR, false>;
-}
-
-// columns [0, ncol) of x (ld n) as ONE launch of k_solve_dep_block<NR>, 1 <= ncol <= NR
-template <int NR>
-void enqueue_solve_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
+void enqueue_solve_dep(b2_solver* s, double* x, int ncol, cudaStream_t st) {
     const Phase& P = s->phase[0];
+    const DevBuf<double>& slots = NR == 1 ? s->d_slots : s->d_bslots;
     SolveArgs a = solve_args(s);
     a.perm = s->d_perm.p;
     a.x = x;
     const int64_t nr = s->cbv_off[s->S.nsuper];
-    a.up = s->d_bslots.p;
-    a.down = s->d_bslots.p + NR * nr;
-    a.ypiv = s->d_bslots.p + 2 * NR * nr;
-    DepSched ds;
-    ds.grp_type = s->d_sched.p + P.dep_type_off; ds.grp_ptr = s->d_sched.p + P.dep_ptr_off; ds.tasks = s->d_sched.p + P.dep_tasks_off;
-    ds.ngroup = P.dep_ngroup;
-    const int w = NR == 2 ? 0 : NR == 4 ? 1 : 2;
-    auto kern = s->pairs ? k_solve_dep_block<NR, true> : k_solve_dep_block<NR, false>;
-    kern<<<P.sol_grid_blk[w], 128, solve_dep_smem<NR>(P.dep_maxf4), st>>>(a, s->d_childrec.p, ds, s->d_counters.p + 4, s->d_flags.p + s->S.nsuper + 1,
-                                                                 s->S.n, ncol, s->d_bslots.p, (int64_t)s->d_bslots.n, s->d_dsub.p);
-}
-
-// the level-launch block kernels of one width: dynamic shared memory above the 48 KB default
-template <int NR>
-cudaError_t set_level_block_attrs() {
-    const void* k[] = {(const void*)k_fwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>, (const void*)k_bwd_warp2_block<1, SOLVE_FUSED_TEAMS, NR>,
-                       (const void*)k_fwd_warp2_block<1, FW_WARPS, NR>, (const void*)k_bwd_warp2_block<1, FW_WARPS, NR>,
-                       (const void*)k_fwd_warp2_block<2, 1, NR>, (const void*)k_bwd_warp2_block<2, 1, NR>,
-                       (const void*)k_bs_head_block<NR>, (const void*)k_bs_fwd_block<NR>, (const void*)k_bs_bwd_block<NR>};
-    for (const void* f : k) {
-        cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-        if (e != cudaSuccess) return e;
+    a.up = slots.p;
+    a.down = slots.p + NR * nr;
+    a.ypiv = slots.p + 2 * NR * nr;
+    const DepSched ds = dep_sched(s, P);
+    const int grid = P.sol_grid[width_index(NR)];
+    const size_t sm = solve_dep_smem<NR>(P.dep_maxf4);       // (dep_maxf4 is 0 on a static tree)
+    int* err = s->d_counters.p + 4;
+    int* ctl = s->d_flags.p + s->S.nsuper + 1;
+    if constexpr (NR == 1) {
+        a.strace = s->d_strace.p;
+        if (s->pairs) k_solve_dep_pairs<<<grid, 128, sm, st>>>(a, s->d_childrec.p, ds, err, ctl, s->S.n, slots.p, (int64_t)slots.n, s->d_dsub.p);
+        else k_solve_dep<<<grid, 128, sm, st>>>(a, s->d_childrec.p, ds, err, ctl, s->S.n, slots.p, (int64_t)slots.n);
+    } else {
+        auto kern = s->pairs ? k_solve_dep_block<NR, true> : k_solve_dep_block<NR, false>;
+        kern<<<grid, 128, sm, st>>>(a, s->d_childrec.p, ds, err, ctl, s->S.n, ncol, slots.p, (int64_t)slots.n, s->d_dsub.p);
     }
-    return cudaSuccess;
 }
 
 int set_smem_attrs() {
-    B2_CUDA(cudaFuncSetAttribute(k_front_smem<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_factor_warp<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_factor_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_factor_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_fwd_warp2<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute((k_fwd_warp2<1, SOLVE_FUSED_TEAMS>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute((k_bwd_warp2<1, SOLVE_FUSED_TEAMS>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_fwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_bwd_warp2<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_solve_dep, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(cudaFuncSetAttribute(k_solve_dep_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    B2_CUDA(set_level_block_attrs<2>());
-    B2_CUDA(set_level_block_attrs<4>());
-    B2_CUDA(set_level_block_attrs<8>());
-    for (bool pairs : {false, true}) {
-        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<2>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<4>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        B2_CUDA(cudaFuncSetAttribute(solve_block_kernel<8>(pairs), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    }
-    B2_CUDA(cudaFuncSetAttribute(k_big_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    constexpr cudaFuncAttribute dyn = cudaFuncAttributeMaxDynamicSharedMemorySize;
+    B2_CUDA(cudaFuncSetAttribute(k_front_smem<512>, dyn, 227 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_factor_warp<1>, dyn, 160 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_factor_warp<2>, dyn, 160 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_factor_dep, dyn, 160 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_factor_dep_pairs, dyn, 160 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(k_big_inv, dyn, 160 * 1024));
+    // the solve kernels of every width that take dynamic shared memory (the one-column big-front kernels take none)
+    cudaError_t e = cudaSuccess;
+    for_each_width([&](auto w) {
+        using K = SolveKernels<w>;
+        std::vector<const void*> k = {(const void*)K::template fwd_warp<1, SOLVE_FUSED_TEAMS>, (const void*)K::template bwd_warp<1, SOLVE_FUSED_TEAMS>,
+                                      (const void*)K::template fwd_warp<1, FW_WARPS>, (const void*)K::template bwd_warp<1, FW_WARPS>,
+                                      (const void*)K::template fwd_warp<2, 1>, (const void*)K::template bwd_warp<2, 1>,
+                                      solve_dep_kernel<w>(false), solve_dep_kernel<w>(true)};
+        if (w > 1) k.insert(k.end(), {(const void*)K::head, (const void*)K::fwd, (const void*)K::bwd});
+        for (const void* f : k)
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(f, dyn, 100 * 1024);
+    });
+    B2_CUDA(e);
     return B2_OK;
 }
 
@@ -518,7 +497,7 @@ void build_schedule(b2_solver* s) {
     };
     for (int ph = 0; ph < 2; ++ph) {
         Phase& P = s->phase[ph];
-        P.lev.clear(); P.fused = WarpLaunch(); P.n_fused_fronts = 0; P.dep_ngroup = 0; P.sol_grid = 0;
+        P.lev.clear(); P.fused = WarpLaunch(); P.n_fused_fronts = 0; P.dep_ngroup = 0; P.sol_grid[0] = 0;
         std::vector<char> mine(ns, 0);
         for (int sn = 0; sn < ns; ++sn) mine[sn] = (ph == 0) ? (S.owner[sn] == rank) : (S.owner[sn] == -1);
         // ---- dependency-driven single launch: every front of the phase is team-class and the tree is not sharded
@@ -875,22 +854,17 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
         build_schedule(s);
         if (set_smem_attrs() != B2_OK) throw std::runtime_error("attr");
         if (Phase& P = s->phase[0]; P.dep_ngroup) {
-            // persistent grid: as many CTAs as fit on the device at once (a size, not a correctness condition), at most one per task
-            int per_sm = 0;
-            B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pairs ? (const void*)k_solve_dep_pairs : (const void*)k_solve_dep,
-                                                                        128, solve_dep_smem<1>(P.dep_maxf4)));
+            // persistent grid of each width: as many CTAs as fit on the device at once (a size, not a correctness condition), at most
+            // one per task
             const int ntask = 2 * P.dep_ngroup;
-            P.sol_grid = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
+            for_each_width([&](auto w) {
+                int per_sm = 0;
+                B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_dep_kernel<w>(pairs), 128, solve_dep_smem<w>(P.dep_maxf4)));
+                P.sol_grid[width_index(w)] = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
+            });
             P.n_solve_launches = 1;
             B2_CUDA_THROW(s->d_slots.alloc((size_t)(2 * s->cbv_off[ns] + n)));
             B2_CUDA_THROW(cudaMemset(s->d_slots.p, SLOT_EMPTY_BYTE, s->d_slots.bytes()));     // every slot SLOT_EMPTY
-            // block solve: each width's grid from its own occupancy
-            const void* bk[3] = {solve_block_kernel<2>(pairs), solve_block_kernel<4>(pairs), solve_block_kernel<8>(pairs)};
-            const size_t bsm[3] = {solve_dep_smem<2>(P.dep_maxf4), solve_dep_smem<4>(P.dep_maxf4), solve_dep_smem<8>(P.dep_maxf4)};
-            for (int w = 0; w < 3; ++w) {
-                B2_CUDA_THROW(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bk[w], 128, bsm[w]));
-                P.sol_grid_blk[w] = std::max(1, std::min(ntask, std::max(1, per_sm) * sm_count()));
-            }
             B2_CUDA_THROW(s->d_bslots.alloc((size_t)8 * (2 * s->cbv_off[ns] + n)));
             B2_CUDA_THROW(cudaMemset(s->d_bslots.p, SLOT_EMPTY_BYTE, s->d_bslots.bytes()));
         } else if (s->opt.n_parts == 1) {
@@ -958,7 +932,7 @@ int solve_level_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
     int64_t nl = 0;
     auto sweeps = [&](cudaStream_t cs) { nl = enqueue_solve<NR>(s, 0, true, cs); enqueue_solve<NR>(s, 0, false, cs); };
     if (s->opt.use_cuda_graph && !stream_is_capturing(st)) {
-        cudaGraphExec_t* g = &P.g_blk[NR == 2 ? 0 : NR == 4 ? 1 : 2];
+        cudaGraphExec_t* g = &P.g_blk[width_index(NR) - 1];
         if (!*g) {
             int rc = capture(s, g, sweeps);
             if (rc != B2_OK) return rc;
@@ -971,6 +945,19 @@ int solve_level_block(b2_solver* s, double* x, int ncol, cudaStream_t st) {
         B2_CUDA(cudaGetLastError());
     }
     B2_CUDA(launch_pdl(k_perm_out_block<NR>, dim3(grid), dim3(256), 0, st, n, ncol, s->d_perm.p, s->d_xblk.p, x));
+    return B2_OK;
+}
+
+// columns [0, nrhs) of x (ld n) in chunks of 8, then the narrowest width that holds the rest (12 columns: 8 + 4, 9: 8 + 1 of 2);
+// walk(Width<NR>(), x, ncol) solves one chunk of ncol <= NR columns, on the single-launch or the level-launch schedule
+template <typename Walk>
+int solve_chunks(b2_solver* s, double* x_d, int nrhs, Walk&& walk) {
+    for (int c0 = 0; c0 < nrhs; c0 += 8) {
+        double* x = x_d + (size_t)c0 * s->S.n;
+        const int m = std::min(8, nrhs - c0);
+        const int rc = m <= 2 ? walk(Width<2>(), x, m) : m <= 4 ? walk(Width<4>(), x, m) : walk(Width<8>(), x, m);
+        if (rc != B2_OK) return rc;
+    }
     return B2_OK;
 }
 
@@ -1129,21 +1116,11 @@ int b2_solve_bwd_local(b2_solver* s, double* x_d, void* stream) {
 int b2_solve(b2_solver* s, double* x_d, int32_t nrhs, void* stream) {
     if (!s || s->symbolic_only || !x_d || nrhs < 1) { set_error("b2_solve: invalid argument"); return B2_ERR_INVALID; }
     if (s->opt.n_parts > 1) { set_error("b2_solve: multi-part solver needs the phased solve"); return B2_ERR_INVALID; }
-    if (s->phase[0].sol_grid) {          // every front team-class: one launch per walk of the tree, in place on x
+    if (s->phase[0].sol_grid[0]) {       // every front team-class: one launch per walk of the tree, in place on x
         if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
         cudaStream_t st = as_stream(stream);
-        if (nrhs == 1) {
-            enqueue_solve_dep(s, x_d, st);
-        } else {
-            // chunks of 8 columns, then the narrowest block width that holds the rest (12 columns: 8 + 4, 9: 8 + 1 of 2)
-            for (int c0 = 0; c0 < nrhs; c0 += 8) {
-                double* x = x_d + (size_t)c0 * s->S.n;
-                const int m = std::min(8, nrhs - c0);
-                if (m <= 2) enqueue_solve_block<2>(s, x, m, st);
-                else if (m <= 4) enqueue_solve_block<4>(s, x, m, st);
-                else enqueue_solve_block<8>(s, x, m, st);
-            }
-        }
+        if (nrhs == 1) enqueue_solve_dep<1>(s, x_d, 1, st);
+        else solve_chunks(s, x_d, nrhs, [&](auto w, double* x, int m) { enqueue_solve_dep<w>(s, x, m, st); return (int)B2_OK; });
         s->phase[0].n_solve_launches = 1;  // per right-hand side
         B2_CUDA(cudaGetLastError());
         return B2_OK;
@@ -1153,16 +1130,10 @@ int b2_solve(b2_solver* s, double* x_d, int32_t nrhs, void* stream) {
         if (rc != B2_OK) return rc;
         return b2_solve_bwd_local(s, x_d, stream);
     }
-    // level-launch tree: chunks of 8 columns as on the single-launch schedule, each one walk of the factor
+    // level-launch tree: chunks as on the single-launch schedule, each one walk of the factor
     if (!s->factorized) { set_error("b2_solve: not factorized"); return B2_ERR_SOLVE; }
     cudaStream_t st = as_stream(stream);
-    for (int c0 = 0; c0 < nrhs; c0 += 8) {
-        double* x = x_d + (size_t)c0 * s->S.n;
-        const int m = std::min(8, nrhs - c0);
-        int rc = m <= 2 ? solve_level_block<2>(s, x, m, st) : m <= 4 ? solve_level_block<4>(s, x, m, st) : solve_level_block<8>(s, x, m, st);
-        if (rc != B2_OK) return rc;
-    }
-    return B2_OK;
+    return solve_chunks(s, x_d, nrhs, [&](auto w, double* x, int m) { return solve_level_block<w>(s, x, m, st); });
 }
 
 int b2_improve(b2_solver* s, int32_t* changed) {

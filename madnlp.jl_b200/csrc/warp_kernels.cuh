@@ -554,6 +554,12 @@ __global__ void k_factor_team_profile(FactorArgs a, const ChildRec* childrec, in
     for (int r = 0; r < reps; ++r) front_factor_team<NW>(a, childrec, sn, sm, threadIdx.x, 0, maxf, nneg, npert, prof + 8 * r);
 }
 
+// a team's pivot counts into the factorisation's counters (negative pivots, perturbed pivots)
+__device__ __forceinline__ void flush_counters(int* counters, int nneg, int npert) {
+    if (nneg) atomicAdd(counters + 0, nneg);
+    if (npert) atomicAdd(counters + 1, npert);
+}
+
 // teams per CTA: FW_WARPS one-warp teams, or ONE two-warp team (its staging area is large)
 template <int NW> struct TeamsPerCta { static constexpr int value = (NW == 1) ? FW_WARPS : 1; };
 
@@ -570,10 +576,7 @@ __global__ void __launch_bounds__(TeamsPerCta<NW>::value * NW * 32) k_factor_war
         for (int q = team; q < cnt; q += NTEAM) front_factor_team<NW>(a, childrec, ws.list[off + q], smt, tid, team, maxf, nneg, npert);
         if (s1 - s0 > 1) __syncthreads();
     }
-    if (tid == 0) {
-        if (nneg) atomicAdd(a.counters + 0, nneg);
-        if (npert) atomicAdd(a.counters + 1, npert);
-    }
+    if (tid == 0) flush_counters(a.counters, nneg, npert);
 }
 
 // ------------------------------------------------------------------------------------------------ solves
@@ -1200,39 +1203,11 @@ __device__ __forceinline__ void front_bwd_block(const SolveArgs& a, int s, doubl
 // CTA instead of 4 is SLOWER (fewer resident CTAs, wider barriers), while smaller subtrees (fuse_max_fronts 16 -> 8) are
 // faster -- so the fused launches keep TeamsPerCta teams.
 constexpr int SOLVE_FUSED_TEAMS = 4;
-template <int NW, int NTEAM = TeamsPerCta<NW>::value>
-__global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2(SolveArgs a, const ChildRec* childrec, WarpSched ws) {
-    extern __shared__ __align__(16) double smd[];
-    double (*sm)[SolveSmem<NW>::doubles] = (double (*)[SolveSmem<NW>::doubles])smd;
-    const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
-    pdl_trigger();
-    const int s0 = ws.cta_ptr[blockIdx.x], s1 = ws.cta_ptr[blockIdx.x + 1];
-    for (int st = s0; st < s1; ++st) {
-        const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
-        for (int q = team; q < cnt; q += NTEAM) front_fwd_team<NW>(a, childrec, ws.list[off + q], sm[team], tid, team);
-        if (s1 - s0 > 1) __syncthreads();
-    }
-    pdl_wait();                                         // (idle teams too: this grid's completion must imply its predecessor's)
-}
-
-template <int NW, int NTEAM = TeamsPerCta<NW>::value>
-__global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2(SolveArgs a, WarpSched ws) {
-    extern __shared__ __align__(16) double smd[];
-    double (*sm)[SolveSmem<NW>::doubles] = (double (*)[SolveSmem<NW>::doubles])smd;
-    const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
-    pdl_trigger();
-    const int s0 = ws.cta_ptr[blockIdx.x], s1 = ws.cta_ptr[blockIdx.x + 1];
-    for (int st = s1 - 1; st >= s0; --st) {
-        const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
-        for (int q = team; q < cnt; q += NTEAM) front_bwd_team<NW>(a, ws.list[off + q], sm[team], tid, team);
-        if (s1 - s0 > 1) __syncthreads();
-    }
-    pdl_wait();
-}
-
-// k_fwd_warp2 / k_bwd_warp2 for NR right-hand sides (b2_solve's level-launch block solve): xp and cbv hold NR interleaved columns
+// One sweep of a level-launch solve: a CTA walks its stages (forward: ascending, backward: descending), its NTEAM teams sharing each
+// stage's fronts.  NR = 1 is the one-column solve on xp / cbv; NR > 1 (b2_solve's level-launch block solve) holds NR interleaved columns
+// of xp and cbv, with front_bwd_block as the backward front.  The kernels below keep their names as thin wrappers.
 template <int NW, int NTEAM, int NR>
-__global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2_block(SolveArgs a, const ChildRec* childrec, WarpSched ws) {
+__device__ __forceinline__ void fwd_warp_sweep(const SolveArgs& a, const ChildRec* childrec, const WarpSched& ws) {
     extern __shared__ __align__(16) double smd[];
     double (*sm)[SolveSmem<NW, NR>::doubles] = (double (*)[SolveSmem<NW, NR>::doubles])smd;
     const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
@@ -1243,11 +1218,11 @@ __global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2_block(SolveArgs a
         for (int q = team; q < cnt; q += NTEAM) front_fwd_team<NW, false, NR>(a, childrec, ws.list[off + q], sm[team], tid, team);
         if (s1 - s0 > 1) __syncthreads();
     }
-    pdl_wait();
+    pdl_wait();                                         // (idle teams too: this grid's completion must imply its predecessor's)
 }
 
 template <int NW, int NTEAM, int NR>
-__global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a, WarpSched ws) {
+__device__ __forceinline__ void bwd_warp_sweep(const SolveArgs& a, const WarpSched& ws) {
     extern __shared__ __align__(16) double smd[];
     double (*sm)[SolveSmem<NW, NR>::doubles] = (double (*)[SolveSmem<NW, NR>::doubles])smd;
     const int team = threadIdx.x / (32 * NW), tid = threadIdx.x % (32 * NW);
@@ -1255,11 +1230,30 @@ __global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a
     const int s0 = ws.cta_ptr[blockIdx.x], s1 = ws.cta_ptr[blockIdx.x + 1];
     for (int st = s1 - 1; st >= s0; --st) {
         const int off = ws.stage_off[st], cnt = ws.stage_cnt[st];
-        for (int q = team; q < cnt; q += NTEAM)
-            front_bwd_block<NW, false, NR, false>(a, ws.list[off + q], sm[team], tid, team, nullptr, nullptr, nullptr, 0, 0);
+        for (int q = team; q < cnt; q += NTEAM) {
+            if constexpr (NR == 1) front_bwd_team<NW>(a, ws.list[off + q], sm[team], tid, team);
+            else front_bwd_block<NW, false, NR, false>(a, ws.list[off + q], sm[team], tid, team, nullptr, nullptr, nullptr, 0, 0);
+        }
         if (s1 - s0 > 1) __syncthreads();
     }
     pdl_wait();
+}
+
+template <int NW, int NTEAM = TeamsPerCta<NW>::value>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2(SolveArgs a, const ChildRec* childrec, WarpSched ws) {
+    fwd_warp_sweep<NW, NTEAM, 1>(a, childrec, ws);
+}
+template <int NW, int NTEAM = TeamsPerCta<NW>::value>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2(SolveArgs a, WarpSched ws) {
+    bwd_warp_sweep<NW, NTEAM, 1>(a, ws);
+}
+template <int NW, int NTEAM, int NR>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_fwd_warp2_block(SolveArgs a, const ChildRec* childrec, WarpSched ws) {
+    fwd_warp_sweep<NW, NTEAM, NR>(a, childrec, ws);
+}
+template <int NW, int NTEAM, int NR>
+__global__ void __launch_bounds__(NTEAM * NW * 32) k_bwd_warp2_block(SolveArgs a, WarpSched ws) {
+    bwd_warp_sweep<NW, NTEAM, NR>(a, ws);
 }
 
 
@@ -1290,47 +1284,48 @@ __device__ __forceinline__ int claim_group(int* ticket, int ngroup) {
     return g_sh;
 }
 
-__global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec* childrec, DepSched ds, int maxf1, int maxf2,
-                                                    int* done, int* err, int* ticket) {
+// A group's team and the thread's index in it: type 1 is four one-warp teams, type 2 one two-warp team, type 4 (PAIRS only) one
+// four-warp team.
+template <bool PAIRS>
+__device__ __forceinline__ void group_team(int type, int& team, int& tid) {
+    team = (type == 1) ? (threadIdx.x >> 5) : (!PAIRS || type == 2) ? (threadIdx.x >> 6) : 0;
+    tid = (type == 1) ? (threadIdx.x & 31) : (!PAIRS || type == 2) ? (threadIdx.x & 63) : threadIdx.x;
+}
+
+// PAIRS (b2_options.sparse_pivoting = B2_SPARSE_PIVOT_PAIRS): front_factor_team's pivot loop with candidate 2 x 2 pivots, and type-4
+// groups, one front of order 65..96 as a four-warp team (the pair ordering makes fronts larger: DESIGN.md section 3).  maxf4 and pa
+// are unused without PAIRS.  The static instance folds every PAIRS test away and compiles to the same machine code as a body written
+// for it alone (tools/sass_diff.py compares the builds).
+template <bool PAIRS>
+__device__ __forceinline__ void factor_dep_body(const FactorArgs& a, const ChildRec* childrec, const DepSched& ds, int maxf1, int maxf2,
+                                                int maxf4, int* done, int* err, int* ticket, const PairArgs& pa) {
     extern __shared__ __align__(16) double sm[];
     const int g = claim_group(ticket, ds.ngroup);
     const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
-    int nneg = 0, npert = 0;
+    int npert = 0, nneg = 0;                            // (declared in this order, the static kernel's code is unchanged)
     if (type == 1) {
         const int team = threadIdx.x >> 5, tid = threadIdx.x & 31;
-        if (team < n) front_factor_team<1, true>(a, childrec, ds.tasks[t0 + team], sm + (size_t)team * TeamSmem<1>::doubles(maxf1),
-                                                 tid, team, maxf1, nneg, npert, nullptr, done, err);
-        if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
-    } else {
+        if (team < n) front_factor_team<1, true, PAIRS>(a, childrec, ds.tasks[t0 + team], sm + (size_t)team * TeamSmem<1>::doubles(maxf1),
+                                                        tid, team, maxf1, nneg, npert, nullptr, done, err, pa);
+        if (tid == 0) flush_counters(a.counters, nneg, npert);
+    } else if (!PAIRS || type == 2) {
         const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
-        if (team < n) front_factor_team<2, true>(a, childrec, ds.tasks[t0 + team], sm, tid, team, maxf2, nneg, npert, nullptr, done, err);
-        if (tid == 0 && team < n) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
+        if (team < n) front_factor_team<2, true, PAIRS>(a, childrec, ds.tasks[t0 + team], sm, tid, team, maxf2, nneg, npert, nullptr, done, err, pa);
+        if (tid == 0 && team < n) flush_counters(a.counters, nneg, npert);
+    } else if constexpr (PAIRS) {
+        front_factor_team<4, true, true>(a, childrec, ds.tasks[t0], sm, threadIdx.x, 0, maxf4, nneg, npert, nullptr, done, err, pa);
+        if (threadIdx.x == 0) flush_counters(a.counters, nneg, npert);
     }
 }
 
-// k_factor_dep with candidate 2 x 2 pivots (b2_options.sparse_pivoting = B2_SPARSE_PIVOT_PAIRS): the same schedule and hand-offs,
-// front_factor_team's PAIRS pivot loop.  A separate kernel, so that the static one is compiled exactly as before.  Its groups also
-// come as type 4: one front of order 65..96 as a four-warp team (the pair ordering makes fronts larger: DESIGN.md section 3).
+__global__ void __launch_bounds__(128) k_factor_dep(FactorArgs a, const ChildRec* childrec, DepSched ds, int maxf1, int maxf2,
+                                                    int* done, int* err, int* ticket) {
+    factor_dep_body<false>(a, childrec, ds, maxf1, maxf2, 0, done, err, ticket, PairArgs());
+}
+
 __global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const ChildRec* childrec, DepSched ds, int maxf1, int maxf2,
                                                           int maxf4, int* done, int* err, int* ticket, PairArgs pa) {
-    extern __shared__ __align__(16) double sm[];
-    const int g = claim_group(ticket, ds.ngroup);
-    const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], n = ds.grp_ptr[g + 1] - t0;
-    int nneg = 0, npert = 0;
-    if (type == 1) {
-        const int team = threadIdx.x >> 5, tid = threadIdx.x & 31;
-        if (team < n) front_factor_team<1, true, true>(a, childrec, ds.tasks[t0 + team], sm + (size_t)team * TeamSmem<1>::doubles(maxf1),
-                                                       tid, team, maxf1, nneg, npert, nullptr, done, err, pa);
-        if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
-    } else if (type == 2) {
-        const int team = threadIdx.x >> 6, tid = threadIdx.x & 63;
-        if (team < n) front_factor_team<2, true, true>(a, childrec, ds.tasks[t0 + team], sm, tid, team, maxf2, nneg, npert, nullptr, done, err, pa);
-        if (tid == 0 && team < n) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
-    } else {
-        const int tid = threadIdx.x;
-        front_factor_team<4, true, true>(a, childrec, ds.tasks[t0], sm, tid, 0, maxf4, nneg, npert, nullptr, done, err, pa);
-        if (tid == 0) { if (nneg) atomicAdd(a.counters + 0, nneg); if (npert) atomicAdd(a.counters + 1, npert); }
-    }
+    factor_dep_body<true>(a, childrec, ds, maxf1, maxf2, maxf4, done, err, ticket, pa);
 }
 
 // ------------------------------------------------------------------------------------------------ single-launch solve
@@ -1363,34 +1358,20 @@ __global__ void __launch_bounds__(128) k_factor_dep_pairs(FactorArgs a, const Ch
 // that Richardson refinement rejects the step, and fills every slot with SLOT_EMPTY again: a slot whose consumer gave up may
 // hold a value the next launch must not see.
 // (six CTAs per SM: what the 35 KB of shared memory allows; the bound also keeps ptxas from spilling)
-__global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
-                                                   double* slots, int64_t nslot) {
-    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
-    double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
-    __shared__ int tk_sh, bad_sh;
-    const int ntask = 2 * ds.ngroup;
-    for (;;) {
-        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
-        __syncthreads();
-        const int t = tk_sh;
-        if (t >= ntask) break;
-        const bool fwd = t < ds.ngroup;
-        const int g = fwd ? t : ntask - 1 - t;
-        const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
-        const int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
-        const int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
-        if (team < cnt) {
-            const int s = ds.tasks[t0 + team];
-            if (fwd) {
-                if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, err);
-                else front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
-            } else {
-                if (type == 1) front_bwd_team<1, true>(a, s, sm1[team], tid, team, childrec, err);
-                else front_bwd_team<2, true>(a, s, smd, tid, team, childrec, err);
-            }
-        }
-        __syncthreads();                                // (tk_sh is rewritten by the next claim)
-    }
+//
+// The ticket claim and the count-out / time-out path are shared with k_solve_dep_block; each kernel writes its own claim loop around
+// them, because one loop body inlined into all of them compiles the block kernels to different machine code (tools/sass_diff.py).
+__device__ __forceinline__ int claim_task(int* ctl) {
+    __shared__ int tk_sh;
+    if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
+    __syncthreads();
+    return tk_sh;
+}
+
+// after the last claim: count the CTA out, re-arm the counters once every CTA is out, and on a time-out anywhere write NaN into the
+// ncol columns of x (ld n) and SLOT_EMPTY into every slot
+__device__ __forceinline__ void solve_dep_finish(double* x, int n, int ncol, int* err, int* ctl, double* slots, int64_t nslot) {
+    __shared__ int bad_sh;
     if (threadIdx.x == 0) {
         bad_sh = 0;
         __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
@@ -1403,58 +1384,53 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRe
     }
     __syncthreads();
     if (bad_sh) {
-        for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
+        for (int q = 0; q < ncol; ++q)
+            for (int i = threadIdx.x; i < n; i += blockDim.x) x[(int64_t)q * n + i] = __longlong_as_double((long long)CANON_NAN);
         for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
     }
 }
 
-// k_solve_dep for a PAIRS factor (D with 2 x 2 blocks, front_bwd_team<.., PAIRS>); a separate kernel, so that the static one is
-// compiled exactly as before.  A type-4 group is one front of order 65..96 on a four-warp slice (SolveSmem<4>::doubles_panel).
-__global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl,
-                                                         int n, double* slots, int64_t nslot, const double* dsub) {
-    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice, 1 four-warp slice)
+// PAIRS: D has 2 x 2 blocks (dsub, front_bwd_team<.., PAIRS>), and a type-4 group is one front of order 65..96 on a four-warp slice
+// (SolveSmem<4>::doubles_panel).  The static kernel compiles to the same machine code as a body written for it alone.
+template <bool PAIRS>
+__device__ __forceinline__ void solve_dep_body(const SolveArgs& a, const ChildRec* childrec, const DepSched& ds, int* err, int* ctl, int n,
+                                               double* slots, int64_t nslot, const double* dsub) {
+    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice, PAIRS: 1 four-warp slice)
     double (*sm1)[SolveSmem<1>::doubles] = (double (*)[SolveSmem<1>::doubles])smd;
-    __shared__ int tk_sh, bad_sh;
     const int ntask = 2 * ds.ngroup;
     for (;;) {
-        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
-        __syncthreads();
-        const int t = tk_sh;
+        const int t = claim_task(ctl);
         if (t >= ntask) break;
         const bool fwd = t < ds.ngroup;
         const int g = fwd ? t : ntask - 1 - t;
         const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
-        const int team = (type == 1) ? (threadIdx.x >> 5) : (type == 2) ? (threadIdx.x >> 6) : 0;
-        const int tid = (type == 1) ? (threadIdx.x & 31) : (type == 2) ? (threadIdx.x & 63) : threadIdx.x;
+        int team, tid;
+        group_team<PAIRS>(type, team, tid);
         if (team < cnt) {
             const int s = ds.tasks[t0 + team];
             if (fwd) {
                 if (type == 1) front_fwd_team<1, true>(a, childrec, s, sm1[team], tid, team, err);
-                else if (type == 2) front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
+                else if (!PAIRS || type == 2) front_fwd_team<2, true>(a, childrec, s, smd, tid, team, err);
                 else front_fwd_team<4, true>(a, childrec, s, smd, tid, 0, err);
             } else {
-                if (type == 1) front_bwd_team<1, true, true>(a, s, sm1[team], tid, team, childrec, err, dsub);
-                else if (type == 2) front_bwd_team<2, true, true>(a, s, smd, tid, team, childrec, err, dsub);
-                else front_bwd_team<4, true, true>(a, s, smd, tid, 0, childrec, err, dsub);
+                if (type == 1) front_bwd_team<1, true, PAIRS>(a, s, sm1[team], tid, team, childrec, err, dsub);
+                else if (!PAIRS || type == 2) front_bwd_team<2, true, PAIRS>(a, s, smd, tid, team, childrec, err, dsub);
+                else front_bwd_team<4, true, PAIRS>(a, s, smd, tid, 0, childrec, err, dsub);
             }
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)
     }
-    if (threadIdx.x == 0) {
-        bad_sh = 0;
-        __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
-        if (atomicAdd(ctl + 1, 1) == (int)gridDim.x - 1) {
-            atomicExch(ctl, 0);
-            atomicExch(ctl + 1, 0);
-            __threadfence();
-            bad_sh = *(volatile int*)err;
-        }
-    }
-    __syncthreads();
-    if (bad_sh) {
-        for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[i] = __longlong_as_double((long long)CANON_NAN);
-        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
-    }
+    solve_dep_finish(a.x, n, 1, err, ctl, slots, nslot);
+}
+
+__global__ void __launch_bounds__(128, 6) k_solve_dep(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
+                                                   double* slots, int64_t nslot) {
+    solve_dep_body<false>(a, childrec, ds, err, ctl, n, slots, nslot, nullptr);
+}
+
+__global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl,
+                                                         int n, double* slots, int64_t nslot, const double* dsub) {
+    solve_dep_body<true>(a, childrec, ds, err, ctl, n, slots, nslot, dsub);
 }
 
 // k_solve_dep (PAIRS: k_solve_dep_pairs) for NR right-hand sides in one walk of the tree: the same tasks, tickets, count-out and
@@ -1468,21 +1444,18 @@ __global__ void __launch_bounds__(128, 6) k_solve_dep_pairs(SolveArgs a, const C
 template <int NR, bool PAIRS>
 __global__ void __launch_bounds__(128, PAIRS ? 1 : 0) k_solve_dep_block(SolveArgs a, const ChildRec* childrec, DepSched ds, int* err, int* ctl, int n,
                                                          int ncol, double* slots, int64_t nslot, const double* dsub) {
-    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice)
+    extern __shared__ __align__(16) double smd[];       // max(4 one-warp slices, 1 two-warp slice, PAIRS: 1 four-warp slice)
     double (*sm1)[SolveSmem<1, NR>::doubles] = (double (*)[SolveSmem<1, NR>::doubles])smd;
-    __shared__ int tk_sh, bad_sh;
     const int ntask = 2 * ds.ngroup;
     for (;;) {
-        if (threadIdx.x == 0) tk_sh = atomicAdd(ctl, 1);
-        __syncthreads();
-        const int t = tk_sh;
+        const int t = claim_task(ctl);
         if (t >= ntask) break;
         const bool fwd = t < ds.ngroup;
         const int g = fwd ? t : ntask - 1 - t;
         const int type = ds.grp_type[g], t0 = ds.grp_ptr[g], cnt = ds.grp_ptr[g + 1] - t0;
-        int team = (type == 1) ? (threadIdx.x >> 5) : (threadIdx.x >> 6);
-        int tid = (type == 1) ? (threadIdx.x & 31) : (threadIdx.x & 63);
-        if constexpr (PAIRS) {                          // (type 4: one front of order 65..96 as a four-warp team)
+        int team, tid;
+        group_team<false>(type, team, tid);
+        if constexpr (PAIRS) {                          // (type 4 after the others: group_team<true> compiles this kernel differently)
             if (type == 4) { team = 0; tid = threadIdx.x; }
         }
         if (team < cnt) {
@@ -1503,22 +1476,7 @@ __global__ void __launch_bounds__(128, PAIRS ? 1 : 0) k_solve_dep_block(SolveArg
         }
         __syncthreads();                                // (tk_sh is rewritten by the next claim)
     }
-    if (threadIdx.x == 0) {
-        bad_sh = 0;
-        __threadfence();                                // this CTA's stores (the barrier above orders the whole CTA's) before it counts out
-        if (atomicAdd(ctl + 1, 1) == (int)gridDim.x - 1) {
-            atomicExch(ctl, 0);
-            atomicExch(ctl + 1, 0);
-            __threadfence();
-            bad_sh = *(volatile int*)err;
-        }
-    }
-    __syncthreads();
-    if (bad_sh) {
-        for (int q = 0; q < ncol; ++q)
-            for (int i = threadIdx.x; i < n; i += blockDim.x) a.x[(int64_t)q * n + i] = __longlong_as_double((long long)CANON_NAN);
-        for (int64_t i = threadIdx.x; i < nslot; i += blockDim.x) st_relaxed_b64(slots + i, SLOT_EMPTY);
-    }
+    solve_dep_finish(a.x, n, ncol, err, ctl, slots, nslot);
 }
 
 }  // namespace b2
