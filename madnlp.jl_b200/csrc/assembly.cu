@@ -98,7 +98,7 @@ extern "C" int b2_transfer_plan_create(int64_t nnz_coo, int64_t nnz_csc, const i
 extern "C" int b2_transfer_plan_destroy(b2_transfer_plan* p) { delete p; return B2_OK; }
 
 extern "C" int b2_transfer(b2_transfer_plan* p, double* dst_nz_d, const double* V_d, void* stream) {
-    if (!p || !dst_nz_d || !V_d) { set_error("b2_transfer: invalid argument"); return B2_ERR_INVALID; }
+    if (!p || (p->nnz_csc && (!dst_nz_d || !V_d))) { set_error("b2_transfer: invalid argument"); return B2_ERR_INVALID; }   // empty: may be null
     if (p->nnz_csc == 0) return B2_OK;
     const int grid = (int)std::min<int64_t>((p->nnz_csc + 255) / 256, 8 * sm_count());
     launch_pdl(k_transfer, dim3(grid), dim3(256), 0, as_stream(stream), p->nnz_csc, p->ptr.p, p->src.p, V_d, dst_nz_d);
@@ -278,7 +278,10 @@ extern "C" int b2_condensed_plan_destroy(b2_condensed_plan* p) { delete p; retur
 
 extern "C" int b2_condensed_assemble(b2_condensed_plan* p, double* aug_nz_d, const double* pr_diag_d, const double* du_diag_d,
                                      const double* H_nz_d, const double* Jt_nz_d, double* diag_buffer_d, void* stream) {
-    if (!p || !aug_nz_d || !pr_diag_d || !du_diag_d || !diag_buffer_d) { set_error("b2_condensed_assemble: invalid argument"); return B2_ERR_INVALID; }
+    if (!p || !aug_nz_d || !pr_diag_d || (p->m && (!du_diag_d || !diag_buffer_d))) {   // m = 0: empty du_diag and diag_buffer may be null
+        set_error("b2_condensed_assemble: invalid argument");
+        return B2_ERR_INVALID;
+    }
     if (!p->hsrc.p) { set_error("b2_condensed_assemble: plan has no device state (no CUDA device at creation)"); return B2_ERR_NO_DEVICE; }
     cudaStream_t st = as_stream(stream);
     if (p->m > 0) {

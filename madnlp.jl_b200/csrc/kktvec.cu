@@ -630,7 +630,7 @@ static CondArgs make_cond(b2_bounds* b, int64_t n, int64_t m, const double* l_di
 static int cond_pre(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d, const double* pr_diag_d,
                     const double* diag_buffer_d, const double* l_diag_d, const double* u_diag_d, double* buffer_d, double* w_d,
                     double* norms_d, void* stream) {
-    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m || jt->nrow != n || jt->ncol != m) {
+    if (!b || !jt || !w_d || (m && !buffer_d) || b->n_tot != n + m || jt->nrow != n || jt->ncol != m) {
         set_error(std::string(name) + ": invalid argument");
         return B2_ERR_INVALID;
     }
@@ -645,7 +645,7 @@ template <bool UPDATE>
 static int cond_post(const char* name, b2_bounds* b, b2_spmv_plan* jt, int64_t n, int64_t m, const double* jt_nz_d, const double* pr_diag_d,
                      const double* diag_buffer_d, const double* l_lower_d, const double* u_lower_d, const double* l_diag_d,
                      const double* u_diag_d, const double* buffer_d, double* w_d, double* x_d, double* norms_d, void* stream) {
-    if (!b || !jt || !w_d || !buffer_d || b->n_tot != n + m || jt->nrow != n || jt->ncol != m || (UPDATE && (!x_d || !norms_d))) {
+    if (!b || !jt || !w_d || (m && !buffer_d) || b->n_tot != n + m || jt->nrow != n || jt->ncol != m || (UPDATE && (!x_d || !norms_d))) {
         set_error(std::string(name) + ": invalid argument");
         return B2_ERR_INVALID;
     }
