@@ -100,11 +100,18 @@ typedef struct b2_options {
                                 analysis (fronts of order 65..96 run as four-warp teams) (B2_ERR_INVALID otherwise, before any device work; b2_create_symbolic_only skips the front-order
                                 condition so that tooling can inspect the tree).  The dense solver (b2d_create) rejects any value but
                                 STATIC.                                                                                    */
-    int32_t reserved[1];
+    int32_t dense_algorithm; /* dense solver (b2d_*) only, B2_DENSE_ALG_*: LDLT (default) factors A = L D L' with the pivoting chosen
+                                by dense_pivoting; LU mirrors the lower triangle into the full matrix and factors it with partial
+                                pivoting, LAPACK dgetrf's pivot sequence (MadNLP's lapack_algorithm = LU).  LU reports no inertia
+                                (b2d_inertia* return B2_ERR_INVALID), needs dense_pivoting = STATIC and, like BUNCH_KAUFMAN,
+                                N <= 128 * (number of SMs of the device); b2d_create rejects anything else (B2_ERR_INVALID).
+                                The sparse solver (b2_create*) rejects any value but LDLT.                                  */
 } b2_options;
 
 #define B2_DENSE_PIVOT_STATIC        0
 #define B2_DENSE_PIVOT_BUNCH_KAUFMAN 1
+#define B2_DENSE_ALG_LDLT            0
+#define B2_DENSE_ALG_LU              1
 #define B2_SPARSE_PIVOT_STATIC       0
 #define B2_SPARSE_PIVOT_PAIRS        1
 
@@ -231,6 +238,7 @@ int b2d_destroy(b2d_solver* s);
  * uint64 values (0 when tracing is off); stamps are copied when capacity >= *count. */
 int b2d_debug_trace(b2d_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t* count);
 int b2d_factorize(b2d_solver* s, void* stream);
+/* the three inertia entries return B2_ERR_INVALID on an LU handle (opt.dense_algorithm = B2_DENSE_ALG_LU): LU reports no inertia */
 int b2d_inertia(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg, void* stream);
 int b2d_inertia_enqueue(b2d_solver* s, void* stream);
 int b2d_inertia_fetch(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg);
@@ -240,6 +248,11 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream);
  * e_h D's subdiagonal (0 for a 1x1 pivot, d21 at the first index of a 2x2 block).  A zero column is reported with its perturbed
  * pivot +-pivot_eps.  Synchronises the device; B2_ERR_INVALID on a static-pivoting handle. */
 int b2d_get_pivots(b2d_solver* s, int32_t* ipiv_h, double* d_h, double* e_h);
+/* Export of an LU factor (opt.dense_algorithm = B2_DENSE_ALG_LU) as LAPACK dgetrf leaves it, on the host: ipiv_h (N entries,
+ * 1-based: row k was interchanged with row ipiv[k]), *info_h (the first exactly-zero pivot of U, 1-based, else 0) and lu_h (N x N
+ * column-major, unit-lower L below the diagonal, U on and above it).  Any pointer may be NULL.  Synchronises the device;
+ * B2_ERR_SOLVE if a device-wide wait of the factorisation or of a solve timed out, B2_ERR_INVALID on an LDLT handle. */
+int b2d_get_lu(b2d_solver* s, int32_t* ipiv_h, int32_t* info_h, double* lu_h);
 
 /* ------------------------------------------------------------------ assembly: COO -> CSC */
 /* Host, one-time: CSC pattern of a COO matrix with duplicate merging and the COO->CSC map

@@ -17,6 +17,7 @@ B2_ERR_INVALID, B2_ERR_CUDA, B2_ERR_SYMBOLIC, B2_ERR_FACTORIZATION, B2_ERR_SOLVE
 ORDER_METIS_ND, ORDER_MINDEG, ORDER_NATURAL, ORDER_USER = 0, 1, 2, 3
 QN_BFGS, QN_DAMPED_BFGS = 1, 2
 B2_DENSE_PIVOT_STATIC, B2_DENSE_PIVOT_BUNCH_KAUFMAN = 0, 1
+B2_DENSE_ALG_LDLT, B2_DENSE_ALG_LU = 0, 1
 B2_SPARSE_PIVOT_STATIC, B2_SPARSE_PIVOT_PAIRS = 0, 1
 B2_PIVOT_1X1, B2_PIVOT_1X1_PERTURBED, B2_PIVOT_2X2_FIRST, B2_PIVOT_2X2_SECOND = 0, 1, 2, 3
 # layout of b2_mul_hess_blk_tail's curvature-test result (B2_CURV_* in include/b200kkt.h)
@@ -59,13 +60,13 @@ class InertiaException(RuntimeError):
 
 
 class _Pivoting(C.Structure):
-    _fields_ = [("dense_pivoting", C.c_int32), ("sparse_pivoting", C.c_int32)]
+    _fields_ = [("dense_pivoting", C.c_int32), ("sparse_pivoting", C.c_int32), ("dense_algorithm", C.c_int32)]
 
 
 class _OptionsTail(C.Union):
-    """the three int32 after kkt_n_dual: `dense_pivoting` and `sparse_pivoting` took the first two (include/b200kkt.h).
+    """the three int32 after kkt_n_dual: `dense_pivoting`, `sparse_pivoting` and `dense_algorithm` (include/b200kkt.h).
     `reserved` keeps the view of all three at the offset it always had, so that code which reads `Options.reserved` still finds
-    it there; the header's `reserved[1]` (and the Julia shim's) is `reserved[2:]` here."""
+    it there."""
     _anonymous_ = ("_pivoting",)
     _fields_ = [("_pivoting", _Pivoting), ("reserved", C.c_int32 * 3)]
 
@@ -184,6 +185,7 @@ PROTOTYPES = {
     "b2d_inertia_fetch": (C.c_int, [_p, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "b2d_solve": (C.c_int, [_p, _p, _i32, _p]),
     "b2d_get_pivots": (C.c_int, [_p, _p, _p, _p]),
+    "b2d_get_lu": (C.c_int, [_p, _p, _p, _p]),
     "b2_condensed_symbolic_device": (C.c_int, [_i32, _i32, _p, _p, _p, _p, _PP, C.POINTER(_i64), _p]),
     "b2_coo_to_csc_device": (C.c_int, [_i32, _i32, _i64, _p, _p, _p, _p, _p, C.POINTER(_i64), _p]),
     "b2d_ozaki_plan_create": (C.c_int, [_i32, _i32, _PP]),

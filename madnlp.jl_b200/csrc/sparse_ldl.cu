@@ -17,6 +17,7 @@
 #include "bigsolve_kernels.cuh"
 #include "densesolve_kernels.cuh"
 #include "dense_bk.cuh"
+#include "dense_lu.cuh"
 
 using namespace b2;
 
@@ -674,6 +675,10 @@ int create_common(int32_t n, int64_t nnz, const int32_t* colptr_h, const int32_t
     if (colptr_h[n] != nnz) { set_error("b2_create: colptr[n] != nnz"); return B2_ERR_INVALID; }
     if (opt && opt->dense_pivoting != B2_DENSE_PIVOT_STATIC) {
         set_error("b2_create: dense_pivoting applies to the dense solver (b2d_create) only; the sparse solver pivots statically");
+        return B2_ERR_INVALID;
+    }
+    if (opt && opt->dense_algorithm != B2_DENSE_ALG_LDLT) {
+        set_error("b2_create: dense_algorithm applies to the dense solver (b2d_create) only; the sparse solver factors L D L'");
         return B2_ERR_INVALID;
     }
     if (opt && opt->kkt_n_dual != 0) {
@@ -1347,6 +1352,8 @@ struct b2d_solver {
     bool factorized = false;
     bool bunch_kaufman = false;                      // opt.dense_pivoting == B2_DENSE_PIVOT_BUNCH_KAUFMAN (dense_bk.cu)
     DenseBK bk;
+    bool lu = false;                                 // opt.dense_algorithm == B2_DENSE_ALG_LU (dense_lu.cu)
+    DenseLU lum;
     ~b2d_solver() {
         if (g_factor) cudaGraphExecDestroy(g_factor);
         for (auto e : ev_pool) cudaEventDestroy(e);
@@ -1465,6 +1472,10 @@ void enqueue_dense_factor_lookahead(b2d_solver* s, cudaStream_t S1) {
 }
 
 void enqueue_dense_factor(b2d_solver* s, cudaStream_t st) {
+    if (s->lu) {
+        lu_enqueue_factor(s->lum, s->lda, s->A_d, s->fact.p, s->linv.p, s->counters.p, st);
+        return;
+    }
     if (s->bunch_kaufman) {
         bk_enqueue_factor(s->bk, s->lda, s->A_d, s->fact.p, s->linv.p, s->dvec.p, s->counters.p, s->opt.pivot_eps, st);
         return;
@@ -1488,6 +1499,14 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
         set_error("b2d_create: dense_pivoting must be B2_DENSE_PIVOT_STATIC (0) or B2_DENSE_PIVOT_BUNCH_KAUFMAN (1)");
         return B2_ERR_INVALID;
     }
+    if (opt && opt->dense_algorithm != B2_DENSE_ALG_LDLT && opt->dense_algorithm != B2_DENSE_ALG_LU) {
+        set_error("b2d_create: dense_algorithm must be B2_DENSE_ALG_LDLT (0) or B2_DENSE_ALG_LU (1)");
+        return B2_ERR_INVALID;
+    }
+    if (opt && opt->dense_algorithm == B2_DENSE_ALG_LU && opt->dense_pivoting != B2_DENSE_PIVOT_STATIC) {
+        set_error("b2d_create: dense_algorithm = B2_DENSE_ALG_LU pivots by rows and needs dense_pivoting = B2_DENSE_PIVOT_STATIC (0)");
+        return B2_ERR_INVALID;
+    }
     if (opt && opt->sparse_pivoting != B2_SPARSE_PIVOT_STATIC) {
         set_error("b2d_create: sparse_pivoting applies to the sparse solver (b2_create) only");
         return B2_ERR_INVALID;
@@ -1502,10 +1521,15 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
         set_error("b2d_create: the Bunch-Kaufman solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
         return B2_ERR_INVALID;
     }
+    if (opt && opt->dense_algorithm == B2_DENSE_ALG_LU && (N + BS - 1) / BS > sm_count()) {
+        set_error("b2d_create: the LU solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
+        return B2_ERR_INVALID;
+    }
     auto* s = new b2d_solver();
     s->N = N; s->lda = lda; s->A_d = A_d;
     if (opt) s->opt = *opt; else b2_options_default(&s->opt);
     s->bunch_kaufman = s->opt.dense_pivoting == B2_DENSE_PIVOT_BUNCH_KAUFMAN;
+    s->lu = s->opt.dense_algorithm == B2_DENSE_ALG_LU;
     FrontDesc d;
     std::memset(&d, 0, sizeof(d));
     d.col0 = 0; d.w = N; d.f = N;
@@ -1522,7 +1546,7 @@ int b2d_create(int32_t N, int32_t lda, const double* A_d, const b2_options* opt,
         s->tilecnt.alloc((size_t)((N + DB - 1) / DB)) != cudaSuccess ||
         (getenv("B2_DENSE_TRACE") && atoi(getenv("B2_DENSE_TRACE")) && s->trace.alloc((size_t)16 * ((N + DB - 1) / DB)) != cudaSuccess) ||
         cudaMemset(s->fact.p, 0, s->fact.bytes()) != cudaSuccess || cudaMemset(s->counters.p, 0, 4 * sizeof(int32_t)) != cudaSuccess ||
-        (s->bunch_kaufman && bk_alloc(s->bk, N) != cudaSuccess)) {
+        (s->bunch_kaufman && bk_alloc(s->bk, N) != cudaSuccess) || (s->lu && lu_alloc(s->lum, N) != cudaSuccess)) {
         delete s;
         return cuda_fail(cudaGetLastError(), "b2d_create allocation", __FILE__, __LINE__);
     }
@@ -1566,12 +1590,14 @@ int b2d_debug_trace(b2d_solver* s, uint64_t* stamps_h, int64_t capacity, int64_t
 }
 
 int b2d_inertia_enqueue(b2d_solver* s, void* stream) {
+    if (s && s->lu) { set_error("b2d_inertia: an LU factorisation reports no inertia (opt.dense_algorithm = B2_DENSE_ALG_LU)"); return B2_ERR_INVALID; }
     if (!s || !s->factorized) { set_error("b2d_inertia: not factorized"); return B2_ERR_FACTORIZATION; }
     B2_CUDA(cudaMemcpyAsync(s->h_counters, s->counters.p, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, as_stream(stream)));
     return B2_OK;
 }
 
 int b2d_inertia_fetch(b2d_solver* s, int64_t* num_pos, int64_t* num_zero, int64_t* num_neg) {
+    if (s && s->lu) { set_error("b2d_inertia: an LU factorisation reports no inertia (opt.dense_algorithm = B2_DENSE_ALG_LU)"); return B2_ERR_INVALID; }
     if (!s || !s->factorized) { set_error("b2d_inertia: not factorized"); return B2_ERR_FACTORIZATION; }
     if (s->h_counters[2]) { set_error("b2d: a device-wide wait timed out (single-launch solve or Bunch-Kaufman panel)"); return B2_ERR_SOLVE; }
     const int64_t neg = s->h_counters[0], zero = s->h_counters[1];
@@ -1598,12 +1624,24 @@ int b2d_solve(b2d_solver* s, double* x_d, int32_t nrhs, void* stream) {
         cudaFuncSetAttribute(k_dense_solve_flow<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
     static const bool flow_bk_ok =
         cudaFuncSetAttribute(k_dense_solve_flow<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
+    static const bool flow_lu_ok =
+        cudaFuncSetAttribute(k_dense_solve_flow<DenseSolveKind::LU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_SMEM) == cudaSuccess;
+    if (s->lu && !(flow_lu_ok && nblk <= sm_count())) {
+        set_error("b2d_solve: the LU solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
+        return B2_ERR_INVALID;
+    }
     if (s->bunch_kaufman && !(flow_bk_ok && nblk <= sm_count())) {
         set_error("b2d_solve: the Bunch-Kaufman solve runs in one launch with one CTA per 128 rows and needs N <= 128 * (number of SMs)");
         return B2_ERR_INVALID;
     }
     for (int c = 0; c < nrhs; ++c) {
         double* x = x_d + (size_t)c * N;
+        if (s->lu) {
+            B2_CUDA(cudaMemsetAsync(s->flow.p, SLOT_EMPTY_BYTE, s->flow.bytes(), st));
+            k_dense_solve_flow<DenseSolveKind::LU><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->lum.uinv.p, x, s->flow.p,
+                                                                s->flow.p + (size_t)nblk * BS, s->counters.p + 2, s->lum.perm.p);
+            continue;
+        }
         if (s->bunch_kaufman) {
             B2_CUDA(cudaMemsetAsync(s->flow.p, SLOT_EMPTY_BYTE, s->flow.bytes(), st));
             k_dense_solve_flow<true><<<nblk, DS_NT, DS_SMEM, st>>>(N, s->fact.p, s->linv.p, s->dvec.p, x, s->flow.p, s->flow.p + (size_t)nblk * BS,
@@ -1644,6 +1682,20 @@ int b2d_get_pivots(b2d_solver* s, int32_t* ipiv_h, double* d_h, double* e_h) {
     B2_CUDA(cudaMemcpy(ipiv_h, s->bk.ipiv.p, s->bk.ipiv.bytes(), cudaMemcpyDeviceToHost));
     B2_CUDA(cudaMemcpy(d_h, s->dvec.p, (size_t)s->N * sizeof(double), cudaMemcpyDeviceToHost));
     B2_CUDA(cudaMemcpy(e_h, s->bk.evec.p, s->bk.evec.bytes(), cudaMemcpyDeviceToHost));
+    return B2_OK;
+}
+
+int b2d_get_lu(b2d_solver* s, int32_t* ipiv_h, int32_t* info_h, double* lu_h) {
+    if (!s) { set_error("b2d_get_lu: invalid argument"); return B2_ERR_INVALID; }
+    if (!s->lu) { set_error("b2d_get_lu: the handle factors L D L' (opt.dense_algorithm = 0)"); return B2_ERR_INVALID; }
+    if (!s->factorized) { set_error("b2d_get_lu: not factorized"); return B2_ERR_FACTORIZATION; }
+    B2_CUDA(cudaDeviceSynchronize());
+    int32_t c[3];
+    B2_CUDA(cudaMemcpy(c, s->counters.p, sizeof(c), cudaMemcpyDeviceToHost));
+    if (c[2]) { set_error("b2d_get_lu: a device-wide wait timed out (LU panel or single-launch solve)"); return B2_ERR_SOLVE; }
+    if (info_h) *info_h = c[0];
+    if (ipiv_h) B2_CUDA(cudaMemcpy(ipiv_h, s->lum.ipiv.p, s->lum.ipiv.bytes(), cudaMemcpyDeviceToHost));
+    if (lu_h) B2_CUDA(cudaMemcpy(lu_h, s->fact.p, (size_t)s->N * s->N * sizeof(double), cudaMemcpyDeviceToHost));
     return B2_OK;
 }
 

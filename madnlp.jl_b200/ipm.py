@@ -94,6 +94,10 @@ def resolve_inertia_correction_method(method, linear_solver):
         raise ValueError(f"inertia_correction_method must be one of {', '.join(INERTIA_CORRECTION_METHODS)}; got {method!r}")
     if method == "InertiaAuto":
         return "InertiaBased" if linear_solver.is_inertia() else "InertiaFree"
+    if method == "InertiaBased" and not linear_solver.is_inertia():
+        # (the reference fails later, when inertia() has no method for the solver)
+        raise ValueError(f"inertia_correction_method = InertiaBased needs a linear solver that reports inertia; "
+                         f"{type(linear_solver).__name__} ({linear_solver.introduce()}) does not: use InertiaAuto or InertiaFree")
     return method
 
 
@@ -136,8 +140,8 @@ class IPMLinearAlgebra:
     """Owns the work vectors of MadNLPSolver that the hot path touches (d, p, _w4) and drives one iteration.
 
     inertia_correction_method (MadNLP's option of the same name): "InertiaBased" (the default), "InertiaFree" (the curvature test
-    of Chiang & Zavala; it reads solver_vectors, which load_ifr_inputs fills), "InertiaIgnore", or "InertiaAuto" (InertiaBased with every
-    solver of this package, since each reports inertia).  inertia_free_tol is the curvature test's tolerance (default 0).
+    of Chiang & Zavala; it reads solver_vectors, which load_ifr_inputs fills), "InertiaIgnore", or "InertiaAuto" (InertiaBased when the
+    linear solver reports inertia, InertiaFree otherwise: B200DenseSolver with LU reports none).  inertia_free_tol is the curvature test's tolerance (default 0).
 
     iterator (MadNLP's option of the same name): "RichardsonIterator" (the default) or "KrylovIterator" (krylov.py: restarted GMRES
     preconditioned on the right by the KKT solve, with krylov_options passed to it, e.g. krylov_restart, krylov_max_iter).  With

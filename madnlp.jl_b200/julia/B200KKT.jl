@@ -39,17 +39,20 @@ Base.@kwdef mutable struct B200Options <: AbstractOptions
                                         # lapack_algorithm = BUNCHKAUFMAN (B2_DENSE_PIVOT_BUNCH_KAUFMAN); B200Solver needs 0
     b200_sparse_pivoting::Int32 = 0     # B200Solver only: 0 static (B2_SPARSE_PIVOT_STATIC), 1 2x2 pivots on matched
                                         # primal-dual pairs (B2_SPARSE_PIVOT_PAIRS); B200DenseSolver needs 0
+    b200_dense_algorithm::Int32 = 0     # B200DenseSolver only: 0 LDL' (B2_DENSE_ALG_LDLT), 1 LU with partial pivoting, as
+                                        # lapack_algorithm = LU (B2_DENSE_ALG_LU, no inertia: InertiaAuto is InertiaFree);
+                                        # B200Solver needs 0
 end
 
 struct CB2Options
     ordering::Int32; nemin::Int32; relax_zeros::Float64; pivot_eps::Float64
     use_cuda_graph::Int32; small_front_max::Int32; n_parts::Int32; part_rank::Int32
     kkt_n_primal::Int32; fuse_max_fronts::Int32; dep_schedule::Int32; chain_merge_f::Int32; kkt_n_dual::Int32; dense_pivoting::Int32
-    sparse_pivoting::Int32; reserved::NTuple{1,Int32}
+    sparse_pivoting::Int32; dense_algorithm::Int32
 end
 CB2Options(o::B200Options) = CB2Options(o.b200_ordering, o.b200_nemin, o.b200_relax_zeros, o.b200_pivot_eps,
     o.b200_use_cuda_graph, o.b200_small_front_max, 1, 0, o.b200_kkt_n_primal, o.b200_fuse_max_fronts, o.b200_dep_schedule, o.b200_chain_merge_f,
-    o.b200_kkt_n_dual, o.b200_dense_pivoting, o.b200_sparse_pivoting, ntuple(_ -> Int32(0), 1))
+    o.b200_kkt_n_dual, o.b200_dense_pivoting, o.b200_sparse_pivoting, o.b200_dense_algorithm)
 
 last_error() = unsafe_string(ccall((:b2_last_error, libb200kkt), Cstring, ()))
 function check(rc::Cint, exc)
@@ -245,14 +248,16 @@ end
 factorize!(M::B200DenseSolver) = (check(ccall((:b2d_factorize, libb200kkt), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), M.handle, stream_ptr()), FactorizationException); M)
 solve_linear_system!(M::B200DenseSolver{T}, x::CuVector{T}) where T =
     (check(ccall((:b2d_solve, libb200kkt), Cint, (Ptr{Cvoid}, CuPtr{T}, Int32, Ptr{Cvoid}), M.handle, pointer(x), 1, stream_ptr()), SolveException); x)
-is_inertia(::B200DenseSolver) = true
+is_inertia(M::B200DenseSolver) = M.opt.b200_dense_algorithm == 0     # LU reports no inertia (lapack_common.jl:91)
 function inertia(M::B200DenseSolver)
+    M.opt.b200_dense_algorithm == 0 || error("B200DenseSolver: an LU factorisation (b200_dense_algorithm = 1) reports no inertia")
     p = Ref{Int64}(0); z = Ref{Int64}(0); n = Ref{Int64}(0)
     check(ccall((:b2d_inertia, libb200kkt), Cint, (Ptr{Cvoid}, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Cvoid}), M.handle, p, z, n, stream_ptr()), FactorizationException)
     return (Int(p[]), Int(z[]), Int(n[]))
 end
 improve!(::B200DenseSolver) = false
-introduce(M::B200DenseSolver) = M.opt.b200_dense_pivoting == 1 ? "b200kkt dense LDL' (Bunch-Kaufman pivoting)" : "b200kkt dense LDL' (DMMA)"
+introduce(M::B200DenseSolver) = M.opt.b200_dense_algorithm == 1 ? "b200kkt dense LU (partial pivoting)" :
+    M.opt.b200_dense_pivoting == 1 ? "b200kkt dense LDL' (Bunch-Kaufman pivoting)" : "b200kkt dense LDL' (DMMA)"
 input_type(::Type{<:B200DenseSolver}) = :dense
 default_options(::Type{<:B200DenseSolver}) = B200Options()
 is_supported(::Type{<:B200DenseSolver}, ::Type{Float64}) = true

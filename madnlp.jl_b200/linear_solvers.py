@@ -135,8 +135,9 @@ class B200SparseSolver:
 
 class B200DenseSolver:
     """Blocked dense LDL^T on the fp64 tensor pipe (role of LapackCUDASolver / LapackCPUSolver{BUNCHKAUFMAN},
-    src/LinearSolvers/lapack.jl:164-172, cusolver.jl:150-187).  `A` is an N x N column-major device matrix kept by
-    reference; only its lower triangle is read."""
+    src/LinearSolvers/lapack.jl:164-172, cusolver.jl:150-187), or with opt.dense_algorithm = B2_DENSE_ALG_LU the LU with
+    partial pivoting of the mirrored matrix (lapack_algorithm = LU, lapack.jl:174-187), which reports no inertia.  `A` is an
+    N x N column-major device matrix kept by reference; only its lower triangle is read."""
     input_type = "dense"
 
     def __init__(self, A, opt: capi.Options | None = None, stream=None):
@@ -164,7 +165,12 @@ class B200DenseSolver:
     def is_supported(dtype) -> bool:
         return np.dtype(dtype) == np.float64
 
+    def _is_lu(self) -> bool:
+        return self.opt.dense_algorithm == capi.B2_DENSE_ALG_LU
+
     def introduce(self) -> str:
+        if self._is_lu():
+            return f"b200kkt dense LU (partial pivoting) v{lib.b2_version()}"
         if self.opt.dense_pivoting == capi.B2_DENSE_PIVOT_BUNCH_KAUFMAN:
             return f"b200kkt dense LDL^T (Bunch-Kaufman pivoting) v{lib.b2_version()}"
         return f"b200kkt dense LDL^T (DMMA) v{lib.b2_version()}"
@@ -176,6 +182,14 @@ class B200DenseSolver:
         e = np.empty(self.n, dtype=np.float64)
         check(lib.b2d_get_pivots(self._h, ipiv.ctypes.data, d.ctypes.data, e.ctypes.data))
         return ipiv, d, e
+
+    def lu(self, factors: bool = True):
+        """An LU factor as LAPACK dgetrf leaves it (b2d_get_lu): (ipiv 1-based, info, the packed N x N LU or None); synchronises."""
+        ipiv = np.empty(self.n, dtype=np.int32)
+        info = C.c_int32()
+        lu = np.empty((self.n, self.n), dtype=np.float64, order="F") if factors else None
+        check(lib.b2d_get_lu(self._h, ipiv.ctypes.data, C.byref(info), lu.ctypes.data if factors else None))
+        return ipiv, int(info.value), lu
 
     def is_async(self) -> bool:
         return True
@@ -190,7 +204,7 @@ class B200DenseSolver:
         return x
 
     def is_inertia(self) -> bool:
-        return True
+        return not self._is_lu()             # LU reports no inertia (lapack_common.jl:91)
 
     def inertia(self):
         p, z, n = C.c_int64(), C.c_int64(), C.c_int64()
